@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- headline benchmark: Atlas (floating base, nv = 36) forward-dynamics evaluations per second.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch B] [--dtype f32|f64]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--batch B] [--dtype f32|f64] [--dump-outputs DIR]
 
 Workload (BASELINE.json metric, SURVEY 8(d) "Headline"): Atlas v5 with a QuaternionFloating root (nq 37, nv 36, 31 bodies),
 `dynamics!` with joint torques, fp32, batch 2^20 per GPU.  A "step" is one pass of the forward-dynamics kernel over the whole
@@ -14,6 +14,10 @@ One JSON line on stdout (rank 0).  `value` = evaluations/s with inputs resident 
 `cpu_baseline` = the CPU oracle (port of the reference's CRBA + RNEA + Cholesky path) on a bounded sample.
 
 `--impl reference` times that CPU path alone (the reference itself is Julia and cannot run here; see DESIGN.md).
+
+`--dump-outputs DIR` writes, after the timed steps, the v̇ of the last timed step as DIR/vd.npy ([36, n], the run's dtype): every
+column when the batch has at most 2^18 (fp64: 2^17) samples, else that many columns chosen by numpy PCG64 seed 0 (sorted), so
+that two builds can be compared output for output on identical inputs.
 """
 from __future__ import annotations
 
@@ -34,6 +38,22 @@ BYTES_PER_EVAL = {"f32": 580, "f64": 1160}      # (37 + 36 + 36 in, 36 out) scal
 METRIC = "ABA evals/sec for Atlas 30-DoF at batch 2^20; achieved HBM GB/s vs peak"
 
 
+H100_HBM_GBS = 3350.0       # NVIDIA H100 SXM data sheet; used only when no measured peak is at hand
+DUMP_COLUMNS = 1 << 18      # 36 x 2^18 fp64 = 75 MB would exceed 64 MB: fp64 dumps take half as many columns
+
+
+def dump_outputs(d, vd):
+    """v̇ of the last timed step -> d/vd.npy: every column, or a fixed seeded sample of them (see the module docstring)."""
+    import torch
+    os.makedirs(d, exist_ok=True)
+    B = vd.shape[1]
+    n = DUMP_COLUMNS if vd.dtype == torch.float32 else DUMP_COLUMNS // 2
+    if B > n:
+        cols = np.sort(np.random.Generator(np.random.PCG64(0)).choice(B, n, replace=False))
+        vd = vd[:, torch.from_numpy(cols).to(vd.device)]
+    np.save(os.path.join(d, "vd.npy"), vd.cpu().numpy())
+
+
 def make_inputs(mech, B, seed):
     """rand!(state) + random torques, host fp64, [rows, B]."""
     rng = np.random.Generator(np.random.PCG64(seed))
@@ -49,7 +69,7 @@ def make_inputs(mech, B, seed):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled while the GPU is under load (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled while the GPU is under load."""
     FIELDS = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
               "clocks_event_reasons.sw_power_cap")
@@ -307,8 +327,7 @@ def other_configs(steps):
 
 
 def add_rooflines(cfgs, peak):
-    """Per-config roofline objects (HBM, algorithmic bytes) next to the raw rates; ncu summaries of the kernels behind them are under
-    profiles/r2_*_summary.txt (dram__bytes_read/write, issue-active, stall reasons)."""
+    """Per-config roofline objects (HBM, algorithmic bytes) next to the raw rates."""
     for k, c in cfgs.items():
         if isinstance(c, dict) and "algorithmic_GBps" in c:
             c["roofline"] = {"bound": "hbm", "achieved": c["algorithmic_GBps"], "peak": peak, "unit": "GB/s",
@@ -387,15 +406,15 @@ def run_config5(rbd, mech, dist, world, rank, args, tdt):
             "nvlink_bytes_sent_per_gpu_per_step": (world - 1) * nv * Bl * es,
             "nvlink_bytes_received_per_gpu_per_step": (world - 1) * nv * Bl * es,
             "note": "an all-gather of v̇ needs every GPU to RECEIVE (N-1)/N of the 604 MB result per step, so NVLink ingress bounds "
-                    "any gather at N=8 near 0.59 ms per 2^22 samples (7.1 G evals/s at 900 GB/s)"},
+                    "any gather at N=8 near 1.2 ms per 2^22 samples (3.6 G evals/s at H100's 450 GB/s per direction)"},
         "strong_scaling": {"value": no_gather, "unit": "evals/s", "total_batch": total, "batch_per_gpu": Bl,
                            "note": "same total work at every N (config 5 without the gather); the headline `value` is weak scaling"},
     }
 
 
 def bind_to_gpu_numa_node(local_rank):
-    """Run this rank's threads on, and allocate its pinned buffers from, the NUMA node its GPU hangs off (nvidia-smi topo: on the
-    8-GPU boxes GPUs 0-3 sit on node 0 and 4-7 on node 1; unbound ranks were measured at 38.7 instead of 62.9 GB/s of PCIe)."""
+    """Run this rank's threads on, and allocate its pinned buffers from, the NUMA node its GPU hangs off (nvidia-smi topo): a
+    rank bound to the other socket's node crosses the inter-socket link for every host copy."""
     info = {"node": None, "cpus": None}
     try:
         import torch
@@ -487,6 +506,8 @@ def main():
     ap.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg")
     ap.add_argument("--no-config5", action="store_true", help="N > 1: skip BASELINE config 5 (2^22 samples in total, result gather timed)")
     ap.add_argument("--no-other", action="store_true", help="skip the secondary configs (fp64, RNEA, CRBA, ext. wrenches)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's v̇ (a seeded sample of its "
+                    "columns beyond 2^18 samples) to DIR/vd.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.impl == "reference":
@@ -538,6 +559,8 @@ def main():
     barrier()
     t_wall1 = time.time()
     ms = ev0.elapsed_time(ev1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, result.vd)
     # keep the GPU under the same load until the sampler has a few readings inside a loaded window
     t_load_end = t_wall1
     if sampler and (t_wall1 - t_wall0) < 0.6:
@@ -595,24 +618,15 @@ def main():
                 peaks = json.load(f)
         except OSError:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
+        peak = float(peaks.get("hbm_gbs", H100_HBM_GBS))
         bpe = BYTES_PER_EVAL[args.dtype]
         achieved = (B * args.steps / (ms * 1e-3)) * bpe / 1e9       # per GPU
-        traffic, traffic_src = None, None
-        try:        # DRAM bytes per launch from the committed ncu --set full capture of this exact workload (same kernels, same batch)
-            with open(os.path.join(ROOT, "profiles", "r2_traffic.json")) as f:
-                for name, rec in json.load(f).items():
-                    if rec["samples"] == B and args.dtype == "f32":
-                        traffic = rec["dram_bytes_read"] + rec["dram_bytes_write"]
-                        traffic_src = {"capture": name, "command": rec.get("command"), "bytes_per_sample": traffic / B}
-        except (OSError, KeyError, ValueError):
-            pass
         out = {
             "metric": METRIC, "value": value, "unit": "evals/s", "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ms / args.steps, "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None, "dtype": args.dtype, "data": "synthetic",
             "config": {"workload": f"atlas floating-base (nq 37, nv 36) dynamics! = ABA, batch {B} per GPU, {args.dtype}",
-                       "batch_per_gpu": B, "l2": "inputs (109 rows x batch) exceed the 126 MB L2; no reuse between steps",
+                       "batch_per_gpu": B, "l2": f"inputs (109 rows x batch = {109 * B * es / 1e6:.0f} MB) against the 50 MB L2",
                        "parallelism": f"batch-sharded x{world}, no data-path collective"},
             "clocks": clocks,
             "e2e": {"value": e2e_val, "unit": "evals/s", "h2d_bytes_per_step": (37 + 36 + 36) * B * es,
@@ -621,28 +635,12 @@ def main():
             "launch": {"grid": linfo.grid, "block": linfo.block, "smem_bytes": linfo.smem_bytes,
                        "blocks_per_sm": linfo.blocks_per_sm},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": traffic, "traffic_source": traffic_src, "algorithmic_bytes_per_launch": B * bpe,
-                         "peak_source": "MEASURED_PEAKS.json" if peaks else "fallback 6650 GB/s",
-                         "kernels": "model-specialised (NVRTC) pair / unified CTA" if linfo.specialised else "generic kernel pair",
-                         "note": "algorithmic bytes/eval x evals/s per GPU; traffic = ncu dram bytes per launch of the same workload "
-                                 "(profiles/r2_traffic.json, not measured in this run).  The kernel is bound by instruction supply, not by "
-                                 "HBM: the model-specialised program is ~12.4 k warp-instructions per 32 samples (generic: 27.5 k) but "
-                                 "streams from L2 at ~1.4 instr/clk/SM (ncu: no_instruction stalls dominate, profiles/r2_jit_aba_*)"},
+                         "algorithmic_bytes_per_launch": B * bpe,
+                         "peak_source": "MEASURED_PEAKS.json" if peaks else "H100 SXM data sheet (3.35 TB/s), not measured",
+                         "kernels": "model-specialised (NVRTC) kernel" if linfo.specialised else "generic kernel",
+                         "note": "algorithmic bytes/eval x evals/s per GPU.  The kernel is latency- and instruction-bound, not "
+                                 "HBM-bound: this fraction is far below 1 by design (DESIGN.md)"},
         }
-        # The roofline that actually bounds this kernel: warp-instruction ISSUE (4 schedulers x 1 instruction/clk per SM).  The executed
-        # instruction count per 32 samples is ncu's smsp__inst_executed of the specialised program (profiles/r2_jit_aba_*: 12.4 k; the
-        # generic kernel pair: 27.5 k, profiles/r1_aba_f32_fast_smem_kernel_2p20_summary.txt) -- a constant of the program, not measured
-        # in this run; the clock is the one sampled under load above.
-        try:
-            if args.dtype == "f32" and clocks and clocks.get("sm_mhz"):
-                wi = 12.4e3 if linfo.specialised else 27.5e3
-                ipc_peak = 148 * 4 * float(clocks["sm_mhz"]) * 1e6
-                issued = value / world / 32.0 * wi
-                out["roofline_issue"] = {"bound": "warp-instruction issue", "achieved": issued / 1e9, "peak": ipc_peak / 1e9,
-                                         "unit": "G warp-instr/s", "frac": issued / ipc_peak, "warp_instr_per_32_samples": wi,
-                                         "evals_per_s_at_peak_issue": ipc_peak / wi * 32.0}
-        except Exception:      # a descriptor, never a reason to lose the bench line
-            pass
         if config5:
             out["with_nccl_gather"] = config5["with_nccl_gather"]
             out["strong_scaling"] = config5["strong_scaling"]

@@ -1,7 +1,7 @@
 /*
- * rbd_b200.h -- C ABI of librbd_b200.so: batched rigid-body dynamics on NVIDIA B200 (sm_100a).
+ * rbd_b200.h -- C ABI of librbd_b200.so: batched rigid-body dynamics on NVIDIA H100 (sm_90a).
  *
- * This is the drop-in boundary for ONE path of RigidBodyDynamics.jl v2.5.0 (reference at /root/reference):
+ * This is the drop-in boundary for ONE path of RigidBodyDynamics.jl v2.5.0 (the reference):
  * dynamics!, inverse_dynamics!, mass_matrix!, dynamics_bias! evaluated over a batch of (q, v, tau) states.
  * The reference has no FFI of its own (it is 100 % Julia; SURVEY.md finding 2), so each entry point below
  * names the Julia generic function it replaces; a Julia shim (julia/RBDB200.jl, INTEGRATION.md) `ccall`s
@@ -135,7 +135,7 @@ int32_t rbd_get_launch_info(rbd_launch_info* info);
 /*
  * Model-specialised kernels.  For a given handle the library can generate straight-line CUDA code for dynamics! /
  * inverse_dynamics! / dynamics_bias! / mass_matrix! of THAT mechanism (tree walk unrolled, joint classes resolved, model constants folded,
- * structural zeros removed), compile it with NVRTC for sm_100a and keep the cubin in a disk cache
+ * structural zeros removed), compile it with NVRTC for sm_90a and keep the cubin in a disk cache
  * ($RBD_JIT_CACHE, else <library dir>/jit_cache, else ~/.cache/rbd_b200).  This is the analogue of the reference compiling
  * its generic functions for a concrete MechanismState{X,M,C} on first call (Julia's JIT).
  * Entry points use a specialised kernel when its cubin is cached or the batch is at least RBD_JIT_MIN_BATCH (default 32768)

@@ -13,7 +13,7 @@
 // "pinned by identities + agreement of independent formulations", not by reference-produced vectors;
 // quaternion/MRP -> rotation for NON-unit inputs is "parity unpinned" (Rotations.jl is not in the tree).
 //
-// What is restated (file:line relative to /root/reference/src):
+// What is restated (file:line relative to the reference's src/, RigidBodyDynamics.jl v2.5.0):
 //   kinematic caches, world frame      mechanism_state.jl:687-868
 //   CRBA  mass_matrix!                 mechanism_algorithms.jl:248-272
 //   RNEA  bias/spatial accelerations   mechanism_algorithms.jl:377-417

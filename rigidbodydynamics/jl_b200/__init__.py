@@ -1,7 +1,7 @@
-"""rigidbodydynamics.jl_b200 -- batched rigid-body dynamics on NVIDIA B200.
+"""rigidbodydynamics.jl_b200 -- batched rigid-body dynamics on NVIDIA H100.
 
 Drop-in for ONE path of RigidBodyDynamics.jl: ``dynamics!``, ``inverse_dynamics!``, ``mass_matrix!``, ``dynamics_bias!``
-on ``Mechanism`` / ``MechanismState`` / ``DynamicsResult``, evaluated over a batch of states by hand-written sm_100a
+on ``Mechanism`` / ``MechanismState`` / ``DynamicsResult``, evaluated over a batch of states by hand-written sm_90a
 kernels behind a C ABI (``include/rbd_b200.h``, ``csrc/librbd_b200.so``).  This Python package is the host side above
 that ABI (Julia, the reference's language, is not available in the build image; ``julia/RBDB200.jl`` is the
 equivalent shim).  Importing the package does not need a GPU; calling a dynamics function does.

@@ -1,4 +1,4 @@
-// librbd_b200.so -- C ABI (include/rbd_b200.h) over the sm_100a kernels.
+// librbd_b200.so -- C ABI (include/rbd_b200.h) over the sm_90a kernels.
 //
 // Kernel design (DESIGN.md has the long version):
 //   * one THREAD owns one sample; a block is one or more independent warps; there are no block-level barriers;
@@ -28,7 +28,6 @@
 #include "rbd_kin.cuh"
 #include "rbd_dual.cuh"
 #include "rbd_integrate.cuh"
-#include "rbd_tmem.cuh"
 #include "rbd_model.h"
 
 using namespace rbd;
@@ -95,12 +94,11 @@ __device__ __forceinline__ void prefetch_rows(const T* base, int rows, int64_t l
 template <class T> struct AbaArgs {
   const T* q; const T* v; const T* tau; const T* wext;
   T* vd; T* qd;
-  T* scratch;            // [6 * nb][scratch_ld] body-frame external wrenches (EXT only), one column per resident thread
+  T* scratch;            // [6 * nb][grid threads] body-frame external wrenches (EXT only), one column per resident thread
   int64_t ld, B;
-  unsigned long long* counter;   // work queue shared by the two kernels of launch_duo
-  int64_t scratch_ld;            // columns of `scratch` (queue kernels)
-  int64_t scratch_off;           // first scratch column of the Tensor-Memory kernel's threads (after the shared-memory kernel's)
   const int* gate;               // non-NULL: run only if *gate != 0 (fallback behind the model-specialised kernels, rbd_spec.cpp)
+  // mixed CTA (launch_mix): work-queue counter, stash of the warps beyond `sw` in L2, stash rows, columns of `scratch`
+  unsigned long long* counter; T* l2; int sw, rows; int64_t scratch_ld;
 };
 
 // KINDS: compile-time promise about the 1-DoF kinds present (kAllKinds, or 0 = revolute / sin-cos-revolute only).
@@ -140,73 +138,13 @@ aba_kernel(const __grid_constant__ ModelDev<T> M, const AbaArgs<T> a) {
   }
 }
 
-// Work-queue variants for running the shared-memory kernel and the Tensor-Memory kernel SIDE BY SIDE on every SM (two
-// launches on two streams; groups of 32 samples are claimed from one atomic counter, so the kernels balance themselves).
-__device__ __forceinline__ int64_t claim_group(unsigned long long* counter) {
-  unsigned long long g = 0;
-  if ((threadIdx.x & 31) == 0) g = atomicAdd(counter, 1ull);
-  return (int64_t)__shfl_sync(0xffffffffu, g, 0);
-}
-template <class T, class ST, int KINDS, bool EXT>
-__device__ __forceinline__ void aba_queue_loop(const ModelDev<T>& M, const AbaArgs<T>& a, const ST& st, int64_t tid) {
-  constexpr int NT = 32;
-  const int lane = threadIdx.x & 31;
-  unsigned long long* counter = a.counter;
-  const int64_t ngroups = (a.B + NT - 1) / NT;
-  int64_t g = claim_group(counter);
-  while (g < ngroups) {
-    const int64_t gn = claim_group(counter);
-    if (gn < ngroups) {
-      const int64_t bn = gn * NT;
-      prefetch_rows(a.q, M.nq, a.ld, bn);
-      prefetch_rows(a.v, M.nv, a.ld, bn);
-      prefetch_rows(a.tau, M.nv, a.ld, bn);
-      if (EXT) prefetch_rows(a.wext, 6 * M.nb, a.ld, bn);
-    }
-    const int64_t b = g * NT + lane;
-    const bool active = b < a.B;
-    const int64_t bl = active ? b : a.B - 1;
-    AbaIO<T, EXT, KINDS> io;
-    io.q = {a.q + bl, a.ld};
-    io.v = {a.v + bl, a.ld};
-    io.tau = {a.tau ? a.tau + bl : nullptr, a.ld};
-    io.wext = {EXT ? a.wext + bl : nullptr, a.ld};
-    io.vd = {a.vd + bl, a.ld, active};
-    io.qd = {a.qd ? a.qd + bl : nullptr, a.ld, active};
-    io.ext = {EXT ? a.scratch + tid : nullptr, a.scratch_ld};
-    if (EXT) ext_wrench_pass(M, io.q, io.wext, io.ext, st, M.slot_base, kSlotRowsAba);
-    aba_sample<T, ST, false>(M, io, st);
-    g = gn;
-  }
-}
-template <class T, int KINDS, bool EXT>
-__global__ void __launch_bounds__(32, sizeof(T) == 4 ? 16 : 1) aba_kernel_smem_q(const __grid_constant__ ModelDev<T> M, const AbaArgs<T> a) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  aba_queue_loop<T, Stash<T, 32>, KINDS, EXT>(M, a, Stash<T, 32>{reinterpret_cast<T*>(smem_raw) + threadIdx.x},
-                                              (int64_t)blockIdx.x * 32 + threadIdx.x);
-}
-// CTA of NW = 4 or 8 warps over COLS TMEM columns.  Warp w may only touch TMEM lane quadrant w % 4, so warps 0-3 keep their
-// stash in the first COLS / (NW / 4) columns and warps 4-7 (same lanes) in the second half: in fp32 (one column per row,
-// <= 256 rows) one CTA fills all 512 columns with the working sets of 8 warps; fp64 needs two columns per row, 4 warps.
-// Register budget: the CTA shares the SM with the 8 single-warp blocks of aba_kernel_smem_q, 16 warps x 32 x 128 = 64 K.
-template <class T, int COLS, int KINDS, int NW, bool EXT>
-__global__ void __launch_bounds__(32 * NW, NW == 8 ? 2 : 1)
-aba_kernel_tmem_q(const __grid_constant__ ModelDev<T> M, const AbaArgs<T> a) {
-  __shared__ uint32_t tm_slot;
-  const uint32_t tm_base = tmem_alloc_cta<COLS>(&tm_slot);
-  using ST = typename StashTMFor<T>::type;
-  const uint32_t w = threadIdx.x >> 5;
-  aba_queue_loop<T, ST, KINDS, EXT>(M, a, ST{tm_base + (((w & 3u) * 32u) << 16) + (w >> 2) * (uint32_t)(COLS / (NW / 4))},
-                                    a.scratch_off + (int64_t)blockIdx.x * (32 * NW) + threadIdx.x);
-  tmem_free_cta<COLS>(tm_base);
-}
-
-
 // dynamics! on Dual{Float64,6} arrays: thread t of the launch owns (sample t / 6, partial direction t % 6).
 struct DualArgs {
   const double* q; const double* v; const double* tau;
   double* vd;
   int64_t ld, B;
+  unsigned long long* counter; Dual64* l2; int sw, rows;     // mixed CTA (launch_mix), see AbaArgs
+  double* scratch; int64_t scratch_ld;                         // unused: no external wrenches on this path
 };
 template <int NT, bool GENERAL>
 __global__ void __launch_bounds__(NT) aba_dual_kernel(const __grid_constant__ ModelDev<Dual64> M, const DualArgs a) {
@@ -233,41 +171,14 @@ __global__ void __launch_bounds__(NT) aba_dual_kernel(const __grid_constant__ Mo
   }
 }
 
-// Same evaluation with the stash split between shared memory (value parts) and Tensor Memory (partial parts): one 4-warp CTA/SM.
-__global__ void __launch_bounds__(128) aba_dual_kernel_tm(const __grid_constant__ ModelDev<Dual64> M, const DualArgs a) {
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  __shared__ uint32_t tm_slot;
-  const uint32_t tm_base = tmem_alloc_cta<512>(&tm_slot);
-  const StashDualTM st{reinterpret_cast<double*>(smem_raw) + threadIdx.x, tm_base + ((uint32_t)((threadIdx.x >> 5) * 32) << 16)};
-  const int64_t total = a.B * 6;
-  const int64_t ngroups = (total + 127) / 128;
-  for (int64_t g = blockIdx.x; g < ngroups; g += gridDim.x) {
-    const int64_t t = g * 128 + threadIdx.x;
-    const bool active = t < total;
-    const int64_t tl = active ? t : total - 1;
-    const int64_t b = tl / 6;
-    const int dir = (int)(tl - b * 6);
-    AbaIO<Dual64, false> io;
-    io.q = {a.q + b * kDualWidth, a.ld, dir};
-    io.v = {a.v + b * kDualWidth, a.ld, dir};
-    io.tau = {a.tau ? a.tau + b * kDualWidth : nullptr, a.ld, dir};
-    io.wext = {nullptr, a.ld, dir};
-    io.vd = {a.vd + b * kDualWidth, a.ld, dir, active};
-    io.qd = {nullptr, a.ld, dir, active};
-    io.ext = {nullptr, 0};
-    aba_sample<Dual64, StashDualTM, false>(M, io, st);
-  }
-  tmem_free_cta<512>(tm_base);
-}
-
 template <class T> struct RneaArgs {
   const T* q; const T* v; const T* vd; const T* wext;
   T* tau;
   T* scratch;
   int64_t ld, B;
-  unsigned long long* counter;
-  int64_t scratch_ld, scratch_off;
   const int* gate;               // see AbaArgs
+  // mixed CTA (launch_mix): work-queue counter, stash of the warps beyond `sw` in L2, stash rows, columns of `scratch`
+  unsigned long long* counter; T* l2; int sw, rows; int64_t scratch_ld;
 };
 
 template <class T, int NT, bool EXT>
@@ -300,24 +211,72 @@ __global__ void __launch_bounds__(NT, sizeof(T) == 4 ? 32 : 1) rnea_kernel(const
   }
 }
 
-// Work-queue variants of the RNEA kernel (no external wrenches): shared-memory blocks + one Tensor-Memory CTA per SM.
-template <class T, class ST, bool EXT>
-__device__ __forceinline__ void rnea_queue_loop(const ModelDev<T>& M, const RneaArgs<T>& a, const ST& st, int64_t tid) {
-  constexpr int NT = 32;
+// ---- mixed CTA: a second home for the stash in L2 -------------------------------------------------------------------------
+// One CTA of up to kMixWarps<T> warps per SM (launch_mix).  Warps 0 .. sw-1 keep their stash in the CTA's shared memory, the
+// others in a pool-allocated global scratch [block][warp][row][lane] small enough to stay resident in L2.  On H100 shared
+// memory holds 8 Atlas fp32 stashes (4 in fp64, 2 of Dual<6>) while the register file has room for twice as many warps; the
+// L2 warps fill it.  Warps claim groups of 32 samples from one counter, so the slower L2 warps simply take fewer groups.
+template <class T> constexpr int kMixWarps = sizeof(T) == 4 ? 16 : 8;     // x 32 threads x 128 / 255 registers: the register file
+template <class E>
+__device__ __forceinline__ E* mix_stash(E* smem, E* l2, int sw, int rows) {
+  const int w = threadIdx.x >> 5, nw = blockDim.x >> 5;
+  E* base = w < sw ? smem + (size_t)w * rows * 32 : l2 + ((size_t)blockIdx.x * (nw - sw) + (w - sw)) * rows * 32;
+  return base + (threadIdx.x & 31);
+}
+__device__ __forceinline__ int64_t claim_group(unsigned long long* counter) {
+  unsigned long long g = 0;
+  if ((threadIdx.x & 31) == 0) g = atomicAdd(counter, 1ull);
+  return (int64_t)__shfl_sync(0xffffffffu, g, 0);
+}
+// (No external wrenches: with them the mixed CTA measured slower on H100 than the shared-memory kernel, DESIGN.md 4.1.)
+template <class T, int KINDS>
+__global__ void __launch_bounds__(32 * kMixWarps<T>, 1) aba_kernel_mix(const __grid_constant__ ModelDev<T> M, const AbaArgs<T> a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const Stash<T, 32> st{mix_stash(reinterpret_cast<T*>(smem_raw), a.l2, a.sw, a.rows)};
   const int lane = threadIdx.x & 31;
-  unsigned long long* counter = a.counter;
-  const int64_t ngroups = (a.B + NT - 1) / NT;
-  int64_t g = claim_group(counter);
+  const int64_t ngroups = (a.B + 31) / 32;
+  int64_t g = claim_group(a.counter);
   while (g < ngroups) {
-    const int64_t gn = claim_group(counter);
+    const int64_t gn = claim_group(a.counter);
     if (gn < ngroups) {
-      const int64_t bn = gn * NT;
+      const int64_t bn = gn * 32;
+      prefetch_rows(a.q, M.nq, a.ld, bn);
+      prefetch_rows(a.v, M.nv, a.ld, bn);
+      prefetch_rows(a.tau, M.nv, a.ld, bn);
+    }
+    const int64_t b = g * 32 + lane;
+    const bool active = b < a.B;
+    const int64_t bl = active ? b : a.B - 1;
+    AbaIO<T, false, KINDS> io;
+    io.q = {a.q + bl, a.ld};
+    io.v = {a.v + bl, a.ld};
+    io.tau = {a.tau ? a.tau + bl : nullptr, a.ld};
+    io.wext = {nullptr, a.ld};
+    io.vd = {a.vd + bl, a.ld, active};
+    io.qd = {a.qd ? a.qd + bl : nullptr, a.ld, active};
+    io.ext = {nullptr, 0};
+    aba_sample<T, Stash<T, 32>, false>(M, io, st);
+    g = gn;
+  }
+}
+template <class T, bool EXT>
+__global__ void __launch_bounds__(32 * kMixWarps<T>, 1) rnea_kernel_mix(const __grid_constant__ ModelDev<T> M, const RneaArgs<T> a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const Stash<T, 32> st{mix_stash(reinterpret_cast<T*>(smem_raw), a.l2, a.sw, a.rows)};
+  const int64_t tid = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const int lane = threadIdx.x & 31;
+  const int64_t ngroups = (a.B + 31) / 32;
+  int64_t g = claim_group(a.counter);
+  while (g < ngroups) {
+    const int64_t gn = claim_group(a.counter);
+    if (gn < ngroups) {
+      const int64_t bn = gn * 32;
       prefetch_rows(a.q, M.nq, a.ld, bn);
       prefetch_rows(a.v, M.nv, a.ld, bn);
       prefetch_rows(a.vd, M.nv, a.ld, bn);
       if (EXT) prefetch_rows(a.wext, 6 * M.nb, a.ld, bn);
     }
-    const int64_t b = g * NT + lane;
+    const int64_t b = g * 32 + lane;
     const bool active = b < a.B;
     const int64_t bl = active ? b : a.B - 1;
     RneaIO<T> io;
@@ -331,23 +290,27 @@ __device__ __forceinline__ void rnea_queue_loop(const ModelDev<T>& M, const Rnea
     g = gn;
   }
 }
-template <class T, bool EXT>
-__global__ void __launch_bounds__(32, sizeof(T) == 4 ? 16 : 1) rnea_kernel_smem_q(const __grid_constant__ ModelDev<T> M,
-                                                                                   const RneaArgs<T> a) {
+__global__ void __launch_bounds__(32 * kMixWarps<double>, 1) aba_dual_kernel_mix(const __grid_constant__ ModelDev<Dual64> M, const DualArgs a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  rnea_queue_loop<T, Stash<T, 32>, EXT>(M, a, Stash<T, 32>{reinterpret_cast<T*>(smem_raw) + threadIdx.x},
-                                        (int64_t)blockIdx.x * 32 + threadIdx.x);
-}
-template <class T, int COLS, int NW, bool EXT>
-__global__ void __launch_bounds__(32 * NW, NW == 8 ? 2 : 1)
-rnea_kernel_tmem_q(const __grid_constant__ ModelDev<T> M, const RneaArgs<T> a) {
-  __shared__ uint32_t tm_slot;
-  const uint32_t tm_base = tmem_alloc_cta<COLS>(&tm_slot);
-  using ST = typename StashTMFor<T>::type;
-  const uint32_t w = threadIdx.x >> 5;
-  rnea_queue_loop<T, ST, EXT>(M, a, ST{tm_base + (((w & 3u) * 32u) << 16) + (w >> 2) * (uint32_t)(COLS / (NW / 4))},
-                              a.scratch_off + (int64_t)blockIdx.x * (32 * NW) + threadIdx.x);
-  tmem_free_cta<COLS>(tm_base);
+  const Stash<Dual64, 32> st{mix_stash(reinterpret_cast<Dual64*>(smem_raw), a.l2, a.sw, a.rows)};
+  const int64_t total = a.B * 6;
+  const int64_t ngroups = (total + 31) / 32;
+  for (int64_t g = claim_group(a.counter); g < ngroups; g = claim_group(a.counter)) {
+    const int64_t t = g * 32 + (threadIdx.x & 31);
+    const bool active = t < total;
+    const int64_t tl = active ? t : total - 1;
+    const int64_t b = tl / 6;
+    const int dir = (int)(tl - b * 6);
+    AbaIO<Dual64, false> io;
+    io.q = {a.q + b * kDualWidth, a.ld, dir};
+    io.v = {a.v + b * kDualWidth, a.ld, dir};
+    io.tau = {a.tau ? a.tau + b * kDualWidth : nullptr, a.ld, dir};
+    io.wext = {nullptr, a.ld, dir};
+    io.vd = {a.vd + b * kDualWidth, a.ld, dir, active};
+    io.qd = {nullptr, a.ld, dir, active};
+    io.ext = {nullptr, 0};
+    aba_sample<Dual64, Stash<Dual64, 32>, false>(M, io, st);
+  }
 }
 
 template <class T> struct CrbaArgs {
@@ -528,74 +491,48 @@ template <class T> void set_scratch(CrbaArgs<T>&, T*) {}
 
 constexpr int kNT = 32;   // threads per block: one warp; warps never synchronise with each other
 
-// Shared-memory kernel on `stream` plus Tensor-Memory kernel (one CTA per SM, stash in TMEM, no shared memory) on the handle's
-// side stream, both claiming groups of 32 samples from one atomic counter.  fp32: one stash row = one TMEM column, so the 512
-// columns hold the stash of 8 warps (two column halves x four lane quadrants); fp64: two columns per row, 4 warps.  On Atlas
-// that is 8 + 8 resident warps/SM in fp32 (16 x 32 x 128 registers = the whole register file) and 4 + 4 in fp64.
-// `used` = false (and nothing launched) when the batch is too small to feed both kernels or RBD_NO_TMEM is set.
-// Which entry points use the kernel pair by default (RBD_DUO_RNEA=0/1, RBD_DUO_EXT=0/1 override).
-constexpr bool kDuoRneaDefault = true, kDuoExtDefault = true;
-inline bool duo_enabled(const char* env, bool dflt) {
-  const char* e = getenv(env);
-  return e ? (e[0] != '0') : dflt;
-}
-
-template <class T, class KS, class KT, class Args>
-int launch_duo(const rbd_model* model, KS ks, KT kt, int tm_warps, const ModelDev<T>& M, Args a, int rows, int scratch_rows,
-               cudaStream_t stream, bool& used) {
+// The mixed CTA (see aba_kernel_mix) in place of the shared-memory kernel `ks`: one CTA of up to `nw` warps per SM, as many
+// as the registers allow, `sw` of them with their stash in shared memory and the rest in an L2 scratch of at most 60 % of
+// the L2.  `used` = false (nothing launched) when that does not put at least 15 % more warps on the SM than `ks` gets, when
+// the batch has fewer groups of 32 than the CTAs have warps, or with RBD_JIT_VARIANT=1 (shared-memory kernels only).
+template <class KS, class KM, class Dev, class Args>
+int launch_mix(const rbd_model* model, KS ks, KM km, int nw, const Dev& M, Args a, size_t warp_bytes, int64_t ngroups,
+               int scratch_rows, cudaStream_t stream, bool& used) {
   used = false;
-  static const bool no_tmem = getenv("RBD_NO_TMEM") != nullptr;
-  static const int smem_blocks = getenv("RBD_SMEM_BLOCKS") ? atoi(getenv("RBD_SMEM_BLOCKS")) : 0;
-  if (no_tmem) return RBD_OK;
+  if (const char* f = getenv("RBD_JIT_VARIANT")) if (atoi(f) == 1) return RBD_OK;
   DeviceProps p;
   if (int rc = get_props(p)) return rc;
-  const int64_t ngroups = (a.B + kNT - 1) / kNT;
-  const size_t smem = (size_t)rows * kNT * sizeof(T);
-  int bps = 0;
-  if (int rc = configure(ks, kNT, smem, p, bps)) return rc;
-  if (int rc = configure_once((const void*)kt, p)) return rc;
-  {
-    // leave room in the register file for the Tensor-Memory CTA: small models are not limited by shared memory and the
-    // persistent shared-memory blocks would otherwise keep that CTA off the SM until they drain the queue
-    cudaFuncAttributes fs{}, ft{};
-    CUDA_TRY(cudaFuncGetAttributes(&fs, ks));
-    CUDA_TRY(cudaFuncGetAttributes(&ft, kt));
-    const int rs = ((fs.numRegs + 7) / 8) * 8 * kNT, rt = ((ft.numRegs + 7) / 8) * 8 * 32 * tm_warps;
-    const int with_pair = std::max(1, std::min(bps, (65536 - rt) / rs));
-    // The pair only pays when shared memory (not the register file) limits the single kernel's residency: small models
-    // already fill the SM with shared-memory blocks and are faster on the single-kernel path.
-    if ((with_pair + tm_warps) * 100 < bps * 115) return RBD_OK;
-    bps = with_pair;
-  }
-  if (smem_blocks > 0) bps = std::max(1, std::min(bps, smem_blocks));
-  if (ngroups < (int64_t)(bps + tm_warps / 2) * p.sms) return RBD_OK;     // not enough work to keep both kernels' warps busy
-  rbd_model* mm = const_cast<rbd_model*>(model);
-  PairCtx ctx;      // side stream, fork / join events and a zeroed queue counter, all cached in the handle
-  CUDA_TRY(pair_begin(mm, stream, ctx));
-  cudaStream_t side = ctx.side;
-  cudaEvent_t fork = ctx.fork, join = ctx.join;
+  int bps = 0, l2 = 0;
+  if (int rc = configure(ks, kNT, warp_bytes, p, bps)) return rc;
+  if (int rc = configure_once((const void*)km, p)) return rc;
+  cudaFuncAttributes fa{};
+  CUDA_TRY(cudaFuncGetAttributes(&fa, km));
+  CUDA_TRY(cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, p.dev));
+  const int fit = std::min(nw, 65536 / (((fa.numRegs + 7) / 8) * 8 * 32));
+  const int sw = std::min<int>(fit, (int)((p.max_smem_optin - (int)fa.sharedSizeBytes) / warp_bytes));
+  const int gw = (int)std::min<int64_t>(fit - sw, (int64_t)(0.6 * l2) / ((int64_t)p.sms * (int64_t)warp_bytes));
+  const int total = sw + std::max(0, gw);
+  if (sw < 1 || total * 100 < bps * 115 || ngroups < (int64_t)total * p.sms) return RBD_OK;
+  QueueCtx ctx;      // zeroed work-queue counter, cached in the handle
+  CUDA_TRY(queue_begin(const_cast<rbd_model*>(model), stream, ctx));
   a.counter = ctx.counter;
+  a.sw = sw;
+  void* l2s = nullptr;
   void* scratch = nullptr;
-  if (scratch_rows > 0) {       // external wrenches in body frames: one column per resident thread of either kernel
-    a.scratch_off = (int64_t)bps * p.sms * kNT;
-    a.scratch_ld = a.scratch_off + (int64_t)p.sms * 32 * tm_warps;
-    CUDA_TRY(cudaMallocAsync(&scratch, (size_t)scratch_rows * a.scratch_ld * sizeof(T), stream));
-    a.scratch = (T*)scratch;
+  if (gw > 0) CUDA_TRY(cudaMallocAsync(&l2s, (size_t)gw * p.sms * warp_bytes, stream));
+  a.l2 = static_cast<decltype(a.l2)>(l2s);
+  if (scratch_rows > 0) {       // external wrenches in body frames: one column per resident thread
+    a.scratch_ld = (int64_t)p.sms * total * 32;
+    CUDA_TRY(cudaMallocAsync(&scratch, (size_t)scratch_rows * a.scratch_ld * sizeof(*a.scratch), stream));
+    a.scratch = static_cast<decltype(a.scratch)>(scratch);
   }
-  CUDA_TRY(cudaEventRecord(fork, stream));
-  CUDA_TRY(cudaStreamWaitEvent(side, fork, 0));
-  // (profiling aid: under ncu kernels are serialised and the first one drains the queue; RBD_ONLY=smem|tmem launches
-  //  just one of the two so each can be captured doing the whole batch)
-  static const char* const only = getenv("RBD_ONLY");
-  if (!only || only[0] == 's') ks<<<bps * p.sms, kNT, smem, stream>>>(M, a);
-  if (!only || only[0] == 't') kt<<<p.sms, 32 * tm_warps, 0, side>>>(M, a);
+  km<<<p.sms, 32 * total, sw * warp_bytes, stream>>>(M, a);
   cudaError_t e = cudaGetLastError();
-  cudaEventRecord(join, side);
-  cudaStreamWaitEvent(stream, join, 0);
+  if (l2s) cudaFreeAsync(l2s, stream);
   if (scratch) cudaFreeAsync(scratch, stream);
   if (e != cudaSuccess) return fail_cuda(e, "kernel launch");
-  g_launch.kernels_launched += 2;
-  g_launch.grid = bps * p.sms; g_launch.block = kNT; g_launch.smem_bytes = (int)smem; g_launch.blocks_per_sm = bps;
+  g_launch.kernels_launched += 1;
+  g_launch.grid = p.sms; g_launch.block = 32 * total; g_launch.smem_bytes = (int)(sw * warp_bytes); g_launch.blocks_per_sm = 1;
   used = true;
   return RBD_OK;
 }
@@ -632,14 +569,11 @@ int dynamics_t(const rbd_model* model, int64_t B, int64_t ld, const void* q, con
       return rc;
     }
   }
-  if (!hm.general && !other_kinds && rows <= 256 && (!wext || duo_enabled("RBD_DUO_EXT", kDuoExtDefault))) {
-    // Default path for all-revolute trees whose stash fits Tensor Memory: see launch_duo
-    constexpr int kTmWarps = sizeof(T) == 4 ? 8 : 4;
+  if (!wext && !hm.general && !other_kinds && rows <= 256) {   // all-revolute trees (floating root allowed): the mixed CTA, see launch_mix
     bool used = false;
-    const int rc = wext ? launch_duo<T>(model, aba_kernel_smem_q<T, 0, true>, aba_kernel_tmem_q<T, 512, 0, kTmWarps, true>,
-                                        kTmWarps, M, a, rows, sr, stream, used)
-                        : launch_duo<T>(model, aba_kernel_smem_q<T, 0, false>, aba_kernel_tmem_q<T, 512, 0, kTmWarps, false>,
-                                        kTmWarps, M, a, rows, 0, stream, used);
+    a.rows = rows;
+    const int rc = launch_mix(model, aba_kernel<T, kNT, false, false, 0>, aba_kernel_mix<T, 0>, kMixWarps<T>, M, a,
+                              (size_t)rows * kNT * sizeof(T), (B + kNT - 1) / kNT, 0, stream, used);
     if (rc) return rc;
     if (used) return RBD_OK;
   }
@@ -675,13 +609,14 @@ int inverse_dynamics_t(const rbd_model* model, int64_t B, int64_t ld, const void
       return rc;
     }
   }
-  if (rows <= 256 && duo_enabled("RBD_DUO_RNEA", kDuoRneaDefault) && (!wext || duo_enabled("RBD_DUO_EXT", kDuoExtDefault))) {
-    constexpr int kTmWarps = sizeof(T) == 4 ? 8 : 4;
+  if (rows <= 256) {             // the mixed CTA, see launch_mix
     bool used = false;
-    const int rc = wext ? launch_duo<T>(model, rnea_kernel_smem_q<T, true>, rnea_kernel_tmem_q<T, 512, kTmWarps, true>, kTmWarps,
-                                        M, a, rows, 6 * hm.nb, stream, used)
-                        : launch_duo<T>(model, rnea_kernel_smem_q<T, false>, rnea_kernel_tmem_q<T, 512, kTmWarps, false>, kTmWarps,
-                                        M, a, rows, 0, stream, used);
+    a.rows = rows;
+    const int64_t ng = (B + kNT - 1) / kNT;
+    const int rc = wext ? launch_mix(model, rnea_kernel<T, kNT, true>, rnea_kernel_mix<T, true>, kMixWarps<T>, M, a,
+                                     (size_t)rows * kNT * sizeof(T), ng, 6 * hm.nb, stream, used)
+                        : launch_mix(model, rnea_kernel<T, kNT, false>, rnea_kernel_mix<T, false>, kMixWarps<T>, M, a,
+                                     (size_t)rows * kNT * sizeof(T), ng, 0, stream, used);
     if (rc) return rc;
     if (used) return RBD_OK;
   }
@@ -799,21 +734,15 @@ int dynamics_dual(const rbd_model* model, int64_t B, int64_t ld, const void* q, 
     d.kind = s.kind; d.parent = s.parent; d.qrow = s.qrow; d.vrow = s.vrow; d.row0 = s.row0;
     d.oslot = s.oslot; d.pslot = s.pslot; d.flags = s.flags; d.refidx = s.refidx;
   }
-  const DualArgs a{(const double*)q, (const double*)v, (const double*)tau, (double*)vd, ld, B};
+  DualArgs a{(const double*)q, (const double*)v, (const double*)tau, (double*)vd, ld, B};
   DeviceProps p;
   if (int rc = get_props(p)) return rc;
-  // split stash (shared memory + Tensor Memory): 4 warps/SM instead of 2 on Atlas
-  const size_t smem_tm = (size_t)S.nrows * 128 * sizeof(double);
-  if (!hm.general && S.nrows <= 256 && (int)smem_tm <= p.max_smem_optin && B * 6 >= (int64_t)p.sms * 128 && !getenv("RBD_NO_TMEM")) {
-    int bps_tm = 0;
-    if (int rc = configure(aba_dual_kernel_tm, 128, smem_tm, p, bps_tm)) return rc;
-    const int64_t ng = (B * 6 + 127) / 128;
-    const int grid_tm = (int)std::min<int64_t>(ng, p.sms);
-    aba_dual_kernel_tm<<<grid_tm, 128, smem_tm, stream>>>(*Mp, a);
-    CUDA_TRY(cudaGetLastError());
-    g_launch.kernels_launched += 1;
-    g_launch.grid = grid_tm; g_launch.block = 128; g_launch.smem_bytes = (int)smem_tm; g_launch.blocks_per_sm = 1;
-    return RBD_OK;
+  if (!hm.general && S.nrows <= 256) {      // the mixed CTA, see launch_mix
+    bool used = false;
+    a.rows = S.nrows;
+    if (int rc = launch_mix(model, aba_dual_kernel<kNT, false>, aba_dual_kernel_mix, kMixWarps<double>, *Mp, a,
+                            (size_t)S.nrows * kNT * sizeof(Dual64), (B * 6 + kNT - 1) / kNT, 0, stream, used)) return rc;
+    if (used) return RBD_OK;
   }
   const size_t smem = (size_t)S.nrows * kNT * sizeof(Dual64);
   int bps = 0;
@@ -872,7 +801,7 @@ __global__ void __launch_bounds__(128) integrate_stage_kernel(const __grid_const
 }
 // Revolute / prismatic joints (the bulk of a robot): q_s = q0 + wa phid_prev, v_s = v0 + wa vd_prev, phid = v_s -- plain row
 // arithmetic, done VEC samples per thread with 16-byte accesses so that enough loads are in flight to approach the HBM rate (the
-// per-(sample, joint) kernel above sits at 15 % of it, long_scoreboard 13 warps per issue: profiles/r2_gen_rk4_stage_summary.txt).
+// per-(sample, joint) kernel above is latency-bound: too few loads in flight per thread).
 template <class T> struct VecOf { using type = float4; static constexpr int N = 4; };
 template <> struct VecOf<double> { using type = double2; static constexpr int N = 2; };
 template <class T> __device__ __forceinline__ void vec_axpy(const typename VecOf<T>::type& a, T w, const typename VecOf<T>::type& x,
@@ -1356,11 +1285,7 @@ int32_t rbd_model_destroy(rbd_model* m) {
     if (m->streams[i]) cudaStreamDestroy(m->streams[i]);
   }
   spec_release(m);
-  if (m->side_stream) {
-    cudaStreamDestroy(m->side_stream);
-    for (int i = 0; i < kEventRing; ++i) { cudaEventDestroy(m->fork_ev[i]); cudaEventDestroy(m->join_ev[i]); }
-    cudaFree(m->counters);
-  }
+  if (m->counters) cudaFree(m->counters);
   if (m->ev0) cudaEventDestroy(m->ev0);
   if (m->ev1) cudaEventDestroy(m->ev1);
   delete m;

@@ -15,7 +15,7 @@
 namespace rbd {
 namespace {
 
-constexpr int kGeneratorVersion = 24;   // bump when the emitted code changes (part of the cubin cache key)
+constexpr int kGeneratorVersion = 26;   // bump when the emitted code changes (part of the cubin cache key)
 
 template <class F> const ModelDev<F>& devm(const HostModel& m);
 template <> const ModelDev<float>& devm<float>(const HostModel& m) { return m.dev32; }
@@ -106,7 +106,7 @@ struct Emitter {
 
   // Explicit fused multiply-adds (the translation units are compiled with --fmad=false): a product with exactly one use, by an
   // addition or subtraction, is folded into it.  Doing the contraction HERE rather than leaving it to the compiler makes the
-  // shared-memory and the Tensor-Memory kernel (two separately optimised functions) and the CPU flavour bit-identical.
+  // kernel and the CPU flavour bit-identical.
   void plan_fma() {
     const auto& N = tr.nodes;
     uses.assign(N.size(), 0);
@@ -180,7 +180,6 @@ struct Emitter {
     char line[256];
     stats.nodes_traced = (int)N.size();
     int since = 0;
-    size_t sst_done = 0;
     for (size_t i = 0; i < N.size(); ++i) {
       if (!live[i]) continue;
       const SymNode& n = N[i];
@@ -235,61 +234,15 @@ struct Emitter {
           break;
         case S_SLD: {
           ++stats.n_sld;
-          if (flavor != FLAVOR_TMEM && flavor != FLAVOR_UNI) {
-            snprintf(line, sizeof line, "const rbd_v t%zu = RBD_SLD(%d);\n", i, n.row);
-            out += line;
-            break;
-          }
-          // Tensor Memory: issue the whole ldv<N> batch, then one wait
-          if (n.grp != (int)i) break;                      // emitted with the head of its batch
-          size_t e = i;
-          while (e < N.size() && N[e].op == S_SLD && N[e].grp == (int)i) ++e;
-          bool any = false;
-          for (size_t k = i; k < e; ++k) if (live[k]) any = true;
-          if (!any) break;
-          if (flavor == FLAVOR_UNI) {          // one warp-uniform branch per batch: Tensor Memory or shared memory
-            for (size_t k = i; k < e; ++k)
-              if (live[k]) { snprintf(line, sizeof line, "rbd_v t%zu;\n", k); out += line; }
-            out += "if (use_tm) {\n";
-            for (size_t k = i; k < e; ++k)
-              if (live[k]) { snprintf(line, sizeof line, "RBD_TM_REG u%zu; RBD_TM_LD(u%zu, %d);\n", k, k, N[k].row); out += line; }
-            out += "RBD_TM_WAIT_LD();\n";
-            for (size_t k = i; k < e; ++k)
-              if (live[k]) { snprintf(line, sizeof line, "t%zu = RBD_TM_VAL(u%zu);\n", k, k); out += line; }
-            out += "} else {\n";
-            for (size_t k = i; k < e; ++k)
-              if (live[k]) { snprintf(line, sizeof line, "t%zu = RBD_SLD(%d);\n", k, N[k].row); out += line; }
-            out += "}\n";
-            break;
-          }
-          for (size_t k = i; k < e; ++k)
-            if (live[k]) { snprintf(line, sizeof line, "RBD_TM_REG u%zu; RBD_TM_LD(u%zu, %d);\n", k, k, N[k].row); out += line; }
-          out += "RBD_TM_WAIT_LD();\n";
-          for (size_t k = i; k < e; ++k)
-            if (live[k]) { snprintf(line, sizeof line, "const rbd_v t%zu = RBD_TM_VAL(u%zu);\n", k, k); out += line; }
+          snprintf(line, sizeof line, "const rbd_v t%zu = RBD_SLD(%d);\n", i, n.row);
+          out += line;
           break;
         }
-        case S_SST: {
+        case S_SST:
           ++stats.n_sst;
-          if (flavor != FLAVOR_UNI) {
-            snprintf(line, sizeof line, "RBD_SST(%d, %s);\n", n.row, ref(n.a).c_str());
-            out += line;
-            break;
-          }
-          if (sst_done > i) break;             // part of a run already emitted
-          // run of adjacent stash stores (only dead nodes / constants in between): one warp-uniform branch for the run
-          size_t e = i;
-          std::vector<size_t> run;
-          while (e < N.size() && (N[e].op == S_SST || !live[e] || N[e].op == S_CONST || fused[e])) { if (N[e].op == S_SST) run.push_back(e); ++e; }
-          sst_done = e;
-          stats.n_sst += (int)run.size() - 1;
-          out += "if (use_tm) {\n";
-          for (size_t k : run) { snprintf(line, sizeof line, "RBD_TM_ST(%d, %s);\n", N[k].row, ref(N[k].a).c_str()); out += line; }
-          out += "} else {\n";
-          for (size_t k : run) { snprintf(line, sizeof line, "RBD_SST(%d, %s);\n", N[k].row, ref(N[k].a).c_str()); out += line; }
-          out += "}\n";
+          snprintf(line, sizeof line, "RBD_SST(%d, %s);\n", n.row, ref(n.a).c_str());
+          out += line;
           break;
-        }
         case S_SFENCE: out += "RBD_SFENCE();\n"; break;
         case S_XLD: snprintf(line, sizeof line, "const rbd_v t%zu = RBD_XLD(%d);\n", i, n.row); out += line; break;
         case S_XST: snprintf(line, sizeof line, "RBD_XST(%d, %s);\n", n.row, ref(n.a).c_str()); out += line; break;
@@ -298,22 +251,6 @@ struct Emitter {
   }
 };
 
-// In the Tensor-Memory flavour a live load whose batch head is dead would be skipped by the `grp != i` test above: make the
-// first LIVE node of every batch its head.
-void regroup_batches(SymTrace& tr, const std::vector<uint8_t>& live) {
-  auto& N = tr.nodes;
-  for (size_t i = 0; i < N.size();) {
-    if (N[i].op != S_SLD) { ++i; continue; }
-    const int g = N[i].grp;
-    size_t e = i;
-    while (e < N.size() && N[e].op == S_SLD && N[e].grp == g) ++e;
-    int head = -1;
-    for (size_t k = i; k < e; ++k) if (live[k]) { head = (int)k; break; }
-    for (size_t k = i; k < e; ++k) N[k].grp = head >= 0 ? head : (int)i;
-    i = e;
-  }
-}
-
 }  // namespace
 
 bool spec_emit_function(const HostModel& hm, const SpecKey& key, int flavor, const std::string& name, std::string& out,
@@ -321,11 +258,6 @@ bool spec_emit_function(const HostModel& hm, const SpecKey& key, int flavor, con
   SymTrace tr;
   int rows = 0;
   if (!run_trace(hm, key, tr, rows, err)) return false;
-  {
-    Emitter pre(tr, key, flavor);
-    pre.mark();
-    regroup_batches(tr, pre.live);
-  }
   Emitter em(tr, key, flavor);
   if (flavor != FLAVOR_CPU) {
     // One basic block of 10^4 instructions lets ptxas stretch live ranges until it spills (Atlas: 128 registers + 350 B of
@@ -363,13 +295,6 @@ int spec_stash_rows(const HostModel& hm, const SpecKey& key) {
   return key.algo == SPEC_ABA ? hm.dev64.nrows : (key.algo == SPEC_RNEA ? rnea_rows(hm) : std::max(1, crba_rows(hm)));
 }
 
-int spec_uni_smem_warps(const HostModel& hm, const SpecKey& key) {
-  const int per_warp = std::max(1, spec_stash_rows(hm, key)) * 32 * (key.f64 ? 8 : 4);
-  const int fit = (227 * 1024 - 1024) / per_warp;
-  const int want = key.f64 ? 4 : 8;
-  return fit >= want ? want : (fit >= 4 ? 4 : 0);
-}
-
 uint64_t spec_hash(const HostModel& hm, const SpecKey& key) {
   uint64_t h = 0xcbf29ce484222325ull;
   auto mix = [&](const void* p, size_t n) {
@@ -390,12 +315,10 @@ uint64_t spec_hash(const HostModel& hm, const SpecKey& key) {
 }
 
 bool spec_emit_cuda_tu(const HostModel& hm, const SpecKey& key, std::string& out, SpecStats* stats, std::string& err) {
-  // the three per-sample functions first (their size decides a code-shape switch in the header)
-  std::string fn_smem, fn_tmem, fn_uni;
+  // the per-sample function first (its statistics go into the header)
+  std::string fn_smem;
   SpecStats st;
   if (!spec_emit_function(hm, key, FLAVOR_SMEM, "rbd_spec_smem", fn_smem, &st, err)) return false;
-  if (!spec_emit_function(hm, key, FLAVOR_TMEM, "rbd_spec_tmem", fn_tmem, nullptr, err)) return false;
-  if (!spec_emit_function(hm, key, FLAVOR_UNI, "rbd_spec_uni", fn_uni, nullptr, err)) return false;
   if (stats) *stats = st;
   char buf[768];
   const int rows = spec_stash_rows(hm, key);
@@ -404,15 +327,13 @@ bool spec_emit_cuda_tu(const HostModel& hm, const SpecKey& key, std::string& out
            "%d global loads, %d stash loads, %d stash stores)\n"
            "#define RBD_SPEC_F64 %d\n#define RBD_SPEC_NQ %d\n#define RBD_SPEC_NV %d\n#define RBD_SPEC_ROWS %d\n"
            "#define RBD_SPEC_HAS_IN2 %d\n#define RBD_SPEC_HAS_OUT1 %d\n#define RBD_SPEC_OUT0_ROWS %d\n#define RBD_SPEC_OUT1_ROWS %d\n"
-           "#define RBD_UNI_SW %d\n#define RBD_SPEC_ROW32 %d\n#define RBD_SPEC_KIN %d\n#define RBD_SPEC_USES_V %d\n#include \"rbd_jit_prelude.cuh\"\n",
+           "#define RBD_SPEC_ROW32 %d\n#define RBD_SPEC_KIN %d\n#define RBD_SPEC_USES_V %d\n#include \"rbd_jit_prelude.cuh\"\n",
            st.nodes_live, st.n_add, st.n_mul, st.n_div, st.n_sincos, st.n_load, st.n_sld, st.n_sst,
            key.f64 ? 1 : 0, hm.nq, hm.nv, rows, key.has_in2 ? 1 : 0, key.has_out1 ? 1 : 0, key.algo == SPEC_CRBA ? hm.nv * hm.nv : hm.nv, hm.nq,
-           std::max(4, spec_uni_smem_warps(hm, key)), key.algo == SPEC_CRBA ? 1 : 0, key.algo == SPEC_KIN ? 1 : 0, st.n_load_v > 0 ? 1 : 0);
+           key.algo == SPEC_CRBA ? 1 : 0, key.algo == SPEC_KIN ? 1 : 0, st.n_load_v > 0 ? 1 : 0);
   out += buf;
   out += "#define RBD_FLAVOR_SMEM 1\n#include \"rbd_jit_flavor.cuh\"\n" + fn_smem;
-  out += "#undef RBD_FLAVOR_SMEM\n#define RBD_FLAVOR_TMEM 1\n#include \"rbd_jit_flavor.cuh\"\n" + fn_tmem;
-  out += "#undef RBD_FLAVOR_TMEM\n#define RBD_FLAVOR_UNI 1\n#include \"rbd_jit_flavor.cuh\"\n" + fn_uni;
-  out += "#undef RBD_FLAVOR_UNI\n#include \"rbd_jit_kernels.cuh\"\n";
+  out += "#include \"rbd_jit_kernels.cuh\"\n";
   return true;
 }
 

@@ -28,18 +28,16 @@ struct SpecStats {
   int n_load_v = 0;      // global loads of the v array (0: the kernel shell does not prefetch it)
 };
 
-enum SpecFlavor : int { FLAVOR_CPU = 0, FLAVOR_SMEM = 1, FLAVOR_TMEM = 2, FLAVOR_UNI = 3 };   // UNI emits like TMEM (batched loads)
+enum SpecFlavor : int { FLAVOR_CPU = 0, FLAVOR_SMEM = 1 };
 
 // Body of one per-sample function `name(...)` for the given flavour (see rbd_jit_prelude.cuh for the calling convention).
 // Returns false (with `err`) if the model / key cannot be specialised.
 bool spec_emit_function(const HostModel& hm, const SpecKey& key, int flavor, const std::string& name, std::string& out,
                         SpecStats* stats, std::string& err);
 
-// Whole NVRTC translation unit for `key`: defines + the smem and tmem sample functions + the kernel shells of the prelude.
+// Whole NVRTC translation unit for `key`: defines + the per-sample function + the kernel shell of the prelude.
 bool spec_emit_cuda_tu(const HostModel& hm, const SpecKey& key, std::string& out, SpecStats* stats, std::string& err);
 int spec_stash_rows(const HostModel& hm, const SpecKey& key);
-// Warps with a shared-memory stash in the unified CTA (a multiple of 4, 0 = the stash does not fit).
-int spec_uni_smem_warps(const HostModel& hm, const SpecKey& key);
 
 // Self-contained C++ translation unit (needs csrc/ on the include path) defining `extern "C" void name(q, v, in2, o0, o1, ld, sh)`
 // for ONE sample: column pointers with leading dimension ld, `sh` = stash_rows scalars of scratch.  Test tier only.

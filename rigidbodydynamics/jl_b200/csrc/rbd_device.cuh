@@ -5,7 +5,7 @@
 // that carries  v_i, (sin, cos)_i  from the outward pass to the inward pass and  U~_i, u~_i  from the inward pass
 // to the second outward pass, plus one pending slot per simultaneously-open branch node of the tree.
 //
-// What is computed, in the reference's terms (citations relative to /root/reference/src):
+// What is computed, in the reference's terms (citations relative to the reference's src/):
 //   joint transforms / twists      joint_types/*.jl (joint_transform, joint_twist), mechanism_state.jl:687-780
 //   velocity-product accelerations mechanism_state.jl:814-830 (bias_accelerations_wrt_world), spatialmotion.jl:375-401
 //   Newton-Euler wrench            spatial/motion_force_interaction.jl:244-263, spatial/util.jl:110-114

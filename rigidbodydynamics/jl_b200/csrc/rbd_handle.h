@@ -13,14 +13,14 @@
 
 namespace rbd {
 
-// One model-specialised kernel pair (shared-memory + Tensor-Memory stash), loaded from a cubin.
+// One model-specialised program, loaded from a cubin: shared-memory blocks and the mixed shared-memory / L2 CTA.
 struct SpecEntry {
   int state = 0;                 // 0 = not tried, 1 = ready, -1 = unavailable (generic kernels are used)
   cudaLibrary_t lib = nullptr;
-  cudaKernel_t k_smem = nullptr, k_tmem = nullptr, k_uni = nullptr;   // shared-memory blocks / Tensor-Memory CTA / unified CTA
-  int regs_smem = 0, regs_tmem = 0, regs_uni = 0;
-  int choice = 0;                // 0 = not tuned yet, 1 = kernel pair, 2 = unified CTA (for batches that fill the SMs)
-  int uni_sw = 0;                // warps with a shared-memory stash in the unified CTA (0 = unified kernel unusable)
+  cudaKernel_t k_smem = nullptr, k_mix = nullptr;
+  int regs_smem = 0, regs_mix = 0;
+  int mix_sw = 0;                // warps of the mixed CTA whose stash fits its shared memory
+  int choice = 0;                // 0 = not timed yet, 1 = shared-memory blocks, 2 = mixed CTA (for batches that fill the SMs)
   int rows = 0;
   bool from_cache = false;
   std::string why;               // reason for state -1
@@ -29,7 +29,6 @@ struct SpecEntry {
 };
 
 constexpr int kCounterRing = 256;   // work-queue counters, one per call in flight
-constexpr int kEventRing = 8;
 
 }  // namespace rbd
 
@@ -41,11 +40,9 @@ struct rbd_model {
   size_t stage_bytes = 0;
   cudaStream_t streams[3] = {nullptr, nullptr, nullptr};
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  // kernel pairs: the Tensor-Memory kernel runs on the side stream next to the shared-memory kernel (per device)
-  std::mutex side_mu;
-  int side_device = -1;
-  cudaStream_t side_stream = nullptr;
-  cudaEvent_t fork_ev[rbd::kEventRing] = {}, join_ev[rbd::kEventRing] = {};
+  // work queues of the model-specialised kernels (per device)
+  std::mutex queue_mu;
+  int queue_device = -1;
   unsigned long long* counters = nullptr;     // [kCounterRing][2] device memory: work-queue counter, "needs generic kernel" flag
   unsigned next_call = 0;
   // model-specialised kernels, keyed by SpecKey bits
@@ -55,15 +52,13 @@ struct rbd_model {
 
 namespace rbd {
 
-// Resources of one kernel-pair launch: side stream, fork/join events and a zeroed work-queue counter (enqueued on `stream`).
-struct PairCtx {
-  cudaStream_t side = nullptr;
-  cudaEvent_t fork = nullptr, join = nullptr;
+// Resources of one work-queue launch: a zeroed work-queue counter and flag (the zeroing is enqueued on `stream`).
+struct QueueCtx {
   unsigned long long* counter = nullptr;
   int* flag = nullptr;       // zeroed with the counter; raised by a specialised kernel that met an angle beyond its fast sin / cos
 };
 // Returns a cudaError_t (cudaSuccess = 0).
-cudaError_t pair_begin(rbd_model* m, cudaStream_t stream, PairCtx& ctx);
+cudaError_t queue_begin(rbd_model* m, cudaStream_t stream, QueueCtx& ctx);
 
 inline uint64_t spec_key_bits(const SpecKey& k) {
   uint64_t b = (uint64_t)k.algo | (k.f64 ? 8u : 0u) | (k.has_in2 ? 16u : 0u) | (k.has_out1 ? 32u : 0u) | (k.lower ? 64u : 0u) | (k.peers ? 128u : 0u);

@@ -1,6 +1,6 @@
 // Munthe-Kaas RK4 step around `dynamics` (SURVEY 8(f) rank 1): the per-joint local <-> global coordinate maps.
 //
-// Reference (relative to /root/reference/src):
+// Reference (relative to the reference's src/):
 //   step(::MuntheKaasIntegrator, t, dt)      ode_integrators.jl:233-300   (stages in local coordinates phi around q0)
 //   runge_kutta_4                            ode_integrators.jl:48-55     a21 = a32 = 1/2, a43 = 1, b = (1/6, 1/3, 1/3, 1/6)
 //   local_coordinates! / global_coordinates! mechanism_state.jl:1057-1085, defaults joint_types/joint_types.jl:9-18

@@ -88,17 +88,27 @@ void write_file_atomic(const std::string& path, const char* data, size_t n) {
   if (ok) rename(t.c_str(), path.c_str()); else remove(t.c_str());
 }
 
+std::string library_cache_dir() {
+  Dl_info info;
+  if (!dladdr((void*)&jit_cache_dir, &info) || !info.dli_fname) return "./jit_cache";
+  const std::string p(info.dli_fname);
+  const size_t s = p.find_last_of('/');
+  return (s == std::string::npos ? std::string(".") : p.substr(0, s)) + "/jit_cache";
+}
+
+// A cached cubin from the cache directory, else (no $RBD_JIT_CACHE) from <library dir>/jit_cache: build() precompiles there,
+// and the tree may be read-only at run time, which sends jit_cache_dir() elsewhere.
+bool read_cached(const std::string& name, std::vector<char>& out) {
+  if (read_file(jit_cache_dir() + "/" + name, out)) return true;
+  return !getenv("RBD_JIT_CACHE") && read_file(library_cache_dir() + "/" + name, out);
+}
+
 }  // namespace
 
 std::string jit_cache_dir() {
   if (const char* e = getenv("RBD_JIT_CACHE")) { if (dir_writable(e)) return e; }
-  Dl_info info;
-  if (dladdr((void*)&jit_cache_dir, &info) && info.dli_fname) {
-    std::string p(info.dli_fname);
-    const size_t s = p.find_last_of('/');
-    const std::string d = (s == std::string::npos ? std::string(".") : p.substr(0, s)) + "/jit_cache";
-    if (dir_writable(d)) return d;
-  }
+  const std::string lib = library_cache_dir();
+  if (dir_writable(lib)) return lib;
   if (const char* home = getenv("HOME")) {
     const std::string c = std::string(home) + "/.cache";
     mkdir(c.c_str(), 0755);
@@ -108,7 +118,7 @@ std::string jit_cache_dir() {
   return "/tmp";
 }
 
-// NVRTC for sm_100a on a complete source text; the embedded headers are offered to every program.
+// NVRTC for sm_90a on a complete source text; the embedded headers are offered to every program.
 static bool nvrtc_compile(const std::string& src, bool fmad, std::vector<char>& cubin, std::string& err) {
   Nvrtc& n = nvrtc();
   if (!n.h) { err = n.err; return false; }
@@ -118,7 +128,7 @@ static bool nvrtc_compile(const std::string& src, bool fmad, std::vector<char>& 
   nvrtcProgram prog = nullptr;
   nvrtcResult r = n.CreateProgram(&prog, src.c_str(), "rbd_spec.cu", nh, ht.data(), hn.data());
   if (r != NVRTC_SUCCESS) { err = std::string("nvrtcCreateProgram: ") + n.GetErrorString(r); return false; }
-  const char* opts[] = {"--gpu-architecture=sm_100a", "-std=c++17", "-lineinfo", "--fmad=false"};
+  const char* opts[] = {"--gpu-architecture=sm_90a", "-std=c++17", "-lineinfo", "--fmad=false"};
   r = n.CompileProgram(prog, fmad ? 3 : 4, opts);
   if (r != NVRTC_SUCCESS) {
     size_t ls = 0;
@@ -140,9 +150,9 @@ static bool nvrtc_compile(const std::string& src, bool fmad, std::vector<char>& 
 
 bool jit_get_cubin(const HostModel& hm, const SpecKey& key, std::vector<char>& cubin, bool compile_if_missing, bool* from_cache,
                    SpecStats* stats, std::string& err) {
-  const std::string path = jit_cache_dir() + "/" + key_name(hm, key) + ".cubin";
+  const std::string name = key_name(hm, key) + ".cubin";
   if (from_cache) *from_cache = false;
-  if (!getenv("RBD_JIT_NO_CACHE") && read_file(path, cubin)) {
+  if (!getenv("RBD_JIT_NO_CACHE") && read_cached(name, cubin)) {
     if (from_cache) *from_cache = true;
     return true;
   }
@@ -150,7 +160,7 @@ bool jit_get_cubin(const HostModel& hm, const SpecKey& key, std::vector<char>& c
   std::string src;
   if (!spec_emit_cuda_tu(hm, key, src, stats, err)) return false;
   if (!nvrtc_compile(src, false, cubin, err)) return false;
-  if (!getenv("RBD_JIT_NO_CACHE")) write_file_atomic(path, cubin.data(), cubin.size());
+  if (!getenv("RBD_JIT_NO_CACHE")) write_file_atomic(jit_cache_dir() + "/" + name, cubin.data(), cubin.size());
   return true;
 }
 
@@ -160,15 +170,15 @@ bool jit_compile_text(const std::string& tag, const std::string& src, bool fmad,
   for (unsigned char c : src) { h ^= c; h *= 1099511628211ull; }
   char buf[64];
   snprintf(buf, sizeof buf, "%016llx_%s", h, tag.c_str());
-  const std::string path = jit_cache_dir() + "/" + buf + ".cubin";
+  const std::string name = std::string(buf) + ".cubin";
   if (from_cache) *from_cache = false;
-  if (!getenv("RBD_JIT_NO_CACHE") && read_file(path, cubin)) {
+  if (!getenv("RBD_JIT_NO_CACHE") && read_cached(name, cubin)) {
     if (from_cache) *from_cache = true;
     return true;
   }
   if (!compile_if_missing) { err = "no cached cubin"; return false; }
   if (!nvrtc_compile(src, fmad, cubin, err)) return false;
-  if (!getenv("RBD_JIT_NO_CACHE")) write_file_atomic(path, cubin.data(), cubin.size());
+  if (!getenv("RBD_JIT_NO_CACHE")) write_file_atomic(jit_cache_dir() + "/" + name, cubin.data(), cubin.size());
   return true;
 }
 

@@ -1,13 +1,8 @@
-// Stash access macros of the generated per-sample function, for one stash home (no include guard: included once per flavour).
+// Stash access macros of the generated per-sample function (no include guard: the header undefines and redefines them).
 #undef RBD_STASH_ARG
 #undef RBD_SLD
 #undef RBD_SST
 #undef RBD_SFENCE
-#undef RBD_TM_REG
-#undef RBD_TM_LD
-#undef RBD_TM_WAIT_LD
-#undef RBD_TM_VAL
-#undef RBD_TM_ST
 #if defined(RBD_FLAVOR_SMEM)
 // shared memory, [row][lane] of a single warp: conflict-free, constant offsets.  volatile: with every row a compile-time constant the
 // compiler would otherwise forward each pass-1 store to its pass-2 load THROUGH REGISTERS (and spill them) -- the stash exists to
@@ -16,49 +11,4 @@
 #define RBD_SLD(r) sh[(r) * 32]
 #define RBD_SST(r, val_) sh[(r) * 32] = (val_)
 #define RBD_SFENCE()
-#elif defined(RBD_FLAVOR_UNI)
-// ONE program for both stash homes: warps of the unified CTA (rbd_jit_kernels.cuh) keep their stash either in shared memory or
-// in Tensor Memory, selected by the warp-uniform `use_tm`; the generator wraps every batch of stash loads / run of stash stores
-// in one `if (use_tm) ... else ...`.  All 16 warps of an SM then execute the same instruction stream and share its fetches (two
-// separately compiled kernels side by side were measured to starve each other's instruction supply, DESIGN.md 4.8).
-#define RBD_STASH_ARG const unsigned tm, volatile rbd_f* sh, const bool use_tm
-#define RBD_SLD(r) sh[(r) * 32]
-#define RBD_SST(r, val_) sh[(r) * 32] = (val_)
-#define RBD_SFENCE() do { if (use_tm) asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); } while (0)
-#define RBD_TM_WAIT_LD() asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory")
-#if RBD_SPEC_F64
-#ifndef RBD_U2_DEFINED
-#define RBD_U2_DEFINED
-struct rbd_u2 { unsigned lo, hi; };
-#endif
-#define RBD_TM_REG rbd_u2
-#define RBD_TM_LD(u, r) asm volatile("tcgen05.ld.sync.aligned.32x32b.x2.b32 {%0, %1}, [%2];" : "=r"(u.lo), "=r"(u.hi) : "r"(tm + 2u * (r)) : "memory")
-#define RBD_TM_VAL(u) __hiloint2double((int)u.hi, (int)u.lo)
-#define RBD_TM_ST(r, val_) asm volatile("tcgen05.st.sync.aligned.32x32b.x2.b32 [%0], {%1, %2};" ::"r"(tm + 2u * (r)), "r"((unsigned)__double2loint(val_)), "r"((unsigned)__double2hiint(val_)) : "memory")
-#else
-#define RBD_TM_REG unsigned
-#define RBD_TM_LD(u, r) asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(u) : "r"(tm + (r)) : "memory")
-#define RBD_TM_VAL(u) __uint_as_float(u)
-#define RBD_TM_ST(r, val_) asm volatile("tcgen05.st.sync.aligned.32x32b.x1.b32 [%0], {%1};" ::"r"(tm + (r)), "r"(__float_as_uint(val_)) : "memory")
-#endif
-#elif defined(RBD_FLAVOR_TMEM)
-// Tensor Memory (rbd_tmem.cuh): lane l of warp w owns TMEM lane 32 (w % 4) + l; one 32-bit column per fp32 row, two per fp64 row
-#define RBD_STASH_ARG const unsigned tm
-#define RBD_SFENCE() asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory")
-#define RBD_TM_WAIT_LD() asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory")
-#if RBD_SPEC_F64
-#ifndef RBD_U2_DEFINED
-#define RBD_U2_DEFINED
-struct rbd_u2 { unsigned lo, hi; };
-#endif
-#define RBD_TM_REG rbd_u2
-#define RBD_TM_LD(u, r) asm volatile("tcgen05.ld.sync.aligned.32x32b.x2.b32 {%0, %1}, [%2];" : "=r"(u.lo), "=r"(u.hi) : "r"(tm + 2u * (r)) : "memory")
-#define RBD_TM_VAL(u) __hiloint2double((int)u.hi, (int)u.lo)
-#define RBD_SST(r, val_) asm volatile("tcgen05.st.sync.aligned.32x32b.x2.b32 [%0], {%1, %2};" ::"r"(tm + 2u * (r)), "r"((unsigned)__double2loint(val_)), "r"((unsigned)__double2hiint(val_)) : "memory")
-#else
-#define RBD_TM_REG unsigned
-#define RBD_TM_LD(u, r) asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(u) : "r"(tm + (r)) : "memory")
-#define RBD_TM_VAL(u) __uint_as_float(u)
-#define RBD_SST(r, val_) asm volatile("tcgen05.st.sync.aligned.32x32b.x1.b32 [%0], {%1};" ::"r"(tm + (r)), "r"(__float_as_uint(val_)) : "memory")
-#endif
 #endif

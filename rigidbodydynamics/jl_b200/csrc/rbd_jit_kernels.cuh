@@ -1,11 +1,10 @@
-// Persistent kernels around the generated per-sample functions (see rbd_jit_prelude.cuh): warps claim groups of 32 consecutive
+// Persistent kernel around the generated per-sample function (see rbd_jit_prelude.cuh): warps claim groups of 32 consecutive
 // samples from an atomic counter; the next group's input lines are prefetched into L2 while the current one is computed; warps
-// never synchronise with each other.  Three ways to fill an SM with warps (rbd_spec.cpp picks one per model and entry point):
-//   rbd_jit_smem alone       single-warp blocks, stash in shared memory -- models whose stash is small;
-//   rbd_jit_smem + _tmem     the kernel pair of the generic path: shared-memory blocks and a Tensor-Memory CTA side by side;
-//   rbd_jit_uni              one CTA per SM, half of its warps' stashes in shared memory, half in Tensor Memory, one program.
-// Which of the last two is faster depends on the program (Atlas forward dynamics: pair 1.03 vs 0.93 G evals/s; Atlas inverse
-// dynamics: 2.23 vs 2.72 G; 31-joint chain: 0.66 vs 0.81 G), so the first large call times both once and keeps the winner.  (Tried and dropped: multi-warp CTAs walking the program as a convoy behind CTA
+// never synchronise with each other.  Two ways to fill an SM with warps (rbd_spec.cpp picks one per model and entry point):
+//   rbd_jit_smem   single-warp blocks with their stash in shared memory ([row][lane]), as many per SM as the stash allows;
+//   rbd_jit_mix    one CTA per SM of up to 16 warps: those shared memory can hold keep their stash there, the others in a global
+//                  scratch small enough to stay in the 50 MB L2 -- the register file holds 16 warps where shared memory holds 8
+//                  Atlas stashes.  (Tried and dropped: multi-warp CTAs walking the program as a convoy behind CTA
 // barriers every 64 ... 1024 statements, to share instruction fetches -- no measurable change, DESIGN.md section 4.8.)
 #pragma once
 
@@ -36,59 +35,14 @@ extern "C" __global__ void __launch_bounds__(32, RBD_SPEC_F64 ? 1 : 16) rbd_jit_
   RBD_QUEUE_LOOP(RBD_CALL_SMEM)
 }
 
-// Tensor-Memory CTA of the kernel PAIR (rbd_jit_smem blocks + one of these per SM, two launches on two streams sharing the
-// work queue): 8 (fp32) / 4 (fp64) warps over all 512 TMEM columns -- warp w uses lane quadrant w % 4 and, with 8 warps, column
-// half w / 4 (256 fp32 rows per warp; fp64 rows take two columns).
-#define RBD_TM_WARPS (RBD_SPEC_F64 ? 4 : 8)
-extern "C" __global__ void __launch_bounds__(32 * RBD_TM_WARPS, RBD_SPEC_F64 ? 1 : 2) rbd_jit_tmem(const RbdJitArgs a) {
-  __shared__ unsigned tm_slot;
-  if (threadIdx.x < 32) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"((unsigned)__cvta_generic_to_shared(&tm_slot)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const unsigned tm_base = tm_slot;
-  const unsigned w = threadIdx.x >> 5;
-  const unsigned tm = tm_base + (((w & 3u) * 32u) << 16) + (w >> 2) * 256u;
-#define RBD_CALL_TMEM(q_, v_, i_, o0_, o1_, ld_, act_, fl_, pa_, pb_) rbd_spec_tmem(q_, v_, i_, o0_, o1_, ld_, act_, fl_, pa_, pb_, tm)
-  {
-    RBD_QUEUE_LOOP(RBD_CALL_TMEM)
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (threadIdx.x < 32) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tm_base) : "memory");
-}
-
-// Unified CTA, one per SM: RBD_UNI_SW warps with their stash in shared memory ([row][lane] slices of the dynamic shared memory)
-// followed by RBD_TM_WARPS warps with theirs in Tensor Memory (same layout as above).  All warps run the SAME per-sample
-// function (flavour UNI): one instruction stream per SM instead of two.
-#ifndef RBD_UNI_SW
-#define RBD_UNI_SW RBD_TM_WARPS
-#endif
-extern "C" __global__ void __launch_bounds__(32 * (RBD_UNI_SW + RBD_TM_WARPS), 1) rbd_jit_uni(const RbdJitArgs a) {
+// All warps run the same program through a generic stash pointer, so the SM fetches ONE instruction stream (two kernels side by
+// side starve each other's instruction supply, DESIGN.md 4.8).
+#define RBD_STASH_ROWS (RBD_SPEC_ROWS > 0 ? RBD_SPEC_ROWS : 1)
+extern "C" __global__ void __launch_bounds__(512, 1) rbd_jit_mix(const RbdJitArgs a) {
   extern __shared__ __align__(16) unsigned char rbd_smem_raw[];
-  __shared__ unsigned tm_slot;
-  if (threadIdx.x < 32) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"((unsigned)__cvta_generic_to_shared(&tm_slot)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const unsigned tm_base = tm_slot;
   const unsigned w = threadIdx.x >> 5;
-  const bool use_tm = w >= RBD_UNI_SW;
-  const unsigned wt = use_tm ? w - RBD_UNI_SW : 0u;            // RBD_UNI_SW is a multiple of 4, so wt % 4 == w % 4 = this warp's lane quadrant
-  const unsigned tm = tm_base + (((w & 3u) * 32u) << 16) + (wt >> 2) * 256u;
-  const unsigned ws = use_tm ? 0u : w;
-  volatile rbd_f* sh = reinterpret_cast<volatile rbd_f*>(rbd_smem_raw) + ws * (RBD_SPEC_ROWS * 32u) + (threadIdx.x & 31u);
-#define RBD_CALL_UNI(q_, v_, i_, o0_, o1_, ld_, act_, fl_, pa_, pb_) rbd_spec_uni(q_, v_, i_, o0_, o1_, ld_, act_, fl_, pa_, pb_, tm, sh, use_tm)
-  {
-    RBD_QUEUE_LOOP(RBD_CALL_UNI)
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (threadIdx.x < 32) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tm_base) : "memory");
+  const unsigned sw = (unsigned)a.smem_warps, gw = blockDim.x / 32u - sw;
+  volatile rbd_f* sh = w < sw ? reinterpret_cast<volatile rbd_f*>(rbd_smem_raw) + w * (RBD_STASH_ROWS * 32u) + (threadIdx.x & 31u)
+                              : a.l2_stash + ((unsigned long long)blockIdx.x * gw + (w - sw)) * (RBD_STASH_ROWS * 32u) + (threadIdx.x & 31u);
+  RBD_QUEUE_LOOP(RBD_CALL_SMEM)
 }

@@ -1,5 +1,5 @@
 // Per-sample kinematics by-products in the ROOT frame (SURVEY 8(f) rank 2), one thread per sample, same depth-first order,
-// register hand-over and pending slots as the dynamics passes.  Reference (relative to /root/reference/src):
+// register hand-over and pending slots as the dynamics passes.  Reference (relative to the reference's src/):
 //   transform_to_root               mechanism_state.jl:687-714      T_i = T_parent * joint_to_predecessor_i * J_i(q_i)
 //   center_of_mass                  mechanism_algorithms.jl:30-49
 //   kinetic_energy                  mechanism_state.jl:886-888, :989-994 ; spatial/motion_force_interaction.jl:337-346

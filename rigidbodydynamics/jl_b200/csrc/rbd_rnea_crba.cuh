@@ -1,6 +1,6 @@
 // Per-sample recursive Newton-Euler (inverse_dynamics! / dynamics_bias!), composite-rigid-body algorithm (mass_matrix!)
 // and the external-wrench preparation pass, in the same body-frame / one-hot-subspace / depth-first conventions as the
-// Articulated-Body code in rbd_device.cuh.  Reference (relative to /root/reference/src):
+// Articulated-Body code in rbd_device.cuh.  Reference (relative to the reference's src/):
 //   spatial_accelerations!        mechanism_algorithms.jl:387-417     a_i = a_parent + v_parent x S v + S v̇, a_root = -g
 //   newton_euler!                 mechanism_algorithms.jl:428-439     w_i = I a + v x* I v - w_ext
 //   joint_wrenches_and_torques!   mechanism_algorithms.jl:442-459     w_parent += w_i ; tau_k = S_k . w
@@ -109,8 +109,8 @@ template <class T> struct RneaIO {
   Scr<T> ext;
 };
 
-// ST: Stash<T, STRIDE> (shared memory) or StashTM / StashTM64 (Tensor Memory, whose stores are asynchronous: fence_st()
-// stands wherever a thread re-reads a word it wrote; it is a no-op for shared memory)
+// ST: Stash<T, STRIDE> (shared memory) or the symbolic stash of the code generator (rbd_sym.h); fence_st()
+// stands wherever a thread re-reads a word it wrote; it is a no-op for shared memory
 template <class T, class ST>
 RBD_HD void rnea_sample(const ModelDev<T>& M, const RneaIO<T>& io, const ST& st) {
   const int nb = M.nb;

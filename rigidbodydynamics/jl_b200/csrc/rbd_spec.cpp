@@ -1,7 +1,7 @@
 // Model-specialised kernels: compile (rbd_jit.cpp), load (cudaLibraryLoadData) and launch.  Host-only C++ on the CUDA runtime.
 //
-// The kernels come as a pair, exactly like the generic ones in rbd_b200.cu: single-warp shared-memory blocks on the caller's
-// stream and one Tensor-Memory CTA per SM on the handle's side stream, both claiming groups of 32 samples from one counter.
+// The kernels are persistent and claim groups of 32 samples from one counter: single-warp blocks with their stash in shared
+// memory, or one mixed CTA per SM whose extra warps keep their stash in L2 (rbd_jit_kernels.cuh).
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -13,21 +13,17 @@
 namespace rbd {
 namespace {
 
+constexpr int kMixWarps = 16;       // warps of the mixed CTA: 16 x 32 threads x 128 registers = the whole register file
+
 struct Env {
-  bool jit = true, no_tmem = false, force_pair = false, no_gate = false;
+  bool jit = true, no_gate = false;
   int64_t min_batch = 1 << 15;      // below this a missing cubin is not compiled on the fly (generic kernels serve the call)
   int smem_blocks = 0;
-  int variant = 0;                  // RBD_JIT_VARIANT=1 (pair) / 2 (unified): skip the tuning
-  const char* only = nullptr;       // RBD_ONLY=smem|tmem: launch one kernel of the pair (ncu captures: the profiler serialises them)
   Env() {
     if (const char* e = getenv("RBD_JIT")) jit = e[0] != '0';
-    no_tmem = getenv("RBD_NO_TMEM") != nullptr;
-    force_pair = getenv("RBD_FORCE_PAIR") != nullptr;       // experiments only
     no_gate = getenv("RBD_NO_GATE") != nullptr;
     if (const char* e = getenv("RBD_JIT_MIN_BATCH")) min_batch = atoll(e);
     if (const char* e = getenv("RBD_SMEM_BLOCKS")) smem_blocks = atoi(e);
-    if (const char* e = getenv("RBD_JIT_VARIANT")) variant = atoi(e);
-    only = getenv("RBD_ONLY");
   }
 };
 const Env& env() { static const Env e; return e; }
@@ -43,39 +39,33 @@ cudaError_t props(Props& p) {
   if (dev < 64 && cache[dev].sms) { p = cache[dev]; return cudaSuccess; }
   if ((e = cudaDeviceGetAttribute(&p.sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return e;
   if ((e = cudaDeviceGetAttribute(&p.max_smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev)) != cudaSuccess) return e;
+  {  // the L2 stash of the mixed CTA comes from the stream-ordered pool: keep freed blocks cached in the pool
+    cudaMemPool_t pool;
+    if (cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
+      uint64_t keep = ~0ull;
+      cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
+    }
+  }
   if (dev < 64) cache[dev] = p;
   return cudaSuccess;
 }
 
 }  // namespace
 
-cudaError_t pair_begin(rbd_model* m, cudaStream_t stream, PairCtx& ctx) {
+cudaError_t queue_begin(rbd_model* m, cudaStream_t stream, QueueCtx& ctx) {
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
   unsigned slot;
   {
-    std::lock_guard<std::mutex> lk(m->side_mu);
-    if (m->side_device != dev) {       // first use (or the caller moved to another device): (re)create the per-device resources
-      if (m->side_stream) {
-        cudaStreamDestroy(m->side_stream);
-        for (int i = 0; i < kEventRing; ++i) { cudaEventDestroy(m->fork_ev[i]); cudaEventDestroy(m->join_ev[i]); }
-        cudaFree(m->counters);
-        m->side_stream = nullptr; m->counters = nullptr;
-      }
-      if ((e = cudaStreamCreateWithFlags(&m->side_stream, cudaStreamNonBlocking)) != cudaSuccess) return e;
-      for (int i = 0; i < kEventRing; ++i) {
-        if ((e = cudaEventCreateWithFlags(&m->fork_ev[i], cudaEventDisableTiming)) != cudaSuccess) return e;
-        if ((e = cudaEventCreateWithFlags(&m->join_ev[i], cudaEventDisableTiming)) != cudaSuccess) return e;
-      }
+    std::lock_guard<std::mutex> lk(m->queue_mu);
+    if (m->queue_device != dev) {       // first use (or the caller moved to another device): (re)allocate the counters
+      if (m->counters) { cudaFree(m->counters); m->counters = nullptr; }
       if ((e = cudaMalloc((void**)&m->counters, kCounterRing * 2 * sizeof(unsigned long long))) != cudaSuccess) return e;
-      m->side_device = dev;
+      m->queue_device = dev;
     }
     slot = m->next_call++;
   }
-  ctx.side = m->side_stream;
-  ctx.fork = m->fork_ev[slot % kEventRing];
-  ctx.join = m->join_ev[slot % kEventRing];
   ctx.counter = m->counters + 2 * (slot % kCounterRing);
   ctx.flag = reinterpret_cast<int*>(ctx.counter + 1);
   return cudaMemsetAsync(ctx.counter, 0, 2 * sizeof(unsigned long long), stream);
@@ -87,10 +77,10 @@ void spec_release(rbd_model* m) {
   m->spec.clear();
 }
 
-// Straight-line programs far beyond the instruction caches run at the SM's instruction-fetch rate (~1.4 instr/clk on B200)
-// instead of its issue rate; measured against the generic (looping, cache-resident) kernels on Atlas: fp32 ABA 12.7 k nodes
-// 1.03x, fp32 RNEA 5.8 k nodes 1.46x, 7-DoF arm 2.2 k nodes 2.7x, but fp64 ABA 0.83x (half the resident warps).  fp32 programs
-// are therefore always specialised, fp64 programs only below an estimated size.
+// Straight-line programs far beyond the instruction caches run at the SM's instruction-fetch rate instead of its issue rate,
+// and an fp64 stash halves the resident warps: against the generic (looping, cache-resident) kernels the fp32 programs win,
+// a large fp64 program (Atlas ABA) loses.  fp32 programs are therefore always specialised, fp64 programs only below an
+// estimated size.
 bool spec_worthwhile(const HostModel& hm, const SpecKey& key) {
   if (!key.f64) return true;
   if (key.algo == SPEC_CRBA) return !getenv("RBD_JIT_NO_CRBA64");   // small stash (2 rows per body): fp64 keeps its resident warps
@@ -113,20 +103,21 @@ int spec_prepare(rbd_model* m, const SpecKey& key, bool load_on_device, std::str
   if (!load_on_device) return RBD_OK;      // precompile only (CPU build step): the cubin is in the cache now
   cudaError_t e = cudaLibraryLoadData(&se.lib, cubin.data(), nullptr, nullptr, 0, nullptr, nullptr, 0);
   if (e == cudaSuccess) e = cudaLibraryGetKernel(&se.k_smem, se.lib, "rbd_jit_smem");
-  if (e == cudaSuccess) e = cudaLibraryGetKernel(&se.k_tmem, se.lib, "rbd_jit_tmem");
-  if (e == cudaSuccess) e = cudaLibraryGetKernel(&se.k_uni, se.lib, "rbd_jit_uni");
+  if (e == cudaSuccess) e = cudaLibraryGetKernel(&se.k_mix, se.lib, "rbd_jit_mix");
   cudaFuncAttributes fa{};
   if (e == cudaSuccess) { e = cudaFuncGetAttributes(&fa, (const void*)se.k_smem); se.regs_smem = fa.numRegs; }
-  if (e == cudaSuccess) { e = cudaFuncGetAttributes(&fa, (const void*)se.k_tmem); se.regs_tmem = fa.numRegs; }
-  if (e == cudaSuccess) { e = cudaFuncGetAttributes(&fa, (const void*)se.k_uni); se.regs_uni = fa.numRegs; }
-  if (e == cudaSuccess) e = cudaFuncSetAttribute((const void*)se.k_tmem, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  if (e == cudaSuccess) { e = cudaFuncGetAttributes(&fa, (const void*)se.k_mix); se.regs_mix = fa.numRegs; }
   se.rows = spec_stash_rows(m->hm, key);
   const size_t smem = (size_t)std::max(1, se.rows) * 32 * (key.f64 ? 8 : 4);
+  int optin = 0, dev = 0;
+  if (e == cudaSuccess) e = cudaGetDevice(&dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+  se.mix_sw = std::min<int>(kMixWarps, (int)(optin / smem));
   if (e == cudaSuccess) e = cudaFuncSetAttribute((const void*)se.k_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute((const void*)se.k_smem, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  se.uni_sw = spec_uni_smem_warps(m->hm, key);
-  if (e == cudaSuccess && se.uni_sw > 0) e = cudaFuncSetAttribute((const void*)se.k_uni, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(smem * se.uni_sw));
-  if (e == cudaSuccess) e = cudaFuncSetAttribute((const void*)se.k_uni, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
+  if (e == cudaSuccess && se.mix_sw > 0)
+    e = cudaFuncSetAttribute((const void*)se.k_mix, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(smem * se.mix_sw));
+  if (e == cudaSuccess) e = cudaFuncSetAttribute((const void*)se.k_mix, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   if (e != cudaSuccess) {
     cudaGetLastError();
     se.state = -1;
@@ -147,7 +138,7 @@ int spec_try_launch(rbd_model* m, const SpecKey& key, const SpecLaunchArgs& a, c
   if (!ev.jit || !spec_worthwhile(m->hm, key)) return RBD_OK;
   if (a.ld * (key.f64 ? 8 : 4) >= (1ll << 32)) return RBD_OK;   // the generated code forms row offsets as 32 x 32 -> 64-bit products of the byte stride
   const int rows = spec_stash_rows(m->hm, key);
-  if (rows > 256) return RBD_OK;                     // one warp's share of Tensor Memory: 256 fp32 rows (128 x 2 columns in fp64)
+  if (rows > 256) return RBD_OK;                     // larger stashes leave too few warps per SM: the generic kernels serve
   Props p;
   if (cudaError_t e = props(p)) { err = cudaGetErrorString(e); return RBD_ECUDA; }
   const size_t es = key.f64 ? 8 : 4;
@@ -178,68 +169,57 @@ int spec_try_launch(rbd_model* m, const SpecKey& key, const SpecLaunchArgs& a, c
     }
   }
   const int64_t ngroups = (a.B + 31) / 32;
-  const int tm_warps = key.f64 ? 4 : 8;
   int bps = 0;
   if (cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, (const void*)se->k_smem, 32, smem)) {
     err = cudaGetErrorString(e); return RBD_ECUDA;
   }
   if (bps < 1) return RBD_OK;
-  // Three ways to fill an SM (rbd_jit_kernels.cuh): shared-memory blocks alone, the kernel pair, the unified CTA.  The two
-  // Tensor-Memory variants are used when they put at least 15 % more warps on the SM than shared memory alone and there is work
-  // for them; which of the two is decided by timing both once, on the first call large enough to tell (not while capturing).
   if (ev.smem_blocks > 0) bps = std::max(1, std::min(bps, ev.smem_blocks));
-  const int rs = ((se->regs_smem + 7) / 8) * 8 * 32, rt = ((se->regs_tmem + 7) / 8) * 8 * 32 * tm_warps;
-  const int bps_pair = std::max(1, std::min(bps, (65536 - rt) / rs));
-  const bool pair_ok = !ev.no_tmem && rt + rs <= 65536 && (bps_pair + tm_warps) * 100 >= bps * 115 &&
-                       ngroups >= (int64_t)(bps_pair + tm_warps / 2) * p.sms;
-  const int uni_warps = se->uni_sw > 0 ? se->uni_sw + tm_warps : 0;
-  const bool uni_ok = !ev.no_tmem && uni_warps * 100 >= bps * 115 && ((se->regs_uni + 7) / 8) * 8 * 32 * uni_warps <= 65536 &&
-                      ngroups >= (int64_t)(uni_warps - tm_warps / 2) * p.sms;
+  // The mixed CTA (rbd_jit_kernels.cuh) is worth trying when it puts at least 15 % more warps on the SM than shared-memory blocks
+  // alone and there is a group of samples for each of its warps; which of the two is faster depends on the program, so the first
+  // call large enough to tell times both once and keeps the winner (not while capturing a graph).  RBD_JIT_VARIANT=1 / 2 forces one.
+  const int mix_warps = std::min(kMixWarps, 65536 / (((se->regs_mix + 7) / 8) * 8 * 32));
+  const int mix_sw = std::min(se->mix_sw, mix_warps);
+  const bool mix_ok = mix_sw >= 1 && mix_warps * 100 >= bps * 115 && ngroups >= (int64_t)mix_warps * p.sms;
   struct KArgs {
     const void* q; const void* v; const void* in2; void* o0; void* o1; long long ld, B; unsigned long long* counter; int* flag;
     void* peers[8]; long long peer_ld, peer_col0; void* mc; int npeers;
     void* ko[8];
+    void* l2_stash; int smem_warps;
   };
-  int launched = 0;
   int* last_flag = nullptr;
-  auto run = [&](int variant) -> cudaError_t {        // 0 = shared memory alone, 1 = pair, 2 = unified
-    PairCtx ctx;
-    cudaError_t e = pair_begin(m, stream, ctx);
+  auto run = [&](int variant) -> cudaError_t {        // 1 = shared-memory blocks, 2 = mixed CTA
+    QueueCtx ctx;
+    cudaError_t e = queue_begin(m, stream, ctx);
     if (e != cudaSuccess) return e;
     KArgs ka = {a.q, a.v, a.in2, a.o0, a.o1, (long long)a.ld, (long long)a.B, ctx.counter, ctx.flag, {}, (long long)a.peer_ld,
-                (long long)a.peer_col0, a.mc, a.npeers};
+                (long long)a.peer_col0, a.mc, a.npeers, {}, nullptr, mix_sw};
     for (int i = 0; i < a.npeers && i < 8; ++i) ka.peers[i] = a.peers[i];
     for (int i = 0; i < 8; ++i) ka.ko[i] = a.ko[i];
     void* params[] = {&ka};
     if (variant == 2) {
-      e = cudaLaunchKernel((const void*)se->k_uni, dim3(p.sms), dim3(32 * uni_warps), params, smem * se->uni_sw, stream);
-      ++launched;
-      li.grid = p.sms; li.block = 32 * uni_warps; li.blocks_per_sm = 1; li.smem_bytes = (int)(smem * se->uni_sw);
-    } else if (variant == 1) {
-      e = cudaEventRecord(ctx.fork, stream);
-      if (e == cudaSuccess) e = cudaStreamWaitEvent(ctx.side, ctx.fork, 0);
-      if (e == cudaSuccess && (!ev.only || ev.only[0] == 's')) { e = cudaLaunchKernel((const void*)se->k_smem, dim3(bps_pair * p.sms), dim3(32), params, smem, stream); ++launched; }
-      if (e == cudaSuccess && (!ev.only || ev.only[0] == 't')) { e = cudaLaunchKernel((const void*)se->k_tmem, dim3(p.sms), dim3(32 * tm_warps), params, 0, ctx.side); ++launched; }
-      if (e == cudaSuccess) e = cudaEventRecord(ctx.join, ctx.side);
-      if (e == cudaSuccess) e = cudaStreamWaitEvent(stream, ctx.join, 0);
-      li.grid = bps_pair * p.sms; li.block = 32; li.blocks_per_sm = bps_pair; li.smem_bytes = (int)smem;
+      e = cudaMallocAsync(&ka.l2_stash, (size_t)(mix_warps - mix_sw) * p.sms * smem, stream);
+      if (e == cudaSuccess) e = cudaLaunchKernel((const void*)se->k_mix, dim3(p.sms), dim3(32 * mix_warps), params, smem * mix_sw, stream);
+      if (ka.l2_stash) cudaFreeAsync(ka.l2_stash, stream);
+      li.grid = p.sms; li.block = 32 * mix_warps; li.blocks_per_sm = 1; li.smem_bytes = (int)(smem * mix_sw);
     } else {
       const int grid = (int)std::min<int64_t>(ngroups, (int64_t)bps * p.sms);
       e = cudaLaunchKernel((const void*)se->k_smem, dim3(grid), dim3(32), params, smem, stream);
-      ++launched;
       li.grid = grid; li.block = 32; li.blocks_per_sm = bps; li.smem_bytes = (int)smem;
     }
     last_flag = ctx.flag;
     return e;
   };
   cudaError_t e = cudaSuccess;
-  int variant = 0;
-  if (pair_ok && uni_ok) {
-    variant = ev.variant ? ev.variant : se->choice;
+  int variant = 1;
+  const char* force = getenv("RBD_JIT_VARIANT");
+  if (force && mix_ok) variant = atoi(force) == 2 ? 2 : 1;
+  else if (mix_ok) {
+    variant = se->choice;
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
     cudaStreamIsCapturing(stream, &cap);
     if (variant == 0 && cap == cudaStreamCaptureStatusNone && a.B >= (int64_t)p.sms * 32 * 64) {
-      // tune: each variant once to warm up, then timed; outputs are simply overwritten with the same values
+      // each variant once to warm up, then timed; the outputs are simply overwritten with the same values
       float best = 0.f;
       cudaEvent_t t0, t1;
       cudaEventCreate(&t0); cudaEventCreate(&t1);
@@ -255,15 +235,12 @@ int spec_try_launch(rbd_model* m, const SpecKey& key, const SpecLaunchArgs& a, c
       }
       cudaEventDestroy(t0); cudaEventDestroy(t1);
       if (e == cudaSuccess) se->choice = variant;
-      launched = 0;
     }
     if (variant == 0) variant = 1;
-  } else if (uni_ok) variant = 2;
-  else if (pair_ok) variant = 1;
-  if (ev.force_pair && uni_warps) variant = 2;
+  }
   if (e == cudaSuccess) e = run(variant);
   if (e != cudaSuccess) { err = std::string("specialised kernel launch: ") + cudaGetErrorString(e); return RBD_ECUDA; }
-  li.kernels_launched += launched;
+  li.kernels_launched += 1;
   if (gate && !key.f64 && !ev.no_gate) *gate = last_flag;
   used = true;
   return RBD_OK;

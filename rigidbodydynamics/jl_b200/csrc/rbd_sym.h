@@ -31,7 +31,7 @@ enum SymOp : int32_t {
   S_STORE,               // global output: arr, row, a = value
   S_SLD,                 // stash load:  row; grp = id of the first load of its ldv<N> batch
   S_SST,                 // stash store: row, a = value
-  S_SFENCE,              // stash store fence (Tensor Memory stores are asynchronous)
+  S_SFENCE,              // stash store fence: where a thread re-reads its own stash writes (a no-op in shared memory)
   S_XLD, S_XST,          // per-thread global scratch (body-frame external wrenches): row[, a]
 };
 

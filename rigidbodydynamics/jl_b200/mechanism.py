@@ -1,6 +1,6 @@
 """Host-side model: RigidBody / Joint / Mechanism, mirroring the reference's user-facing types.
 
-Reference (all under /root/reference/src):
+Reference (all under the reference's src/, RigidBodyDynamics.jl v2.5.0):
   RigidBody                 rigid_body.jl:12-29
   Joint                     joint.jl:43-67   (joint_to_predecessor :49, joint_to_successor :50)
   Mechanism                 mechanism.jl:10-34, default gravity (0,0,-9.81) mechanism.jl:1

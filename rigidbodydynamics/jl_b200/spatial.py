@@ -4,7 +4,7 @@ These are used ONLY to build and flatten a model on the host (URDF parsing, fixe
 merging, frame canonicalisation).  The batched dynamics never run through this file: they
 run in the CUDA kernels behind the C-ABI (``csrc/``).
 
-Conventions follow the reference (all citations relative to /root/reference):
+Conventions follow the reference (all citations relative to the root of RigidBodyDynamics.jl v2.5.0):
   * 6-vectors are [angular; linear]                      -- src/spatial/common.jl:13
   * ``Transform3D`` maps coordinates FROM one frame TO another: x_to = R x_from + p
                                                           -- src/spatial/transform3d.jl:7-69

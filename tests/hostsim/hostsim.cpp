@@ -179,7 +179,7 @@ void run_integrate(const HostModel& hm, int64_t B, T* q, T* v, const T* tau, dou
 
 extern "C" {
 // Model-specialised program (csrc/rbd_codegen.cpp) for the mechanism: flavor 0 = self-contained C++ (one sample per call),
-// 1 / 2 = the per-sample CUDA function bodies, 3 = the whole NVRTC translation unit.  Returns a malloc'ed string (free with
+// 1 = the per-sample CUDA function body, 3 = the whole NVRTC translation unit.  Returns a malloc'ed string (free with
 // hostsim_free) or NULL; stats = {nodes_traced, nodes_live, add, mul, div, neg, sincos, load, store, sld, sst, stash_rows}.
 // kin_mask / kin_sign (reference joint order, may be NULL): the rbd_kinematics variant (algo 3)
 static int g_kin_mask = 0;

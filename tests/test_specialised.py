@@ -102,7 +102,7 @@ def test_specialised_program_is_smaller_than_the_generic_walk(built):
 
 
 def test_nvrtc_compiles_without_a_gpu(built, tmp_path, monkeypatch):
-    """rbd_model_precompile(load = 0): generate + NVRTC-compile for sm_100a on this CPU-only machine, cubin lands in the cache."""
+    """rbd_model_precompile(load = 0): generate + NVRTC-compile for sm_90a without a GPU, cubin lands in the cache."""
     monkeypatch.setenv("RBD_JIT_CACHE", str(tmp_path))
     mech = rbd.load_model("double_pendulum")
     h = _cabi.ModelHandle(mech.flatten())
@@ -115,9 +115,10 @@ def test_nvrtc_compiles_without_a_gpu(built, tmp_path, monkeypatch):
     files = sorted(os.listdir(tmp_path))
     assert len(files) == 2 and all(f.endswith(".cubin") for f in files)
     assert any("_aba_f32_" in f for f in files) and any("_rnea_f32_" in f for f in files)
-    # it is a real sm_100a ELF holding both kernels
+    # it is a real sm_90a ELF holding the kernel (the low byte of e_flags is the SM version)
     blob = open(tmp_path / files[0], "rb").read()
-    assert blob[:4] == b"\x7fELF" and b"rbd_jit_smem" in blob and b"rbd_jit_tmem" in blob
+    assert blob[:4] == b"\x7fELF" and b"rbd_jit_smem" in blob
+    assert blob[48] == 90
 
 
 # ---------------------------------------------------------------------------------------------------------------- GPU tier
@@ -165,6 +166,38 @@ def test_specialised_kernels_match_oracle_gpu(built, name, floating, B):
     assert rel_err(out[:, :512].double().cpu().numpy(), o.inverse_dynamics(q[:, :512], v[:, :512], vd[:, :512])) < FP32_TOL
     rbd.dynamics_bias_(out, st)
     assert rel_err(out[:, :512].double().cpu().numpy(), o.dynamics_bias(q[:, :512], v[:, :512])) < FP32_TOL
+
+
+@pytest.mark.gpu
+def test_mixed_cta_with_l2_stash_matches_shared_memory_blocks_gpu(built, monkeypatch):
+    """Atlas at 2^19 samples is large enough for the mixed CTA (warps whose stash does not fit shared memory keep it in L2).
+    Forced either way, forward and inverse dynamics must be bit-identical and match the oracle."""
+    import torch
+    mech = rbd.load_model("atlas", floating=True)
+    B = 1 << 19
+    base = rand_inputs(mech, 512, 13)
+    q, v, tau, vd = (np.tile(a, (1, B // 512)) for a in base[:4])
+    o = Oracle(mech.flatten())
+    st = rbd.MechanismState(mech, B, torch.float32)
+    st.q.copy_(torch.from_numpy(q).float()); st.v.copy_(torch.from_numpy(v).float())
+    tau_d, vd_d = torch.from_numpy(tau).float().cuda(), torch.from_numpy(vd).float().cuda()
+    outs = {}
+    for variant in ("1", "2"):
+        monkeypatch.setenv("RBD_JIT_VARIANT", variant)
+        res = rbd.DynamicsResult(mech, B, torch.float32)
+        rbd.dynamics_(res, st, tau_d, want_qd=False)
+        info = rbd.launch_info()
+        assert info.specialised == 1 and info.block == (32 if variant == "1" else 512), (variant, info.block)
+        tau_out = torch.empty((st.nv, B), dtype=torch.float32, device="cuda")
+        rbd.inverse_dynamics_(tau_out, st, vd_d)
+        assert rbd.launch_info().block == (32 if variant == "1" else 512)
+        torch.cuda.synchronize()
+        outs[variant] = (res.vd.clone(), tau_out)
+    assert torch.equal(outs["1"][0], outs["2"][0]) and torch.equal(outs["1"][1], outs["2"][1])
+    got = outs["2"][0].double().cpu().numpy()
+    assert rel_err(got[:, :512], o.dynamics(q[:, :512], v[:, :512], tau[:, :512])) < FP32_TOL
+    assert np.array_equal(got.reshape(got.shape[0], -1, 512), np.broadcast_to(got[:, None, :512], (got.shape[0], B // 512, 512)))
+    assert rel_err(outs["2"][1][:, :512].double().cpu().numpy(), o.inverse_dynamics(q[:, :512], v[:, :512], vd[:, :512])) < FP32_TOL
 
 
 @pytest.mark.gpu

@@ -1,11 +1,13 @@
 """Shared helpers for the test-suite: models, seeded inputs, error metrics."""
+import gzip
 import os
 
 import numpy as np
 
 import rigidbodydynamics.jl_b200 as rbd
 
-REF_URDF = "/root/reference/test/urdf"
+# the reference's test URDFs (RigidBodyDynamics.jl v2.5.0, test/urdf/), stored gzip-compressed
+REF_URDF = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "urdf")
 ALL_JOINT_TYPES = ([rbd.QuaternionFloating] + [rbd.Revolute] * 5 + [rbd.Fixed] * 5 + [rbd.Prismatic] * 5
                    + [rbd.Planar] * 5 + [rbd.SPQuatFloating] * 2 + [rbd.SinCosRevolute] * 2
                    + [rbd.QuaternionSpherical] * 2)
@@ -48,8 +50,12 @@ def rel_err(got, ref):
     return float((np.abs(got - ref).max(0) / np.maximum(1.0, np.abs(ref).max(0))).max())
 
 
-def have_reference():
-    return os.path.isdir(REF_URDF)
+def ref_urdf(name, tmp_dir):
+    """Path of the reference's test URDF `name`, decompressed into `tmp_dir`."""
+    path = os.path.join(str(tmp_dir), name + ".urdf")
+    with gzip.open(os.path.join(REF_URDF, name + ".urdf.gz"), "rb") as src, open(path, "wb") as dst:
+        dst.write(src.read())
+    return path
 
 
 def make_duals(mech, q, v, tau, seed):

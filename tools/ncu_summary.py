@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Summarise an .ncu-rep (read with `ncu -i`): headline metrics, opcode mix, stall reasons per opcode class.
-    python tools/ncu_summary.py gpurun_out/prof.ncu-rep [kernel-index]
+    python tools/ncu_summary.py prof.ncu-rep [kernel-index]
 """
 import csv, subprocess, sys, io
 from collections import Counter

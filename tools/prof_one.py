@@ -1,4 +1,4 @@
-"""Run ONE fp32 forward-dynamics call (batch from argv, default 2^18) -- the target of the ncu captures in profiles/.
+"""Run ONE fp32 forward-dynamics call (batch from argv, default 2^18) -- the target of an ncu capture.
     prof_one.py [batch] [atlas|valkyrie|iiwa14|chainN] [dynamics|id]"""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,5 +1,5 @@
-"""Workload for compute-sanitizer (profiles/sanitizer_*.txt): every kernel family once, at batch sizes that take the production
-paths (shared-memory + Tensor-Memory kernel pair at 2^16; single kernels at 257)."""
+"""Workload for compute-sanitizer: every kernel family once, at batch sizes that take the production paths (model-specialised
+kernels at 2^16; generic kernels at 257)."""
 import os
 import sys
 
