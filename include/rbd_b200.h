@@ -222,6 +222,52 @@ typedef struct rbd_contact_desc {
 int32_t rbd_contact_dynamics(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                              const rbd_contact_desc* contact, void* state, void* state_deriv_out, void* wrenches_out, void* stream);
 
+/* Next row of the scope table (SURVEY 8(f) rank 4, second half): dynamics! for mechanisms WITH kinematic loops
+ *                                                             src/mechanism_algorithms.jl:845-864, :574-673, :747-822
+ * The model handle stays a TREE handle (the spanning tree, num_non_tree_joints = 0); the non-tree joints arrive per call in this
+ * descriptor (plain host arrays, read on the host), in non_tree_joints(mechanism) order.  Constraint rows are concatenated in that
+ * order (mechanism_state.jl:105-107).  Per loop joint:
+ *   predecessor / successor   tree-joint index whose successor is that body, -1 = the root body; predecessor != successor
+ *   joint_to_predecessor      frame before the joint -> predecessor body frame: rotation row-major (9), translation (3)
+ *   joint_to_successor        frame after the joint  -> successor body frame, same layout (Joint.joint_to_successor)
+ *   nconstraints, wrench_basis  constraint_wrench_subspace(joint_type, tf): nconstraints (0..6) columns [torque; force] in the frame
+ *                             after the joint, in the reference's column order (fixed.jl:42, revolute.jl:91, prismatic.jl:96,
+ *                             planar.jl:95, quaternion_spherical.jl:60, sin_cos_revolute.jl:125; 0 columns for floating joints)
+ *   gains                     Baumgarte stabilisation SE3PDGains: angular k, d, linear k, d (default 100, 20, 100, 20,
+ *                             mechanism_algorithms.jl:610-612); gains == NULL disables stabilisation (stabilization_gains = nothing).
+ * The library derives each loop's path (TreePath predecessor -> successor) from the model's parent[]. */
+#define RBD_MAX_LOOP_JOINTS 16
+#define RBD_MAX_CONSTRAINTS 96
+typedef struct rbd_loop_desc {
+  int32_t nloops;
+  const int32_t* predecessor;          /* [nloops]                        */
+  const int32_t* successor;            /* [nloops]                        */
+  const double* joint_to_predecessor;  /* [nloops][12]                    */
+  const double* joint_to_successor;    /* [nloops][12]                    */
+  const int32_t* nconstraints;         /* [nloops] 0..6                   */
+  const double* wrench_basis;          /* [sum nconstraints][6]           */
+  const double* gains;                 /* [nloops][4] or NULL             */
+} rbd_loop_desc;
+
+/*   q [nq x B], v [nv x B], tau [nv x B] or NULL (zero), wext [6*nb x B] or NULL (root-frame wrenches as in rbd_dynamics)
+ *   -> vd_out [nv x B] (result.v̇), qd_out [nq x B] (result.q̇), lambda_out [nl x B] (result.λ), K_out [nl*nv x B]
+ *      (result.constraintjacobian, entry (c, j) at row c + j*nl, column-major), k_out [nl x B] (result.constraintbias);
+ *      every output except vd_out may be NULL.  nl = sum of nconstraints.
+ * The reference's BLAS solve (dynamics_solve!, :747-822):  M = L L^T,  Y = K L^-T,  z = L^-1 (tau - c),  A = Y Y^T,  b = Y z + k,
+ * lambda = gelsy(A, b, rcond)  (minimum-norm solution of the rank-truncated system: A is only positive SEMI-definite),
+ * v̇ = M^-1 (tau - c - K^T lambda).  Here the rank of A is decided by a diagonally pivoted Cholesky factorisation A ~ P^T G G^T P
+ * that stops at the first pivot with  G_ii^2 <= rcond * G_11^2, and lambda = P^T G (G^T G)^-2 G^T P b, the minimum-norm
+ * least-squares solution of the truncated system (equal to gelsy's wherever the rank gap is clear).
+ * rcond: 1e-10 in fp64, the reference's constant (:804).  fp32: 1e-5 (about 100 fp32 epsilons): the Schur complement left by a
+ * structurally zero constraint row (three of the five rows of a planar four-bar's revolute loop joint) carries rounding of order
+ * eps_32 * G_11^2 ~ 1e-7 G_11^2, which 1e-10 would keep as rank and amplify into lambda.
+ * fp32 / fp64 only (RBD_DUAL64X6 -> RBD_EUNSUPPORTED); more than RBD_MAX_LOOP_JOINTS loops or RBD_MAX_CONSTRAINTS rows ->
+ * RBD_EUNSUPPORTED (callers fall back to the reference); a malformed descriptor (index out of range, predecessor == successor,
+ * nconstraints outside 0..6) -> RBD_EINVAL.  With nloops = 0 the result is v̇ = M^-1 (tau - c). */
+int32_t rbd_dynamics_loops(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
+                           const void* tau, const void* wext, const rbd_loop_desc* loops,
+                           void* vd_out, void* qd_out, void* lambda_out, void* K_out, void* k_out, void* stream);
+
 /* dynamics!(result, ...) INCLUDING the by-products the reference leaves in the DynamicsResult (src/dynamics_result.jl:11-85,
  * mechanism_algorithms.jl:849-863): besides v̇ / q̇, any of  result.massmatrix (M_out [nv*nv x B], see rbd_mass_matrix),
  * result.dynamicsbias (c_out [nv x B]), result.accelerations and result.jointwrenches (see rbd_inverse_dynamics_bodies, evaluated

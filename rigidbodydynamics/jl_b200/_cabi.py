@@ -12,6 +12,7 @@ from ctypes import POINTER, Structure, c_char_p, c_double, c_float, c_int32, c_i
 import numpy as np
 
 RBD_MAX_BODIES = 64
+RBD_MAX_LOOP_JOINTS, RBD_MAX_CONSTRAINTS = 16, 96
 
 RBD_OK, RBD_EINVAL, RBD_EDIM, RBD_ELOOP, RBD_ESTALE, RBD_ECUDA, RBD_EUNSUPPORTED, RBD_ENOMEM = range(8)
 RBD_F32, RBD_F64, RBD_DUAL64X6 = 0, 1, 2
@@ -111,6 +112,7 @@ SYMBOLS = {
     "rbd_inverse_dynamics": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rbd_inverse_dynamics_bodies": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rbd_contact_dynamics": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "rbd_dynamics_loops": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rbd_dynamics_result": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rbd_dynamics_derivatives": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rbd_model_precompile_derivatives": (c_int32, [_vp, _i32]),

@@ -49,6 +49,13 @@ def _call(status):
     _cabi.check(status)
 
 
+def _require_tree(state: MechanismState, what: str):
+    """Paths that cannot honour loop constraints refuse a mechanism with non-tree joints before anything is launched, with the
+    reference's error (mechanism_algorithms.jl:549), instead of silently evaluating the spanning tree."""
+    if state.mechanism.has_loops():
+        raise _cabi.RbdError(_cabi.RBD_ELOOP, f"{what}: This method can currently only handle tree Mechanisms.")
+
+
 def dynamics_(result: DynamicsResult, state: MechanismState, torques: Optional[torch.Tensor] = None,
               externalwrenches: Optional[torch.Tensor] = None, want_qd: bool = True, byproducts=()):
     """``dynamics!(result, state, torques, externalwrenches)``: fills ``result.vd`` (v̇) and ``result.qd`` (q̇).
@@ -59,8 +66,22 @@ def dynamics_(result: DynamicsResult, state: MechanismState, torques: Optional[t
     The reference's ``dynamics!`` also leaves ``result.massmatrix``, ``result.dynamicsbias`` (it solves M v̇ = tau - c) and, on
     request, ``result.accelerations`` / ``result.jointwrenches`` behind (dynamics_result.jl:11-85).  The Articulated-Body kernel
     needs none of them, so they are computed only when named in ``byproducts`` (any of "massmatrix", "dynamicsbias",
-    "accelerations", "jointwrenches", or "all") -- a drop-in caller that reads those fields passes ``byproducts="all"``."""
+    "accelerations", "jointwrenches", or "all") -- a drop-in caller that reads those fields passes ``byproducts="all"``.
+
+    A mechanism with loops goes to ``dynamics_loops_`` with the default stabilisation gains, as the reference's ``dynamics!`` does
+    (mechanism_algorithms.jl:858-862); of the by-products it leaves ``massmatrix`` and ``dynamicsbias`` (spanning tree)."""
     state.check_modcount()
+    if state.mechanism.has_loops():
+        from .loops import dynamics_loops_
+        want = {"massmatrix", "dynamicsbias"} if byproducts == "all" else set(byproducts or ())
+        if want - {"massmatrix", "dynamicsbias"}:
+            raise _cabi.RbdError(_cabi.RBD_ELOOP, "dynamics_: accelerations / jointwrenches of a mechanism with loops are not available")
+        dynamics_loops_(result, state, torques, externalwrenches, want_qd=want_qd)
+        if "massmatrix" in want:
+            mass_matrix_(result, state)
+        if "dynamicsbias" in want:
+            dynamics_bias_(result, state, externalwrenches)
+        return result
     lib = _cabi.load_library()
     _check(torques, state.nv, state, "torques")
     _check(externalwrenches, 6 * len(state.mechanism.joints), state, "externalwrenches")
@@ -85,6 +106,7 @@ def dynamics_dual_(vd_out: torch.Tensor, state: MechanismState, q: torch.Tensor,
     """``dynamics!`` on ``ForwardDiff.Dual{Tag,Float64,6}`` inputs (BASELINE config 4; the reference reaches this through
     its generic-scalar path, examples/5 + src/caches.jl:46-64).  Arrays are float64 ``[rows, B, 7]`` = (value, 6 partials)
     per element, which is the memory layout of a Julia ``Matrix{Dual}(B, n)``.  ``state`` only supplies the model handle."""
+    _require_tree(state, "dynamics_dual_")
     state.check_modcount()
     lib = _cabi.load_library()
     B = q.shape[1]
@@ -107,6 +129,7 @@ def dynamics_derivatives_(dvd_dq: torch.Tensor, dvd_dv: torch.Tensor, result: Dy
     test/test_mechanism_algorithms.jl:600-675).  ``dvd_dq`` / ``dvd_dv`` are [nv*nv, B], entry (i, j) at row i + j*nv (column-major
     like ``M.data``); ``dvd_dq[:, j]`` is the derivative along ``velocity_to_configuration_derivative(e_j)``, i.e.
     ``(d v̇/d q) * velocity_to_configuration_derivative_jacobian(state)``.  ``result.vd`` receives v̇."""
+    _require_tree(state, "dynamics_derivatives_")
     state.check_modcount()
     lib = _cabi.load_library()
     _check(torques, state.nv, state, "torques")
@@ -138,6 +161,7 @@ def simulate_(state: MechanismState, final_time: float, torques: Optional[torch.
     steps (src/ode_integrators.jl:233-300) until ``t >= final_time``; ``state.q`` / ``state.v`` are advanced in place.  The
     control is the default passive one (``torques=None``) or a constant torque array [nv, B] (zero-order hold over the call);
     a time-varying controller calls this once per control interval.  Returns the number of steps taken."""
+    _require_tree(state, "simulate_")
     state.check_modcount()
     lib = _cabi.load_library()
     nsteps, t = 0, 0.0
@@ -168,6 +192,7 @@ def inverse_dynamics_(torquesout: torch.Tensor, state: MechanismState, vd: torch
     """``inverse_dynamics!(torquesout, jointwrenchesout, accelerations, state, v̇, externalwrenches)`` (mechanism_algorithms.jl:542-553):
     tau = M(q) v̇ + c(q, v, w_ext).  ``jointwrenchesout`` / ``accelerations`` [6*nb, B] (optional) receive the reference's per-body
     outputs, root frame, rows 6i..6i+5 for the successor of tree joint i."""
+    _require_tree(state, "inverse_dynamics_")
     state.check_modcount()
     lib = _cabi.load_library()
     nb6 = 6 * len(state.mechanism.joints)

@@ -25,7 +25,7 @@ import numpy as np
 import torch
 
 from . import _cabi
-from .algorithms import DimensionMismatch, _call, _check, _ptr, _stream, dynamics_
+from .algorithms import DimensionMismatch, _call, _check, _ptr, _require_tree, _stream, dynamics_
 from .state import DynamicsResult, MechanismState, _DT
 
 __all__ = ["HuntCrossleyModel", "hunt_crossley_hertz", "ViscoelasticCoulombModel", "SoftContactModel", "ContactPoint", "HalfSpace3D",
@@ -179,6 +179,7 @@ def dynamics_contact_(result: DynamicsResult, state: MechanismState, torques: Op
     """``dynamics!`` for a mechanism with contact points (mechanism_algorithms.jl:845-866): contact_dynamics!, then the contact
     wrench of every body is added to its external wrench and the forward dynamics run on the sum.  Leaves
     ``result.contactwrenches`` and ``result.totalwrenches`` ([6*nb, B]) behind like the reference's DynamicsResult."""
+    _require_tree(state, "dynamics_contact_")
     nb6 = 6 * len(state.mechanism.joints)
     _check(externalwrenches, nb6, state, "externalwrenches")
     cw = getattr(result, "contactwrenches", None)

@@ -6,6 +6,7 @@ Reference (all under the reference's src/, RigidBodyDynamics.jl v2.5.0):
   Mechanism                 mechanism.jl:10-34, default gravity (0,0,-9.81) mechanism.jl:1
   attach!                   mechanism_modification.jl:21-46
   remove_fixed_tree_joints! mechanism_modification.jl:260-317
+  maximal_coordinates       mechanism_modification.jl:335-362
   rand_*_mechanism          mechanism_modification.jl:382-426
 
 A ``Mechanism`` is immutable while a batch is being evaluated; ``flatten()`` turns it into the plain
@@ -51,6 +52,9 @@ class Joint:
         self.name = name
         self.joint_type = joint_type
         self.joint_to_predecessor = Transform3D.identity()   # frame before joint -> predecessor body frame
+        # frame after joint -> successor body frame: the identity for tree joints (the body frame IS the frame after the joint),
+        # inv(successor_pose) for non-tree joints (mechanism_modification.jl:34)
+        self.joint_to_successor = Transform3D.identity()
         self.predecessor: Optional[RigidBody] = None
         self.successor: Optional[RigidBody] = None
 
@@ -86,8 +90,8 @@ class ModelDesc:
 
 
 class Mechanism:
-    """mechanism.jl:10-34 (tree part; non-tree joints are recorded so the hot path can refuse them,
-    as inverse_dynamics! does at mechanism_algorithms.jl:549)."""
+    """mechanism.jl:10-34.  ``joints`` is the spanning tree (the q/v order); non-tree (loop) joints are kept in
+    ``non_tree_joints`` with their attachment transforms and enter dynamics! as constraints (loops.py)."""
 
     def __init__(self, root_body: Optional[RigidBody] = None, gravity=DEFAULT_GRAVITATIONAL_ACCELERATION):
         self.root_body = root_body if root_body is not None else RigidBody("world")
@@ -147,8 +151,11 @@ class Mechanism:
         joint.joint_to_predecessor = joint_pose if joint_pose is not None else Transform3D.identity()
         joint.predecessor, joint.successor = predecessor, successor
         if successor in self.bodies:
-            self.non_tree_joints.append(joint)      # loop joint: recorded, not evaluated on the GPU path
+            # loop joint: the successor keeps its frame, the joint records where it attaches (mechanism_modification.jl:34)
+            joint.joint_to_successor = successor_pose.inv() if successor_pose is not None else Transform3D.identity()
+            self.non_tree_joints.append(joint)
         else:
+            joint.joint_to_successor = Transform3D.identity()
             if successor.inertia is None:
                 successor.inertia = SpatialInertia.zero()
             if successor_pose is not None:
@@ -178,6 +185,7 @@ class Mechanism:
                     j.joint_to_predecessor = to_pred * j.joint_to_predecessor
                 if j.successor is succ:                   # only possible for non-tree joints
                     j.successor = pred
+                    j.joint_to_successor = to_pred * j.joint_to_successor
             self.bodies.remove(succ)
             self.joints.remove(fj)
         self.modcount += 1
@@ -226,6 +234,30 @@ class Mechanism:
     def __repr__(self):
         return (f"Mechanism({len(self.bodies) - 1} bodies, nq={self.num_positions()}, "
                 f"nv={self.num_velocities()})")
+
+
+def maximal_coordinates(mechanism: Mechanism, floating_joint_type: type = QuaternionFloating, bodymap: Optional[dict] = None,
+                        jointmap: Optional[dict] = None) -> Mechanism:
+    """mechanism_modification.jl:335-362: every non-root body is attached to the root by a floating joint and every joint of
+    ``mechanism`` (tree and non-tree) becomes a non-tree joint between the copies.  ``bodymap`` / ``jointmap`` (optional dicts)
+    receive original -> copy, like the reference's keyword arguments."""
+    import copy
+    if not floating_joint_type.isfloating:
+        raise ValueError("floating_joint_type must be a floating joint type")
+    bodymap = {} if bodymap is None else bodymap
+    jointmap = {} if jointmap is None else jointmap
+    bodymap.clear()
+    jointmap.clear()
+    root = bodymap[mechanism.root_body] = RigidBody(mechanism.root_body.name)
+    ret = Mechanism(root, gravity=mechanism.gravitational_acceleration)
+    for src in mechanism.non_root_bodies():
+        body = bodymap[src] = RigidBody(src.name, src.inertia.copy())
+        ret.attach(root, body, Joint(str(src.name), floating_joint_type()))
+    for src in mechanism.joints + mechanism.non_tree_joints:             # _copyjoint! (:48-63)
+        joint = jointmap[src] = Joint(src.name, copy.deepcopy(src.joint_type))
+        ret.attach(bodymap[src.predecessor], bodymap[src.successor], joint, joint_pose=src.joint_to_predecessor,
+                   successor_pose=src.joint_to_successor.inv())
+    return ret
 
 
 # -------------------------------------------------------------------------------------------------

@@ -82,8 +82,9 @@ def dynamics_gather_(gathered: GatheredResult, state, torques=None):
     reading columns owned by other ranks."""
     import ctypes
     from . import _cabi
-    from .algorithms import _check, _ptr, _stream
+    from .algorithms import _check, _ptr, _require_tree, _stream
     from .state import _DT
+    _require_tree(state, "dynamics_gather_")
     state.check_modcount()
     if state.batch != gathered.B_local or gathered.rows != state.nv or gathered.tensor.dtype != state.dtype:
         raise ValueError("gathered array does not match the state (rows = nv, B_local = state.batch, same dtype)")

@@ -22,11 +22,12 @@ _DT = {torch.float32: _cabi.RBD_F32, torch.float64: _cabi.RBD_F64}
 def _model_handle(mechanism: Mechanism) -> "_cabi.ModelHandle":
     """Flatten once per (mechanism, modcount): the analogue of constructing a MechanismState
     (mechanism_state.jl:79-172).  A modified mechanism gets a fresh handle; stale states are caught by
-    ``rbd_model_check_modcount`` (ModificationCountMismatch, src/util.jl:56-72)."""
+    ``rbd_model_check_modcount`` (ModificationCountMismatch, src/util.jl:56-72).  The handle describes the spanning tree only;
+    the non-tree joints of a mechanism with loops are passed per call by ``dynamics_loops_`` (loops.py)."""
     cache = getattr(mechanism, "_rbd_handle", None)
     if cache is None or cache[0] != mechanism.modcount:
         desc = mechanism.flatten()
-        h = _cabi.ModelHandle(desc, num_non_tree_joints=len(mechanism.non_tree_joints))
+        h = _cabi.ModelHandle(desc, num_non_tree_joints=0)
         mechanism._rbd_handle = (mechanism.modcount, h, desc)
     return mechanism._rbd_handle[1]
 
@@ -150,7 +151,8 @@ def rand_(state: MechanismState, rng: np.random.Generator):
 
 class DynamicsResult:
     """dynamics_result.jl:11-85, batched: ``vd`` (v̇) [nv, B], ``qd`` (q̇) [nq, B], ``massmatrix`` [nv*nv, B]
-    (entry (i, j) at row i + j*nv, both triangles), ``dynamicsbias`` [nv, B]."""
+    (entry (i, j) at row i + j*nv, both triangles), ``dynamicsbias`` [nv, B]; for mechanisms with loops also ``lam`` (λ) [nl, B],
+    ``constraintjacobian`` [nl*nv, B] (entry (c, j) at row c + j*nl) and ``constraintbias`` [nl, B]."""
 
     def __init__(self, mechanism: Mechanism, batch: int = 1, dtype: torch.dtype = torch.float64,
                  device: Optional[torch.device] = None, with_massmatrix: bool = False):
@@ -164,7 +166,9 @@ class DynamicsResult:
         self._mm = torch.empty((nv * nv, batch), dtype=dtype, device=device) if with_massmatrix else None
         self._mm_args = (nv, batch, dtype, device)
         self._nb6 = 6 * len(mechanism.joints)
+        self._nl = sum(6 - j.nv for j in mechanism.non_tree_joints)      # constraint rows (loops.num_constraints)
         self._acc = self._jw = None
+        self._lam = self._K = self._k = None
 
     @property
     def accelerations(self) -> torch.Tensor:
@@ -181,6 +185,31 @@ class DynamicsResult:
             _, batch, dtype, device = self._mm_args
             self._jw = torch.empty((self._nb6, batch), dtype=dtype, device=device)
         return self._jw
+
+    def _rows(self, rows):
+        _, batch, dtype, device = self._mm_args
+        return torch.empty((rows, batch), dtype=dtype, device=device)
+
+    @property
+    def lam(self) -> torch.Tensor:
+        """result.λ: constraint forces [nl, B], allocated on first use."""
+        if self._lam is None:
+            self._lam = self._rows(self._nl)
+        return self._lam
+
+    @property
+    def constraintjacobian(self) -> torch.Tensor:
+        """result.constraintjacobian K: [nl*nv, B], entry (c, j) at row c + j*nl, allocated on first use."""
+        if self._K is None:
+            self._K = self._rows(self._nl * self._mm_args[0])
+        return self._K
+
+    @property
+    def constraintbias(self) -> torch.Tensor:
+        """result.constraintbias k: [nl, B], allocated on first use."""
+        if self._k is None:
+            self._k = self._rows(self._nl)
+        return self._k
 
     @property
     def massmatrix(self) -> torch.Tensor:
