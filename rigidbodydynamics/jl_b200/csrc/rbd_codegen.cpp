@@ -5,8 +5,13 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <array>
+#include <functional>
+#include <map>
 #include <memory>
+#include <set>
 #include <unordered_map>
+#include <unordered_set>
 
 #include "rbd_rnea_crba.cuh"
 #include "rbd_sym.h"
@@ -15,7 +20,7 @@
 namespace rbd {
 namespace {
 
-constexpr int kGeneratorVersion = 26;   // bump when the emitted code changes (part of the cubin cache key)
+constexpr int kGeneratorVersion = 28;   // bump when the emitted code changes (part of the cubin cache key)
 
 template <class F> const ModelDev<F>& devm(const HostModel& m);
 template <> const ModelDev<float>& devm<float>(const HostModel& m) { return m.dev32; }
@@ -35,7 +40,19 @@ bool run_trace(const HostModel& hm, const SpecKey& key, SymTrace& tr, int& stash
   tr.single = !key.f64;
   TraceScope scope(&tr);
   std::unique_ptr<ModelDev<Sym>> M(new ModelDev<Sym>());
-  if (key.f64) sym_model(hm.dev64, *M); else sym_model(hm.dev32, *M);
+  const std::vector<FoldPair>* pairs = key.algo == SPEC_ABA ? &hm.pairs : nullptr;
+  if (key.f64) sym_model(hm.dev64, *M, pairs); else sym_model(hm.dev32, *M, pairs);
+  if (pairs)
+    for (const FoldPair& fp : *pairs)
+      for (int pass = 1; pass <= 3; ++pass) {
+        const int a = pass == 2 ? fp.l0 + 2 * fp.len - 1 : fp.l0, b = pass == 2 ? fp.l0 + fp.len - 1 : fp.l0 + fp.len;
+        tr.fresh_steps.insert({pass, a});
+        tr.fresh_steps.insert({pass, b});
+        // the step before the pair already requests the first body's joint scalars (prefetch_body)
+        if (pass == 2) tr.fresh_steps.insert(a + 1 < hm.nb ? std::make_pair(2, a + 1) : std::make_pair(1, -1));
+        else if (a > 1) tr.fresh_steps.insert({pass, a - 1});
+        else if (pass == 3) tr.fresh_steps.insert({2, -1});
+      }
   const SymStash st;
   if (key.algo == SPEC_ABA) {
     AbaIO<Sym, false, kAllKinds> io;
@@ -155,7 +172,7 @@ struct Emitter {
   }
   std::string ref(int id) const {
     const SymNode& n = tr.nodes[id];
-    if (n.op == S_CONST) return "RBD_K(" + lit(n.c) + ")";
+    if (n.op == S_CONST || n.op == S_PARAM) return "RBD_K(" + lit(n.c) + ")";   // straight-line code: a parameter is its value
     return "t" + std::to_string(id);
   }
   static const char* arr_name(int arr) {
@@ -172,93 +189,410 @@ struct Emitter {
     }
     return "?";
   }
+  bool stmt_node(int i) const {
+    const int op = tr.nodes[i].op;
+    return live[i] && op != S_CONST && op != S_LOAD && op != S_PARAM;
+  }
+
+  // Text of statement i: name(j) = variable of node j, opnd(j, k) = operand k (0: a, 1: b) of node j, row(j) = its row expression.
+  using NameFn = std::function<std::string(int)>;
+  using OpFn = std::function<std::string(int, int)>;
+  std::string stmt(int i, const NameFn& name, const OpFn& opnd, const NameFn& row) {
+    const SymNode& n = tr.nodes[i];
+    const std::string v = "const rbd_v " + name(i) + " = ";
+    switch (n.op) {
+      case S_ADD:
+      case S_SUB: {
+        ++stats.n_add;
+        auto it = fma_of.find(i);
+        if (it == fma_of.end()) return v + (n.op == S_ADD ? "RBD_ADD(" : "RBD_SUB(") + opnd(i, 0) + ", " + opnd(i, 1) + ");\n";
+        const int p = it->second;
+        const char* f = n.op == S_ADD ? "RBD_FMA" : (p == n.a ? "RBD_FMS" /* x*y - c */ : "RBD_FNMA" /* c - x*y */);
+        return v + f + "(" + opnd(p, 0) + ", " + opnd(p, 1) + ", " + opnd(i, p == n.a ? 1 : 0) + ");\n";
+      }
+      case S_MUL: ++stats.n_mul; return v + "RBD_MUL(" + opnd(i, 0) + ", " + opnd(i, 1) + ");\n";
+      case S_DIV:
+        ++stats.n_div;
+        if (tr.is_const(n.a, 1.0)) return v + "RBD_RCP(" + opnd(i, 1) + ");\n";
+        return v + "RBD_DIV(" + opnd(i, 0) + ", " + opnd(i, 1) + ");\n";
+      case S_NEG: ++stats.n_neg; return v + "RBD_NEG(" + opnd(i, 0) + ");\n";
+      case S_SIN:
+        ++stats.n_sincos;
+        return "rbd_v " + name(i) + ", " + name(i + 1) + "; RBD_SINCOS(" + opnd(i, 0) + ", " + name(i) + ", " + name(i + 1) + ");\n";
+      case S_LOAD:
+        ++stats.n_load;
+        if (n.arr == A_V) ++stats.n_load_v;
+        return v + "RBD_LDG(" + arr_name(n.arr) + ", " + row(i) + ");\n";
+      case S_STORE:
+        ++stats.n_store;
+        if (key.peers && n.arr == A_OUT0 && flavor != FLAVOR_CPU) return "RBD_STG_PEERS(" + row(i) + ", " + opnd(i, 0) + ");\n";
+        return std::string("RBD_STG(") + arr_name(n.arr) + ", " + row(i) + ", " + opnd(i, 0) + ");\n";
+      case S_SLD: ++stats.n_sld; return v + "RBD_SLD(" + row(i) + ");\n";
+      case S_SST: ++stats.n_sst; return "RBD_SST(" + row(i) + ", " + opnd(i, 0) + ");\n";
+      case S_SFENCE: return "RBD_SFENCE();\n";
+      case S_XLD: return v + "RBD_XLD(" + row(i) + ");\n";
+      case S_XST: return "RBD_XST(" + row(i) + ", " + opnd(i, 0) + ");\n";
+    }
+    return "";
+  }
+  std::string split_point(int i, int& since) {
+    const SymNode& n = tr.nodes[i];
+    if (split_every > 0 && n.op != S_COS && ++since >= split_every && !(n.op == S_SLD && n.grp != i)) {
+      since = 0;
+      return "RBD_SPLIT();\n";
+    }
+    return "";
+  }
+
+  // ---- folding mirror-image chains ------------------------------------------------------------------------------------
+  // In each ABA pass the two chains of a HostModel pair are walked back to back: segment A (the first walked: the left chain
+  // outward, the right chain inward), then segment B.  B is folded onto A when it is the same program statement by statement:
+  // same operations and FMA contractions, operands that correspond (B's own statements <-> A's, parameters by slot, global
+  // loads and stash rows by a per-statement row offset), except for the nodes inside each body's trace_conn brackets (the
+  // link to the parent, which differs between a first child and a sibling).  A is then emitted once as the body of a
+  // two-iteration loop: iteration 0 is A, iteration 1 is B; rows become row_A + it * offset, parameters come from a
+  // per-instance table, the connection nodes run in a branch on the iteration, and every value the loop hands on is
+  // assigned to a variable declared before it.  Both iterations execute exactly the statements of the straight-line program.
+  struct Fold {
+    int a0 = 0, mid = 0, b1 = 0, instA = 0, first = 0, len = 0, pass = 0;
+    std::vector<int32_t> la, lb;                                     // matched statements of A and B, in order
+    std::vector<std::vector<int32_t>> ca, cb;                        // connection statements of step k
+    std::vector<int> cat;                                            // matched statements before connection k (-1: none)
+    std::unordered_map<int32_t, int> connk;                          // connection statement -> k
+    std::unordered_map<int32_t, int32_t> b2a;
+    std::unordered_set<int32_t> amatched;
+    std::unordered_map<int32_t, std::array<std::string, 2>> opa;    // operand texts of A's statements
+    std::unordered_map<int32_t, int> drow;                           // A statement -> row offset of its B twin
+    std::map<int32_t, int> dload;                                    // A-side load -> row offset of B's
+    std::vector<std::array<int32_t, 3>> pv;                          // per-instance values: A node, B node, connection k (-1: none)
+    std::set<std::pair<int32_t, int32_t>> pvs;
+    std::vector<int32_t> outs;                                       // nodes of A or B used after the loop
+  };
+  bool fold = true;
+  const HostModel* hm = nullptr;
+  std::vector<Fold> folds;
+  std::vector<int32_t> fold_at, in_fold;
+  std::vector<uint8_t> remat;
+
+  static std::string pvname(int32_t x, int32_t y) { return "x" + std::to_string(x) + "_" + std::to_string(y); }
+
+  // operand x of an A statement against operand y of its B twin
+  struct Bind { int kind = 0, x = -1, y = -1, d = 0, k = -1; std::string txt; };
+  bool bind(const Fold& f, int x, int y, Bind& o) const {
+    const SymNode& nx = tr.nodes[x];
+    const SymNode& ny = tr.nodes[y];
+    o = Bind();
+    if (nx.op == S_CONST || ny.op == S_CONST) { o.txt = ref(x); return x == y; }
+    if (nx.op == S_PARAM || ny.op == S_PARAM) {
+      o.txt = "RBD_PAR(" + std::to_string(nx.row) + ")";
+      return nx.op == ny.op && nx.row == ny.row && nx.arr == f.instA && ny.arr == 1 - f.instA;
+    }
+    const bool xl = nx.op == S_LOAD, yl = ny.op == S_LOAD;
+    if (xl && yl && nx.arr == ny.arr) {
+      o.kind = 1; o.x = x; o.d = ny.row - nx.row;
+      auto it = f.dload.find(x);
+      o.txt = "l" + std::to_string(x);
+      return it == f.dload.end() || it->second == o.d;
+    }
+    const bool xa = x >= f.a0 && x < f.mid, yb = y >= f.mid && y < f.b1;
+    if (!xl && xa && f.amatched.count(x)) {
+      auto it = f.b2a.find(y);
+      o.txt = "u" + std::to_string(x);
+      return yb && it != f.b2a.end() && it->second == x;
+    }
+    // otherwise a per-instance value: a load, a node before the pair, or a connection node, on either side
+    const bool xcon = !xl && xa && f.connk.count(x), ycon = !yl && yb && f.connk.count(y);
+    if (!(xl || xcon || (x < f.a0 && !fused[x]))) return false;
+    if (!(yl || ycon || (y < f.a0 && !fused[y]))) return false;
+    if (x == y) { o.txt = ref(x); return true; }                     // the same value outside the pair
+    const int kx = xcon ? f.connk.at(x) : -1, ky = ycon ? f.connk.at(y) : -1;
+    if (kx >= 0 && ky >= 0 && kx != ky) return false;
+    o.kind = 2; o.x = x; o.y = y; o.k = std::max(kx, ky);
+    o.txt = pvname(x, y);
+    return true;
+  }
+  void commit(Fold& f, const Bind& b) {
+    if (b.kind == 1) f.dload[b.x] = b.d;
+    if (b.kind == 2 && f.pvs.insert({b.x, b.y}).second) f.pv.push_back({b.x, b.y, b.k});
+  }
+  // operand text inside a connection branch (side 0: A, 1: B); "" = not expressible
+  std::string conn_ref(const Fold& f, int side, int x) const {
+    const SymNode& n = tr.nodes[x];
+    if (n.op == S_CONST) return ref(x);
+    if (n.op == S_PARAM) return n.arr == (side ? 1 - f.instA : f.instA) ? "RBD_PAR(" + std::to_string(n.row) + ")" : "";
+    if (n.op == S_LOAD) return std::string("RBD_LDG(") + arr_name(n.arr) + ", " + std::to_string(n.row) + ")";
+    if (f.connk.count(x) && (side ? x >= f.mid : x < f.mid)) return "c" + std::to_string(x);
+    if (side == 0 && f.amatched.count(x)) return "u" + std::to_string(x);
+    if (side == 1) { auto it = f.b2a.find(x); if (it != f.b2a.end()) return "u" + std::to_string(it->second); }
+    if (x < f.a0 && !fused[x]) return ref(x);
+    return "";
+  }
+
+  bool try_fold(Fold& f, const std::vector<int>& sa, const std::vector<int>& sb, const std::map<int, std::vector<int>>& conn_of_step) {
+    const auto& N = tr.nodes;
+    const int L = (int)sa.size();
+    f.ca.assign(L, {}); f.cb.assign(L, {}); f.cat.assign(L, -1);
+    std::vector<std::array<int, 2>> ra(L, {-1, -1}), rb(L, {-1, -1});
+    auto conn_range = [&](int step, std::array<int, 2>& r) {
+      auto it = conn_of_step.find(step);
+      if (it == conn_of_step.end()) return true;
+      if (it->second.size() != 2 || !tr.conns[it->second[0]].begin || tr.conns[it->second[1]].begin) return false;
+      r = {tr.conns[it->second[0]].node, tr.conns[it->second[1]].node};
+      return true;
+    };
+    for (int k = 0; k < L; ++k) {
+      if (!conn_range(sa[k], ra[k]) || !conn_range(sb[k], rb[k]) || (ra[k][0] < 0) != (rb[k][0] < 0)) return false;
+      for (int i = ra[k][0]; i >= 0 && i < ra[k][1]; ++i) if (stmt_node(i)) { f.ca[k].push_back(i); f.connk[i] = k; }
+      for (int i = rb[k][0]; i >= 0 && i < rb[k][1]; ++i) if (stmt_node(i)) { f.cb[k].push_back(i); f.connk[i] = k; }
+    }
+    for (int i = f.a0; i < f.mid; ++i) if (stmt_node(i) && !f.connk.count(i)) f.la.push_back(i);
+    for (int i = f.mid; i < f.b1; ++i) if (stmt_node(i) && !f.connk.count(i)) f.lb.push_back(i);
+    if (f.la.size() != f.lb.size() || f.la.empty()) return false;
+    for (int k = 0; k < L; ++k) {
+      if (ra[k][0] < 0) continue;
+      const int na = (int)(std::lower_bound(f.la.begin(), f.la.end(), ra[k][0]) - f.la.begin());
+      const int nb = (int)(std::lower_bound(f.lb.begin(), f.lb.end(), rb[k][0]) - f.lb.begin());
+      if (na != nb) return false;
+      f.cat[k] = na;
+    }
+    f.amatched.insert(f.la.begin(), f.la.end());
+    // a contraction never crosses the boundary of A, B or the pair
+    for (const auto& e : fma_of) {
+      const int i = (int)e.first, p = e.second;
+      auto seg = [&](int x) { return x < f.a0 || x >= f.b1 ? 0 : (x < f.mid ? 1 : 2); };
+      if (seg(i) != seg(p) && seg(i) != 0) return false;         // (out of the pair: see the values handed on below)
+    }
+    for (size_t k = 0; k < f.la.size(); ++k) {
+      const int a = f.la[k], b = f.lb[k];
+      const SymNode& na = N[a];
+      const SymNode& nb = N[b];
+      f.b2a[b] = a;
+      if (na.op != nb.op || fused[a] != fused[b]) return false;
+      auto fa = fma_of.find(a), fb = fma_of.find(b);
+      if ((fa == fma_of.end()) != (fb == fma_of.end())) return false;
+      if (fa != fma_of.end()) {
+        auto m = f.b2a.find(fb->second);
+        if (m == f.b2a.end() || m->second != fa->second) return false;
+      }
+      std::array<std::string, 2>& txt = f.opa[a];
+      Bind b0, b1;
+      switch (na.op) {
+        case S_ADD: case S_MUL: case S_SUB: case S_DIV: {
+          bool ok = bind(f, na.a, nb.a, b0) && bind(f, na.b, nb.b, b1);
+          if (!ok && (na.op == S_ADD || na.op == S_MUL)) ok = bind(f, na.a, nb.b, b0) && bind(f, na.b, nb.a, b1);
+          if (!ok) return false;
+          if (b0.kind == 1 && b1.kind == 1 && b0.x == b1.x && b0.d != b1.d) return false;
+          commit(f, b0); commit(f, b1);
+          txt = {b0.txt, b1.txt};
+          break;
+        }
+        case S_NEG: case S_SIN: case S_SST: case S_STORE: case S_COS:
+          if (!bind(f, na.a, nb.a, b0)) return false;
+          commit(f, b0);
+          txt[0] = b0.txt;
+          if (na.op == S_COS) { auto m = f.b2a.find(nb.b); if (m == f.b2a.end() || m->second != na.b) return false; }
+          if (na.op == S_STORE && na.arr != nb.arr) return false;
+          if (na.op == S_SST || na.op == S_STORE) f.drow[a] = nb.row - na.row;
+          break;
+        case S_SLD: f.drow[a] = nb.row - na.row; break;
+        case S_SFENCE: break;
+        default: return false;
+      }
+    }
+    for (int k = 0; k < L; ++k) {
+      for (int x : f.ca[k]) for (int o : {N[x].a, N[x].b}) if (o >= 0 && N[x].op != S_COS && conn_ref(f, 0, o).empty()) return false;
+      for (int x : f.cb[k]) for (int o : {N[x].a, N[x].b}) if (o >= 0 && N[x].op != S_COS && conn_ref(f, 1, o).empty()) return false;
+    }
+    // values the loop hands on
+    std::set<int32_t> outs;
+    for (size_t i = f.b1; i < N.size(); ++i) {
+      if (!live[i]) continue;
+      for (int o : {N[i].a, N[i].b})
+        if (o >= f.a0 && o < f.b1 && stmt_node(o)) {
+          if (fused[o]) {          // a product contracted into a statement after the loop: its operands are handed on
+            for (int po : {N[o].a, N[o].b}) if (po >= f.a0 && po < f.b1 && stmt_node(po)) outs.insert(po);
+          } else {
+            outs.insert(o);
+          }
+        }
+    }
+    f.outs.assign(outs.begin(), outs.end());
+    return true;
+  }
+
+  void analyse_folds() {
+    const auto& N = tr.nodes;
+    fold_at.assign(N.size(), -1);
+    in_fold.assign(N.size(), -1);
+    remat.assign(N.size(), 0);
+    if (!hm || hm->pairs.empty() || tr.steps.empty()) return;
+    std::map<std::pair<int, int>, int> sidx;
+    for (size_t s = 0; s < tr.steps.size(); ++s) sidx[{tr.steps[s].pass, tr.steps[s].body}] = (int)s;
+    std::map<int, std::vector<int>> conn_of_step;
+    for (size_t c = 0; c < tr.conns.size(); ++c) conn_of_step[tr.conns[c].step].push_back((int)c);
+    for (int pass = 1; pass <= 3; ++pass)
+      for (const FoldPair& fp : hm->pairs) {
+        if (fp.l0 < 1) continue;
+        std::vector<int> sa, sb;
+        bool ok = true;
+        for (int k = 0; k < fp.len && ok; ++k) {
+          const int a = pass == 2 ? fp.l0 + 2 * fp.len - 1 - k : fp.l0 + k;
+          const int b = pass == 2 ? fp.l0 + fp.len - 1 - k : fp.l0 + fp.len + k;
+          auto ia = sidx.find({pass, a}), ib = sidx.find({pass, b});
+          ok = ia != sidx.end() && ib != sidx.end();
+          if (ok) { sa.push_back(ia->second); sb.push_back(ib->second); }
+        }
+        if (!ok || sb.back() + 1 >= (int)tr.steps.size()) continue;
+        Fold f;
+        f.pass = pass; f.len = fp.len; f.instA = pass == 2 ? 1 : 0;
+        f.first = pass == 2 ? fp.l0 + 2 * fp.len - 1 : fp.l0;
+        f.a0 = tr.steps[sa[0]].node; f.mid = tr.steps[sb[0]].node; f.b1 = tr.steps[sb.back() + 1].node;
+        if (!try_fold(f, sa, sb, conn_of_step)) continue;
+        fold_at[f.a0] = (int)folds.size();
+        for (int i = f.a0; i < f.b1; ++i) in_fold[i] = (int)folds.size();
+        folds.push_back(std::move(f));
+      }
+  }
+
+  std::string outer_operand(int x) {
+    const SymNode& n = tr.nodes[x];
+    if (n.op == S_LOAD && in_fold[x] >= 0 && !remat[x]) {     // a load inside a loop is simply issued again
+      remat[x] = 1;
+      ++stats.n_load;
+      out += "const rbd_v t" + std::to_string(x) + " = RBD_LDG(" + arr_name(n.arr) + ", " + std::to_string(n.row) + ");\n";
+    }
+    return ref(x);
+  }
+
+  void emit_fold(const Fold& f, int& since) {
+    const auto& N = tr.nodes;
+    auto rowx = [](int row, int d) { return d ? "(" + std::to_string(row) + " + rbd_it * " + std::to_string(d) + ")" : std::to_string(row); };
+    char hdr[160];
+    snprintf(hdr, sizeof hdr, "// ABA pass %d: bodies %d..%d and their mirror images run one copy of the code\n", f.pass,
+             std::min(f.first, f.first + (f.pass == 2 ? 1 - f.len : f.len - 1)), std::max(f.first, f.first + (f.pass == 2 ? 1 - f.len : f.len - 1)));
+    out += hdr;
+    for (int x : f.outs) out += "rbd_v t" + std::to_string(x) + ";\n";
+    out += "#pragma unroll 1\nfor (int rbd_it = 0; rbd_it < 2; ++rbd_it) {\n";
+    out += "const int rbd_s = rbd_it ^ " + std::to_string(f.instA) + "; (void)rbd_s;\n";
+    for (const auto& e : f.dload) {
+      const int x = e.first;
+      if (x >= f.a0 && x < f.mid && !f.connk.count(x)) continue;
+      ++stats.n_load;
+      out += "const rbd_v l" + std::to_string(x) + " = RBD_LDG(" + arr_name(N[x].arr) + ", " + rowx(N[x].row, e.second) + ");\n";
+    }
+    for (const auto& p : f.pv) {
+      if (p[2] >= 0) out += "rbd_v " + pvname(p[0], p[1]) + ";\n";
+      else out += "const rbd_v " + pvname(p[0], p[1]) + " = rbd_it ? " + conn_ref(f, 1, p[1]) + " : " + conn_ref(f, 0, p[0]) + ";\n";
+    }
+    const NameFn uname = [](int j) { return "u" + std::to_string(j); };
+    const NameFn cname = [](int j) { return "c" + std::to_string(j); };
+    const OpFn aop = [&](int j, int k) { return f.opa.at(j)[k]; };
+    const NameFn arow = [&](int j) { auto it = f.drow.find(j); return rowx(N[j].row, it == f.drow.end() ? 0 : it->second); };
+    const NameFn absrow = [&](int j) { return std::to_string(N[j].row); };
+    std::set<int32_t> outset(f.outs.begin(), f.outs.end());
+    auto branches = [&](size_t at) {
+      for (size_t k = 0; k < f.ca.size(); ++k) {
+        if (f.cat[k] != (int)at) continue;
+        bool any = !f.ca[k].empty() || !f.cb[k].empty();
+        for (const auto& p : f.pv) any = any || p[2] == (int)k;
+        if (!any) continue;
+        for (int side = 0; side < 2; ++side) {
+          out += side ? "} else {\n" : "if (rbd_it == 0) {\n";
+          const OpFn cop = [&, side](int j, int q) { return conn_ref(f, side, q ? N[j].b : N[j].a); };
+          for (int x : side ? f.cb[k] : f.ca[k]) {
+            if (!fused[x] && N[x].op != S_COS) out += stmt(x, cname, cop, absrow);
+            if (outset.count(x)) out += "t" + std::to_string(x) + " = c" + std::to_string(x) + ";\n";
+          }
+          for (const auto& p : f.pv)
+            if (p[2] == (int)k) out += pvname(p[0], p[1]) + " = " + conn_ref(f, side, p[side]) + ";\n";
+        }
+        out += "}\n";
+      }
+    };
+    size_t j = 0;
+    for (int i = f.a0; i < f.mid; ++i) {
+      if (N[i].op == S_LOAD && f.dload.count(i) && !f.connk.count(i)) {
+        ++stats.n_load;
+        out += "const rbd_v l" + std::to_string(i) + " = RBD_LDG(" + arr_name(N[i].arr) + ", " + rowx(N[i].row, f.dload.at(i)) + ");\n";
+        continue;
+      }
+      if (j < f.la.size() && f.la[j] == i) {
+        branches(j);
+        ++j;
+        if (fused[i] || N[i].op == S_COS) continue;
+        out += split_point(i, since);
+        out += stmt(i, uname, aop, arow);
+      }
+    }
+    branches(f.la.size());
+    std::string oa, ob;
+    for (int x : f.outs) {
+      if (f.connk.count(x)) continue;
+      if (x < f.mid) oa += "t" + std::to_string(x) + " = u" + std::to_string(x) + ";\n";
+      else ob += "t" + std::to_string(x) + " = u" + std::to_string(f.b2a.at(x)) + ";\n";
+    }
+    if (!oa.empty() || !ob.empty()) out += "if (rbd_it == 0) {\n" + oa + "} else {\n" + ob + "}\n";
+    out += "}\n";
+    ++stats.n_fold_loops;
+    stats.n_fold_bodies += f.len;
+  }
 
   void emit() {
     mark();
     plan_fma();
+    if (fold) analyse_folds();
+    else { fold_at.assign(tr.nodes.size(), -1); in_fold.assign(tr.nodes.size(), -1); remat.assign(tr.nodes.size(), 0); }
     const auto& N = tr.nodes;
-    char line[256];
     stats.nodes_traced = (int)N.size();
+    for (size_t i = 0; i < N.size(); ++i) if (live[i] && N[i].op != S_CONST && N[i].op != S_PARAM) ++stats.nodes_live;
+    const NameFn tname = [](int j) { return "t" + std::to_string(j); };
+    const OpFn top = [&](int j, int k) { return outer_operand(k ? N[j].b : N[j].a); };
+    const NameFn trow = [&](int j) { return std::to_string(N[j].row); };
     int since = 0;
     for (size_t i = 0; i < N.size(); ++i) {
+      if (fold_at[i] >= 0) {
+        const Fold& f = folds[fold_at[i]];
+        emit_fold(f, since);
+        i = f.b1 - 1;
+        continue;
+      }
       if (!live[i]) continue;
       const SymNode& n = N[i];
-      if (n.op != S_CONST) ++stats.nodes_live;
-      if (fused[i]) continue;
-      if (split_every > 0 && n.op != S_CONST && n.op != S_COS && ++since >= split_every && !(n.op == S_SLD && n.grp != (int)i)) {
-        out += "RBD_SPLIT();\n";
-        since = 0;
-      }
-      switch (n.op) {
-        case S_CONST: break;
-        case S_ADD:
-        case S_SUB: {
-          ++stats.n_add;
-          auto it = fma_of.find(i);
-          if (it == fma_of.end()) {
-            snprintf(line, sizeof line, "const rbd_v t%zu = %s(%s, %s);\n", i, n.op == S_ADD ? "RBD_ADD" : "RBD_SUB", ref(n.a).c_str(), ref(n.b).c_str());
-          } else {
-            const SymNode& p = N[it->second];
-            const int other = it->second == n.a ? n.b : n.a;
-            const char* f = n.op == S_ADD ? "RBD_FMA" : (it->second == n.a ? "RBD_FMS" /* x*y - c */ : "RBD_FNMA" /* c - x*y */);
-            snprintf(line, sizeof line, "const rbd_v t%zu = %s(%s, %s, %s);\n", i, f, ref(p.a).c_str(), ref(p.b).c_str(), ref(other).c_str());
-          }
-          out += line;
-          break;
-        }
-        case S_MUL: ++stats.n_mul; snprintf(line, sizeof line, "const rbd_v t%zu = RBD_MUL(%s, %s);\n", i, ref(n.a).c_str(), ref(n.b).c_str()); out += line; break;
-        case S_DIV:
-          ++stats.n_div;
-          if (tr.is_const(n.a, 1.0)) snprintf(line, sizeof line, "const rbd_v t%zu = RBD_RCP(%s);\n", i, ref(n.b).c_str());
-          else snprintf(line, sizeof line, "const rbd_v t%zu = RBD_DIV(%s, %s);\n", i, ref(n.a).c_str(), ref(n.b).c_str());
-          out += line;
-          break;
-        case S_NEG: ++stats.n_neg; snprintf(line, sizeof line, "const rbd_v t%zu = RBD_NEG(%s);\n", i, ref(n.a).c_str()); out += line; break;
-        case S_SIN:
-          ++stats.n_sincos;
-          snprintf(line, sizeof line, "rbd_v t%zu, t%zu; RBD_SINCOS(%s, t%zu, t%zu);\n", i, i + 1, ref(n.a).c_str(), i, i + 1);
-          out += line;
-          break;
-        case S_COS: break;
-        case S_LOAD:
-          ++stats.n_load;
-          if (n.arr == A_V) ++stats.n_load_v;
-          snprintf(line, sizeof line, "const rbd_v t%zu = RBD_LDG(%s, %d);\n", i, arr_name(n.arr), n.row);
-          out += line;
-          break;
-        case S_STORE:
-          ++stats.n_store;
-          if (key.peers && n.arr == A_OUT0 && flavor != FLAVOR_CPU) snprintf(line, sizeof line, "RBD_STG_PEERS(%d, %s);\n", n.row, ref(n.a).c_str());
-          else snprintf(line, sizeof line, "RBD_STG(%s, %d, %s);\n", arr_name(n.arr), n.row, ref(n.a).c_str());
-          out += line;
-          break;
-        case S_SLD: {
-          ++stats.n_sld;
-          snprintf(line, sizeof line, "const rbd_v t%zu = RBD_SLD(%d);\n", i, n.row);
-          out += line;
-          break;
-        }
-        case S_SST:
-          ++stats.n_sst;
-          snprintf(line, sizeof line, "RBD_SST(%d, %s);\n", n.row, ref(n.a).c_str());
-          out += line;
-          break;
-        case S_SFENCE: out += "RBD_SFENCE();\n"; break;
-        case S_XLD: snprintf(line, sizeof line, "const rbd_v t%zu = RBD_XLD(%d);\n", i, n.row); out += line; break;
-        case S_XST: snprintf(line, sizeof line, "RBD_XST(%d, %s);\n", n.row, ref(n.a).c_str()); out += line; break;
-      }
+      if (fused[i] || n.op == S_CONST || n.op == S_PARAM || n.op == S_COS) continue;
+      if (n.op == S_LOAD && in_fold[i] >= 0) continue;
+      out += split_point((int)i, since);
+      if (n.op == S_LOAD) remat[i] = 1;
+      out += stmt((int)i, tname, top, trow);
     }
+  }
+
+  // per-instance parameter table of the folded loops
+  std::string param_table() const {
+    if (folds.empty() || tr.npar == 0) return "";
+    std::vector<double> tab[2];
+    tab[0].assign(tr.npar, 0.0); tab[1].assign(tr.npar, 0.0);
+    for (const SymNode& n : tr.nodes) if (n.op == S_PARAM) tab[n.arr][n.row] = n.c;
+    std::string s = flavor == FLAVOR_CPU ? "static const rbd_v" : "__constant__ rbd_f";
+    s += " rbd_par_tab[2][" + std::to_string(tr.npar) + "] = {";
+    for (int k = 0; k < 2; ++k) {
+      s += k ? "}, {" : "{";
+      for (int j = 0; j < tr.npar; ++j) s += (j ? ", " : "") + lit(tab[k][j]);
+    }
+    s += "}};\n#undef RBD_PAR\n#define RBD_PAR(k_) rbd_par_tab[rbd_s][k_]\n";
+    return s;
   }
 };
 
 }  // namespace
 
 bool spec_emit_function(const HostModel& hm, const SpecKey& key, int flavor, const std::string& name, std::string& out,
-                        SpecStats* stats, std::string& err) {
+                        SpecStats* stats, std::string& err, bool fold) {
   SymTrace tr;
   int rows = 0;
   if (!run_trace(hm, key, tr, rows, err)) return false;
   Emitter em(tr, key, flavor);
+  em.hm = &hm;
+  em.fold = fold;
   if (flavor != FLAVOR_CPU) {
     // One basic block of 10^4 instructions lets ptxas stretch live ranges until it spills (Atlas: 128 registers + 350 B of
     // local memory, -10 % throughput); a never-taken branch every few hundred statements bounds its scheduling regions.
@@ -268,6 +602,7 @@ bool spec_emit_function(const HostModel& hm, const SpecKey& key, int flavor, con
   em.emit();
   em.stats.stash_rows = rows;
   if (stats) *stats = em.stats;
+  out += em.param_table();
   const char* F = key.f64 ? "double" : "float";
   std::string sig;
   if (flavor == FLAVOR_CPU) {
@@ -338,7 +673,7 @@ bool spec_emit_cuda_tu(const HostModel& hm, const SpecKey& key, std::string& out
 }
 
 bool spec_emit_cpu_tu(const HostModel& hm, const SpecKey& key, const std::string& name, std::string& out, SpecStats* stats,
-                      std::string& err) {
+                      std::string& err, bool fold) {
   out += "// generated by librbd_b200.so (rbd_codegen.cpp): model-specialised program, CPU flavour (test tier)\n"
          "#include \"rbd_device.cuh\"\n"
          "#define RBD_LDG(p, r) p[(long long)(r) * ld]\n#define RBD_STG(p, r, x) p[(long long)(r) * ld] = (x)\n"
@@ -349,7 +684,7 @@ bool spec_emit_cpu_tu(const HostModel& hm, const SpecKey& key, const std::string
          "#define RBD_NEG(a) (-(a))\n#define RBD_FMA(a, b, c) std::fma(a, b, c)\n#define RBD_FMS(a, b, c) std::fma(a, b, -(c))\n"
          "#define RBD_FNMA(a, b, c) std::fma(-(a), b, c)\n";
   out += std::string("typedef ") + (key.f64 ? "double" : "float") + " rbd_v;\n";
-  return spec_emit_function(hm, key, FLAVOR_CPU, name, out, stats, err);
+  return spec_emit_function(hm, key, FLAVOR_CPU, name, out, stats, err, fold);
 }
 
 }  // namespace rbd

@@ -26,14 +26,17 @@ struct SpecStats {
   int n_add = 0, n_mul = 0, n_div = 0, n_neg = 0, n_sincos = 0, n_load = 0, n_store = 0, n_sld = 0, n_sst = 0;
   int stash_rows = 0;
   int n_load_v = 0;      // global loads of the v array (0: the kernel shell does not prefetch it)
+  int n_fold_loops = 0;  // (pass, chain pair) steps emitted once as a two-iteration loop for both mirror-image chains
+  int n_fold_bodies = 0; // body steps whose code those loops share (summed over passes)
 };
 
 enum SpecFlavor : int { FLAVOR_CPU = 0, FLAVOR_SMEM = 1 };
 
 // Body of one per-sample function `name(...)` for the given flavour (see rbd_jit_prelude.cuh for the calling convention).
-// Returns false (with `err`) if the model / key cannot be specialised.
+// Returns false (with `err`) if the model / key cannot be specialised.  `fold` = false keeps mirror-image chains straight-line
+// (the reference form the folded program is tested against; not a user option).
 bool spec_emit_function(const HostModel& hm, const SpecKey& key, int flavor, const std::string& name, std::string& out,
-                        SpecStats* stats, std::string& err);
+                        SpecStats* stats, std::string& err, bool fold = true);
 
 // Whole NVRTC translation unit for `key`: defines + the per-sample function + the kernel shell of the prelude.
 bool spec_emit_cuda_tu(const HostModel& hm, const SpecKey& key, std::string& out, SpecStats* stats, std::string& err);
@@ -42,7 +45,7 @@ int spec_stash_rows(const HostModel& hm, const SpecKey& key);
 // Self-contained C++ translation unit (needs csrc/ on the include path) defining `extern "C" void name(q, v, in2, o0, o1, ld, sh)`
 // for ONE sample: column pointers with leading dimension ld, `sh` = stash_rows scalars of scratch.  Test tier only.
 bool spec_emit_cpu_tu(const HostModel& hm, const SpecKey& key, const std::string& name, std::string& out, SpecStats* stats,
-                      std::string& err);
+                      std::string& err, bool fold = true);
 
 // 64-bit content hash of a model + key + generator version (cubin cache key).
 uint64_t spec_hash(const HostModel& hm, const SpecKey& key);

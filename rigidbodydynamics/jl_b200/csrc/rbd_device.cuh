@@ -577,17 +577,27 @@ RBD_HD void art_to_parent_z(T s, T c, const T* r, const Art<T>& b, Art<T>& o) {
   }
 }
 
+// Hooks for the expression tracer (rbd_sym.h specialises them for its scalar type; for float / double they compile to nothing):
+// trace_step marks where the step of body `i` in ABA pass `pass` begins (i = -1: the pass is over), trace_conn brackets the
+// nodes that connect a body to its parent through the stash (the parent's v / (v, a), or the pending slot the articulated
+// inertia is handed over in) -- the code generator shares one program image between mirror-image limbs and keeps those
+// connections per instance.
+template <class T> RBD_HD void trace_step(int pass, int i) { (void)pass; (void)i; }
+template <class T> RBD_HD void trace_conn(bool begin) { (void)begin; }
+
 // Hand a finished child contribution (already in `carry`, written there by art_to_parent) to its parent: a first child's
 // stays in registers; any other child's goes to the parent's pending slot.  Writing every contribution into `carry` is safe
 // because a non-first child is followed (in reverse preorder) by the last body of a sibling subtree, a leaf, which does not
 // read `carry` -- and it saves a 27-register copy per body.
 template <class T, class ST>
 RBD_HD void hand_over(const ModelDev<T>& M, const BodyDev<T>& bd, const ST& st, const Art<T>& carry) {
+  trace_conn<T>(true);
   if (!(bd.flags & F_FIRST_CHILD)) {
     const int row = M.slot_base + bd.pslot * kSlotRowsAba;
     if (bd.flags & F_SLOT_INIT) art_store(st.slots(), row, carry);
     else art_accum(st.slots(), row, carry);
   }
+  trace_conn<T>(false);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -679,6 +689,7 @@ template <class T, bool EXT = false, int KINDS = kAllKinds> struct AbaIO {
 // Scalars of one 1-DoF body that come from global memory.  They are requested one body AHEAD of their use (software
 // pipelining in aba_sample) so the load latency overlaps the previous body's arithmetic instead of stalling the warp.
 template <class T> struct Pre { T q0, q1, qd, tau; T w[6]; T qoff; int32_t zflags; };
+
 template <class T, int PASS, class IO>
 RBD_HD void prefetch_body(const ModelDev<T>& M, int i, const IO& io, Pre<T>& p) {
   p.q0 = T(0); p.q1 = T(0); p.qd = T(0); p.tau = T(0);
@@ -719,6 +730,7 @@ RBD_HD void aba_pass1_body(const ModelDev<T>& M, int i, const IO& io, const ST& 
                            const Pre<T>& pre) {
   const BodyDev<T>& bd = M.body[i];
   Mot<T> vp;
+  trace_conn<T>(true);
   if (bd.flags & F_ROOT_CHILD) {
 #pragma unroll
     for (int k = 0; k < 3; ++k) { vp.w[k] = T(0); vp.l[k] = T(0); }
@@ -732,6 +744,7 @@ RBD_HD void aba_pass1_body(const ModelDev<T>& M, int i, const IO& io, const ST& 
 #pragma unroll
     for (int k = 0; k < 3; ++k) { vp.w[k] = t[k]; vp.l[k] = t[3 + k]; }
   }
+  trace_conn<T>(false);
   const int kind = bd.kind;
   T R[9], r[3];
   Mot<T> v;
@@ -1018,6 +1031,7 @@ RBD_HD void aba_pass2_multi(const ModelDev<T>& M, int i, const IO& io, const ST&
 template <class T, class ST>
 RBD_HD void load_parent_va(const ModelDev<T>& M, const BodyDev<T>& bd, const ST& st, const Mot<T>& vcur,
                            const Mot<T>& acur, Mot<T>& vp, Mot<T>& ap) {
+  trace_conn<T>(true);
   if (bd.flags & F_ROOT_CHILD) {
 #pragma unroll
     for (int k = 0; k < 3; ++k) { vp.w[k] = T(0); vp.l[k] = T(0); ap.w[k] = T(0); ap.l[k] = -M.g[k]; }
@@ -1032,6 +1046,7 @@ RBD_HD void load_parent_va(const ModelDev<T>& M, const BodyDev<T>& bd, const ST&
 #pragma unroll
     for (int k = 0; k < 3; ++k) { vp.w[k] = t[k]; vp.l[k] = t[3 + k]; ap.w[k] = t[6 + k]; ap.l[k] = t[9 + k]; }
   }
+  trace_conn<T>(false);
 }
 template <class T, class ST>
 RBD_HD void save_own_va(const ModelDev<T>& M, const BodyDev<T>& bd, const ST& st, const Mot<T>& v, const Mot<T>& a) {
@@ -1156,10 +1171,12 @@ RBD_HD void aba_sample(const ModelDev<T>& M, const IO& io, const ST& st) {
   aba_pass1_body<T, ST, true>(M, 0, io, st, vcur, cur);      // body 0 may be multi-DoF in any model: peeled
   cur = nxt;
   for (int i = 1; i < nb; ++i) {
+    trace_step<T>(1, i);
     prefetch_body<T, 1>(M, i + 1, io, nxt);
     aba_pass1_body<T, ST, GENERAL>(M, i, io, st, vcur, cur);
     cur = nxt;
   }
+  trace_step<T>(1, -1);
   // ---- pass 2 ----
   st.fence_st();
   Art<T> carry;
@@ -1172,6 +1189,7 @@ RBD_HD void aba_sample(const ModelDev<T>& M, const IO& io, const ST& st) {
   prefetch_body<T, 2>(M, nb - 1, io, cur);
   for (int i = nb - 1; i >= 1; --i) {
     const int kind = M.body[i].kind;
+    trace_step<T>(2, i);
     prefetch_body<T, 2>(M, i - 1, io, nxt);
     const Pre<T> now = cur;
     cur = nxt;
@@ -1185,6 +1203,7 @@ RBD_HD void aba_sample(const ModelDev<T>& M, const IO& io, const ST& st) {
       aba_pass2_multi<T, ST, 3, K_QFLOAT, false>(M, i, io, st, carry, vcur, acur);
     }
   }
+  trace_step<T>(2, -1);
   // body 0: inward step, then the outward pass starts here
   {
     const BodyDev<T>& b0 = M.body[0];
@@ -1210,6 +1229,7 @@ RBD_HD void aba_sample(const ModelDev<T>& M, const IO& io, const ST& st) {
   cur = nxt;
   for (int i = 1; i < nb; ++i) {
     const int kind = M.body[i].kind;
+    trace_step<T>(3, i);
     prefetch_body<T, 3>(M, i + 1, io, nxt);
     const Pre<T> now = cur;
     cur = nxt;
@@ -1223,6 +1243,7 @@ RBD_HD void aba_sample(const ModelDev<T>& M, const IO& io, const ST& st) {
       aba_pass3_multi<T, ST, 3, K_QFLOAT>(M, i, io, st, vcur, acur);
     }
   }
+  trace_step<T>(3, -1);
 }
 
 }  // namespace rbd

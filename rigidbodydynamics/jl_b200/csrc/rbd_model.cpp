@@ -143,9 +143,9 @@ int build_host_model(const rbd_model_desc* desc, HostModel& out, std::string& er
   std::vector<std::vector<int>> children(nb);
   std::vector<int> roots;
   for (int i = 0; i < nb; ++i) (desc->parent[i] < 0 ? roots : children[desc->parent[i]]).push_back(i);
-  // Ordering heuristic: sibling subtrees that are pure revolute chains of equal length (the legs / arms of a humanoid) are
-  // placed first and adjacent (L then R).  (It once fed a lock-step walk of such pairs, measured slower and removed; the order
-  // is kept because the slot colouring below and every measurement in DESIGN.md were made with it.)
+  // Sibling subtrees that are pure revolute chains of equal length (the legs / arms of a humanoid) are placed first and
+  // adjacent (L then R), so that each ABA pass walks the two chains back to back: the code generator runs both through one
+  // copy of the chain's code (HostModel::pairs, exported below once the flags are known).
   struct PairRec { int L, R, len; };
   std::vector<PairRec> pairs;
   {
@@ -335,6 +335,19 @@ int build_host_model(const rbd_model_desc* desc, HostModel& out, std::string& er
     if (k <= 1) row += (b.kind == K_FIXED) ? 6 : kRowsOneDof;
     else if (p == 0 && par < 0) row += 6;                 // root multi-DoF joint: only its velocity is stashed
     else row += 7 * k;                                    // U~ (6k) + u~ (k), also holds v (6) between passes 1 and 2
+  }
+  // mirror-image chains that run the same code: same joint kind and fast-class / leaf flags at every depth
+  for (const PairRec& pr : pairs) {
+    const int l0 = out.pos[pr.L], r0 = out.pos[pr.R];
+    if (r0 != l0 + pr.len) continue;
+    bool same = true;
+    for (int d = 0; d < pr.len && same; ++d) {
+      const BodyDev<double>& a = M.body[l0 + d];
+      const BodyDev<double>& b = M.body[r0 + d];
+      const int cls = F_ZPERP | F_ZPAR | F_ZERO_R | F_LEAF;
+      same = a.kind == b.kind && (a.flags & cls) == (b.flags & cls);
+    }
+    if (same) out.pairs.push_back({l0, pr.len});
   }
   // (a non-first child implies >= 2 children, so its parent always owns a slot)
   M.slot_base = row;

@@ -10,6 +10,12 @@
 
 namespace rbd {
 
+// Two sibling revolute chains of equal length (the left / right legs or arms of a humanoid), adjacent in preorder: positions
+// [l0, l0 + len) then [l0 + len, l0 + 2 len).  Listed only when the bodies at each depth have the same joint kind and the same
+// fast-class / leaf flags, so that both chains run the same code and differ in model constants only (rbd_codegen.cpp folds
+// their steps into one program image).
+struct FoldPair { int l0, len; };
+
 struct HostModel {
   int nb = 0, nq = 0, nv = 0;
   int64_t modcount = 0;
@@ -20,6 +26,7 @@ struct HostModel {
   std::vector<int> qstart, vstart;   // reference order
   std::vector<double> alignT;        // preorder position -> A^T (9), canonical body frame <- caller's body frame
   double total_mass = 0;
+  std::vector<FoldPair> pairs;
   ModelDev<double> dev64;    // ABA row layout (row0 / nrows); RNEA and CRBA derive theirs from slot indices
   ModelDev<float> dev32;
 };

@@ -15,11 +15,16 @@
 #pragma once
 #include <cmath>
 #include <cstdint>
+#include <cstring>
+#include <map>
+#include <set>
 #include <string>
+#include <tuple>
 #include <unordered_map>
 #include <vector>
 
 #include "rbd_device.cuh"
+#include "rbd_model.h"
 
 namespace rbd {
 
@@ -33,6 +38,7 @@ enum SymOp : int32_t {
   S_SST,                 // stash store: row, a = value
   S_SFENCE,              // stash store fence: where a thread re-reads its own stash writes (a no-op in shared memory)
   S_XLD, S_XST,          // per-thread global scratch (body-frame external wrenches): row[, a]
+  S_PARAM,               // model constant of one instance of a folded chain pair: row = slot, arr = instance (0 left, 1 right), c = value
 };
 
 // arrays a traced algorithm may touch (the code generator maps them to kernel arguments)
@@ -53,6 +59,23 @@ struct SymTrace {
   std::unordered_map<uint64_t, int32_t> last_load;          // (arr, row) -> most recent load node
   bool single = true;                                        // fold constants in fp32 (kernels for float) or fp64
   int load_window = 400;                                     // a repeated load this close to the previous one re-uses it
+  // trace_step / trace_conn marks (rbd_device.cuh): node index where each ABA body step begins, and the connection brackets
+  struct Step { int32_t pass, body, node; };
+  struct Conn { int32_t node, step; bool begin; };
+  std::vector<Step> steps;
+  std::vector<Conn> conns;
+  // steps (pass, body) that begin the walk of a folded chain: loads issued before one are not re-used after it, so that both
+  // chains of a pair start from their own loads (and re-use nothing computed before them)
+  std::set<std::pair<int32_t, int32_t>> fresh_steps;
+  int32_t load_floor = 0;
+  // Parameter leaves (S_PARAM).  A model constant that differs between the two instances of a folded pair is not a literal but
+  // an opaque leaf: never folded into or sign-normalised like a constant, one node per instance (so the two instances' code
+  // stays apart), one slot shared by both.  An expression of parameters and constants only is folded like a constant
+  // expression, per instance, into a derived parameter; its slot is keyed by the operation and the operand slots / constants,
+  // so mirror-image instances get the same slot.
+  int npar = 0;
+  std::map<std::tuple<int32_t, int64_t, uint64_t, int64_t, uint64_t>, int32_t> dslot;
+  std::map<std::pair<int32_t, int32_t>, int32_t> dnode;      // (slot, instance) -> derived parameter node
 
   int32_t push(const SymNode& n) { nodes.push_back(n); return (int32_t)nodes.size() - 1; }
   double rnd(double x) const { return single ? (double)(float)x : x; }
@@ -71,6 +94,36 @@ struct SymTrace {
     cse[h].push_back(id);
     return id;
   }
+  int32_t param(int32_t slot, int32_t inst, double v) { return push({S_PARAM, -1, -1, inst, slot, 0, rnd(v)}); }
+  bool is_par(int32_t id) const { return nodes[id].op == S_PARAM; }
+  bool is_lit(int32_t id) const { return is_const(id) || is_par(id); }
+  // both operands constants or parameters, at least one a parameter, not of different instances
+  bool par_fold(int32_t a, int32_t b) const {
+    if (!is_lit(a) || (b >= 0 && !is_lit(b))) return false;
+    if (!is_par(a) && !(b >= 0 && is_par(b))) return false;
+    return !(b >= 0 && is_par(a) && is_par(b) && nodes[a].arr != nodes[b].arr);
+  }
+  int32_t derive(int32_t op, int32_t a, int32_t b, double v) {
+    v = rnd(v);
+    if (v == 0.0) v = 0.0;
+    auto key = [&](int32_t x, int64_t& kind, uint64_t& bits) {
+      kind = x < 0 ? -1 : (is_par(x) ? nodes[x].row : -2);
+      bits = 0;
+      if (x >= 0 && !is_par(x)) std::memcpy(&bits, &nodes[x].c, 8);
+    };
+    int64_t ka, kb; uint64_t va, vb;
+    key(a, ka, va); key(b, kb, vb);
+    if ((op == S_ADD || op == S_MUL) && std::make_pair(ka, va) > std::make_pair(kb, vb)) { std::swap(ka, kb); std::swap(va, vb); }
+    auto it = dslot.emplace(std::make_tuple(op, ka, va, kb, vb), npar);
+    if (it.second) ++npar;
+    const int32_t slot = it.first->second;
+    const int32_t inst = is_par(a) ? nodes[a].arr : nodes[b].arr;
+    auto nd = dnode.find({slot, inst});
+    if (nd != dnode.end()) return nd->second;
+    const int32_t id = push({S_PARAM, -1, -1, inst, slot, 0, v});
+    dnode[{slot, inst}] = id;
+    return id;
+  }
   int32_t pure(int32_t op, int32_t a, int32_t b) {
     const uint64_t h = ((uint64_t)(uint32_t)op << 58) ^ ((uint64_t)(uint32_t)a * 0xD6E8FEB86659FD93ull) ^ ((uint64_t)(uint32_t)(b + 7) * 0xA24BAED4963EE407ull);
     for (int32_t id : cse[h]) if (nodes[id].op == op && nodes[id].a == a && nodes[id].b == b) return id;
@@ -80,6 +133,7 @@ struct SymTrace {
   }
   int32_t neg(int32_t a) {
     if (is_const(a)) return constant(-cval(a));
+    if (is_par(a)) return derive(S_NEG, a, -1, -cval(a));
     if (nodes[a].op == S_NEG) return nodes[a].a;
     if (nodes[a].op == S_SUB) return sub(nodes[a].b, nodes[a].a);
     return pure(S_NEG, a, -1);
@@ -88,6 +142,7 @@ struct SymTrace {
     if (is_const(a) && is_const(b)) return constant(cval(a) + cval(b));
     if (is_const(a, 0.0)) return b;
     if (is_const(b, 0.0)) return a;
+    if (par_fold(a, b)) return derive(S_ADD, a, b, cval(a) + cval(b));
     if (nodes[b].op == S_NEG) return sub(a, nodes[b].a);
     if (nodes[a].op == S_NEG) return sub(b, nodes[a].a);
     if (a > b) std::swap(a, b);
@@ -98,6 +153,7 @@ struct SymTrace {
     if (a == b) return constant(0.0);
     if (is_const(b, 0.0)) return a;
     if (is_const(a, 0.0)) return neg(b);
+    if (par_fold(a, b)) return derive(S_SUB, a, b, cval(a) - cval(b));
     if (nodes[b].op == S_NEG) return add(a, nodes[b].a);
     return pure(S_SUB, a, b);
   }
@@ -108,6 +164,7 @@ struct SymTrace {
     if (is_const(b, 1.0)) return a;
     if (is_const(a, -1.0)) return neg(b);
     if (is_const(b, -1.0)) return neg(a);
+    if (par_fold(a, b)) return derive(S_MUL, a, b, cval(a) * cval(b));
     // keep signs out of products so that x*y and (-x)*y share one node (negation is a free operand modifier on the GPU)
     bool negate = false;
     if (nodes[a].op == S_NEG) { a = nodes[a].a; negate = !negate; }
@@ -124,11 +181,14 @@ struct SymTrace {
     if (is_const(a) && is_const(b)) return constant(cval(a) / cval(b));
     if (is_const(a, 0.0)) return constant(0.0);
     if (is_const(b, 1.0)) return a;
+    if (par_fold(a, b)) return derive(S_DIV, a, b, cval(a) / cval(b));
     if (is_const(b)) return mul(a, constant(1.0 / cval(b)));   // only exact for powers of two; used for T(0.5)-style scalings
+    if (is_par(b)) return mul(a, derive(S_DIV, constant(1.0), b, 1.0 / cval(b)));   // the same, with the reciprocal a parameter
     return pure(S_DIV, a, b);
   }
   void sincos(int32_t a, int32_t& s, int32_t& c) {
     if (is_const(a)) { s = constant(std::sin(cval(a))); c = constant(std::cos(cval(a))); return; }
+    if (is_par(a)) { s = derive(S_SIN, a, -1, std::sin(cval(a))); c = derive(S_COS, a, -1, std::cos(cval(a))); return; }
     const uint64_t h = ((uint64_t)S_SIN << 58) ^ ((uint64_t)(uint32_t)a * 0xD6E8FEB86659FD93ull);
     for (int32_t id : cse[h]) if (nodes[id].op == S_SIN && nodes[id].a == a) { s = id; c = id + 1; return; }
     s = push({S_SIN, a, -1, 0, 0, 0, 0.0});
@@ -138,7 +198,7 @@ struct SymTrace {
   int32_t load(int32_t arr, int32_t row) {
     const uint64_t key = ((uint64_t)(uint32_t)arr << 32) | (uint32_t)row;
     auto it = last_load.find(key);
-    if (it != last_load.end() && (int32_t)nodes.size() - it->second <= load_window) return it->second;
+    if (it != last_load.end() && (int32_t)nodes.size() - it->second <= load_window && it->second >= load_floor) return it->second;
     const int32_t id = push({S_LOAD, -1, -1, arr, row, 0, 0.0});
     last_load[key] = id;
     return id;
@@ -164,6 +224,16 @@ struct Sym {
   Sym(Raw, int32_t i) : id(i) {}
 };
 inline Sym mk(int32_t id) { return Sym(Sym::Raw{}, id); }
+
+template <> inline void trace_step<Sym>(int pass, int i) {
+  SymTrace* t = sym_trace();
+  t->steps.push_back({pass, i, (int32_t)t->nodes.size()});
+  if (t->fresh_steps.count({pass, i})) t->load_floor = (int32_t)t->nodes.size();
+}
+template <> inline void trace_conn<Sym>(bool begin) {
+  SymTrace* t = sym_trace();
+  t->conns.push_back({(int32_t)t->nodes.size(), (int32_t)t->steps.size() - 1, begin});
+}
 inline Sym operator+(const Sym& a, const Sym& b) { return mk(sym_trace()->add(a.id, b.id)); }
 inline Sym operator-(const Sym& a, const Sym& b) { return mk(sym_trace()->sub(a.id, b.id)); }
 inline Sym operator*(const Sym& a, const Sym& b) { return mk(sym_trace()->mul(a.id, b.id)); }
@@ -227,8 +297,9 @@ struct SymStash {
   const SymStash& slots() const { return *this; }
 };
 
-// Model constants as literals of the trace.
-template <class F> inline void sym_model(const ModelDev<F>& S, ModelDev<Sym>& D) {
+// Model constants as literals of the trace; with `pairs`, the constants that differ between the two chains of a pair are
+// parameter leaves instead (see SymTrace::param).
+template <class F> inline void sym_model(const ModelDev<F>& S, ModelDev<Sym>& D, const std::vector<FoldPair>* pairs = nullptr) {
   D.nb = S.nb; D.nq = S.nq; D.nv = S.nv; D.nrows = S.nrows; D.slot_base = S.slot_base; D.nslots = S.nslots;
   for (int k = 0; k < 3; ++k) D.g[k] = Sym((double)S.g[k]);
   D.pad_ = Sym(0.0);
@@ -243,6 +314,26 @@ template <class F> inline void sym_model(const ModelDev<F>& S, ModelDev<Sym>& D)
     d.kind = s.kind; d.parent = s.parent; d.qrow = s.qrow; d.vrow = s.vrow; d.row0 = s.row0;
     d.oslot = s.oslot; d.pslot = s.pslot; d.flags = s.flags; d.refidx = s.refidx;
   }
+  if (!pairs) return;
+  SymTrace* t = sym_trace();
+  for (const FoldPair& fp : *pairs)
+    for (int k = 0; k < fp.len; ++k) {
+      const BodyDev<F>& sl = S.body[fp.l0 + k];
+      const BodyDev<F>& sr = S.body[fp.l0 + fp.len + k];
+      BodyDev<Sym>& dl = D.body[fp.l0 + k];
+      BodyDev<Sym>& dr = D.body[fp.l0 + fp.len + k];
+      auto split = [&](F a, F b, Sym& da, Sym& db) {
+        if (a == b) return;
+        const int32_t slot = t->npar++;
+        da = mk(t->param(slot, 0, (double)a));
+        db = mk(t->param(slot, 1, (double)b));
+      };
+      for (int j = 0; j < 9; ++j) split(sl.Rt[j], sr.Rt[j], dl.Rt[j], dr.Rt[j]);
+      for (int j = 0; j < 3; ++j) { split(sl.pt[j], sr.pt[j], dl.pt[j], dr.pt[j]); split(sl.h[j], sr.h[j], dl.h[j], dr.h[j]); }
+      for (int j = 0; j < 6; ++j) split(sl.J[j], sr.J[j], dl.J[j], dr.J[j]);
+      split(sl.m, sr.m, dl.m, dr.m);
+      split(sl.qoff, sr.qoff, dl.qoff, dr.qoff);
+    }
 }
 
 }  // namespace rbd
