@@ -293,6 +293,42 @@ int32_t rbd_dynamics_result(const rbd_model* model, int32_t dtype, int64_t B, in
 int32_t rbd_dynamics_derivatives(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                                  const void* tau, void* vd_out, void* dvd_dq_out, void* dvd_dv_out, void* stream);
 
+/* Reverse mode (SURVEY 8(f) rank 3, second half): vector-Jacobian products of dynamics! / inverse_dynamics! -- what a reference user
+ * gets from reverse-mode AD over those functions (ChainRules / ReverseDiff) -- in O(n) per sample, without forming any nv x nv
+ * Jacobian (csrc/rbd_adjoint.cuh has the derivation).  Per sample, ID = inverse_dynamics! (mechanism_algorithms.jl:542-553):
+ *
+ * rbd_dynamics_vjp: the product  ν̄^T d v̇ / d(q, v, tau, wext)  of dynamics!(result, state, tau, wext) (:845-864).
+ *   inputs   q [nq x B], v [nv x B], tau [nv x B] or NULL (zero), wext [6*nb x B] or NULL (root-frame wrenches as in rbd_dynamics),
+ *            vd [nv x B] = v̇, which MUST be rbd_dynamics' result for the same q, v, tau, wext (the products are evaluated at this
+ *            v̇; it is not recomputed -- tau enters only through it), vd_bar [nv x B] = ν̄
+ *   outputs  tau_bar   [nv x B]    μ = M^-1 ν̄
+ *            v_bar     [nv x B]    -(d ID / d v)^T μ
+ *            q_bar_tan [nv x B]    -(d ID / d q)^T μ along q̇ = velocity_to_configuration_derivative(e_j): row j is
+ *                                  sum_i ν̄_i dvd_dq[i + j*nv] of rbd_dynamics_derivatives
+ *            q_bar_cfg [nq x B]    the same covector in configuration coordinates, mapped as configuration_derivative_to_velocity_adjoint!
+ *                                  does (mechanism_state.jl:912-918, joint_types/*.jl): q_bar_cfg . (N(q) u) = q_bar_tan . u for every u
+ *                                  (N: q̇ = N(q) v), also at non-unit quaternions; equal to q_bar_tan for revolute / prismatic joints.
+ *                                  It has no component along the radial direction of a quaternion: that derivative depends on how the
+ *                                  rotation formula is extended off the unit sphere, which no gradient should depend on.
+ *            wext_bar  [6*nb x B]  ν̄^T d v̇ / d wext = -(d ID / d wext)^T μ: rows 6 i .. 6 i + 5 = the ROOT-frame twist [angular; linear]
+ *                                  of the successor of tree joint i under the joint velocities μ (a motion vector: its pairing with a
+ *                                  wrench perturbation [torque; force] gives the change of ν̄ . v̇)
+ * rbd_inverse_dynamics_vjp: the product  τ̄^T d ID / d(q, v, v̇, wext)  of inverse_dynamics!.
+ *   inputs   q, v, vd = v̇ [nv x B], wext or NULL, tau_bar [nv x B] = τ̄
+ *   outputs  q_bar_tan [nv x B] (d ID / d q)^T τ̄ (tangent coordinates as above), q_bar_cfg [nq x B] (mapped as above),
+ *            v_bar [nv x B] (d ID / d v)^T τ̄, vd_bar [nv x B] = M τ̄, wext_bar [6*nb x B] = (d ID / d wext)^T τ̄ = MINUS the root-frame
+ *            twist of each body under the joint velocities τ̄ (external wrenches are subtracted in newton_euler!, :428-439)
+ * Every output may be NULL (not computed, nothing written).  q, v, vd and the adjoint input must not be NULL (RBD_EINVAL).  fp32 /
+ * fp64 (RBD_DUAL64X6 -> RBD_EUNSUPPORTED); the model limits of rbd_dynamics_derivatives apply; B == 0 or nv == 0: nothing to do. */
+int32_t rbd_dynamics_vjp(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld,
+                         const void* q, const void* v, const void* tau, const void* wext, const void* vd,
+                         const void* vd_bar,
+                         void* q_bar_tan, void* q_bar_cfg, void* v_bar, void* tau_bar, void* wext_bar, void* stream);
+int32_t rbd_inverse_dynamics_vjp(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld,
+                                 const void* q, const void* v, const void* vd, const void* wext,
+                                 const void* tau_bar,
+                                 void* q_bar_tan, void* q_bar_cfg, void* v_bar, void* vd_bar, void* wext_bar, void* stream);
+
 /* The triangular solves of rbd_dynamics_derivatives also exist as a model-specialised kernel (every index a constant, right-hand
  * sides in registers; generated and NVRTC-compiled like the kernels of rbd_model_precompile, same cubin cache).  It is used when
  * its cubin is cached or the batch is at least RBD_JIT_MIN_BATCH (default 4096 for this entry point); RBD_DERIV_JIT=0 / RBD_JIT=0

@@ -28,4 +28,6 @@ from .contact import (ContactDesc, ContactPoint, HalfSpace3D, HuntCrossleyModel,
 from .loops import (LoopDesc, PDGains, SE3PDGains, constraint_wrench_subspace, default_constraint_stabilization_gains,  # noqa: F401
                     dynamics_loops_, loop_desc, num_constraints)
 from .mechanism import maximal_coordinates  # noqa: F401
+from . import autodiff  # noqa: F401  (rbd.autodiff.dynamics / inverse_dynamics: differentiable, kept out of this namespace)
+from .autodiff import dynamics_vjp_, inverse_dynamics_vjp_  # noqa: F401
 from ._cabi import RbdError, launch_info, load_library  # noqa: F401

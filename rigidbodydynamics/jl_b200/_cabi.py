@@ -116,6 +116,8 @@ SYMBOLS = {
     "rbd_dynamics_result": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rbd_dynamics_derivatives": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rbd_model_precompile_derivatives": (c_int32, [_vp, _i32]),
+    "rbd_dynamics_vjp": (c_int32, [_vp, _i32, _i64, _i64] + [_vp] * 12),
+    "rbd_inverse_dynamics_vjp": (c_int32, [_vp, _i32, _i64, _i64] + [_vp] * 11),
     "rbd_dynamics_bias": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp]),
     "rbd_mass_matrix": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp]),
     "rbd_mass_matrix_uplo": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _i32, _vp]),
