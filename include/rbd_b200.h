@@ -373,6 +373,31 @@ int32_t rbd_integrate(const rbd_model* model, int32_t dtype, int64_t B, int64_t 
 int32_t rbd_integrate_schedule(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, const void* tau,
                                int64_t tau_step_stride, int64_t tau_stage_stride, double dt, int32_t nsteps, void* stream);
 
+/* rbd_integrate_schedule that also RECORDS the trajectory: q_traj [(nsteps+1) x nq x B] and v_traj [(nsteps+1) x nv x B] (leading
+ * dimension B inside a block) receive the initial state in block 0 and the state after step s in block s.  q / v are advanced in
+ * place exactly as by rbd_integrate_schedule (bit for bit, also every recorded block).  q_traj / v_traj must not be NULL. */
+int32_t rbd_integrate_trajectory(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, const void* tau,
+                                 int64_t tau_step_stride, int64_t tau_stage_stride, double dt, int32_t nsteps,
+                                 void* q_traj, void* v_traj, void* stream);
+
+/* Reverse mode through a rollout (DESIGN 4.13): the gradient of  L = sum_s q_traj_bar[s] . q_traj[s] + v_traj_bar[s] . v_traj[s]
+ * with respect to the initial state and the torques, for the trajectory rbd_integrate_trajectory recorded with the same tau,
+ * strides, dt and nsteps.  Every array has leading dimension B; tau / tau_bar are the blocks of rbd_integrate_schedule.
+ *   inputs   q_traj, v_traj (the recorded trajectory), tau or NULL (zero torques), q_traj_bar [(nsteps+1) x nq x B] and
+ *            v_traj_bar [(nsteps+1) x nv x B] or NULL (zero)
+ *   outputs  q0_bar_tan [nv x B] (tangent coordinates, the convention of rbd_dynamics_vjp), q0_bar_cfg [nq x B] (the minimal-norm
+ *            configuration covector of rbd_dynamics_vjp), v0_bar [nv x B], and tau_bar (layout of tau; needs tau), which is ADDED TO:
+ *            each (step, stage) adds its gradient to its block, so a block held over several stages or steps receives the sum of
+ *            theirs, and a rollout split into consecutive calls (checkpointing) accumulates exactly like one call.  Each may be NULL.
+ * Per step the four stages are recomputed from the recorded state, so memory is O((nq + nv) B) beyond the trajectory.  fp32 / fp64
+ * only (RBD_EUNSUPPORTED); negative strides, nsteps < 0, dt <= 0, tau_bar without tau or NULL q_traj / v_traj: RBD_EINVAL.
+ * B == 0: nothing to do; nsteps == 0: q0_bar_* from q_traj_bar[0], v0_bar = v_traj_bar[0].  Mechanisms with
+ * loops are not supported (the Python layer refuses them with RBD_ELOOP). */
+int32_t rbd_integrate_vjp(const rbd_model* model, int32_t dtype, int64_t B, const void* q_traj, const void* v_traj,
+                          const void* tau, int64_t tau_step_stride, int64_t tau_stage_stride, double dt, int32_t nsteps,
+                          const void* q_traj_bar, const void* v_traj_bar,
+                          void* q0_bar_tan, void* q0_bar_cfg, void* v0_bar, void* tau_bar, void* stream);
+
 /* Next row of the scope table (SURVEY 8(f) rank 2): kinematics by-products of the same outward sweep, all expressed in the
  * mechanism's root frame, 6-vectors as [angular; linear].  Every output pointer may be NULL (not computed).
  *   transforms_to_root  [12*nb x B]  rows 12 i .. 12 i + 11 = transform_to_root(state, successor of tree joint i):

@@ -18,7 +18,8 @@ from .urdf import (default_urdf_joint_types, load_description, load_model, mecha
 from .state import (DynamicsResult, MechanismState, rand_, rand_configuration_, rand_velocity_, zero_,  # noqa: F401
                     zero_configuration_, zero_velocity_)
 from .algorithms import (DimensionMismatch, dynamics_, dynamics_derivatives_, dynamics_dual_, dynamics_bias, dynamics_bias_, dynamics_ode_,  # noqa: F401
-                         inverse_dynamics, inverse_dynamics_, mass_matrix, mass_matrix_, simulate_)
+                         inverse_dynamics, inverse_dynamics_, mass_matrix, mass_matrix_, simulate_,
+                         simulate_trajectory_)
 from .kinematics import (TreePath, center_of_mass, geometric_jacobian, geometric_jacobian_,  # noqa: F401
                          gravitational_potential_energy, kinematics_, kinetic_energy, momentum, momentum_matrix,
                          momentum_matrix_, momentum_rate_bias, path, transforms_to_root, transforms_to_root_)
@@ -29,5 +30,5 @@ from .loops import (LoopDesc, PDGains, SE3PDGains, constraint_wrench_subspace, d
                     dynamics_loops_, loop_desc, num_constraints)
 from .mechanism import maximal_coordinates  # noqa: F401
 from . import autodiff  # noqa: F401  (rbd.autodiff.dynamics / inverse_dynamics: differentiable, kept out of this namespace)
-from .autodiff import dynamics_vjp_, inverse_dynamics_vjp_  # noqa: F401
+from .autodiff import dynamics_vjp_, integrate_vjp_, inverse_dynamics_vjp_  # noqa: F401
 from ._cabi import RbdError, launch_info, load_library  # noqa: F401

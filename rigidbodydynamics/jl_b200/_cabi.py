@@ -123,6 +123,8 @@ SYMBOLS = {
     "rbd_mass_matrix_uplo": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _i32, _vp]),
     "rbd_integrate": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, c_double, _i32, _vp]),
     "rbd_integrate_schedule": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _i64, _i64, c_double, _i32, _vp]),
+    "rbd_integrate_trajectory": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _i64, _i64, c_double, _i32, _vp, _vp, _vp]),
+    "rbd_integrate_vjp": (c_int32, [_vp, _i32, _i64, _vp, _vp, _vp, _i64, _i64, c_double, _i32] + [_vp] * 7),
     "rbd_kinematics": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, POINTER(RbdKinematicsOut), _vp]),
     "rbd_dynamics_host": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rbd_inverse_dynamics_host": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp]),

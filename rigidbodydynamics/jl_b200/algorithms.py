@@ -18,7 +18,7 @@ import torch
 from . import _cabi
 from .state import DynamicsResult, MechanismState, _DT
 
-__all__ = ["dynamics_", "dynamics_dual_", "dynamics_derivatives_", "dynamics_ode_", "simulate_", "inverse_dynamics_", "inverse_dynamics", "mass_matrix_", "mass_matrix",
+__all__ = ["dynamics_", "dynamics_dual_", "dynamics_derivatives_", "dynamics_ode_", "simulate_", "simulate_trajectory_", "inverse_dynamics_", "inverse_dynamics", "mass_matrix_", "mass_matrix",
            "dynamics_bias_", "dynamics_bias", "DimensionMismatch"]
 
 
@@ -156,6 +156,40 @@ def dynamics_ode_(xdot: torch.Tensor, result: DynamicsResult, state: MechanismSt
     return xdot
 
 
+def _torque_schedule(state: MechanismState, torques: torch.Tensor, nsteps: int):
+    """Element strides (step, stage) of an open-loop torque schedule: [nsteps, nv, B] (zero-order hold over each step) or
+    [nsteps, 4, nv, B] (one block per RK4 stage, the batched form of control!(torques, t, state) evaluated at t, t + dt/2, t + dt/2,
+    t + dt)."""
+    if torques.shape[0] < nsteps or torques.shape[-2:] != (state.nv, state.batch) or (torques.dim() == 4 and torques.shape[1] != 4):
+        raise DimensionMismatch("torque schedule must be [nsteps, nv, B] or [nsteps, 4, nv, B]")
+    if torques.dtype != state.dtype or torques.device != state.q.device or not torques.is_contiguous():
+        raise TypeError("torque schedule: dtype / device must match the state, and it must be contiguous")
+    blk = state.nv * state.batch
+    return (4 * blk, blk) if torques.dim() == 4 else (blk, 0)
+
+
+def simulate_trajectory_(state: MechanismState, nsteps: int, torques: Optional[torch.Tensor] = None, dt: float = 1e-4):
+    """``nsteps`` Munthe-Kaas RK4 steps like ``simulate_``, recording the trajectory: returns ``(q_traj, v_traj)``,
+    [nsteps + 1, nq, B] and [nsteps + 1, nv, B], block 0 the initial state and block s the state after step s.  ``state`` is advanced
+    in place exactly as ``simulate_`` advances it.  ``torques``: None, constant [nv, B], per step [nsteps, nv, B] or per stage
+    [nsteps, 4, nv, B].  The recorded trajectory is what ``autodiff.integrate_vjp_`` differentiates."""
+    _require_tree(state, "simulate_trajectory_")
+    state.check_modcount()
+    if nsteps < 0:
+        raise ValueError("nsteps must be >= 0")
+    lib = _cabi.load_library()
+    step = stage = 0
+    if torques is not None and torques.dim() in (3, 4):
+        step, stage = _torque_schedule(state, torques, nsteps)
+    else:
+        _check(torques, state.nv, state, "torques")
+    q_traj = torch.empty((nsteps + 1, state.nq, state.batch), dtype=state.dtype, device=state.q.device)
+    v_traj = torch.empty((nsteps + 1, state.nv, state.batch), dtype=state.dtype, device=state.q.device)
+    _call(lib.rbd_integrate_trajectory(state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q), _ptr(state.v),
+                                       _ptr(torques), step, stage, float(dt), nsteps, _ptr(q_traj), _ptr(v_traj), _stream()))
+    return q_traj, v_traj
+
+
 def simulate_(state: MechanismState, final_time: float, torques: Optional[torch.Tensor] = None, dt: float = 1e-4) -> int:
     """``simulate(state0, final_time, control!; Δt)`` (src/simulate.jl:36-55) for the whole batch, on the GPU: Munthe-Kaas RK4
     steps (src/ode_integrators.jl:233-300) until ``t >= final_time``; ``state.q`` / ``state.v`` are advanced in place.  The
@@ -169,14 +203,7 @@ def simulate_(state: MechanismState, final_time: float, torques: Optional[torch.
         t += dt
         nsteps += 1
     if torques is not None and torques.dim() in (3, 4):
-        # open-loop schedule: [nsteps, nv, B] (zero-order hold over each step) or [nsteps, 4, nv, B] (one block per RK4 stage, the
-        # batched form of control!(torques, t, state) evaluated at t, t + dt/2, t + dt/2, t + dt)
-        if torques.shape[0] < nsteps or torques.shape[-2:] != (state.nv, state.batch) or (torques.dim() == 4 and torques.shape[1] != 4):
-            raise DimensionMismatch("torque schedule must be [nsteps, nv, B] or [nsteps, 4, nv, B]")
-        if torques.dtype != state.dtype or torques.device != state.q.device or not torques.is_contiguous():
-            raise TypeError("torque schedule: dtype / device must match the state, and it must be contiguous")
-        blk = state.nv * state.batch
-        step, stage = (4 * blk, blk) if torques.dim() == 4 else (blk, 0)
+        step, stage = _torque_schedule(state, torques, nsteps)
         _call(lib.rbd_integrate_schedule(state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q), _ptr(state.v),
                                          _ptr(torques), step, stage, float(dt), nsteps, _stream()))
         return nsteps

@@ -2,8 +2,10 @@
 
     dynamics_vjp_          ν̄ᵀ ∂v̇/∂(q, v, τ, w_ext)        rbd_dynamics_vjp          (include/rbd_b200.h, csrc/rbd_adjoint.cuh)
     inverse_dynamics_vjp_  τ̄ᵀ ∂τ/∂(q, v, v̇, w_ext)         rbd_inverse_dynamics_vjp
+    integrate_vjp_         gradient of a recorded rollout       rbd_integrate_vjp         (csrc/rbd_integrate_adjoint.cuh)
     dynamics(mechanism, q, v, tau=None, externalwrenches=None)         differentiable v̇ = dynamics!(...)
     inverse_dynamics(mechanism, q, v, vd, externalwrenches=None)       differentiable τ = inverse_dynamics!(...)
+    simulate(mechanism, q0, v0, torques=None, *, dt, nsteps, ...)     differentiable RK4 rollout (simulate)
 
 One product costs one Articulated-Body solve (forward dynamics only) plus one outward and one inward sweep: O(n) per sample, no
 nv x nv Jacobian is formed (``dynamics_derivatives_`` builds both full Jacobians instead).  Every tensor is ``[rows, B]``, contiguous,
@@ -28,7 +30,7 @@ from .algorithms import DimensionMismatch, _check, _ptr, _require_tree
 from .mechanism import Mechanism
 from .state import _DT, MechanismState, _model_handle
 
-__all__ = ["dynamics_vjp_", "inverse_dynamics_vjp_", "dynamics", "inverse_dynamics"]
+__all__ = ["dynamics_vjp_", "inverse_dynamics_vjp_", "integrate_vjp_", "dynamics", "inverse_dynamics", "simulate"]
 
 
 def _stream(t: torch.Tensor):
@@ -186,3 +188,140 @@ def inverse_dynamics(mechanism: Mechanism, q: torch.Tensor, v: torch.Tensor, vd:
     """Differentiable ``τ = inverse_dynamics!(τ, state, v̇, externalwrenches)``; backward runs ``rbd_inverse_dynamics_vjp``.  Not
     twice differentiable."""
     return _InverseDynamics.apply(mechanism, q, v, vd, externalwrenches)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# rollouts: rbd_integrate_trajectory / rbd_integrate_vjp
+# ----------------------------------------------------------------------------------------------------------------------
+def _rollout_inputs(mechanism: Mechanism, what: str, q: torch.Tensor, v: torch.Tensor, tau: Optional[torch.Tensor], nsteps: int):
+    """Checks of a rollout: (model handle, B, step stride, stage stride) for q [nq, B], v [nv, B] and torques None / [nv, B] /
+    [nsteps, nv, B] / [nsteps, 4, nv, B]."""
+    h, B = _inputs(mechanism, what, q=q, v=v)
+    nv = h.info.nv
+    if nsteps < 0:
+        raise ValueError(f"{what}: nsteps must be >= 0")
+    if tau is None:
+        return h, B, 0, 0
+    if tau.dtype != q.dtype or tau.device != q.device or not tau.is_contiguous():
+        raise TypeError(f"{what}: torques must be contiguous, with the dtype and device of q")
+    blk = nv * B
+    if tau.dim() == 2 and tuple(tau.shape) == (nv, B):
+        return h, B, 0, 0
+    if tau.dim() == 3 and tuple(tau.shape) == (nsteps, nv, B):
+        return h, B, blk, 0
+    if tau.dim() == 4 and tuple(tau.shape) == (nsteps, 4, nv, B):
+        return h, B, 4 * blk, blk
+    raise DimensionMismatch(f"{what}: torques must be [nv, B], [nsteps, nv, B] or [nsteps, 4, nv, B], got {tuple(tau.shape)}")
+
+
+def integrate_vjp_(mechanism: Mechanism, q_traj: torch.Tensor, v_traj: torch.Tensor, torques: Optional[torch.Tensor] = None, *,
+                   dt: float, q_traj_bar: Optional[torch.Tensor] = None, v_traj_bar: Optional[torch.Tensor] = None,
+                   q0_bar_tan: Optional[torch.Tensor] = None, q0_bar_cfg: Optional[torch.Tensor] = None,
+                   v0_bar: Optional[torch.Tensor] = None, tau_bar: Optional[torch.Tensor] = None):
+    """Gradient of ``L = sum_s q_traj_bar[s] . q_traj[s] + v_traj_bar[s] . v_traj[s]`` over a trajectory recorded by
+    ``simulate_trajectory_`` ([nsteps + 1, nq, B] / [nsteps + 1, nv, B]) with the same ``torques`` and ``dt``.  Outputs (each
+    optional, filled in place): ``q0_bar_tan`` [nv, B], ``q0_bar_cfg`` [nq, B] (the coordinates of ``dynamics_vjp_``), ``v0_bar``
+    [nv, B] and ``tau_bar`` (shape of ``torques``), to which the torque gradient is ADDED."""
+    nsteps = q_traj.shape[0] - 1
+    h, B, step, stage = _rollout_inputs(mechanism, "integrate_vjp_", q_traj[0], v_traj[0], torques, nsteps)
+    nq, nv = h.info.nq, h.info.nv
+    for t, shape, name in ((q_traj, (nsteps + 1, nq, B), "q_traj"), (v_traj, (nsteps + 1, nv, B), "v_traj"),
+                           (q_traj_bar, (nsteps + 1, nq, B), "q_traj_bar"), (v_traj_bar, (nsteps + 1, nv, B), "v_traj_bar"),
+                           (q0_bar_tan, (nv, B), "q0_bar_tan"), (q0_bar_cfg, (nq, B), "q0_bar_cfg"), (v0_bar, (nv, B), "v0_bar"),
+                           (tau_bar, None if torques is None else tuple(torques.shape), "tau_bar")):
+        if t is None:
+            continue
+        if t.dtype != q_traj.dtype or t.device != q_traj.device or not t.is_contiguous():
+            raise TypeError(f"integrate_vjp_: {name} must be contiguous, with the dtype and device of q_traj")
+        if shape is None or tuple(t.shape) != shape:
+            raise DimensionMismatch(f"integrate_vjp_: {name} has wrong size: expected {shape}, got {tuple(t.shape)}")
+    _cabi.check(_cabi.load_library().rbd_integrate_vjp(h.ptr, _DT[q_traj.dtype], B, _ptr(q_traj), _ptr(v_traj), _ptr(torques), step,
+                                                       stage, float(dt), nsteps, _ptr(q_traj_bar), _ptr(v_traj_bar), _ptr(q0_bar_tan),
+                                                       _ptr(q0_bar_cfg), _ptr(v0_bar), _ptr(tau_bar), _stream(q_traj)))
+
+
+def _trajectory(h, q0, v0, tau, s0, m, step, stage, dt):
+    """rbd_integrate_trajectory over steps s0 .. s0 + m from (q0, v0) (not modified): [m + 1, rows, B] blocks."""
+    B = q0.shape[1]
+    q, v = q0.clone(), v0.clone()
+    qt = torch.empty((m + 1,) + tuple(q0.shape), dtype=q0.dtype, device=q0.device)
+    vt = torch.empty((m + 1,) + tuple(v0.shape), dtype=v0.dtype, device=v0.device)
+    t = None if tau is None else (tau if tau.dim() == 2 else tau[s0:])
+    _cabi.check(_cabi.load_library().rbd_integrate_trajectory(h.ptr, _DT[q0.dtype], B, B, _ptr(q), _ptr(v), _ptr(t), step, stage,
+                                                              float(dt), m, _ptr(qt), _ptr(vt), _stream(q0)))
+    return qt, vt
+
+
+class _Simulate(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, mechanism, q0, v0, tau, dt, nsteps, trajectory, every):
+        h, B, step, stage = _rollout_inputs(mechanism, "autodiff.simulate", q0, v0, tau, nsteps)
+        ctx.handle, ctx.dt, ctx.nsteps, ctx.trajectory, ctx.step, ctx.stage = h, dt, nsteps, trajectory, step, stage
+        if trajectory or B == 0:
+            qt, vt = _trajectory(h, q0, v0, tau, 0, nsteps, step, stage, dt)
+            ctx.every = nsteps
+            ctx.save_for_backward(tau, qt, vt)
+            return (qt, vt) if trajectory else (qt[-1].clone(), vt[-1].clone())
+        # checkpoints every `every` steps; backward re-records each segment before its VJP
+        every = max(1, min(every or nsteps, nsteps)) if nsteps else 1
+        ctx.every = every
+        q, v = q0, v0
+        qs, vs = [q0], [v0]
+        for s0 in range(0, nsteps, every):
+            qt, vt = _trajectory(h, q, v, tau, s0, min(every, nsteps - s0), step, stage, dt)
+            q, v = qt[-1].clone(), vt[-1].clone()
+            qs.append(q); vs.append(v)
+        ctx.save_for_backward(tau, torch.stack(qs[:-1]), torch.stack(vs[:-1]))
+        return q, v
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gq, gv):
+        tau, qck, vck = ctx.saved_tensors
+        h, dt, n = ctx.handle, ctx.dt, ctx.nsteps
+        need = ctx.needs_input_grad
+        q0, v0 = qck[0], vck[0]
+        qc, vb = _out(need[1], q0, q0.shape[0]), torch.empty_like(v0)
+        tb = torch.zeros_like(tau) if (need[3] and tau is not None) else None
+        if q0.shape[1] == 0 or not (need[1] or need[2] or tb is not None):
+            return None, qc, (vb if need[2] else None), tb, None, None, None, None
+        if ctx.trajectory:
+            _vjp_call(h, qck, vck, tau, ctx.step, ctx.stage, dt, n, gq.contiguous(), gv.contiguous(), qc, vb, tb)
+            return None, qc, (vb if need[2] else None), tb, None, None, None, None
+        # segments last to first; the adjoint of a segment's end state is its successor's q0_bar_cfg / v0_bar
+        k = ctx.every
+        qa, va = gq.contiguous(), gv.contiguous()
+        starts = list(range(0, n, k)) if n else []
+        if not starts:
+            qc_ = torch.empty_like(q0)
+            _vjp_call(h, qck, vck, tau, ctx.step, ctx.stage, dt, 0, qa[None], va[None], qc_, vb, tb)
+            return None, (qc_ if need[1] else None), (vb if need[2] else None), tb, None, None, None, None
+        for j in reversed(range(len(starts))):
+            s0 = starts[j]
+            m = min(k, n - s0)
+            qt, vt = _trajectory(h, qck[j], vck[j], tau, s0, m, ctx.step, ctx.stage, dt)
+            qtb = torch.zeros_like(qt); vtb = torch.zeros_like(vt)
+            qtb[-1] = qa; vtb[-1] = va
+            t = None if tau is None else (tau if tau.dim() == 2 else tau[s0:])
+            tbs = None if tb is None else (tb if tb.dim() == 2 else tb[s0:])
+            qa, va = torch.empty_like(q0), torch.empty_like(v0)
+            _vjp_call(h, qt, vt, t, ctx.step, ctx.stage, dt, m, qtb, vtb, qa, va, tbs)
+        return None, (qa if need[1] else None), (va if need[2] else None), tb, None, None, None, None
+
+
+def _vjp_call(h, qt, vt, tau, step, stage, dt, n, qtb, vtb, qc, vb, tb):
+    B = qt.shape[2]
+    _cabi.check(_cabi.load_library().rbd_integrate_vjp(h.ptr, _DT[qt.dtype], B, _ptr(qt), _ptr(vt), _ptr(tau), step, stage, float(dt), n,
+                                                       _ptr(qtb), _ptr(vtb), None, _ptr(qc), _ptr(vb), _ptr(tb), _stream(qt)))
+
+
+def simulate(mechanism: Mechanism, q0: torch.Tensor, v0: torch.Tensor, torques: Optional[torch.Tensor] = None, *, dt: float,
+             nsteps: int, trajectory: bool = True, checkpoint_every: Optional[int] = None):
+    """Differentiable ``nsteps`` Munthe-Kaas RK4 steps of ``simulate`` from q0 [nq, B], v0 [nv, B].  ``torques``: None (zero),
+    constant [nv, B], per step [nsteps, nv, B] or per stage [nsteps, 4, nv, B].  Returns ``(q_traj, v_traj)`` ([nsteps + 1, rows, B],
+    block 0 the initial state), or ``(q_final, v_final)`` when ``trajectory=False``.  Gradients flow to q0 (as ``q_bar_cfg``, see the
+    module docstring), v0 and the torques; backward runs ``rbd_integrate_vjp``, which recomputes each step's stages from the recorded
+    states.  With ``trajectory=False`` and ``checkpoint_every=k`` only every k-th state is kept, and backward re-records each
+    segment of k steps before its VJP: peak memory O((nsteps / k + k) (nq + nv) B) instead of O(nsteps (nq + nv) B).  The gradients
+    do not depend on k, bit for bit.  Not twice differentiable."""
+    return _Simulate.apply(mechanism, q0, v0, torques, float(dt), int(nsteps), bool(trajectory), checkpoint_every)

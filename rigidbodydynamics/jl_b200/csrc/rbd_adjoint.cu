@@ -164,6 +164,13 @@ VjpArgs<T> args(int64_t B, int64_t ld, const void* q, const void* v, const void*
 
 }  // namespace
 
+int rbd::dynamics_vjp_dense(const rbd_model* model, int32_t dtype, int64_t B, const void* q, const void* v, const void* vd,
+                            const void* vd_bar, void* q_bar_cfg, void* v_bar, void* tau_bar, cudaStream_t s) {
+  return dtype == RBD_F32
+             ? vjp_t<float>(model, true, B, B, args<float>(B, B, q, v, vd, nullptr, vd_bar, nullptr, q_bar_cfg, v_bar, nullptr, tau_bar, nullptr), s)
+             : vjp_t<double>(model, true, B, B, args<double>(B, B, q, v, vd, nullptr, vd_bar, nullptr, q_bar_cfg, v_bar, nullptr, tau_bar, nullptr), s);
+}
+
 extern "C" int32_t rbd_dynamics_vjp(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                                     const void* tau, const void* wext, const void* vd, const void* vd_bar, void* q_bar_tan,
                                     void* q_bar_cfg, void* v_bar, void* tau_bar, void* wext_bar, void* stream) {

@@ -914,9 +914,13 @@ __global__ void __launch_bounds__(128) integrate_finish_kernel(const __grid_cons
   }
 }
 
+// traj_q / traj_v (rbd_integrate_trajectory): [(nsteps + 1) x rows x B] -- block 0 the initial state, block s + 1 written by the
+// finishing kernels of step s; q / v receive the final state as without them.  stages (rbd_integrate_vjp's recompute, nsteps = 1):
+// the four stages' (qs_i, vs_i, φ̇_i, v̇_i) are kept in [4 nq + 12 nv] x B rows (stage_rows) and the finishing step is skipped.
 template <class T>
 int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v, const void* tau, int64_t step_stride,
-                int64_t stage_stride, double dt, int nsteps, cudaStream_t stream) {
+                int64_t stage_stride, double dt, int nsteps, cudaStream_t stream, T* traj_q = nullptr, T* traj_v = nullptr,
+                T* stages = nullptr) {
   const HostModel& hm = model->hm;
   const ModelDev<T>& M = dev_model<T>(hm);
   DeviceProps p;
@@ -930,6 +934,16 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
   T* phid[4]; T* vd[4];
   for (int i = 0; i < 4; ++i) { phid[i] = vs + (size_t)(1 + i) * nv * B; vd[i] = vs + (size_t)(5 + i) * nv * B; }
   T* taud = vs + (size_t)9 * nv * B;
+  T* qsi[4] = {qs, qs, qs, qs};
+  T* vsi[4] = {vs, vs, vs, vs};
+  if (stages)
+    for (int i = 0; i < 4; ++i) {
+      qsi[i] = stages + (size_t)i * nq * B; vsi[i] = stages + (4 * nq + (size_t)i * nv) * B;
+      phid[i] = stages + (4 * nq + (4 + (size_t)i) * nv) * B; vd[i] = stages + (4 * nq + (8 + (size_t)i) * nv) * B;
+    }
+  T* qout = traj_q ? traj_q : (T*)q;       // the finishing kernels' target (block s + 1 of a trajectory)
+  T* vout = traj_v ? traj_v : (T*)v;
+  const int64_t ldo = traj_q ? B : ld;
   // torques of (step s, stage i): tau + s * step_stride + i * stage_stride (both 0: one array held over the whole call); the
   // dynamics kernels want leading dimension B, so arrays with ld != B are densified per use
   const bool varying = step_stride != 0 || stage_stride != 0;
@@ -944,8 +958,8 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
   const bool vec_ok = B % VecOf<T>::N == 0 && B >= 1024;
   const int grid_lin = (int)std::min<int64_t>((B / VecOf<T>::N + 255) / 256, (int64_t)p.sms * 4);
   // ... and, for the finishing kernel, vector-aligned rows of the caller's arrays too
-  const bool vec_user = vec_ok && ld % VecOf<T>::N == 0 && ((uintptr_t)q % sizeof(typename VecOf<T>::type)) == 0 &&
-                        ((uintptr_t)v % sizeof(typename VecOf<T>::type)) == 0;
+  const bool vec_user = vec_ok && ldo % VecOf<T>::N == 0 && ((uintptr_t)qout % sizeof(typename VecOf<T>::type)) == 0 &&
+                        ((uintptr_t)vout % sizeof(typename VecOf<T>::type)) == 0;
   bool has_other = false;
   for (int i = 0; i < hm.nb; ++i) has_other |= (M.body[i].kind != K_REV && M.body[i].kind != K_PRIS && M.body[i].kind != K_FIXED);
   const double a[4] = {0.0, 0.5, 0.5, 1.0}, bw[4] = {1.0 / 6, 1.0 / 3, 1.0 / 3, 1.0 / 6};   // runge_kutta_4, ode_integrators.jl:48-55
@@ -953,6 +967,10 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
   // (q0, v0): dense copies of the state at the start of the step; the finishing kernel of step s refreshes them for step s + 1
   CUDA_TRY(cudaMemcpy2DAsync(q0, B * sizeof(T), q, ld * sizeof(T), B * sizeof(T), nq, cudaMemcpyDeviceToDevice, stream));
   CUDA_TRY(cudaMemcpy2DAsync(v0, B * sizeof(T), v, ld * sizeof(T), B * sizeof(T), nv, cudaMemcpyDeviceToDevice, stream));
+  if (traj_q) {
+    CUDA_TRY(cudaMemcpyAsync(traj_q, q0, nq * B * sizeof(T), cudaMemcpyDeviceToDevice, stream));
+    CUDA_TRY(cudaMemcpyAsync(traj_v, v0, nv * B * sizeof(T), cudaMemcpyDeviceToDevice, stream));
+  }
   for (int s = 0; s < nsteps && rc == RBD_OK; ++s) {
     for (int i = 0; i < 4 && rc == RBD_OK; ++i) {
       if (varying) {
@@ -962,7 +980,7 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
           tau_dense = taud;
         }
       }
-      StageArgs<T> sa{q0, v0, i ? phid[i - 1] : nullptr, i ? vd[i - 1] : nullptr, phid[i], qs, vs, (T)(dt * a[i]), B, vec_ok};
+      StageArgs<T> sa{q0, v0, i ? phid[i - 1] : nullptr, i ? vd[i - 1] : nullptr, phid[i], qsi[i], vsi[i], (T)(dt * a[i]), B, vec_ok};
       if (vec_ok) {        // revolute / prismatic rows, VEC samples per thread
         integrate_stage_linear_kernel<T><<<dim3(grid_lin, hm.nb), 256, 0, stream>>>(M, sa);
         CUDA_TRY(cudaGetLastError());
@@ -974,12 +992,14 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
         launches += 1;
       }
       const int before = g_launch.kernels_launched;
-      rc = dynamics_t<T>(model, B, B, qs, vs, tau_dense, nullptr, vd[i], nullptr, stream);
+      rc = dynamics_t<T>(model, B, B, qsi[i], vsi[i], tau_dense, nullptr, vd[i], nullptr, stream);
       launches += g_launch.kernels_launched - before;
     }
-    if (rc != RBD_OK) break;
-    FinishArgs<T> fa{q0, v0, {phid[0], phid[1], phid[2], phid[3]}, {vd[0], vd[1], vd[2], vd[3]}, (T*)q, (T*)v,
-                     {(T)bw[0], (T)bw[1], (T)bw[2], (T)bw[3]}, (T)dt, B, ld, s + 1 < nsteps, vec_user};
+    if (rc != RBD_OK || stages) break;
+    T* qo = traj_q ? traj_q + (size_t)(s + 1) * nq * B : (T*)q;
+    T* vo = traj_v ? traj_v + (size_t)(s + 1) * nv * B : (T*)v;
+    FinishArgs<T> fa{q0, v0, {phid[0], phid[1], phid[2], phid[3]}, {vd[0], vd[1], vd[2], vd[3]}, qo, vo,
+                     {(T)bw[0], (T)bw[1], (T)bw[2], (T)bw[3]}, (T)dt, B, ldo, s + 1 < nsteps, vec_user};
     if (vec_user) {
       integrate_finish_linear_kernel<T><<<dim3(grid_lin, hm.nb), 256, 0, stream>>>(M, fa);
       CUDA_TRY(cudaGetLastError());
@@ -990,6 +1010,12 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
       CUDA_TRY(cudaGetLastError());
       launches += 1;
     }
+  }
+  if (rc == RBD_OK && traj_q && nsteps > 0) {      // the final state into the caller's q / v, as rbd_integrate leaves it
+    CUDA_TRY(cudaMemcpy2DAsync(q, ld * sizeof(T), traj_q + (size_t)nsteps * nq * B, B * sizeof(T), B * sizeof(T), nq,
+                               cudaMemcpyDeviceToDevice, stream));
+    CUDA_TRY(cudaMemcpy2DAsync(v, ld * sizeof(T), traj_v + (size_t)nsteps * nv * B, B * sizeof(T), B * sizeof(T), nv,
+                               cudaMemcpyDeviceToDevice, stream));
   }
   g_launch.kernels_launched = launches;
   return rc;
@@ -1131,6 +1157,13 @@ int api_check(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld) { re
 void api_note_launch(int grid, int block, int smem_bytes, int blocks_per_sm) {
   g_launch.kernels_launched += 1;
   g_launch.grid = grid; g_launch.block = block; g_launch.smem_bytes = smem_bytes; g_launch.blocks_per_sm = blocks_per_sm;
+}
+int integrate_record(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, const void* tau, int64_t step_stride,
+                     int64_t stage_stride, double dt, int nsteps, void* q_traj, void* v_traj, void* stages, cudaStream_t stream) {
+  return dtype == RBD_F32 ? integrate_t<float>(model, B, ld, q, v, tau, step_stride, stage_stride, dt, nsteps, stream, (float*)q_traj,
+                                               (float*)v_traj, (float*)stages)
+                          : integrate_t<double>(model, B, ld, q, v, tau, step_stride, stage_stride, dt, nsteps, stream, (double*)q_traj,
+                                                (double*)v_traj, (double*)stages);
 }
 }  // namespace rbd
 
@@ -1401,6 +1434,19 @@ int32_t rbd_integrate_schedule(const rbd_model* model, int32_t dtype, int64_t B,
 int32_t rbd_integrate(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, const void* tau,
                       double dt, int32_t nsteps, void* stream) {
   return rbd_integrate_schedule(model, dtype, B, ld, q, v, tau, 0, 0, dt, nsteps, stream);
+}
+
+int32_t rbd_integrate_trajectory(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, const void* tau,
+                                 int64_t tau_step_stride, int64_t tau_stage_stride, double dt, int32_t nsteps, void* q_traj,
+                                 void* v_traj, void* stream) {
+  if (int rc = check_common(model, dtype, B, ld)) return rc;
+  if (nsteps < 0 || !(dt > 0)) return fail(RBD_EINVAL, "rbd_integrate_trajectory: need dt > 0 and nsteps >= 0");
+  if (tau_step_stride < 0 || tau_stage_stride < 0) return fail(RBD_EINVAL, "rbd_integrate_trajectory: torque strides must be >= 0");
+  g_launch = {0, 0, 0, 0, 0, 0.f, 0};
+  if (B == 0) return RBD_OK;
+  if (!q || !v || !q_traj || !v_traj) return fail(RBD_EINVAL, "rbd_integrate_trajectory: q, v, q_traj and v_traj must not be NULL");
+  return rbd::integrate_record(model, dtype, B, ld, q, v, tau, tau_step_stride, tau_stage_stride, dt, nsteps, q_traj, v_traj, nullptr,
+                               (cudaStream_t)stream);
 }
 
 int32_t rbd_inverse_dynamics(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q,

@@ -8,6 +8,8 @@
 // so thread (b, d) carries Dual1 = (value, d-th partial) through the very same templated ABA code; the 6 threads of a sample
 // sit in adjacent lanes, their value loads coalesce into one request and their partial loads are contiguous.
 #pragma once
+#include <type_traits>
+
 #include "rbd_device.cuh"
 
 namespace rbd {
@@ -19,6 +21,9 @@ template <class F> struct Dual1 {
   RBD_HD Dual1(F a, F b) : v(a), d(b) {}
   template <class U> RBD_HD explicit Dual1(const Dual1<U>& o) : v((F)o.v), d((F)o.d) {}
   RBD_HD explicit Dual1(int a) : v((F)a), d(0) {}
+  // a constant of another floating type, e.g. T(0.5) with T = Dual1<float>: rounded like F(0.5)
+  template <class U, class = typename std::enable_if<std::is_floating_point<U>::value && !std::is_same<U, F>::value>::type>
+  RBD_HD Dual1(U a) : v((F)a), d(0) {}
 };
 template <class F> RBD_HD Dual1<F> operator+(const Dual1<F>& a, const Dual1<F>& b) { return {a.v + b.v, a.d + b.d}; }
 template <class F> RBD_HD Dual1<F> operator-(const Dual1<F>& a, const Dual1<F>& b) { return {a.v - b.v, a.d - b.d}; }

@@ -95,5 +95,13 @@ void spec_release(rbd_model* m);
 int api_fail(int status, const std::string& msg);
 int api_check(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld);
 void api_note_launch(int grid, int block, int smem_bytes, int blocks_per_sm);
+// rbd_b200.cu's RK4 driver for rbd_integrate_trajectory (q_traj / v_traj) and rbd_integrate_vjp's recompute (stages: one step,
+// its four stages kept in stage_rows(nq, nv) x B rows, no finishing step).  fp32 / fp64, arguments checked by the caller.
+inline int64_t stage_rows(int64_t nq, int64_t nv) { return 4 * nq + 12 * nv; }
+int integrate_record(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, const void* tau, int64_t step_stride,
+                     int64_t stage_stride, double dt, int nsteps, void* q_traj, void* v_traj, void* stages, cudaStream_t stream);
+// rbd_adjoint.cu's forward-dynamics VJP on dense [rows x B] arrays (no external wrenches); outputs may be NULL
+int dynamics_vjp_dense(const rbd_model* model, int32_t dtype, int64_t B, const void* q, const void* v, const void* vd, const void* vd_bar,
+                       void* q_bar_cfg, void* v_bar, void* tau_bar, cudaStream_t stream);
 
 }  // namespace rbd

@@ -21,7 +21,11 @@ RBD_HD float sqrt_t(float x) { return sqrtf(x); }
 RBD_HD double sqrt_t(double x) { return sqrt(x); }
 RBD_HD float atan2_t(float y, float x) { return atan2f(y, x); }
 RBD_HD double atan2_t(double y, double x) { return atan2(y, x); }
-template <class T> RBD_HD T small_angle2() { return sizeof(T) == 4 ? T(2.5e-3) : T(1e-6); }   // theta^2 threshold
+// The floating type a scalar type computes in: T itself, or the value type of a dual number (rbd_integrate_adjoint.cuh), so
+// that the adjoints' dual-number runs take the branches the forward pass took.
+template <class T> struct ScalarOf { using type = T; };
+template <class T> RBD_HD constexpr bool is_f32() { return sizeof(typename ScalarOf<T>::type) == 4; }
+template <class T> RBD_HD T small_angle2() { return is_f32<T>() ? T(2.5e-3) : T(1e-6); }   // theta^2 threshold
 
 template <class T> RBD_HD void quat_mul(const T* a, const T* b, T* o) {   // Hamilton product, [w x y z]
   o[0] = a[0] * b[0] - a[1] * b[1] - a[2] * b[2] - a[3] * b[3];
@@ -100,7 +104,7 @@ template <class T> RBD_HD void qfloat_global(const T* q0, const T* phi, T* q) {
   quat_from_rotvec(pr, dq);
   T R0[9], Rr[9], tr[3];
   rot_quat(q0[0], q0[1], q0[2], q0[3], R0);
-  if (t2 < (sizeof(T) == 4 ? T(1e-12) : T(1e-30))) {
+  if (t2 < (is_f32<T>() ? T(1e-12) : T(1e-30))) {
     tr[0] = pt[0]; tr[1] = pt[1]; tr[2] = pt[2];
   } else {
     // trans = (1 - R) (w x v) + w (w . v) theta,  w = pr / theta, v = pt / theta
@@ -170,6 +174,37 @@ template <class T> RBD_HD void qsph_local_rate(const T* q0, const T* q, const T*
   for (int k = 0; k < 3; ++k) phid[k] = w[k] + T(0.5) * c1[k] + g * c2[k];
 }
 
+// ---- SinCosRevolute, Planar, SPQuatFloating: the non-trivial halves of their coordinate maps ----------------------------
+// (s, c) of the angle of (s0, c0) advanced by phi
+template <class T> RBD_HD void sincos_global(T s0, T c0, T phi, T& s1, T& c1) {
+  T s, c;
+  sincos_t(phi, s, c);
+  s1 = s0 * c + c0 * s;
+  c1 = c0 * c - s0 * s;
+}
+// planar q̇ of the two translational velocity coordinates (a, b) at angle th
+template <class T> RBD_HD void planar_rate(T th, T a, T b, T& pa, T& pb) {
+  T s, c;
+  sincos_t(th, s, c);
+  pa = c * a - s * b;
+  pb = s * a + c * b;
+}
+// SPQuatFloating q̇ = N(q) v (q: MRP, translation)
+template <class T> RBD_HD void spq_rate(const T* qq, const T* vv, T* pd) {
+  T e[4];
+  mrp_to_quat(qq[0], qq[1], qq[2], e);
+  const T w = e[0], x = e[1], y = e[2], z = e[3];
+  const T dw = T(0.5) * (-x * vv[0] - y * vv[1] - z * vv[2]);
+  const T dx = T(0.5) * (w * vv[0] - z * vv[1] + y * vv[2]);
+  const T dy = T(0.5) * (z * vv[0] + w * vv[1] - x * vv[2]);
+  const T dz = T(0.5) * (-y * vv[0] + x * vv[1] + w * vv[2]);
+  const T inv = T(1) / (T(1) + w);
+  pd[0] = (dx - x * dw * inv) * inv; pd[1] = (dy - y * dw * inv) * inv; pd[2] = (dz - z * dw * inv) * inv;
+  T R[9];
+  rot_quat(w, x, y, z, R);
+  mat_vec(R, vv + 3, pd + 3);
+}
+
 // ---- one joint: stage configuration from local coordinates, and the rate of the local coordinates ---------------------
 // q_stage = global(q0, phi);  phid = d/dt local(q0, q_stage, v_stage).  Rows are addressed through Col / ColOut views.
 // CP / CV: any row accessor with operator()(row) -- Col<T>, ColRW<T>, or the on-the-fly combinations of the RK4 kernels.
@@ -186,39 +221,27 @@ RBD_HD void joint_stage(const BodyDev<T>& bd, const Col<T>& q0, const CP& phi, c
     case K_FIXED: break;
     case K_SINCOS: {                                   // sin_cos_revolute.jl:186-196, :173-184
       T s, c;
-      sincos_t(phi(v), s, c);
-      const T s0 = q0(q), c0 = q0(q + 1);
-      qs.st(q, s0 * c + c0 * s);
-      qs.st(q + 1, c0 * c - s0 * s);
+      sincos_global(q0(q), q0(q + 1), phi(v), s, c);
+      qs.st(q, s);
+      qs.st(q + 1, c);
       phid.st(v, vs(v));
       break;
     }
     case K_PLANAR: {                                   // defaults: q = q0 + phi, phi_dot = q̇ (planar.jl:123-129)
       const T x = q0(q) + phi(v), y = q0(q + 1) + phi(v + 1), th = q0(q + 2) + phi(v + 2);
       qs.st(q, x); qs.st(q + 1, y); qs.st(q + 2, th);
-      T s, c;
-      sincos_t(th, s, c);
-      const T a = vs(v), b = vs(v + 1);
-      phid.st(v, c * a - s * b); phid.st(v + 1, s * a + c * b); phid.st(v + 2, vs(v + 2));
+      T pa, pb;
+      planar_rate(th, vs(v), vs(v + 1), pa, pb);
+      phid.st(v, pa); phid.st(v + 1, pb); phid.st(v + 2, vs(v + 2));
       break;
     }
     case K_SPQFLOAT: {                                 // defaults with q̇ of spquat_floating.jl:128-138
-      T qq[6], vv[6];
+      T qq[6], vv[6], pd[6];
 #pragma unroll
       for (int k = 0; k < 6; ++k) { qq[k] = q0(q + k) + phi(v + k); vv[k] = vs(v + k); qs.st(q + k, qq[k]); }
-      T e[4];
-      mrp_to_quat(qq[0], qq[1], qq[2], e);
-      const T w = e[0], x = e[1], y = e[2], z = e[3];
-      const T dw = T(0.5) * (-x * vv[0] - y * vv[1] - z * vv[2]);
-      const T dx = T(0.5) * (w * vv[0] - z * vv[1] + y * vv[2]);
-      const T dy = T(0.5) * (z * vv[0] + w * vv[1] - x * vv[2]);
-      const T dz = T(0.5) * (-y * vv[0] + x * vv[1] + w * vv[2]);
-      const T inv = T(1) / (T(1) + w);
-      phid.st(v, (dx - x * dw * inv) * inv); phid.st(v + 1, (dy - y * dw * inv) * inv); phid.st(v + 2, (dz - z * dw * inv) * inv);
-      T R[9], t[3];
-      rot_quat(w, x, y, z, R);
-      mat_vec(R, vv + 3, t);
-      phid.st(v + 3, t[0]); phid.st(v + 4, t[1]); phid.st(v + 5, t[2]);
+      spq_rate(qq, vv, pd);
+#pragma unroll
+      for (int k = 0; k < 6; ++k) phid.st(v + k, pd[k]);
       break;
     }
     case K_QFLOAT: {
