@@ -1,17 +1,15 @@
 // rbd_dynamics_vjp / rbd_inverse_dynamics_vjp: reverse-mode products of dynamics! and inverse_dynamics! (csrc/rbd_adjoint.cuh has
 // the mathematics).
 //
-// One generic persistent kernel per entry point, one thread per sample, one launch per call.  The grid is blocks_per_SM x SMs
-// blocks of one warp looping over groups of 32 samples (rbd_loops.cu's scheme).  The per-sample working set -- 54 rows per body
-// plus μ -- lives in a stream-ordered global workspace of adjoint_rows() rows x RESIDENT threads, laid out [row][thread] so a warp's
-// access to a row is one coalesced line; it is capped at kWorkspaceCap bytes by trimming the grid.  The forward VJP's solve
+// One generic persistent kernel per entry point, one thread per sample, one launch per call: blocks of one warp looping over groups
+// of 32 samples, launched through plan_persistent (rbd_handle.h).  The per-sample working set -- 54 rows per body plus μ -- lives
+// in its stream-ordered workspace of adjoint_rows() rows x RESIDENT threads, laid out [row][thread] so a warp's access to a row is
+// one coalesced line; it is capped at kWorkspaceCap bytes by trimming the grid.  The forward VJP's solve
 // (aba_sample) keeps its stash in shared memory like the generic ABA kernel.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include <algorithm>
-#include <mutex>
-#include <set>
 #include <string>
 
 #include "../../../include/rbd_b200.h"
@@ -26,10 +24,6 @@ namespace {
 
 constexpr int kNT = 32;                               // one warp per block; warps never synchronise
 constexpr size_t kWorkspaceCap = size_t(512) << 20;   // bytes of workspace per call at most (fewer resident warps beyond it)
-
-template <class T> const ModelDev<T>& dev_model(const HostModel& m);
-template <> const ModelDev<float>& dev_model<float>(const HostModel& m) { return m.dev32; }
-template <> const ModelDev<double>& dev_model<double>(const HostModel& m) { return m.dev64; }
 
 template <class T> struct VjpArgs {
   const T *q, *v, *vd, *wext, *wbar;            // wbar: ν̄ (forward) / τ̄ (inverse)
@@ -86,20 +80,6 @@ __global__ void __launch_bounds__(kNT, 1) inverse_dynamics_vjp_kernel(const __gr
   }
 }
 
-int big_smem_once(const void* kernel, int dev, int max_smem_optin) {
-  static std::mutex mu;
-  static std::set<std::pair<const void*, int>> done;
-  std::lock_guard<std::mutex> lk(mu);
-  if (done.count({kernel, dev})) return RBD_OK;
-  cudaFuncAttributes fa{};
-  if (cudaFuncGetAttributes(&fa, kernel) != cudaSuccess ||
-      cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin - (int)fa.sharedSizeBytes) != cudaSuccess)
-    return api_fail(RBD_ECUDA, std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(cudaGetLastError()));
-  cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  done.insert({kernel, dev});
-  return RBD_OK;
-}
-
 // Same model limits as rbd_dynamics_derivatives
 int check_limits(const HostModel& hm, const char* who) {
   DerivDev D;
@@ -117,39 +97,16 @@ int vjp_t(const rbd_model* model, bool fd, int64_t B, int64_t ld, VjpArgs<T> a, 
   if (fd)
     for (int k = 0; k < 3; ++k) M.g[k] = T(0);
   const void* kernel = fd ? (const void*)dynamics_vjp_kernel<T> : (const void*)inverse_dynamics_vjp_kernel<T>;
-  int dev = 0, sms = 0, optin = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return api_fail(RBD_ECUDA, "cudaGetDevice failed");
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
   const size_t smem = fd ? (size_t)std::max(1, (int)M.nrows) * kNT * sizeof(T) : 0;
-  if ((int)smem > optin) return api_fail(RBD_EUNSUPPORTED, "model working set exceeds shared memory per block");
-  if (fd)
-    if (int rc = big_smem_once(kernel, dev, optin)) return rc;
-  int bps = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, kernel, kNT, smem) != cudaSuccess || bps < 1)
-    return api_fail(RBD_EUNSUPPORTED, "rbd_*_vjp: kernel does not fit on an SM");
-  const int rows = adjoint_rows(hm.nb, hm.nv);
-  const size_t col_bytes = (size_t)rows * kNT * sizeof(T);
-  const int64_t ngroups = (B + kNT - 1) / kNT;
-  const int64_t cap = std::max<int64_t>(1, (int64_t)(kWorkspaceCap / col_bytes));
-  const int grid = (int)std::min<int64_t>({ngroups, (int64_t)bps * sms, cap});
-  T* work = nullptr;
-  const size_t nwork = (size_t)rows * grid * kNT + 1;       // + the zero
-  cudaError_t e = cudaMallocAsync((void**)&work, nwork * sizeof(T), stream);
-  if (e != cudaSuccess) return api_fail(e == cudaErrorMemoryAllocation ? RBD_ENOMEM : RBD_ECUDA,
-                                        std::string("rbd_*_vjp workspace: ") + cudaGetErrorString(e));
-  a.work = work;
-  a.zero = work + nwork - 1;
-  e = cudaMemsetAsync(work + nwork - 1, 0, sizeof(T), stream);
-  if (e == cudaSuccess) {
-    if (fd) dynamics_vjp_kernel<T><<<grid, kNT, smem, stream>>>(M, a);
-    else inverse_dynamics_vjp_kernel<T><<<grid, kNT, 0, stream>>>(M, a);
-    e = cudaGetLastError();
-  }
-  cudaFreeAsync(work, stream);
-  if (e != cudaSuccess) return api_fail(RBD_ECUDA, std::string("rbd_*_vjp launch failed: ") + cudaGetErrorString(e));
-  api_note_launch(grid, kNT, (int)smem, bps);
-  return RBD_OK;
+  const size_t row_bytes = (size_t)adjoint_rows(hm.nb, hm.nv) * sizeof(T);
+  LaunchPlan pl;        // the workspace, then the zero
+  if (int rc = plan_persistent(kernel, kNT, smem, (B + kNT - 1) / kNT, stream, pl, row_bytes, sizeof(T), kWorkspaceCap)) return rc;
+  a.work = (T*)pl.work.p;
+  a.zero = a.work + row_bytes / sizeof(T) * pl.grid * kNT;
+  RBD_CUDA_TRY(cudaMemsetAsync(const_cast<T*>(a.zero), 0, sizeof(T), stream));
+  if (fd) dynamics_vjp_kernel<T><<<pl.grid, pl.block, pl.smem, stream>>>(M, a);
+  else inverse_dynamics_vjp_kernel<T><<<pl.grid, pl.block, pl.smem, stream>>>(M, a);
+  return api_launched(&pl);
 }
 
 template <class T>
@@ -175,6 +132,7 @@ extern "C" int32_t rbd_dynamics_vjp(const rbd_model* model, int32_t dtype, int64
                                     const void* tau, const void* wext, const void* vd, const void* vd_bar, void* q_bar_tan,
                                     void* q_bar_cfg, void* v_bar, void* tau_bar, void* wext_bar, void* stream) {
   if (int rc = api_check(model, dtype, B, ld)) return rc;
+  const ApiCall call;
   if (B == 0 || model->hm.nv == 0) return RBD_OK;
   if (!q || !v || !vd || !vd_bar) return api_fail(RBD_EINVAL, "rbd_dynamics_vjp: q, v, vd and vd_bar must not be NULL");
   if (int rc = check_limits(model->hm, "rbd_dynamics_vjp")) return rc;
@@ -189,6 +147,7 @@ extern "C" int32_t rbd_inverse_dynamics_vjp(const rbd_model* model, int32_t dtyp
                                             const void* vd, const void* wext, const void* tau_bar, void* q_bar_tan, void* q_bar_cfg,
                                             void* v_bar, void* vd_bar, void* wext_bar, void* stream) {
   if (int rc = api_check(model, dtype, B, ld)) return rc;
+  const ApiCall call;
   if (B == 0 || model->hm.nv == 0) return RBD_OK;
   if (!q || !v || !vd || !tau_bar) return api_fail(RBD_EINVAL, "rbd_inverse_dynamics_vjp: q, v, vd and tau_bar must not be NULL");
   if (int rc = check_limits(model->hm, "rbd_inverse_dynamics_vjp")) return rc;

@@ -9,6 +9,8 @@
 //     [row][lane] so a warp's access to a row hits 32 distinct banks;
 //   * the flattened mechanism is a __grid_constant__ kernel parameter: it is read through the constant bank with a
 //     warp-uniform index, i.e. as uniform-register operands, not as per-thread loads.
+// The host side of every launch (device properties, kernel configuration, persistent grid and workspace, error mapping, launch
+// record) is the shared plumbing declared in rbd_handle.h and implemented below, used by the library's other units as well.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -19,6 +21,7 @@
 #include <memory>
 #include <mutex>
 #include <new>
+#include <optional>
 #include <set>
 #include <string>
 #include <type_traits>
@@ -41,43 +44,105 @@ namespace {
 
 thread_local std::string g_err;
 thread_local rbd_launch_info g_launch = {0, 0, 0, 0, 0, 0.f, 0};
+thread_local int g_call_depth = 0;     // C-ABI calls in progress on this thread (ApiCall)
 
 int fail(int status, const std::string& msg) { g_err = msg; return status; }
-int fail_cuda(cudaError_t e, const char* what) {
-  g_err = std::string(what) + ": " + cudaGetErrorString(e);
-  return RBD_ECUDA;
-}
-#define CUDA_TRY(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) return fail_cuda(e_, #expr); } while (0)
 
-struct DeviceProps { int dev = 0; int sms = 0; int max_smem_optin = 0; int smem_per_sm = 0; bool ok = false; };
-int get_props(DeviceProps& p) {
+}  // namespace
+
+// ---- the host plumbing of rbd_handle.h, shared by the library's translation units ----------------------------------------
+namespace rbd {
+
+int api_fail(int status, const std::string& msg) { return fail(status, msg); }
+int api_fail_cuda(cudaError_t e, const std::string& what) {
+  cudaGetLastError();      // a non-sticky error must not be reported again by the next launch check
+  return fail(e == cudaErrorMemoryAllocation ? RBD_ENOMEM : RBD_ECUDA, what + ": " + cudaGetErrorString(e));
+}
+
+cudaError_t device_props(DeviceProps& p) {
   static std::mutex mu;
   static DeviceProps cache[64];
   int dev = 0;
-  CUDA_TRY(cudaGetDevice(&dev));
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
   std::lock_guard<std::mutex> lk(mu);
-  if (dev >= 0 && dev < 64 && cache[dev].ok) { p = cache[dev]; return RBD_OK; }
+  if (dev >= 0 && dev < 64 && cache[dev].sms) { p = cache[dev]; return cudaSuccess; }
   DeviceProps q;
   q.dev = dev;
-  CUDA_TRY(cudaDeviceGetAttribute(&q.sms, cudaDevAttrMultiProcessorCount, dev));
-  CUDA_TRY(cudaDeviceGetAttribute(&q.max_smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-  CUDA_TRY(cudaDeviceGetAttribute(&q.smem_per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev));
-  {  // scratch for slots / external wrenches comes from the stream-ordered pool: keep freed blocks cached in the pool
-    cudaMemPool_t pool;
-    if (cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
-      uint64_t keep = ~0ull;
-      cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
-    }
-  }
-  q.ok = true;
+  cudaMemPool_t pool;
+  uint64_t keep = ~0ull;
+  e = cudaDeviceGetAttribute(&q.sms, cudaDevAttrMultiProcessorCount, dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&q.max_smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&q.smem_per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
+  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&q.l2_bytes, cudaDevAttrL2CacheSize, dev);
+  if (e == cudaSuccess) e = cudaDeviceGetDefaultMemPool(&pool, dev);
+  if (e == cudaSuccess) e = cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
+  if (e != cudaSuccess) return e;
   if (dev >= 0 && dev < 64) cache[dev] = q;
   p = q;
+  return cudaSuccess;
+}
+
+int kernel_config(const void* kernel, int block, size_t smem, const DeviceProps& p, int& blocks_per_sm) {
+  if (smem > (size_t)p.max_smem_optin) return fail(RBD_EUNSUPPORTED, "model working set exceeds shared memory per block");
+  if (smem > 0) {
+    static std::mutex mu;
+    static std::set<std::pair<const void*, int>> done;
+    std::lock_guard<std::mutex> lk(mu);
+    if (!done.count({kernel, p.dev})) {
+      cudaFuncAttributes fa{};
+      RBD_CUDA_TRY(cudaFuncGetAttributes(&fa, kernel));
+      RBD_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, p.max_smem_optin - (int)fa.sharedSizeBytes));
+      RBD_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+      done.insert({kernel, p.dev});
+    }
+  }
+  RBD_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, kernel, block, smem));
+  if (blocks_per_sm < 1) return fail(RBD_EUNSUPPORTED, "kernel does not fit on an SM");
   return RBD_OK;
 }
 
-template <class T> const ModelDev<T>& dev_model(const HostModel& m);
-template <> const ModelDev<float>& dev_model<float>(const HostModel& m) { return m.dev32; }
-template <> const ModelDev<double>& dev_model<double>(const HostModel& m) { return m.dev64; }
+int plan_persistent(const void* kernel, int block, size_t smem, int64_t ngroups, cudaStream_t stream, LaunchPlan& plan,
+                    size_t work_per_thread, size_t work_extra, size_t work_cap) {
+  DeviceProps p;
+  RBD_CUDA_TRY(device_props(p));
+  if (int rc = kernel_config(kernel, block, smem, p, plan.blocks_per_sm)) return rc;
+  int64_t grid = std::min<int64_t>(ngroups, (int64_t)plan.blocks_per_sm * p.sms);
+  if (work_cap) grid = std::min<int64_t>(grid, std::max<int64_t>(1, (int64_t)(work_cap / (work_per_thread * block))));
+  plan.grid = (int)grid;
+  plan.block = block;
+  plan.smem = (int)smem;
+  if (work_per_thread) RBD_CUDA_TRY(plan.work.alloc(work_per_thread * grid * block + work_extra, stream));
+  return RBD_OK;
+}
+
+ApiCall::ApiCall() { if (g_call_depth++ == 0) g_launch = {0, 0, 0, 0, 0, 0.f, 0}; }
+ApiCall::~ApiCall() { --g_call_depth; }
+
+void api_note_launch(const LaunchShape* shape, bool specialised) {
+  g_launch.kernels_launched += 1;
+  if (shape) {
+    g_launch.grid = shape->grid; g_launch.block = shape->block; g_launch.smem_bytes = shape->smem;
+    g_launch.blocks_per_sm = shape->blocks_per_sm;
+  }
+  if (specialised) g_launch.specialised = 1;
+}
+int api_launched(const LaunchShape* shape) {
+  RBD_CUDA_TRY(cudaGetLastError());
+  api_note_launch(shape);
+  return RBD_OK;
+}
+
+KeepLaunchRecord::KeepLaunchRecord() : saved(g_launch) {}
+KeepLaunchRecord::~KeepLaunchRecord() {
+  const int n = g_launch.kernels_launched;
+  g_launch = saved;
+  g_launch.kernels_launched = n;
+}
+
+}  // namespace rbd
+
+namespace {
 
 // ------------------------------------------------------------------------------------------------------------------
 // kernels
@@ -379,20 +444,6 @@ __global__ void __launch_bounds__(NT, sizeof(T) == 4 ? 28 : 12) kin_kernel(const
   }
 }
 
-// Opt a kernel into large dynamic shared memory ONCE per (kernel, device): the attribute is process-global per kernel, so
-// setting it to each call's exact size would race between host threads using different model handles.
-int configure_once(const void* kernel, const DeviceProps& p) {
-  static std::mutex mu;
-  static std::set<std::pair<const void*, int>> done;
-  std::lock_guard<std::mutex> lk(mu);
-  if (done.count({kernel, p.dev})) return RBD_OK;
-  cudaFuncAttributes fa{};
-  CUDA_TRY(cudaFuncGetAttributes(&fa, kernel));
-  CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, p.max_smem_optin - (int)fa.sharedSizeBytes));
-  CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-  done.insert({kernel, p.dev});
-  return RBD_OK;
-}
 template <class T> struct BodiesArgs {
   const T* q; const T* v; const T* vd; const T* wext;
   T* acc; T* jw;
@@ -448,48 +499,19 @@ contact_kernel(const __grid_constant__ ModelDev<T> M, const __grid_constant__ Co
   }
 }
 
-template <class K> int configure(K kernel, int nt, size_t smem, const DeviceProps& p, int& blocks_per_sm) {
-  if ((int)smem > p.max_smem_optin) return fail(RBD_EUNSUPPORTED, "model working set exceeds shared memory per block");
-  if (int rc = configure_once((const void*)kernel, p)) return rc;
-  CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks_per_sm, kernel, nt, smem));
-  if (blocks_per_sm < 1) return fail(RBD_EUNSUPPORTED, "kernel does not fit on an SM");
-  return RBD_OK;
-}
-
-template <class T> struct AbaArgs; template <class T> struct RneaArgs; template <class T> struct CrbaArgs;
-template <class T> void set_scratch(AbaArgs<T>& a, T* s);
-template <class T> void set_scratch(RneaArgs<T>& a, T* s);
-template <class T> void set_scratch(CrbaArgs<T>&, T*);
-
-// Launch `kernel` persistently (blocks_per_SM x SMs blocks looping over groups of NT samples).  `scratch_rows` > 0
-// requests a stream-ordered scratch of that many rows per resident thread (the external-wrench path).
-template <class T, class Kern, class Args>
-int launch(Kern kernel, const ModelDev<T>& M, Args a, int nt, int rows, int scratch_rows, cudaStream_t stream) {
-  DeviceProps p;
-  if (int rc = get_props(p)) return rc;
-  const size_t smem = (size_t)rows * nt * sizeof(T);
-  int bps = 0;
-  if (int rc = configure(kernel, nt, smem, p, bps)) return rc;
-  const int64_t ngroups = (a.B + nt - 1) / nt;
-  const int grid = (int)std::min<int64_t>(ngroups, (int64_t)bps * p.sms);
-  void* scratch = nullptr;
-  if (scratch_rows > 0) {
-    CUDA_TRY(cudaMallocAsync(&scratch, (size_t)scratch_rows * grid * nt * sizeof(T), stream));
-    set_scratch(a, (T*)scratch);
-  }
-  kernel<<<grid, nt, smem, stream>>>(M, a);
-  cudaError_t e = cudaGetLastError();
-  if (scratch) cudaFreeAsync(scratch, stream);
-  if (e != cudaSuccess) return fail_cuda(e, "kernel launch");
-  g_launch.kernels_launched += 1;
-  g_launch.grid = grid; g_launch.block = nt; g_launch.smem_bytes = (int)smem; g_launch.blocks_per_sm = bps;
-  return RBD_OK;
-}
-template <class T> void set_scratch(AbaArgs<T>& a, T* s) { a.scratch = s; }
-template <class T> void set_scratch(RneaArgs<T>& a, T* s) { a.scratch = s; }
-template <class T> void set_scratch(CrbaArgs<T>&, T*) {}
-
 constexpr int kNT = 32;   // threads per block: one warp; warps never synchronise with each other
+
+// Launch `kernel` persistently with a stash of `rows` rows per thread in shared memory (plan_persistent).  `scratch_rows` > 0
+// gives the kernel's `scratch` member a workspace of that many rows per resident thread (the external-wrench path).
+template <class T, class Kern, class Args>
+int launch(Kern kernel, const ModelDev<T>& M, Args a, int rows, cudaStream_t stream, T* Args::*scratch = nullptr, int scratch_rows = 0) {
+  LaunchPlan pl;
+  if (int rc = plan_persistent((const void*)kernel, kNT, (size_t)rows * kNT * sizeof(T), (a.B + kNT - 1) / kNT, stream, pl,
+                               (size_t)scratch_rows * sizeof(T))) return rc;
+  if (scratch) a.*scratch = (T*)pl.work.p;
+  kernel<<<pl.grid, pl.block, pl.smem, stream>>>(M, a);
+  return api_launched(&pl);
+}
 
 // The mixed CTA (see aba_kernel_mix) in place of the shared-memory kernel `ks`: one CTA of up to `nw` warps per SM, as many
 // as the registers allow, `sw` of them with their stash in shared memory and the rest in an L2 scratch of at most 60 % of
@@ -499,40 +521,34 @@ template <class KS, class KM, class Dev, class Args>
 int launch_mix(const rbd_model* model, KS ks, KM km, int nw, const Dev& M, Args a, size_t warp_bytes, int64_t ngroups,
                int scratch_rows, cudaStream_t stream, bool& used) {
   used = false;
-  if (const char* f = getenv("RBD_JIT_VARIANT")) if (atoi(f) == 1) return RBD_OK;
+  if (jit_variant() == 1) return RBD_OK;
   DeviceProps p;
-  if (int rc = get_props(p)) return rc;
-  int bps = 0, l2 = 0;
-  if (int rc = configure(ks, kNT, warp_bytes, p, bps)) return rc;
-  if (int rc = configure_once((const void*)km, p)) return rc;
+  RBD_CUDA_TRY(device_props(p));
+  int bps = 0, bps_mix = 0;
+  if (int rc = kernel_config((const void*)ks, kNT, warp_bytes, p, bps)) return rc;
   cudaFuncAttributes fa{};
-  CUDA_TRY(cudaFuncGetAttributes(&fa, km));
-  CUDA_TRY(cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, p.dev));
+  RBD_CUDA_TRY(cudaFuncGetAttributes(&fa, km));
   const int fit = std::min(nw, 65536 / (((fa.numRegs + 7) / 8) * 8 * 32));
   const int sw = std::min<int>(fit, (int)((p.max_smem_optin - (int)fa.sharedSizeBytes) / warp_bytes));
-  const int gw = (int)std::min<int64_t>(fit - sw, (int64_t)(0.6 * l2) / ((int64_t)p.sms * (int64_t)warp_bytes));
+  const int gw = (int)std::min<int64_t>(fit - sw, (int64_t)(0.6 * p.l2_bytes) / ((int64_t)p.sms * (int64_t)warp_bytes));
   const int total = sw + std::max(0, gw);
   if (sw < 1 || total * 100 < bps * 115 || ngroups < (int64_t)total * p.sms) return RBD_OK;
+  const LaunchShape shape{p.sms, 32 * total, (int)(sw * warp_bytes), 1};
+  if (int rc = kernel_config((const void*)km, shape.block, shape.smem, p, bps_mix)) return rc;
   QueueCtx ctx;      // zeroed work-queue counter, cached in the handle
-  CUDA_TRY(queue_begin(const_cast<rbd_model*>(model), stream, ctx));
+  RBD_CUDA_TRY(queue_begin(const_cast<rbd_model*>(model), stream, ctx));
   a.counter = ctx.counter;
   a.sw = sw;
-  void* l2s = nullptr;
-  void* scratch = nullptr;
-  if (gw > 0) CUDA_TRY(cudaMallocAsync(&l2s, (size_t)gw * p.sms * warp_bytes, stream));
-  a.l2 = static_cast<decltype(a.l2)>(l2s);
+  StreamAlloc l2s, scratch;
+  if (gw > 0) RBD_CUDA_TRY(l2s.alloc((size_t)gw * p.sms * warp_bytes, stream));
+  a.l2 = static_cast<decltype(a.l2)>(l2s.p);
   if (scratch_rows > 0) {       // external wrenches in body frames: one column per resident thread
     a.scratch_ld = (int64_t)p.sms * total * 32;
-    CUDA_TRY(cudaMallocAsync(&scratch, (size_t)scratch_rows * a.scratch_ld * sizeof(*a.scratch), stream));
-    a.scratch = static_cast<decltype(a.scratch)>(scratch);
+    RBD_CUDA_TRY(scratch.alloc((size_t)scratch_rows * a.scratch_ld * sizeof(*a.scratch), stream));
+    a.scratch = static_cast<decltype(a.scratch)>(scratch.p);
   }
-  km<<<p.sms, 32 * total, sw * warp_bytes, stream>>>(M, a);
-  cudaError_t e = cudaGetLastError();
-  if (l2s) cudaFreeAsync(l2s, stream);
-  if (scratch) cudaFreeAsync(scratch, stream);
-  if (e != cudaSuccess) return fail_cuda(e, "kernel launch");
-  g_launch.kernels_launched += 1;
-  g_launch.grid = p.sms; g_launch.block = 32 * total; g_launch.smem_bytes = (int)(sw * warp_bytes); g_launch.blocks_per_sm = 1;
+  km<<<shape.grid, shape.block, shape.smem, stream>>>(M, a);
+  if (int rc = api_launched(&shape)) return rc;
   used = true;
   return RBD_OK;
 }
@@ -547,26 +563,19 @@ int dynamics_t(const rbd_model* model, int64_t B, int64_t ld, const void* q, con
   const int sr = wext ? 6 * hm.nb : 0;
   bool other_kinds = false;          // prismatic / fixed joints anywhere -> kernels with those code paths
   for (int i = 0; i < hm.nb; ++i) other_kinds |= (M.body[i].kind == K_PRIS || M.body[i].kind == K_FIXED);
-#define RBD_ABA(G, E, K) launch<T>(aba_kernel<T, kNT, G, E, K>, M, a, kNT, rows, sr, stream)
+#define RBD_ABA(G, E, K) launch<T>(aba_kernel<T, kNT, G, E, K>, M, a, rows, stream, &AbaArgs<T>::scratch, sr)
   if (!wext) {      // model-specialised kernels (rbd_spec.cpp): straight-line code generated for this mechanism
     SpecKey key; key.algo = SPEC_ABA; key.f64 = sizeof(T) == 8; key.has_in2 = tau != nullptr; key.has_out1 = qd != nullptr;
-    const SpecLaunchArgs sa{q, v, tau, vd, qd, ld, B};
     bool used = false;
-    std::string err;
     const int* gate = nullptr;
-    if (int rc = spec_try_launch(const_cast<rbd_model*>(model), key, sa, stream, used, g_launch, &gate, err)) return fail(rc, err);
+    if (int rc = spec_try_launch(const_cast<rbd_model*>(model), key, {q, v, tau, vd, qd, ld, B}, stream, used, &gate)) return rc;
     if (used) {
-      g_launch.specialised = 1;
       if (!gate) return RBD_OK;
       // fp32: the specialised program has no slow sin / cos path; if any sample met an angle beyond 1e4 rad (flag raised on the
       // device) this generic launch redoes the batch with the library path, otherwise it exits at once
-      const rbd_launch_info keep = g_launch;
+      const KeepLaunchRecord keep;
       a.gate = gate;
-      const int rc = hm.general ? RBD_ABA(true, false, kAllKinds) : (other_kinds ? RBD_ABA(false, false, kAllKinds) : RBD_ABA(false, false, 0));
-      const int n = g_launch.kernels_launched;
-      g_launch = keep;
-      g_launch.kernels_launched = n;
-      return rc;
+      return hm.general ? RBD_ABA(true, false, kAllKinds) : (other_kinds ? RBD_ABA(false, false, kAllKinds) : RBD_ABA(false, false, 0));
     }
   }
   if (!wext && !hm.general && !other_kinds && rows <= 256) {   // all-revolute trees (floating root allowed): the mixed CTA, see launch_mix
@@ -592,21 +601,14 @@ int inverse_dynamics_t(const rbd_model* model, int64_t B, int64_t ld, const void
   const int rows = rnea_rows(hm);
   if (!wext) {
     SpecKey key; key.algo = SPEC_RNEA; key.f64 = sizeof(T) == 8; key.has_in2 = vd != nullptr;
-    const SpecLaunchArgs sa{q, v, vd, tau, nullptr, ld, B};
     bool used = false;
-    std::string err;
     const int* gate = nullptr;
-    if (int rc = spec_try_launch(const_cast<rbd_model*>(model), key, sa, stream, used, g_launch, &gate, err)) return fail(rc, err);
+    if (int rc = spec_try_launch(const_cast<rbd_model*>(model), key, {q, v, vd, tau, nullptr, ld, B}, stream, used, &gate)) return rc;
     if (used) {
-      g_launch.specialised = 1;
       if (!gate) return RBD_OK;
-      const rbd_launch_info keep = g_launch;      // gated generic fallback, see dynamics_t
+      const KeepLaunchRecord keep;      // gated generic fallback, see dynamics_t
       a.gate = gate;
-      const int rc = launch<T>(rnea_kernel<T, kNT, false>, M, a, kNT, rows, 0, stream);
-      const int n = g_launch.kernels_launched;
-      g_launch = keep;
-      g_launch.kernels_launched = n;
-      return rc;
+      return launch<T>(rnea_kernel<T, kNT, false>, M, a, rows, stream);
     }
   }
   if (rows <= 256) {             // the mixed CTA, see launch_mix
@@ -620,8 +622,8 @@ int inverse_dynamics_t(const rbd_model* model, int64_t B, int64_t ld, const void
     if (rc) return rc;
     if (used) return RBD_OK;
   }
-  return wext ? launch<T>(rnea_kernel<T, kNT, true>, M, a, kNT, rows, 6 * hm.nb, stream)
-              : launch<T>(rnea_kernel<T, kNT, false>, M, a, kNT, rows, 0, stream);
+  return wext ? launch<T>(rnea_kernel<T, kNT, true>, M, a, rows, stream, &RneaArgs<T>::scratch, 6 * hm.nb)
+              : launch<T>(rnea_kernel<T, kNT, false>, M, a, rows, stream);
 }
 
 template <class T>
@@ -634,26 +636,18 @@ int mass_matrix_t(const rbd_model* model, int64_t B, int64_t ld, const void* q, 
   for (int i = 0; i < hm.nb; ++i) multi |= kind_nv(M.body[i].kind) > 1;
   {      // model-specialised kernel: the composite-rigid-body algorithm traced on this mechanism (rbd_codegen.cpp)
     SpecKey key; key.algo = SPEC_CRBA; key.f64 = sizeof(T) == 8; key.has_in2 = false; key.lower = lower;
-    const SpecLaunchArgs sa{q, nullptr, nullptr, Mout, nullptr, ld, B};
     bool used = false;
-    std::string err;
     const int* gate = nullptr;
-    if (int rc = spec_try_launch(const_cast<rbd_model*>(model), key, sa, stream, used, g_launch, &gate, err)) return fail(rc, err);
-    if (used) {
-      g_launch.specialised = 1;
-      if (!gate) return RBD_OK;
-      const rbd_launch_info keep = g_launch;      // gated generic fallback, see dynamics_t
-      a.gate = gate;
-      const int rc = multi ? launch<T>(crba_kernel<T, kNT, 6>, M, a, kNT, rows, 0, stream)
-                           : launch<T>(crba_kernel<T, kNT, 1>, M, a, kNT, rows, 0, stream);
-      const int n = g_launch.kernels_launched;
-      g_launch = keep;
-      g_launch.kernels_launched = n;
+    if (int rc = spec_try_launch(const_cast<rbd_model*>(model), key, {q, nullptr, nullptr, Mout, nullptr, ld, B}, stream, used, &gate))
       return rc;
+    if (used) {
+      if (!gate) return RBD_OK;
+      const KeepLaunchRecord keep;      // gated generic fallback, see dynamics_t
+      a.gate = gate;
+      return multi ? launch<T>(crba_kernel<T, kNT, 6>, M, a, rows, stream) : launch<T>(crba_kernel<T, kNT, 1>, M, a, rows, stream);
     }
   }
-  return multi ? launch<T>(crba_kernel<T, kNT, 6>, M, a, kNT, rows, 0, stream)
-               : launch<T>(crba_kernel<T, kNT, 1>, M, a, kNT, rows, 0, stream);
+  return multi ? launch<T>(crba_kernel<T, kNT, 6>, M, a, rows, stream) : launch<T>(crba_kernel<T, kNT, 1>, M, a, rows, stream);
 }
 
 // Kinematics by-products (SURVEY 8(f) rank 2).  One launch; the momentum matrix additionally parks the 12 nb pose rows of
@@ -673,8 +667,7 @@ int kinematics_t(const rbd_model* model, int64_t B, int64_t ld, const void* q, c
   KinArgs<T> a{(const T*)q, (const T*)v, (T*)o.transforms_to_root, (T*)o.center_of_mass, (T*)o.kinetic_energy,
                (T*)o.gravitational_potential_energy, (T*)o.momentum, (T*)o.momentum_rate_bias, (T*)o.momentum_matrix,
                (T*)o.geometric_jacobian, nullptr, ld, B, nullptr};
-  DeviceProps p;
-  if (int rc = get_props(p)) return rc;
+  std::optional<KeepLaunchRecord> keep;
   {                              // model-specialised kernel for this output subset (and this jacobian path)
     SpecKey key;
     key.algo = SPEC_KIN; key.f64 = sizeof(T) == 8; key.has_in2 = v != nullptr;
@@ -684,34 +677,22 @@ int kinematics_t(const rbd_model* model, int64_t B, int64_t ld, const void* q, c
     for (int k = 0; k < 8; ++k) { if (outs[k]) key.kin_mask |= 1 << k; sa.ko[k] = outs[k]; }
     for (int i = 0; i < hm.nb; ++i) key.kin_sign[i] = K.sign[i];
     bool used = false;
-    std::string err;
     const int* gate = nullptr;
     if (key.kin_mask)
-      if (int rc = spec_try_launch(const_cast<rbd_model*>(model), key, sa, stream, used, g_launch, &gate, err)) return fail(rc, err);
+      if (int rc = spec_try_launch(const_cast<rbd_model*>(model), key, sa, stream, used, &gate)) return rc;
     if (used) {
-      g_launch.specialised = 1;
       if (!gate) return RBD_OK;
+      keep.emplace();
       a.gate = gate;               // gated generic fallback (angles beyond the fast sin / cos range), see dynamics_t
     }
   }
   auto kernel = kin_kernel<T, kNT>;
-  const size_t smem = (size_t)std::max(1, kin_rows(hm)) * kNT * sizeof(T);
-  int bps = 0;
-  if (int rc = configure(kernel, kNT, smem, p, bps)) return rc;
-  const int64_t ngroups = (B + kNT - 1) / kNT;
-  const int grid = (int)std::min<int64_t>(ngroups, (int64_t)bps * p.sms);
-  void* scratch = nullptr;
-  if (o.momentum_matrix) {
-    CUDA_TRY(cudaMallocAsync(&scratch, (size_t)12 * hm.nb * grid * kNT * sizeof(T), stream));
-    a.scratch = (T*)scratch;
-  }
-  kernel<<<grid, kNT, smem, stream>>>(M, a, K);
-  cudaError_t e = cudaGetLastError();
-  if (scratch) cudaFreeAsync(scratch, stream);
-  if (e != cudaSuccess) return fail_cuda(e, "kernel launch");
-  g_launch.kernels_launched += 1;
-  g_launch.grid = grid; g_launch.block = kNT; g_launch.smem_bytes = (int)smem; g_launch.blocks_per_sm = bps;
-  return RBD_OK;
+  LaunchPlan pl;
+  if (int rc = plan_persistent((const void*)kernel, kNT, (size_t)std::max(1, kin_rows(hm)) * kNT * sizeof(T), (B + kNT - 1) / kNT,
+                               stream, pl, o.momentum_matrix ? (size_t)12 * hm.nb * sizeof(T) : 0)) return rc;
+  a.scratch = (T*)pl.work.p;
+  kernel<<<pl.grid, pl.block, pl.smem, stream>>>(M, a, K);
+  return api_launched(&pl);
 }
 
 // dynamics! on Dual{Float64,6} arrays (config 4).  The Dual model (constants with zero partials, 25 KB) is built per call
@@ -735,27 +716,19 @@ int dynamics_dual(const rbd_model* model, int64_t B, int64_t ld, const void* q, 
     d.oslot = s.oslot; d.pslot = s.pslot; d.flags = s.flags; d.refidx = s.refidx;
   }
   DualArgs a{(const double*)q, (const double*)v, (const double*)tau, (double*)vd, ld, B};
-  DeviceProps p;
-  if (int rc = get_props(p)) return rc;
+  const int64_t ngroups = (B * 6 + kNT - 1) / kNT;      // one thread per (sample, partial direction)
   if (!hm.general && S.nrows <= 256) {      // the mixed CTA, see launch_mix
     bool used = false;
     a.rows = S.nrows;
     if (int rc = launch_mix(model, aba_dual_kernel<kNT, false>, aba_dual_kernel_mix, kMixWarps<double>, *Mp, a,
-                            (size_t)S.nrows * kNT * sizeof(Dual64), (B * 6 + kNT - 1) / kNT, 0, stream, used)) return rc;
+                            (size_t)S.nrows * kNT * sizeof(Dual64), ngroups, 0, stream, used)) return rc;
     if (used) return RBD_OK;
   }
-  const size_t smem = (size_t)S.nrows * kNT * sizeof(Dual64);
-  int bps = 0;
-  if (int rc = hm.general ? configure(aba_dual_kernel<kNT, true>, kNT, smem, p, bps)
-                          : configure(aba_dual_kernel<kNT, false>, kNT, smem, p, bps)) return rc;
-  const int64_t ngroups = (B * 6 + kNT - 1) / kNT;      // one thread per (sample, partial direction)
-  const int grid = (int)std::min<int64_t>(ngroups, (int64_t)bps * p.sms);
-  if (hm.general) aba_dual_kernel<kNT, true><<<grid, kNT, smem, stream>>>(*Mp, a);
-  else aba_dual_kernel<kNT, false><<<grid, kNT, smem, stream>>>(*Mp, a);
-  CUDA_TRY(cudaGetLastError());
-  g_launch.kernels_launched += 1;
-  g_launch.grid = grid; g_launch.block = kNT; g_launch.smem_bytes = (int)smem; g_launch.blocks_per_sm = bps;
-  return RBD_OK;
+  const auto kernel = hm.general ? aba_dual_kernel<kNT, true> : aba_dual_kernel<kNT, false>;
+  LaunchPlan pl;
+  if (int rc = plan_persistent((const void*)kernel, kNT, (size_t)S.nrows * kNT * sizeof(Dual64), ngroups, stream, pl)) return rc;
+  kernel<<<pl.grid, pl.block, pl.smem, stream>>>(*Mp, a);
+  return api_launched(&pl);
 }
 
 // ---- Munthe-Kaas RK4 (rbd_integrate): elementwise stage kernels around the dynamics kernels -----------------------------
@@ -802,8 +775,6 @@ __global__ void __launch_bounds__(128) integrate_stage_kernel(const __grid_const
 // Revolute / prismatic joints (the bulk of a robot): q_s = q0 + wa phid_prev, v_s = v0 + wa vd_prev, phid = v_s -- plain row
 // arithmetic, done VEC samples per thread with 16-byte accesses so that enough loads are in flight to approach the HBM rate (the
 // per-(sample, joint) kernel above is latency-bound: too few loads in flight per thread).
-template <class T> struct VecOf { using type = float4; static constexpr int N = 4; };
-template <> struct VecOf<double> { using type = double2; static constexpr int N = 2; };
 template <class T> __device__ __forceinline__ void vec_axpy(const typename VecOf<T>::type& a, T w, const typename VecOf<T>::type& x,
                                                             typename VecOf<T>::type& o);
 template <> __device__ __forceinline__ void vec_axpy<float>(const float4& a, float w, const float4& x, float4& o) {
@@ -924,13 +895,12 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
   const HostModel& hm = model->hm;
   const ModelDev<T>& M = dev_model<T>(hm);
   DeviceProps p;
-  if (int rc = get_props(p)) return rc;
+  RBD_CUDA_TRY(device_props(p));
   const size_t nq = hm.nq, nv = hm.nv;
   const size_t rows = 2 * nq + 10 * nv + (tau && ld != B ? nv : 0);
-  T* ws = nullptr;
-  CUDA_TRY(cudaMallocAsync((void**)&ws, rows * (size_t)B * sizeof(T), stream));
-  struct Guard { void* p; cudaStream_t s; ~Guard() { if (p) cudaFreeAsync(p, s); } } guard{ws, stream};    // freed on every exit path
-  T* q0 = ws; T* qs = q0 + nq * B; T* v0 = qs + nq * B; T* vs = v0 + nv * B;
+  StreamAlloc work;
+  RBD_CUDA_TRY(work.alloc(rows * (size_t)B * sizeof(T), stream));
+  T* q0 = (T*)work.p; T* qs = q0 + nq * B; T* v0 = qs + nq * B; T* vs = v0 + nv * B;
   T* phid[4]; T* vd[4];
   for (int i = 0; i < 4; ++i) { phid[i] = vs + (size_t)(1 + i) * nv * B; vd[i] = vs + (size_t)(5 + i) * nv * B; }
   T* taud = vs + (size_t)9 * nv * B;
@@ -950,7 +920,7 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
   auto tau_at = [&](int s_, int i_) -> const T* { return tau ? (const T*)tau + (size_t)s_ * step_stride + (size_t)i_ * stage_stride : nullptr; };
   const T* tau_dense = (const T*)tau;
   if (tau && ld != B && !varying) {
-    CUDA_TRY(cudaMemcpy2DAsync(taud, B * sizeof(T), tau, ld * sizeof(T), B * sizeof(T), nv, cudaMemcpyDeviceToDevice, stream));
+    RBD_CUDA_TRY(cudaMemcpy2DAsync(taud, B * sizeof(T), tau, ld * sizeof(T), B * sizeof(T), nv, cudaMemcpyDeviceToDevice, stream));
     tau_dense = taud;
   }
   const int grid = (int)std::min<int64_t>((B + 127) / 128, (int64_t)p.sms * 8);
@@ -963,62 +933,54 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
   bool has_other = false;
   for (int i = 0; i < hm.nb; ++i) has_other |= (M.body[i].kind != K_REV && M.body[i].kind != K_PRIS && M.body[i].kind != K_FIXED);
   const double a[4] = {0.0, 0.5, 0.5, 1.0}, bw[4] = {1.0 / 6, 1.0 / 3, 1.0 / 3, 1.0 / 6};   // runge_kutta_4, ode_integrators.jl:48-55
-  int rc = RBD_OK, launches = 0;
   // (q0, v0): dense copies of the state at the start of the step; the finishing kernel of step s refreshes them for step s + 1
-  CUDA_TRY(cudaMemcpy2DAsync(q0, B * sizeof(T), q, ld * sizeof(T), B * sizeof(T), nq, cudaMemcpyDeviceToDevice, stream));
-  CUDA_TRY(cudaMemcpy2DAsync(v0, B * sizeof(T), v, ld * sizeof(T), B * sizeof(T), nv, cudaMemcpyDeviceToDevice, stream));
+  RBD_CUDA_TRY(cudaMemcpy2DAsync(q0, B * sizeof(T), q, ld * sizeof(T), B * sizeof(T), nq, cudaMemcpyDeviceToDevice, stream));
+  RBD_CUDA_TRY(cudaMemcpy2DAsync(v0, B * sizeof(T), v, ld * sizeof(T), B * sizeof(T), nv, cudaMemcpyDeviceToDevice, stream));
   if (traj_q) {
-    CUDA_TRY(cudaMemcpyAsync(traj_q, q0, nq * B * sizeof(T), cudaMemcpyDeviceToDevice, stream));
-    CUDA_TRY(cudaMemcpyAsync(traj_v, v0, nv * B * sizeof(T), cudaMemcpyDeviceToDevice, stream));
+    RBD_CUDA_TRY(cudaMemcpyAsync(traj_q, q0, nq * B * sizeof(T), cudaMemcpyDeviceToDevice, stream));
+    RBD_CUDA_TRY(cudaMemcpyAsync(traj_v, v0, nv * B * sizeof(T), cudaMemcpyDeviceToDevice, stream));
   }
-  for (int s = 0; s < nsteps && rc == RBD_OK; ++s) {
-    for (int i = 0; i < 4 && rc == RBD_OK; ++i) {
+  for (int s = 0; s < nsteps; ++s) {
+    for (int i = 0; i < 4; ++i) {
       if (varying) {
         tau_dense = tau_at(s, i);
         if (tau && ld != B) {
-          CUDA_TRY(cudaMemcpy2DAsync(taud, B * sizeof(T), tau_dense, ld * sizeof(T), B * sizeof(T), nv, cudaMemcpyDeviceToDevice, stream));
+          RBD_CUDA_TRY(cudaMemcpy2DAsync(taud, B * sizeof(T), tau_dense, ld * sizeof(T), B * sizeof(T), nv, cudaMemcpyDeviceToDevice, stream));
           tau_dense = taud;
         }
       }
       StageArgs<T> sa{q0, v0, i ? phid[i - 1] : nullptr, i ? vd[i - 1] : nullptr, phid[i], qsi[i], vsi[i], (T)(dt * a[i]), B, vec_ok};
       if (vec_ok) {        // revolute / prismatic rows, VEC samples per thread
         integrate_stage_linear_kernel<T><<<dim3(grid_lin, hm.nb), 256, 0, stream>>>(M, sa);
-        CUDA_TRY(cudaGetLastError());
-        launches += 1;
+        if (int rc = api_launched()) return rc;
       }
       if (!vec_ok || has_other) {
         integrate_stage_kernel<T><<<dim3(grid, hm.nb), 128, 0, stream>>>(M, sa);
-        CUDA_TRY(cudaGetLastError());
-        launches += 1;
+        if (int rc = api_launched()) return rc;
       }
-      const int before = g_launch.kernels_launched;
-      rc = dynamics_t<T>(model, B, B, qsi[i], vsi[i], tau_dense, nullptr, vd[i], nullptr, stream);
-      launches += g_launch.kernels_launched - before;
+      if (int rc = dynamics_t<T>(model, B, B, qsi[i], vsi[i], tau_dense, nullptr, vd[i], nullptr, stream)) return rc;
     }
-    if (rc != RBD_OK || stages) break;
+    if (stages) return RBD_OK;
     T* qo = traj_q ? traj_q + (size_t)(s + 1) * nq * B : (T*)q;
     T* vo = traj_v ? traj_v + (size_t)(s + 1) * nv * B : (T*)v;
     FinishArgs<T> fa{q0, v0, {phid[0], phid[1], phid[2], phid[3]}, {vd[0], vd[1], vd[2], vd[3]}, qo, vo,
                      {(T)bw[0], (T)bw[1], (T)bw[2], (T)bw[3]}, (T)dt, B, ldo, s + 1 < nsteps, vec_user};
     if (vec_user) {
       integrate_finish_linear_kernel<T><<<dim3(grid_lin, hm.nb), 256, 0, stream>>>(M, fa);
-      CUDA_TRY(cudaGetLastError());
-      launches += 1;
+      if (int rc = api_launched()) return rc;
     }
     if (!vec_user || has_other) {
       integrate_finish_kernel<T><<<dim3(grid, hm.nb), 128, 0, stream>>>(M, fa);
-      CUDA_TRY(cudaGetLastError());
-      launches += 1;
+      if (int rc = api_launched()) return rc;
     }
   }
-  if (rc == RBD_OK && traj_q && nsteps > 0) {      // the final state into the caller's q / v, as rbd_integrate leaves it
-    CUDA_TRY(cudaMemcpy2DAsync(q, ld * sizeof(T), traj_q + (size_t)nsteps * nq * B, B * sizeof(T), B * sizeof(T), nq,
-                               cudaMemcpyDeviceToDevice, stream));
-    CUDA_TRY(cudaMemcpy2DAsync(v, ld * sizeof(T), traj_v + (size_t)nsteps * nv * B, B * sizeof(T), B * sizeof(T), nv,
-                               cudaMemcpyDeviceToDevice, stream));
+  if (traj_q && nsteps > 0) {      // the final state into the caller's q / v, as rbd_integrate leaves it
+    RBD_CUDA_TRY(cudaMemcpy2DAsync(q, ld * sizeof(T), traj_q + (size_t)nsteps * nq * B, B * sizeof(T), B * sizeof(T), nq,
+                                   cudaMemcpyDeviceToDevice, stream));
+    RBD_CUDA_TRY(cudaMemcpy2DAsync(v, ld * sizeof(T), traj_v + (size_t)nsteps * nv * B, B * sizeof(T), B * sizeof(T), nv,
+                                   cudaMemcpyDeviceToDevice, stream));
   }
-  g_launch.kernels_launched = launches;
-  return rc;
+  return RBD_OK;
 }
 
 // rbd_dynamics_gather.  Fast path: the model-specialised kernels store v̇ straight into every GPU's gathered array (peer-mapped
@@ -1055,43 +1017,34 @@ int dynamics_gather_t(const rbd_model* model, int64_t B, int64_t ld, const void*
     SpecKey key; key.algo = SPEC_ABA; key.f64 = sizeof(T) == 8; key.has_in2 = tau != nullptr; key.peers = true;
     SpecLaunchArgs sa{q, v, tau, nullptr, nullptr, ld, B};
     sa.peers = peers; sa.npeers = npeers; sa.peer_ld = peer_ld; sa.peer_col0 = col0; sa.mc = mc;
-    std::string err;
-    if (int rc = spec_try_launch(const_cast<rbd_model*>(model), key, sa, stream, used, g_launch, &gate, err)) return fail(rc, err);
-    if (used) g_launch.specialised = 1;
+    if (int rc = spec_try_launch(const_cast<rbd_model*>(model), key, sa, stream, used, &gate)) return rc;
     if (used && !gate) return RBD_OK;
   }
-  const rbd_launch_info keep = g_launch;
   // the generic kernels use ONE leading dimension for inputs and outputs, so the scratch is [nv x ld]
-  T* scratch = nullptr;
-  CUDA_TRY(cudaMallocAsync((void**)&scratch, (size_t)hm.nv * (size_t)ld * sizeof(T), stream));
-  int rc;
+  StreamAlloc scratch_;
+  RBD_CUDA_TRY(scratch_.alloc((size_t)hm.nv * (size_t)ld * sizeof(T), stream));
+  T* scratch = (T*)scratch_.p;
+  std::optional<KeepLaunchRecord> keep;      // behind the specialised kernel: gated generic fallback, see dynamics_t
   if (!used) {
-    rc = dynamics_t<T>(model, B, ld, q, v, tau, nullptr, scratch, nullptr, stream);
+    if (int rc = dynamics_t<T>(model, B, ld, q, v, tau, nullptr, scratch, nullptr, stream)) return rc;
   } else {
+    keep.emplace();
     AbaArgs<T> a{(const T*)q, (const T*)v, (const T*)tau, nullptr, scratch, nullptr, nullptr, ld, B};
     a.gate = gate;
     bool other_kinds = false;
     for (int i = 0; i < hm.nb; ++i) other_kinds |= (M.body[i].kind == K_PRIS || M.body[i].kind == K_FIXED);
     const int rows = M.nrows;
-#define RBD_ABA_G(G, K) launch<T>(aba_kernel<T, kNT, G, false, K>, M, a, kNT, rows, 0, stream)
-    rc = hm.general ? RBD_ABA_G(true, kAllKinds) : (other_kinds ? RBD_ABA_G(false, kAllKinds) : RBD_ABA_G(false, 0));
+#define RBD_ABA_G(G, K) launch<T>(aba_kernel<T, kNT, G, false, K>, M, a, rows, stream)
+    if (int rc = hm.general ? RBD_ABA_G(true, kAllKinds) : (other_kinds ? RBD_ABA_G(false, kAllKinds) : RBD_ABA_G(false, 0))) return rc;
 #undef RBD_ABA_G
   }
-  if (rc == RBD_OK) {
-    ScatterArgs<T> sc{};
-    sc.src = scratch; sc.src_ld = ld; sc.dst_ld = peer_ld; sc.ndst = npeers; sc.rows = hm.nv; sc.B = B; sc.gate = gate;
-    for (int p = 0; p < npeers; ++p) sc.dst[p] = (T*)peers[p] + col0;
-    DeviceProps p;
-    if ((rc = get_props(p)) == RBD_OK) {
-      gather_scatter_kernel<T><<<p.sms * 8, 256, 0, stream>>>(sc);
-      if (cudaGetLastError() != cudaSuccess) rc = fail(RBD_ECUDA, "gather_scatter_kernel launch failed");
-      g_launch.kernels_launched += 1;
-    }
-  }
-  cudaFreeAsync(scratch, stream);
-  const int n = g_launch.kernels_launched;
-  if (used) { g_launch = keep; g_launch.kernels_launched = n; }
-  return rc;
+  ScatterArgs<T> sc{};
+  sc.src = scratch; sc.src_ld = ld; sc.dst_ld = peer_ld; sc.ndst = npeers; sc.rows = hm.nv; sc.B = B; sc.gate = gate;
+  for (int p = 0; p < npeers; ++p) sc.dst[p] = (T*)peers[p] + col0;
+  DeviceProps p;
+  RBD_CUDA_TRY(device_props(p));
+  gather_scatter_kernel<T><<<p.sms * 8, 256, 0, stream>>>(sc);
+  return api_launched();
 }
 
 template <class T>
@@ -1100,19 +1053,12 @@ int bodies_t(const rbd_model* model, int64_t B, int64_t ld, const void* q, const
   const HostModel& hm = model->hm;
   const ModelDev<T>& M = dev_model<T>(hm);
   BodiesArgs<T> a{(const T*)q, (const T*)v, (const T*)vd, (const T*)wext, (T*)acc, (T*)jw, ld, B};
-  DeviceProps p;
-  if (int rc = get_props(p)) return rc;
   auto kernel = bodies_kernel<T, kNT>;
-  const size_t smem = (size_t)std::max(1, kin_rows(hm)) * kNT * sizeof(T);
-  int bps = 0;
-  if (int rc = configure(kernel, kNT, smem, p, bps)) return rc;
-  const int64_t ngroups = (B + kNT - 1) / kNT;
-  const int grid = (int)std::min<int64_t>(ngroups, (int64_t)bps * p.sms);
-  kernel<<<grid, kNT, smem, stream>>>(M, a);
-  if (cudaGetLastError() != cudaSuccess) return fail(RBD_ECUDA, "bodies_kernel launch failed");
-  g_launch.kernels_launched += 1;
-  g_launch.grid = grid; g_launch.block = kNT; g_launch.smem_bytes = (int)smem; g_launch.blocks_per_sm = bps;
-  return RBD_OK;
+  LaunchPlan pl;
+  if (int rc = plan_persistent((const void*)kernel, kNT, (size_t)std::max(1, kin_rows(hm)) * kNT * sizeof(T), (B + kNT - 1) / kNT,
+                               stream, pl)) return rc;
+  kernel<<<pl.grid, pl.block, pl.smem, stream>>>(M, a);
+  return api_launched(&pl);
 }
 
 template <class T>
@@ -1123,19 +1069,12 @@ int contact_t(const rbd_model* model, int64_t B, int64_t ld, const void* q, cons
   ContactDev<T> C;
   build_contact_dev<T>(hm.nb, hm.pos.data(), hm.alignT.data(), cd, C);
   ContactArgs<T> a{(const T*)q, (const T*)v, (T*)sx, (T*)sd, (T*)wr, ld, B};
-  DeviceProps p;
-  if (int rc = get_props(p)) return rc;
   auto kernel = contact_kernel<T, kNT>;
-  const size_t smem = (size_t)std::max(1, kin_rows(hm)) * kNT * sizeof(T);
-  int bps = 0;
-  if (int rc = configure(kernel, kNT, smem, p, bps)) return rc;
-  const int64_t ngroups = (B + kNT - 1) / kNT;
-  const int grid = (int)std::min<int64_t>(ngroups, (int64_t)bps * p.sms);
-  kernel<<<grid, kNT, smem, stream>>>(M, C, a);
-  if (cudaGetLastError() != cudaSuccess) return fail(RBD_ECUDA, "contact_kernel launch failed");
-  g_launch.kernels_launched += 1;
-  g_launch.grid = grid; g_launch.block = kNT; g_launch.smem_bytes = (int)smem; g_launch.blocks_per_sm = bps;
-  return RBD_OK;
+  LaunchPlan pl;
+  if (int rc = plan_persistent((const void*)kernel, kNT, (size_t)std::max(1, kin_rows(hm)) * kNT * sizeof(T), (B + kNT - 1) / kNT,
+                               stream, pl)) return rc;
+  kernel<<<pl.grid, pl.block, pl.smem, stream>>>(M, C, a);
+  return api_launched(&pl);
 }
 
 int check_common(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, bool allow_dual = false) {
@@ -1150,14 +1089,9 @@ int check_common(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, b
 
 }  // namespace
 
-// hooks for the other translation units of the library (rbd_deriv.cu): per-thread error text, argument checks, launch statistics
+// hooks for the other translation units of the library: argument checks, the RK4 driver
 namespace rbd {
-int api_fail(int status, const std::string& msg) { return fail(status, msg); }
 int api_check(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld) { return check_common(model, dtype, B, ld); }
-void api_note_launch(int grid, int block, int smem_bytes, int blocks_per_sm) {
-  g_launch.kernels_launched += 1;
-  g_launch.grid = grid; g_launch.block = block; g_launch.smem_bytes = smem_bytes; g_launch.blocks_per_sm = blocks_per_sm;
-}
 int integrate_record(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, const void* tau, int64_t step_stride,
                      int64_t stage_stride, double dt, int nsteps, void* q_traj, void* v_traj, void* stages, cudaStream_t stream) {
   return dtype == RBD_F32 ? integrate_t<float>(model, B, ld, q, v, tau, step_stride, stage_stride, dt, nsteps, stream, (float*)q_traj,
@@ -1173,7 +1107,7 @@ int integrate_record(const rbd_model* model, int32_t dtype, int64_t B, int64_t l
 int32_t rbd_kinematics(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                        const int8_t* path_sign, const rbd_kinematics_out* out, void* stream) {
   if (int rc = check_common(model, dtype, B, ld)) return rc;
-  g_launch = {0, 0, 0, 0, 0, 0.f, 0};
+  const ApiCall call;
   if (dtype != RBD_F32 && dtype != RBD_F64) return fail(RBD_EUNSUPPORTED, "rbd_kinematics: fp32 and fp64 only");
   if (!out) return fail(RBD_EINVAL, "rbd_kinematics: out must not be NULL");
   if (B == 0) return RBD_OK;      // empty batch: nothing to read or write, pointers may be NULL
@@ -1197,13 +1131,13 @@ constexpr int64_t kChunk = 1 << 16;
 
 int ensure_staging(rbd_model* m, size_t bytes_per_stream) {
   for (int i = 0; i < 3; ++i)
-    if (!m->streams[i]) CUDA_TRY(cudaStreamCreateWithFlags(&m->streams[i], cudaStreamNonBlocking));
-  if (!m->ev0) { CUDA_TRY(cudaEventCreate(&m->ev0)); CUDA_TRY(cudaEventCreate(&m->ev1)); }
+    if (!m->streams[i]) RBD_CUDA_TRY(cudaStreamCreateWithFlags(&m->streams[i], cudaStreamNonBlocking));
+  if (!m->ev0) { RBD_CUDA_TRY(cudaEventCreate(&m->ev0)); RBD_CUDA_TRY(cudaEventCreate(&m->ev1)); }
   if (m->stage_bytes >= bytes_per_stream) return RBD_OK;
   m->stage_bytes = 0;               // a failed reallocation must not leave a stale size behind
   for (int i = 0; i < 3; ++i) {
     if (m->d_stage[i]) { cudaFree(m->d_stage[i]); m->d_stage[i] = nullptr; }
-    CUDA_TRY(cudaMalloc(&m->d_stage[i], bytes_per_stream));
+    RBD_CUDA_TRY(cudaMalloc(&m->d_stage[i], bytes_per_stream));
   }
   m->stage_bytes = bytes_per_stream;
   return RBD_OK;
@@ -1212,7 +1146,7 @@ int ensure_staging(rbd_model* m, size_t bytes_per_stream) {
 // copy rows x C block between a host array with leading dimension ld and a dense device tile (leading dimension C)
 int copy_rows(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, int rows, cudaMemcpyKind kind,
               cudaStream_t s) {
-  CUDA_TRY(cudaMemcpy2DAsync(dst, dpitch, src, spitch, width, rows, kind, s));
+  RBD_CUDA_TRY(cudaMemcpy2DAsync(dst, dpitch, src, spitch, width, rows, kind, s));
   return RBD_OK;
 }
 }  // namespace
@@ -1238,15 +1172,12 @@ template <class Launch>
 int host_pipeline_impl(rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const HostArr* ins, int nin, const HostArr* outs,
                        int nout, Launch launch_chunk) {
   const size_t es = dtype == RBD_F32 ? 4 : 8;
-  int64_t chunk = kChunk;
-  if (const char* e = getenv("RBD_HOST_CHUNK")) chunk = std::max<int64_t>(1024, atoll(e));     // tuning knob
-  const int64_t C = std::min<int64_t>(chunk, B);
+  const int64_t C = std::min<int64_t>(kChunk, B);
   size_t rows_total = 0;
   for (int i = 0; i < nin; ++i) rows_total += ins[i].in ? ins[i].rows : 0;
   for (int i = 0; i < nout; ++i) rows_total += outs[i].out ? outs[i].rows : 0;
   if (int rc = ensure_staging(model, rows_total * C * es)) return rc;
-  int launches = 0, nchunk = 0;
-  rbd_launch_info last = g_launch;
+  int nchunk = 0;
   for (int64_t b0 = 0; b0 < B; b0 += C, ++nchunk) {
     const int64_t n = std::min<int64_t>(C, B - b0);
     const int si = nchunk % 3;
@@ -1267,16 +1198,12 @@ int host_pipeline_impl(rbd_model* model, int32_t dtype, int64_t B, int64_t ld, c
       cur += (size_t)outs[i].rows * C * es;
     }
     if (int rc = launch_chunk(n, C, din, dout, s)) return rc;
-    launches += g_launch.kernels_launched;
-    last = g_launch;
     for (int i = 0; i < nout; ++i) {
       if (!outs[i].out) continue;
       if (int rc = copy_rows((char*)outs[i].out + off, ld * es, dout[i], C * es, n * es, outs[i].rows, cudaMemcpyDeviceToHost, s)) return rc;
     }
   }
-  for (int i = 0; i < 3; ++i) CUDA_TRY(cudaStreamSynchronize(model->streams[i]));
-  g_launch = last;
-  g_launch.kernels_launched = launches;
+  for (int i = 0; i < 3; ++i) RBD_CUDA_TRY(cudaStreamSynchronize(model->streams[i]));
   return RBD_OK;
 }
 }  // namespace
@@ -1391,7 +1318,7 @@ int32_t rbd_model_precompile(rbd_model* model, int32_t dtype, int32_t what, int3
 int32_t rbd_dynamics(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                      const void* tau, const void* wext, void* vd_out, void* qd_out, void* stream) {
   if (int rc = check_common(model, dtype, B, ld, true)) return rc;
-  g_launch = {0, 0, 0, 0, 0, 0.f, 0};
+  const ApiCall call;
   if (B == 0) return RBD_OK;      // empty batch: nothing to read or write, pointers may be NULL
   if (!q || !v || !vd_out) return fail(RBD_EINVAL, "rbd_dynamics: q, v and vd_out must not be NULL");
   cudaStream_t s = (cudaStream_t)stream;
@@ -1407,7 +1334,7 @@ int32_t rbd_dynamics_gather(const rbd_model* model, int32_t dtype, int64_t B, in
                             const void* tau, int32_t npeers, void* const* vd_peers, void* vd_multicast, int64_t peer_ld, int64_t col0,
                             void* stream) {
   if (int rc = check_common(model, dtype, B, ld)) return rc;
-  g_launch = {0, 0, 0, 0, 0, 0.f, 0};
+  const ApiCall call;
   if (npeers < 1 || npeers > 8 || !vd_peers) return fail(RBD_EINVAL, "rbd_dynamics_gather: need 1..8 peer arrays");
   for (int p = 0; p < npeers; ++p) if (!vd_peers[p]) return fail(RBD_EINVAL, "rbd_dynamics_gather: NULL peer array");
   if (col0 < 0 || peer_ld < col0 + B) return fail(RBD_EDIM, "rbd_dynamics_gather: columns [col0, col0 + B) exceed the gathered array");
@@ -1423,7 +1350,7 @@ int32_t rbd_integrate_schedule(const rbd_model* model, int32_t dtype, int64_t B,
   if (int rc = check_common(model, dtype, B, ld)) return rc;
   if (nsteps < 0 || !(dt > 0)) return fail(RBD_EINVAL, "rbd_integrate: need dt > 0 and nsteps >= 0");
   if (tau_step_stride < 0 || tau_stage_stride < 0) return fail(RBD_EINVAL, "rbd_integrate: torque strides must be >= 0");
-  g_launch = {0, 0, 0, 0, 0, 0.f, 0};
+  const ApiCall call;
   if (B == 0 || nsteps == 0) return RBD_OK;
   if (!q || !v) return fail(RBD_EINVAL, "rbd_integrate: q and v must not be NULL");
   cudaStream_t s = (cudaStream_t)stream;
@@ -1442,7 +1369,7 @@ int32_t rbd_integrate_trajectory(const rbd_model* model, int32_t dtype, int64_t 
   if (int rc = check_common(model, dtype, B, ld)) return rc;
   if (nsteps < 0 || !(dt > 0)) return fail(RBD_EINVAL, "rbd_integrate_trajectory: need dt > 0 and nsteps >= 0");
   if (tau_step_stride < 0 || tau_stage_stride < 0) return fail(RBD_EINVAL, "rbd_integrate_trajectory: torque strides must be >= 0");
-  g_launch = {0, 0, 0, 0, 0, 0.f, 0};
+  const ApiCall call;
   if (B == 0) return RBD_OK;
   if (!q || !v || !q_traj || !v_traj) return fail(RBD_EINVAL, "rbd_integrate_trajectory: q, v, q_traj and v_traj must not be NULL");
   return rbd::integrate_record(model, dtype, B, ld, q, v, tau, tau_step_stride, tau_stage_stride, dt, nsteps, q_traj, v_traj, nullptr,
@@ -1452,7 +1379,7 @@ int32_t rbd_integrate_trajectory(const rbd_model* model, int32_t dtype, int64_t 
 int32_t rbd_inverse_dynamics(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q,
                              const void* v, const void* vd, const void* wext, void* tau_out, void* stream) {
   if (int rc = check_common(model, dtype, B, ld)) return rc;
-  g_launch = {0, 0, 0, 0, 0, 0.f, 0};
+  const ApiCall call;
   if (B == 0) return RBD_OK;      // empty batch: nothing to read or write, pointers may be NULL
   if (!q || !v || !vd || !tau_out) return fail(RBD_EINVAL, "rbd_inverse_dynamics: q, v, vd and tau_out must not be NULL");
   cudaStream_t s = (cudaStream_t)stream;
@@ -1463,7 +1390,7 @@ int32_t rbd_inverse_dynamics(const rbd_model* model, int32_t dtype, int64_t B, i
 int32_t rbd_inverse_dynamics_bodies(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                                     const void* vd, const void* wext, void* accelerations_out, void* jointwrenches_out, void* stream) {
   if (int rc = check_common(model, dtype, B, ld)) return rc;
-  g_launch = {0, 0, 0, 0, 0, 0.f, 0};
+  const ApiCall call;
   if (B == 0 || (!accelerations_out && !jointwrenches_out)) return RBD_OK;
   if (!q || !v) return fail(RBD_EINVAL, "rbd_inverse_dynamics_bodies: q and v must not be NULL");
   cudaStream_t s = (cudaStream_t)stream;
@@ -1474,7 +1401,7 @@ int32_t rbd_inverse_dynamics_bodies(const rbd_model* model, int32_t dtype, int64
 int32_t rbd_contact_dynamics(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                              const rbd_contact_desc* contact, void* state, void* state_deriv_out, void* wrenches_out, void* stream) {
   if (int rc = check_common(model, dtype, B, ld)) return rc;
-  g_launch = {0, 0, 0, 0, 0, 0.f, 0};
+  const ApiCall call;
   if (!contact) return fail(RBD_EINVAL, "rbd_contact_dynamics: contact must not be NULL");
   if (contact->npoints < 0 || contact->nhalfspaces < 0) return fail(RBD_EINVAL, "rbd_contact_dynamics: negative counts");
   if (contact->npoints > kMaxContactPoints || contact->nhalfspaces > kMaxHalfSpaces)
@@ -1500,26 +1427,23 @@ int32_t rbd_contact_dynamics(const rbd_model* model, int32_t dtype, int64_t B, i
 int32_t rbd_dynamics_result(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                             const void* tau, const void* wext, void* vd_out, void* qd_out, void* M_out, void* c_out,
                             void* accelerations_out, void* jointwrenches_out, void* stream) {
+  const ApiCall call;
   int rc = rbd_dynamics(model, dtype, B, ld, q, v, tau, wext, vd_out, qd_out, stream);
   if (rc != RBD_OK || B == 0) return rc;
   if (dtype == RBD_DUAL64X6 && (M_out || c_out || accelerations_out || jointwrenches_out))
     return fail(RBD_EUNSUPPORTED, "rbd_dynamics_result: by-products are fp32 / fp64 only");
-  rbd_launch_info acc = g_launch;
-  auto merge = [&]() { acc.kernels_launched += g_launch.kernels_launched; };
-  if (c_out) { if ((rc = rbd_dynamics_bias(model, dtype, B, ld, q, v, wext, c_out, stream)) != RBD_OK) return rc; merge(); }
-  if (M_out) { if ((rc = rbd_mass_matrix(model, dtype, B, ld, q, M_out, stream)) != RBD_OK) return rc; merge(); }
-  if (accelerations_out || jointwrenches_out) {
-    if ((rc = rbd_inverse_dynamics_bodies(model, dtype, B, ld, q, v, vd_out, wext, accelerations_out, jointwrenches_out, stream)) != RBD_OK) return rc;
-    merge();
-  }
-  g_launch = acc;
+  const KeepLaunchRecord keep;      // the record describes the dynamics kernel; the by-products add their launches
+  if (c_out && (rc = rbd_dynamics_bias(model, dtype, B, ld, q, v, wext, c_out, stream)) != RBD_OK) return rc;
+  if (M_out && (rc = rbd_mass_matrix(model, dtype, B, ld, q, M_out, stream)) != RBD_OK) return rc;
+  if (accelerations_out || jointwrenches_out)
+    return rbd_inverse_dynamics_bodies(model, dtype, B, ld, q, v, vd_out, wext, accelerations_out, jointwrenches_out, stream);
   return RBD_OK;
 }
 
 int32_t rbd_dynamics_bias(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q,
                           const void* v, const void* wext, void* c_out, void* stream) {
   if (int rc = check_common(model, dtype, B, ld)) return rc;
-  g_launch = {0, 0, 0, 0, 0, 0.f, 0};
+  const ApiCall call;
   if (B == 0) return RBD_OK;      // empty batch: nothing to read or write, pointers may be NULL
   if (!q || !v || !c_out) return fail(RBD_EINVAL, "rbd_dynamics_bias: q, v and c_out must not be NULL");
   cudaStream_t s = (cudaStream_t)stream;
@@ -1530,7 +1454,7 @@ int32_t rbd_dynamics_bias(const rbd_model* model, int32_t dtype, int64_t B, int6
 int32_t rbd_mass_matrix_uplo(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, void* M_out,
                              int32_t uplo, void* stream) {
   if (int rc = check_common(model, dtype, B, ld)) return rc;
-  g_launch = {0, 0, 0, 0, 0, 0.f, 0};
+  const ApiCall call;
   if (uplo != RBD_UPLO_FULL && uplo != RBD_UPLO_LOWER) return fail(RBD_EINVAL, "rbd_mass_matrix: uplo must be RBD_UPLO_FULL or RBD_UPLO_LOWER");
   if (B == 0) return RBD_OK;      // empty batch: nothing to read or write, pointers may be NULL
   if (!q || !M_out) return fail(RBD_EINVAL, "rbd_mass_matrix: q and M_out must not be NULL");
@@ -1550,7 +1474,7 @@ int32_t rbd_mass_matrix(const rbd_model* model, int32_t dtype, int64_t B, int64_
 int32_t rbd_dynamics_host(rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                           const void* tau, const void* wext, void* vd_out, void* qd_out) {
   if (int rc = check_common(model, dtype, B, ld)) return rc;
-  g_launch = {0, 0, 0, 0, 0, 0.f, 0};
+  const ApiCall call;
   if (B == 0) return RBD_OK;      // empty batch: nothing to read or write, pointers may be NULL
   if (!q || !v || !vd_out) return fail(RBD_EINVAL, "rbd_dynamics_host: q, v and vd_out must not be NULL");
   const HostModel& hm = model->hm;
@@ -1558,7 +1482,6 @@ int32_t rbd_dynamics_host(rbd_model* model, int32_t dtype, int64_t B, int64_t ld
   const HostArr outs[2] = {{nullptr, vd_out, hm.nv}, {nullptr, qd_out, hm.nq}};
   return host_pipeline(model, dtype, B, ld, ins, 4, outs, 2,
                        [&](int64_t n, int64_t C, const void** di, void** dq, cudaStream_t s) {
-                         g_launch.kernels_launched = 0;
                          return dtype == RBD_F32 ? dynamics_t<float>(model, n, C, di[0], di[1], di[2], di[3], dq[0], dq[1], s)
                                                  : dynamics_t<double>(model, n, C, di[0], di[1], di[2], di[3], dq[0], dq[1], s);
                        });
@@ -1567,7 +1490,7 @@ int32_t rbd_dynamics_host(rbd_model* model, int32_t dtype, int64_t B, int64_t ld
 int32_t rbd_inverse_dynamics_host(rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q,
                                   const void* v, const void* vd, const void* wext, void* tau_out) {
   if (int rc = check_common(model, dtype, B, ld)) return rc;
-  g_launch = {0, 0, 0, 0, 0, 0.f, 0};
+  const ApiCall call;
   if (B == 0) return RBD_OK;      // empty batch: nothing to read or write, pointers may be NULL
   if (!q || !v || !vd || !tau_out) return fail(RBD_EINVAL, "rbd_inverse_dynamics_host: q, v, vd and tau_out must not be NULL");
   const HostModel& hm = model->hm;
@@ -1575,7 +1498,6 @@ int32_t rbd_inverse_dynamics_host(rbd_model* model, int32_t dtype, int64_t B, in
   const HostArr outs[1] = {{nullptr, tau_out, hm.nv}};
   return host_pipeline(model, dtype, B, ld, ins, 4, outs, 1,
                        [&](int64_t n, int64_t C, const void** di, void** dq, cudaStream_t s) {
-                         g_launch.kernels_launched = 0;
                          return dtype == RBD_F32 ? inverse_dynamics_t<float>(model, n, C, di[0], di[1], di[2], di[3], dq[0], s)
                                                  : inverse_dynamics_t<double>(model, n, C, di[0], di[1], di[2], di[3], dq[0], s);
                        });
@@ -1584,7 +1506,7 @@ int32_t rbd_inverse_dynamics_host(rbd_model* model, int32_t dtype, int64_t B, in
 int32_t rbd_dynamics_bias_host(rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q,
                                const void* v, const void* wext, void* c_out) {
   if (int rc = check_common(model, dtype, B, ld)) return rc;
-  g_launch = {0, 0, 0, 0, 0, 0.f, 0};
+  const ApiCall call;
   if (B == 0) return RBD_OK;      // empty batch: nothing to read or write, pointers may be NULL
   if (!q || !v || !c_out) return fail(RBD_EINVAL, "rbd_dynamics_bias_host: q, v and c_out must not be NULL");
   const HostModel& hm = model->hm;
@@ -1592,7 +1514,6 @@ int32_t rbd_dynamics_bias_host(rbd_model* model, int32_t dtype, int64_t B, int64
   const HostArr outs[1] = {{nullptr, c_out, hm.nv}};
   return host_pipeline(model, dtype, B, ld, ins, 3, outs, 1,
                        [&](int64_t n, int64_t C, const void** di, void** dq, cudaStream_t s) {
-                         g_launch.kernels_launched = 0;
                          return dtype == RBD_F32 ? inverse_dynamics_t<float>(model, n, C, di[0], di[1], nullptr, di[2], dq[0], s)
                                                  : inverse_dynamics_t<double>(model, n, C, di[0], di[1], nullptr, di[2], dq[0], s);
                        });
@@ -1600,7 +1521,7 @@ int32_t rbd_dynamics_bias_host(rbd_model* model, int32_t dtype, int64_t B, int64
 
 int32_t rbd_mass_matrix_host(rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, void* M_out) {
   if (int rc = check_common(model, dtype, B, ld)) return rc;
-  g_launch = {0, 0, 0, 0, 0, 0.f, 0};
+  const ApiCall call;
   if (B == 0) return RBD_OK;      // empty batch: nothing to read or write, pointers may be NULL
   if (!q || !M_out) return fail(RBD_EINVAL, "rbd_mass_matrix_host: q and M_out must not be NULL");
   const HostModel& hm = model->hm;
@@ -1608,7 +1529,6 @@ int32_t rbd_mass_matrix_host(rbd_model* model, int32_t dtype, int64_t B, int64_t
   const HostArr outs[1] = {{nullptr, M_out, hm.nv * hm.nv}};
   return host_pipeline(model, dtype, B, ld, ins, 1, outs, 1,
                        [&](int64_t n, int64_t C, const void** di, void** dq, cudaStream_t s) {
-                         g_launch.kernels_launched = 0;
                          return dtype == RBD_F32 ? mass_matrix_t<float>(model, n, C, di[0], dq[0], s)
                                                  : mass_matrix_t<double>(model, n, C, di[0], dq[0], s);
                        });

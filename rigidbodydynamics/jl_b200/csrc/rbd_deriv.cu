@@ -10,7 +10,8 @@
 //                        columns in place with its right-hand side in shared memory, [row][lane]
 //   (deriv_factor_kernel one thread per sample, on the scratch: only when M does not fit into shared memory)
 // Intermediates: a global scratch of DerivDev::rows rows per sample, allocated from the stream-ordered pool per call and
-// bounded by RBD_DERIV_SCRATCH_MB (default 2048): larger batches are processed in chunks on the same stream.
+// bounded by RBD_DERIV_SCRATCH_MB (default 2048): larger batches are processed in chunks on the same stream.  The launch record
+// (rbd_handle.h) counts the kernels of every chunk, the forward dynamics included.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -20,7 +21,6 @@
 #include <cstring>
 #include <map>
 #include <mutex>
-#include <set>
 #include <string>
 #include <vector>
 
@@ -38,10 +38,6 @@ using namespace rbd;
 namespace {
 
 constexpr int kNT = 128;
-
-template <class T> const ModelDev<T>& dev_model(const HostModel& m);
-template <> const ModelDev<float>& dev_model<float>(const HostModel& m) { return m.dev32; }
-template <> const ModelDev<double>& dev_model<double>(const HostModel& m) { return m.dev64; }
 
 template <class T> struct DerivArgs {
   const T* q; const T* v; const T* vd;
@@ -148,30 +144,6 @@ __global__ void deriv_solve_kernel(const __grid_constant__ DerivDev D, const __g
   }
 }
 
-struct Props { int dev = 0, sms = 0, max_smem_optin = 0, smem_per_sm = 0; };
-int get_props(Props& p) {
-  if (cudaGetDevice(&p.dev) != cudaSuccess) return api_fail(RBD_ECUDA, "cudaGetDevice failed");
-  cudaDeviceGetAttribute(&p.sms, cudaDevAttrMultiProcessorCount, p.dev);
-  cudaDeviceGetAttribute(&p.max_smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, p.dev);
-  cudaDeviceGetAttribute(&p.smem_per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, p.dev);
-  return RBD_OK;
-}
-// opt a kernel into large dynamic shared memory once per (kernel, device)
-int big_smem_once(const void* kernel, const Props& p) {
-  static std::mutex mu;
-  static std::set<std::pair<const void*, int>> done;
-  std::lock_guard<std::mutex> lk(mu);
-  if (done.count({kernel, p.dev})) return RBD_OK;
-  cudaFuncAttributes fa{};
-  if (cudaFuncGetAttributes(&fa, kernel) != cudaSuccess ||
-      cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, p.max_smem_optin - (int)fa.sharedSizeBytes) != cudaSuccess)
-    return api_fail(RBD_ECUDA, std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(cudaGetLastError()));
-  cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  done.insert({kernel, p.dev});
-  return RBD_OK;
-}
-#define LAUNCH_CHECK(name) do { cudaError_t e_ = cudaGetLastError(); if (e_ != cudaSuccess) { rc = api_fail(RBD_ECUDA, std::string(name " launch failed: ") + cudaGetErrorString(e_)); goto done; } } while (0)
-
 // ---- model-specialised solve kernel (rbd_deriv_jit.cpp): compiled with NVRTC on the first large call (or ahead of time by
 // rbd_model_precompile_derivatives), cubin cached on disk, module cached per (tables, dtype, device) ----
 struct JitSolve {
@@ -208,7 +180,7 @@ bool jit_solve_cubin(const DerivDev& D, const DerivAnc& A, bool f64, bool compil
   bool from_cache = false;
   return jit_compile_text(f64 ? "deriv_f64" : "deriv_f32", src, true, cubin, compile, &from_cache, err);
 }
-JitSolve* jit_solve_get(const DerivDev& D, const DerivAnc& A, bool f64, int64_t B, const Props& p) {
+JitSolve* jit_solve_get(const DerivDev& D, const DerivAnc& A, bool f64, int64_t B, const DeviceProps& p) {
   if (!jit_enabled()) return nullptr;
   std::string key((const char*)&D, sizeof(D));
   key.append((const char*)A.anc, sizeof(int16_t) * D.nnz);
@@ -254,20 +226,18 @@ int derivatives_t(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, 
   if (!build_deriv_dev(M, D, A))
     return api_fail(RBD_EUNSUPPORTED, "rbd_dynamics_derivatives: more than 128 velocity coordinates or 4096 mass-matrix entries");
   if (D.nv == 0) return RBD_OK;        // nothing to differentiate (only fixed joints): no outputs have any rows
-  Props p;
-  if (int rc = get_props(p)) return rc;
+  DeviceProps p;
+  RBD_CUDA_TRY(device_props(p));
   // chunk size from the scratch budget
   int64_t budget_mb = 2048;
   if (const char* e = std::getenv("RBD_DERIV_SCRATCH_MB")) budget_mb = std::max<int64_t>(1, std::atoll(e));
   const int64_t per_sample = (int64_t)D.rows * (int64_t)sizeof(T);
   int64_t C = std::min<int64_t>(B, std::max<int64_t>(kNT, (budget_mb << 20) / per_sample / kNT * kNT));
   const int64_t sld = (C + 31) / 32 * 32;
-  T* scratch = nullptr;
-  if (cudaMallocAsync((void**)&scratch, (size_t)per_sample * sld, stream) != cudaSuccess) {
-    cudaGetLastError();
-    return api_fail(RBD_ENOMEM, "rbd_dynamics_derivatives: scratch allocation failed (lower RBD_DERIV_SCRATCH_MB)");
-  }
-  int rc = RBD_OK;
+  StreamAlloc scratch_;
+  if (cudaError_t e = scratch_.alloc((size_t)per_sample * sld, stream))
+    return api_fail_cuda(e, "rbd_dynamics_derivatives: scratch allocation (lower RBD_DERIV_SCRATCH_MB)");
+  T* scratch = (T*)scratch_.p;
   // solve kernel geometry: warps per block so that factor + right-hand sides fit, maximising resident warps
   const size_t hbytes = (size_t)D.nnz * 32 * sizeof(T), xbytes = (size_t)D.nv * 32 * sizeof(T);
   int bestW = 0, bestNb = 0;
@@ -290,52 +260,44 @@ int derivatives_t(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, 
   auto kworld = deriv_world_kernel<T, kNT>;
   auto ksolve_s = deriv_solve_kernel<T, true>;
   auto ksolve_g = deriv_solve_kernel<T, false>;
-  if ((rc = big_smem_once((const void*)kworld, p)) != RBD_OK) goto done;
-  if ((rc = big_smem_once(hs ? (const void*)ksolve_s : (const void*)ksolve_g, p)) != RBD_OK) goto done;
-  if (world_smem > (size_t)p.max_smem_optin) { rc = api_fail(RBD_EUNSUPPORTED, "rbd_dynamics_derivatives: too many open branch nodes"); goto done; }
+  int bps_world = 0, bps_solve = 0;
+  if (int rc = kernel_config((const void*)kworld, kNT, world_smem, p, bps_world)) return rc;
+  if (int rc = kernel_config(hs ? (const void*)ksolve_s : (const void*)ksolve_g, 32 * bestW, solve_smem, p, bps_solve)) return rc;
   for (int64_t b0 = 0; b0 < B; b0 += C) {
     const int64_t c = std::min<int64_t>(C, B - b0);
     T* vd = vd_out + b0;
     // v̇ itself: the library's own forward dynamics (model-specialised kernels when available)
-    if ((rc = rbd_dynamics(model, dtype, c, ld, q + b0, v + b0, tau ? tau + b0 : nullptr, nullptr, vd, nullptr, stream)) != RBD_OK) goto done;
+    if (int rc = rbd_dynamics(model, dtype, c, ld, q + b0, v + b0, tau ? tau + b0 : nullptr, nullptr, vd, nullptr, stream)) return rc;
     DerivArgs<T> a{q + b0, v + b0, vd, dq + b0, dv + b0, scratch, ld, sld, c};
     const int gx = (int)((c + kNT - 1) / kNT);
-    kworld<<<std::min(gx, 8 * p.sms), kNT, world_smem, stream>>>(M, D, a);
-    LAUNCH_CHECK("deriv_world_kernel");
-    api_note_launch(gx, kNT, (int)world_smem, 0);
+    const LaunchShape world{std::min(gx, 8 * p.sms), kNT, (int)world_smem}, accum{gx * kBodyRows, kNT}, pairs{gx * D.nb, kNT},
+        factor{gx, kNT};
+    kworld<<<world.grid, kNT, world_smem, stream>>>(M, D, a);
+    if (int rc = api_launched(&world)) return rc;
     deriv_accum_kernel<T, kNT><<<dim3(gx, kBodyRows), kNT, 0, stream>>>(M, D, a);
-    LAUNCH_CHECK("deriv_accum_kernel");
-    api_note_launch(gx * kBodyRows, kNT, 0, 0);
+    if (int rc = api_launched(&accum)) return rc;
     deriv_pairs_kernel<T, kNT><<<dim3(D.nb, gx), kNT, 0, stream>>>(D, A, a);
-    LAUNCH_CHECK("deriv_pairs_kernel");
-    api_note_launch(gx * D.nb, kNT, 0, 0);
+    if (int rc = api_launched(&pairs)) return rc;
     if (!hs) {
       deriv_factor_kernel<T, kNT><<<gx, kNT, 0, stream>>>(D, A, a);
-      LAUNCH_CHECK("deriv_factor_kernel");
-      api_note_launch(gx, kNT, 0, 0);
+      if (int rc = api_launched(&factor)) return rc;
     }
     if (js) {
       const T* Hg = scratch + (int64_t)D.h_base * sld;
       long long sld_ = sld, ld_ = ld, c_ = c;
       T* dq_ = dq + b0; T* dv_ = dv + b0;
       void* params[] = {(void*)&Hg, (void*)&sld_, (void*)&dq_, (void*)&dv_, (void*)&ld_, (void*)&c_};
-      const int sgj = (int)std::min<int64_t>((c + 31) / 32, (int64_t)js->bps * p.sms);
-      if (cudaLaunchKernel((const void*)js->kernel, dim3(sgj), dim3(32 * js->plan.warps), params, js->smem, stream) != cudaSuccess) {
-        rc = api_fail(RBD_ECUDA, std::string("rbd_deriv_solve launch failed: ") + cudaGetErrorString(cudaGetLastError()));
-        goto done;
-      }
-      api_note_launch(sgj, 32 * js->plan.warps, (int)js->smem, js->bps);
+      const LaunchShape solve{(int)std::min<int64_t>((c + 31) / 32, (int64_t)js->bps * p.sms), 32 * js->plan.warps, (int)js->smem, js->bps};
+      RBD_CUDA_TRY(cudaLaunchKernel((const void*)js->kernel, dim3(solve.grid), dim3(solve.block), params, js->smem, stream));
+      api_note_launch(&solve);
       continue;
     }
-    const int sg = (int)std::min<int64_t>((c + 31) / 32, (int64_t)bestNb * p.sms);
-    if (hs) ksolve_s<<<sg, dim3(32, bestW), solve_smem, stream>>>(D, A, a);
-    else ksolve_g<<<sg, dim3(32, bestW), solve_smem, stream>>>(D, A, a);
-    LAUNCH_CHECK("deriv_solve_kernel");
-    api_note_launch(sg, 32 * bestW, (int)solve_smem, bestNb);
+    const LaunchShape solve{(int)std::min<int64_t>((c + 31) / 32, (int64_t)bestNb * p.sms), 32 * bestW, (int)solve_smem, bestNb};
+    if (hs) ksolve_s<<<solve.grid, dim3(32, bestW), solve_smem, stream>>>(D, A, a);
+    else ksolve_g<<<solve.grid, dim3(32, bestW), solve_smem, stream>>>(D, A, a);
+    if (int rc = api_launched(&solve)) return rc;
   }
-done:
-  cudaFreeAsync(scratch, stream);
-  return rc;
+  return RBD_OK;
 }
 
 }  // namespace
@@ -343,6 +305,7 @@ done:
 extern "C" int32_t rbd_dynamics_derivatives(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                                             const void* tau, void* vd_out, void* dvd_dq_out, void* dvd_dv_out, void* stream) {
   if (int rc = api_check(model, dtype, B, ld)) return rc;
+  const ApiCall call;
   if (B == 0) return RBD_OK;
   if (!q || !v || !vd_out || !dvd_dq_out || !dvd_dv_out)
     return api_fail(RBD_EINVAL, "rbd_dynamics_derivatives: q, v, vd_out, dvd_dq_out and dvd_dv_out must not be NULL");

@@ -1,5 +1,6 @@
-// The opaque model handle of the C ABI (include/rbd_b200.h), shared by rbd_b200.cu (generic kernels, entry points) and
-// rbd_spec.cpp (model-specialised kernels).
+// The opaque model handle of the C ABI (include/rbd_b200.h) and the host plumbing that every translation unit of the library
+// launches through (rbd_b200.cu: generic kernels, entry points; rbd_spec.cpp: model-specialised kernels; rbd_deriv.cu, rbd_loops.cu,
+// rbd_adjoint.cu, rbd_integrate_vjp.cu).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -81,20 +82,76 @@ struct SpecLaunchArgs {
   int64_t peer_ld = 0, peer_col0 = 0;
   void* ko[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};   // SPEC_KIN: the rbd_kinematics_out pointers
 };
-// Tries the model-specialised kernels for (model, key).  `used` = false (and RBD_OK) when they are unavailable, not yet
-// compiled and the batch is below the compile threshold, or the batch is too small: the caller then runs the generic kernels.
-// `gate` (fp32 only, else NULL): device flag the specialised kernels raise when a sample needs the library sin / cos; the caller
-// must enqueue the generic kernel gated on it right behind.
-int spec_try_launch(rbd_model* m, const SpecKey& key, const SpecLaunchArgs& a, cudaStream_t stream, bool& used,
-                    rbd_launch_info& li, const int** gate, std::string& err);
+// Tries the model-specialised kernels for (model, key) and notes the launch as specialised.  `used` = false (and RBD_OK) when
+// they are unavailable, not yet compiled and the batch is below the compile threshold, or the batch is too small: the caller
+// then runs the generic kernels.  `gate` (fp32 only, else NULL): device flag the specialised kernels raise when a sample needs
+// the library sin / cos; the caller must enqueue the generic kernel gated on it right behind (under a KeepLaunchRecord).
+int spec_try_launch(rbd_model* m, const SpecKey& key, const SpecLaunchArgs& a, cudaStream_t stream, bool& used, const int** gate);
 // Compile (or load from the cubin cache) without launching; RBD_OK / RBD_EUNSUPPORTED.
 int spec_prepare(rbd_model* m, const SpecKey& key, bool load_on_device, std::string& err);
 void spec_release(rbd_model* m);
+// RBD_JIT_VARIANT (read at every call): 1 = shared-memory kernels only, 2 = the specialised kernels use the mixed CTA, 0 = unset
+int jit_variant();
 
-// rbd_b200.cu's per-thread error text / argument checks / launch statistics, for the library's other translation units
+// ---- host plumbing shared by the library's translation units (rbd_b200.cu implements it) ----------------------------------
+// Per-thread error text and argument checks.  A failed CUDA call returns RBD_ENOMEM if it was an allocation, else RBD_ECUDA.
 int api_fail(int status, const std::string& msg);
+int api_fail_cuda(cudaError_t e, const std::string& what);
+#define RBD_CUDA_TRY(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) return ::rbd::api_fail_cuda(e_, #expr); } while (0)
 int api_check(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld);
-void api_note_launch(int grid, int block, int smem_bytes, int blocks_per_sm);
+
+// The current device, cached per device.  The first query on a device keeps freed blocks of its stream-ordered pool cached
+// (cudaMemPoolAttrReleaseThreshold): every entry point takes its workspaces from that pool per call.
+struct DeviceProps { int dev = 0, sms = 0, max_smem_optin = 0, smem_per_sm = 0, l2_bytes = 0; };
+cudaError_t device_props(DeviceProps& p);
+// Checks that `smem` bytes of dynamic shared memory fit a block, opts the kernel into large dynamic shared memory with the
+// maximum shared-memory carveout ONCE per (kernel, device) -- the attribute is process-global per kernel, so setting it to each
+// call's exact size would race between host threads using different model handles -- and returns the resident blocks per SM.
+// Kernels without dynamic shared memory keep the default carveout (their workspace traffic goes through L1).
+int kernel_config(const void* kernel, int block, size_t smem, const DeviceProps& p, int& blocks_per_sm);
+
+// A stream-ordered allocation, freed on its stream when it goes out of scope (after the launches using it were enqueued).
+struct StreamAlloc {
+  void* p = nullptr;
+  cudaStream_t stream = nullptr;
+  StreamAlloc() = default;
+  StreamAlloc(const StreamAlloc&) = delete;
+  StreamAlloc& operator=(const StreamAlloc&) = delete;
+  ~StreamAlloc() { if (p) cudaFreeAsync(p, stream); }
+  cudaError_t alloc(size_t bytes, cudaStream_t s) { stream = s; return cudaMallocAsync(&p, bytes, s); }
+};
+
+// Launch record (rbd_get_launch_info): the outermost C-ABI call on a thread resets it (one ApiCall at its entry); calls nested
+// in it (rbd_dynamics_result -> rbd_dynamics, rbd_dynamics_derivatives -> rbd_dynamics) add to it.
+struct ApiCall {
+  ApiCall();
+  ~ApiCall();
+  ApiCall(const ApiCall&) = delete;
+  ApiCall& operator=(const ApiCall&) = delete;
+};
+struct LaunchShape { int grid = 0, block = 0, smem = 0, blocks_per_sm = 0; };
+// Counts one enqueued kernel.  With a shape the record describes that kernel; the elementwise kernels around the dynamics
+// kernels (RK4 stages, integrate-VJP phases, the gather scatter) are counted only.
+void api_note_launch(const LaunchShape* shape = nullptr, bool specialised = false);
+// The status of the kernel launch just enqueued (cudaGetLastError); noted as above when it succeeded.
+int api_launched(const LaunchShape* shape = nullptr);
+// Restores the record, except its count, at scope exit: a gated generic fallback (and rbd_dynamics_result's by-products) add
+// their launches while the record keeps describing the kernel that serves the call.
+struct KeepLaunchRecord {
+  rbd_launch_info saved;
+  KeepLaunchRecord();
+  ~KeepLaunchRecord();
+  KeepLaunchRecord(const KeepLaunchRecord&) = delete;
+  KeepLaunchRecord& operator=(const KeepLaunchRecord&) = delete;
+};
+
+// A persistent launch: min(groups, blocks_per_SM x SMs) blocks of `block` threads looping over the groups, plus -- when
+// `work_per_thread` > 0 -- a stream-ordered workspace of that many bytes per resident thread (and `work_extra` bytes behind it),
+// freed when the plan goes out of scope.  `work_cap` > 0 trims the grid so that the workspace stays within that many bytes.
+// The caller launches `kernel<<<grid, block, smem, stream>>>` with its own arguments, then returns api_launched(&plan).
+struct LaunchPlan : LaunchShape { StreamAlloc work; };
+int plan_persistent(const void* kernel, int block, size_t smem, int64_t ngroups, cudaStream_t stream, LaunchPlan& plan,
+                    size_t work_per_thread = 0, size_t work_extra = 0, size_t work_cap = 0);
 // rbd_b200.cu's RK4 driver for rbd_integrate_trajectory (q_traj / v_traj) and rbd_integrate_vjp's recompute (stages: one step,
 // its four stages kept in stage_rows(nq, nv) x B rows, no finishing step).  fp32 / fp64, arguments checked by the caller.
 inline int64_t stage_rows(int64_t nq, int64_t nv) { return 4 * nq + 12 * nv; }

@@ -275,4 +275,10 @@ RBD_HD void joint_stage(const BodyDev<T>& bd, const Col<T>& q0, const CP& phi, c
   }
 }
 
+#if defined(__CUDACC__)
+// 16-byte vector of T for the kernels that treat revolute / prismatic rows VEC samples per thread (rbd_integrate, rbd_integrate_vjp)
+template <class T> struct VecOf { using type = float4; static constexpr int N = 4; };
+template <> struct VecOf<double> { using type = double2; static constexpr int N = 2; };
+#endif
+
 }  // namespace rbd

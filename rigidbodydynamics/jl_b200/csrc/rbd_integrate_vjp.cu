@@ -6,6 +6,7 @@
 //   finish + L3 | VJP 3 | G3 + L2 | VJP 2 | G2 + L1 | VJP 1 | G1 + L0 | VJP 0 | G0 (+ the trajectory adjoints of the step's start)
 // An elementwise phase is one thread per (sample, joint) for the joints with non-linear maps (blockIdx.y = body) and, when the
 // batch allows, a vectorised kernel over the revolute / prismatic rows (16-byte accesses, like integrate_stage_linear_kernel).
+// Every launch, the recompute's and the VJPs' included, counts in the call's launch record (rbd_handle.h).
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -20,13 +21,6 @@
 using namespace rbd;
 
 namespace {
-
-template <class T> const ModelDev<T>& dev_model(const HostModel& m);
-template <> const ModelDev<float>& dev_model<float>(const HostModel& m) { return m.dev32; }
-template <> const ModelDev<double>& dev_model<double>(const HostModel& m) { return m.dev64; }
-
-template <class T> struct VecOf { using type = float4; static constexpr int N = 4; };
-template <> struct VecOf<double> { using type = double2; static constexpr int N = 2; };
 
 template <class T>
 __global__ void __launch_bounds__(128) integrate_adjoint_kernel(const __grid_constant__ ModelDev<T> M, const AdjStepArgs<T> a,
@@ -102,12 +96,6 @@ __global__ void __launch_bounds__(128) integrate_adjoint_out_kernel(const __grid
     adj_out(bd, a.q, a.qb, a.qt, a.qc, a.B, b);
 }
 
-int fail_cuda(cudaError_t e, const char* what) {
-  return api_fail(e == cudaErrorMemoryAllocation ? RBD_ENOMEM : RBD_ECUDA, std::string("rbd_integrate_vjp: ") + what + ": " +
-                                                                            cudaGetErrorString(e));
-}
-#define TRY_CUDA(x, what) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) return fail_cuda(e_, what); } while (0)
-
 template <class T>
 int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q_traj, const T* v_traj, const T* tau, int64_t step_stride,
                     int64_t stage_stride, double dt, int nsteps, const T* qtb, const T* vtb, T* q0t, T* q0c, T* v0b, T* taub,
@@ -115,24 +103,22 @@ int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q
   const HostModel& hm = model->hm;
   const ModelDev<T>& M = dev_model<T>(hm);
   const int64_t nq = hm.nq, nv = hm.nv;
-  int dev = 0, sms = 0;
-  TRY_CUDA(cudaGetDevice(&dev), "cudaGetDevice");
-  TRY_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev), "device attributes");
+  DeviceProps p;
+  RBD_CUDA_TRY(device_props(p));
   // workspace: the four stages, then q̄_cfg / q̄ / q̄0 / q̄s (nq rows each), v̄ / τ̄ / v̄ / v̄0 / v̄s / v̇̄ / Φ̄ (nv rows each)
   const int64_t srows = stage_rows(nq, nv), rows = srows + 4 * nq + 7 * nv;
-  T* ws = nullptr;
-  TRY_CUDA(cudaMallocAsync((void**)&ws, (size_t)rows * B * sizeof(T), stream), "workspace");
-  struct Guard { void* p; cudaStream_t s; ~Guard() { if (p) cudaFreeAsync(p, s); } } guard{ws, stream};    // freed on every exit path
-  T* stages = ws;
-  T* p = ws + srows * B;
-  auto take = [&](int64_t r) { T* o = p; p += r * B; return o; };
+  StreamAlloc work;
+  RBD_CUDA_TRY(work.alloc((size_t)rows * B * sizeof(T), stream));
+  T* stages = (T*)work.p;
+  T* next = stages + srows * B;
+  auto take = [&](int64_t r) { T* o = next; next += r * B; return o; };
   T *qcb = take(nq), *qb = take(nq), *qb0 = take(nq), *qsb = take(nq);
   T *vvb = take(nv), *tb = take(nv), *vb = take(nv), *vb0 = take(nv), *vsb = take(nv), *vdb = take(nv), *phib = take(nv);
   const size_t qbytes = (size_t)nq * B * sizeof(T), vbytes = (size_t)nv * B * sizeof(T);
-  if (qtb) TRY_CUDA(cudaMemcpyAsync(qb, qtb + (size_t)nsteps * nq * B, qbytes, cudaMemcpyDeviceToDevice, stream), "copy");
-  else TRY_CUDA(cudaMemsetAsync(qb, 0, qbytes, stream), "memset");
-  if (vtb) TRY_CUDA(cudaMemcpyAsync(vb, vtb + (size_t)nsteps * nv * B, vbytes, cudaMemcpyDeviceToDevice, stream), "copy");
-  else TRY_CUDA(cudaMemsetAsync(vb, 0, vbytes, stream), "memset");
+  if (qtb) RBD_CUDA_TRY(cudaMemcpyAsync(qb, qtb + (size_t)nsteps * nq * B, qbytes, cudaMemcpyDeviceToDevice, stream));
+  else RBD_CUDA_TRY(cudaMemsetAsync(qb, 0, qbytes, stream));
+  if (vtb) RBD_CUDA_TRY(cudaMemcpyAsync(vb, vtb + (size_t)nsteps * nv * B, vbytes, cudaMemcpyDeviceToDevice, stream));
+  else RBD_CUDA_TRY(cudaMemsetAsync(vb, 0, vbytes, stream));
   bool has_other = false;
   for (int i = 0; i < hm.nb; ++i) has_other |= (M.body[i].kind != K_REV && M.body[i].kind != K_PRIS && M.body[i].kind != K_FIXED);
   constexpr int N = VecOf<T>::N;
@@ -140,8 +126,8 @@ int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q
   auto aligned = [&](const T* x, int64_t stride) { return !x || ((uintptr_t)x % va == 0 && stride % N == 0); };
   const bool vec_ok = B % N == 0 && B >= 1024 && aligned(taub, step_stride) && aligned(taub, stage_stride) && aligned(qtb, 0) &&
                       aligned(vtb, 0) && aligned(q_traj, 0);
-  const int grid = (int)std::min<int64_t>((B + 127) / 128, (int64_t)sms * 8);
-  const int grid_lin = (int)std::min<int64_t>((B / N + 255) / 256, (int64_t)sms * 4);
+  const int grid = (int)std::min<int64_t>((B + 127) / 128, (int64_t)p.sms * 8);
+  const int grid_lin = (int)std::min<int64_t>((B / N + 255) / 256, (int64_t)p.sms * 4);
   const double ca[4] = {0.0, 0.5, 0.5, 1.0}, cb[4] = {1.0 / 6, 1.0 / 3, 1.0 / 3, 1.0 / 6};   // runge_kutta_4, as integrate_t
   AdjStepArgs<T> a{};
   for (int i = 0; i < 4; ++i) {
@@ -167,16 +153,16 @@ int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q
       a.tau_bar = (taub && g < 4) ? taub + s * step_stride + g * stage_stride : nullptr;
       if (vec_ok) {
         integrate_adjoint_linear_kernel<T><<<dim3(grid_lin, hm.nb), 256, 0, stream>>>(M, a);
-        TRY_CUDA(cudaGetLastError(), "launch");
+        if (int rc = api_launched()) return rc;
       }
       if (!vec_ok || has_other) {
         integrate_adjoint_kernel<T><<<dim3(grid, hm.nb), 128, 0, stream>>>(M, a, vec_ok);
-        TRY_CUDA(cudaGetLastError(), "launch");
+        if (int rc = api_launched()) return rc;
       }
       if (a.l < 0) {
         if (s > 0) {
           integrate_adjoint_out_kernel<T><<<dim3(grid, hm.nb), 128, 0, stream>>>(M, OutArgs<T>{q0, qb, nullptr, qb, B});
-          TRY_CUDA(cudaGetLastError(), "launch");
+          if (int rc = api_launched()) return rc;
         }
         continue;
       }
@@ -185,9 +171,9 @@ int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q
   }
   if (q0t || q0c) {
     integrate_adjoint_out_kernel<T><<<dim3(grid, hm.nb), 128, 0, stream>>>(M, OutArgs<T>{q_traj, qb, q0t, q0c, B});
-    TRY_CUDA(cudaGetLastError(), "launch");
+    if (int rc = api_launched()) return rc;
   }
-  if (v0b) TRY_CUDA(cudaMemcpyAsync(v0b, vb, vbytes, cudaMemcpyDeviceToDevice, stream), "copy");
+  if (v0b) RBD_CUDA_TRY(cudaMemcpyAsync(v0b, vb, vbytes, cudaMemcpyDeviceToDevice, stream));
   return RBD_OK;
 }
 
@@ -198,6 +184,7 @@ extern "C" int32_t rbd_integrate_vjp(const rbd_model* model, int32_t dtype, int6
                                      const void* q_traj_bar, const void* v_traj_bar, void* q0_bar_tan, void* q0_bar_cfg, void* v0_bar,
                                      void* tau_bar, void* stream) {
   if (int rc = api_check(model, dtype, B, B)) return rc;
+  const ApiCall call;
   if (dtype != RBD_F32 && dtype != RBD_F64) return api_fail(RBD_EUNSUPPORTED, "rbd_integrate_vjp: fp32 and fp64 only");
   if (nsteps < 0 || !(dt > 0)) return api_fail(RBD_EINVAL, "rbd_integrate_vjp: need dt > 0 and nsteps >= 0");
   if (tau_step_stride < 0 || tau_stage_stride < 0) return api_fail(RBD_EINVAL, "rbd_integrate_vjp: torque strides must be >= 0");

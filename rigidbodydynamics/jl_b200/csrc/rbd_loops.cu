@@ -2,15 +2,13 @@
 //
 // One generic persistent kernel, one thread per sample, one launch per call: CRBA, RNEA bias, q̇, the constraint Jacobian / bias
 // sweep and the KKT solve run back to back in the same thread, so no intermediate crosses a launch boundary.  The per-sample
-// working set (M, K / Y, A, ...) lives in a stream-ordered global workspace of LoopRows::total rows x RESIDENT threads (the grid is
-// blocks_per_SM x SMs blocks of one warp looping over groups of 32 samples), laid out [row][thread] so a warp's access to a row is
+// working set (M, K / Y, A, ...) lives in the stream-ordered workspace of plan_persistent (rbd_handle.h): LoopRows::total rows x
+// RESIDENT threads (blocks of one warp looping over groups of 32 samples), laid out [row][thread] so a warp's access to a row is
 // one coalesced line; the pending slots of the tree sweeps live in shared memory as in the other kernels.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include <algorithm>
-#include <mutex>
-#include <set>
 #include <string>
 
 #include "../../../include/rbd_b200.h"
@@ -24,10 +22,6 @@ using namespace rbd;
 namespace {
 
 constexpr int kNT = 32;     // one warp per block; warps never synchronise
-
-template <class T> const ModelDev<T>& dev_model(const HostModel& m);
-template <> const ModelDev<float>& dev_model<float>(const HostModel& m) { return m.dev32; }
-template <> const ModelDev<double>& dev_model<double>(const HostModel& m) { return m.dev64; }
 
 template <class T> struct LoopArgs {
   const T *q, *v, *tau, *wext;
@@ -64,20 +58,6 @@ loops_kernel(const __grid_constant__ ModelDev<T> M, const __grid_constant__ Loop
   }
 }
 
-int big_smem_once(const void* kernel, int dev, int max_smem_optin) {
-  static std::mutex mu;
-  static std::set<std::pair<const void*, int>> done;
-  std::lock_guard<std::mutex> lk(mu);
-  if (done.count({kernel, dev})) return RBD_OK;
-  cudaFuncAttributes fa{};
-  if (cudaFuncGetAttributes(&fa, kernel) != cudaSuccess ||
-      cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem_optin - (int)fa.sharedSizeBytes) != cudaSuccess)
-    return api_fail(RBD_ECUDA, std::string("cudaFuncSetAttribute: ") + cudaGetErrorString(cudaGetLastError()));
-  cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-  done.insert({kernel, dev});
-  return RBD_OK;
-}
-
 template <class T>
 int loops_t(const rbd_model* model, int64_t B, int64_t ld, const void* q, const void* v, const void* tau, const void* wext,
             const rbd_loop_desc& desc, void* vd, void* qd, void* lam, void* K, void* k, cudaStream_t stream) {
@@ -89,31 +69,15 @@ int loops_t(const rbd_model* model, int64_t B, int64_t ld, const void* q, const 
   bool multi = false;
   for (int i = 0; i < hm.nb; ++i) multi |= kind_nv(M.body[i].kind) > 1;
   const void* kernel = multi ? (const void*)loops_kernel<T, kNT, 6> : (const void*)loops_kernel<T, kNT, 1>;
-  int dev = 0, sms = 0, optin = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return api_fail(RBD_ECUDA, "cudaGetDevice failed");
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
   const int stash = std::max({1, crba_rows(hm), rnea_rows(hm), kin_rows(hm)});
-  const size_t smem = (size_t)stash * kNT * sizeof(T);
-  if ((int)smem > optin) return api_fail(RBD_EUNSUPPORTED, "model working set exceeds shared memory per block");
-  if (int rc = big_smem_once(kernel, dev, optin)) return rc;
-  int bps = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, kernel, kNT, smem) != cudaSuccess || bps < 1)
-    return api_fail(RBD_EUNSUPPORTED, "rbd_dynamics_loops: kernel does not fit on an SM");
-  const int64_t ngroups = (B + kNT - 1) / kNT;
-  const int grid = (int)std::min<int64_t>(ngroups, (int64_t)bps * sms);
-  T* work = nullptr;
-  cudaError_t e = cudaMallocAsync((void**)&work, (size_t)rows.total * grid * kNT * sizeof(T), stream);
-  if (e != cudaSuccess) return api_fail(e == cudaErrorMemoryAllocation ? RBD_ENOMEM : RBD_ECUDA,
-                                        std::string("rbd_dynamics_loops workspace: ") + cudaGetErrorString(e));
-  const LoopArgs<T> a{(const T*)q, (const T*)v, (const T*)tau, (const T*)wext, (T*)vd, (T*)qd, (T*)lam, (T*)K, (T*)k, work, rows, ld, B};
-  if (multi) loops_kernel<T, kNT, 6><<<grid, kNT, smem, stream>>>(M, L, a);
-  else loops_kernel<T, kNT, 1><<<grid, kNT, smem, stream>>>(M, L, a);
-  e = cudaGetLastError();
-  cudaFreeAsync(work, stream);
-  if (e != cudaSuccess) return api_fail(RBD_ECUDA, std::string("loops_kernel launch failed: ") + cudaGetErrorString(e));
-  api_note_launch(grid, kNT, (int)smem, bps);
-  return RBD_OK;
+  LaunchPlan pl;
+  if (int rc = plan_persistent(kernel, kNT, (size_t)stash * kNT * sizeof(T), (B + kNT - 1) / kNT, stream, pl,
+                               (size_t)rows.total * sizeof(T))) return rc;
+  const LoopArgs<T> a{(const T*)q, (const T*)v, (const T*)tau, (const T*)wext, (T*)vd, (T*)qd, (T*)lam, (T*)K, (T*)k,
+                      (T*)pl.work.p, rows, ld, B};
+  if (multi) loops_kernel<T, kNT, 6><<<pl.grid, pl.block, pl.smem, stream>>>(M, L, a);
+  else loops_kernel<T, kNT, 1><<<pl.grid, pl.block, pl.smem, stream>>>(M, L, a);
+  return api_launched(&pl);
 }
 
 }  // namespace
@@ -122,6 +86,7 @@ extern "C" int32_t rbd_dynamics_loops(const rbd_model* model, int32_t dtype, int
                                       const void* tau, const void* wext, const rbd_loop_desc* loops, void* vd_out, void* qd_out,
                                       void* lambda_out, void* K_out, void* k_out, void* stream) {
   if (int rc = api_check(model, dtype, B, ld)) return rc;
+  const ApiCall call;
   std::string err;
   if (int rc = check_loop_desc(model->hm, loops, err)) return api_fail(rc, err);
   if (!q || !v || !vd_out) return api_fail(RBD_EINVAL, "rbd_dynamics_loops: q, v and vd_out must not be NULL");

@@ -1,7 +1,8 @@
 // Model-specialised kernels: compile (rbd_jit.cpp), load (cudaLibraryLoadData) and launch.  Host-only C++ on the CUDA runtime.
 //
 // The kernels are persistent and claim groups of 32 samples from one counter: single-warp blocks with their stash in shared
-// memory, or one mixed CTA per SM whose extra warps keep their stash in L2 (rbd_jit_kernels.cuh).
+// memory, or one mixed CTA per SM whose extra warps keep their stash in L2 (rbd_jit_kernels.cuh).  Device properties, error
+// mapping and the launch record are the shared plumbing of rbd_handle.h; the cubin kernels get exact shared-memory sizes here.
 #include <algorithm>
 #include <cstdio>
 #include <cstdlib>
@@ -16,41 +17,21 @@ namespace {
 constexpr int kMixWarps = 16;       // warps of the mixed CTA: 16 x 32 threads x 128 registers = the whole register file
 
 struct Env {
-  bool jit = true, no_gate = false;
+  bool jit = true;
   int64_t min_batch = 1 << 15;      // below this a missing cubin is not compiled on the fly (generic kernels serve the call)
-  int smem_blocks = 0;
   Env() {
     if (const char* e = getenv("RBD_JIT")) jit = e[0] != '0';
-    no_gate = getenv("RBD_NO_GATE") != nullptr;
     if (const char* e = getenv("RBD_JIT_MIN_BATCH")) min_batch = atoll(e);
-    if (const char* e = getenv("RBD_SMEM_BLOCKS")) smem_blocks = atoi(e);
   }
 };
 const Env& env() { static const Env e; return e; }
 
-struct Props { int sms = 0, max_smem_optin = 0; };
-cudaError_t props(Props& p) {
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return e;
-  static std::mutex mu;
-  static Props cache[64];
-  std::lock_guard<std::mutex> lk(mu);
-  if (dev < 64 && cache[dev].sms) { p = cache[dev]; return cudaSuccess; }
-  if ((e = cudaDeviceGetAttribute(&p.sms, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return e;
-  if ((e = cudaDeviceGetAttribute(&p.max_smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev)) != cudaSuccess) return e;
-  {  // the L2 stash of the mixed CTA comes from the stream-ordered pool: keep freed blocks cached in the pool
-    cudaMemPool_t pool;
-    if (cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) {
-      uint64_t keep = ~0ull;
-      cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep);
-    }
-  }
-  if (dev < 64) cache[dev] = p;
-  return cudaSuccess;
-}
-
 }  // namespace
+
+int jit_variant() {
+  const char* e = getenv("RBD_JIT_VARIANT");
+  return e ? atoi(e) : 0;
+}
 
 cudaError_t queue_begin(rbd_model* m, cudaStream_t stream, QueueCtx& ctx) {
   int dev = 0;
@@ -83,8 +64,8 @@ void spec_release(rbd_model* m) {
 // estimated size.
 bool spec_worthwhile(const HostModel& hm, const SpecKey& key) {
   if (!key.f64) return true;
-  if (key.algo == SPEC_CRBA) return !getenv("RBD_JIT_NO_CRBA64");   // small stash (2 rows per body): fp64 keeps its resident warps
-  if (key.algo == SPEC_KIN) return true;                             // stash = the pending branch nodes only
+  // small stashes (CRBA: 2 rows per body, kinematics: the pending branch nodes only): fp64 keeps its resident warps
+  if (key.algo == SPEC_CRBA || key.algo == SPEC_KIN) return true;
   const int est = hm.nb * (key.algo == SPEC_ABA ? 410 : 190);
   return est <= 6500;
 }
@@ -109,10 +90,9 @@ int spec_prepare(rbd_model* m, const SpecKey& key, bool load_on_device, std::str
   if (e == cudaSuccess) { e = cudaFuncGetAttributes(&fa, (const void*)se.k_mix); se.regs_mix = fa.numRegs; }
   se.rows = spec_stash_rows(m->hm, key);
   const size_t smem = (size_t)std::max(1, se.rows) * 32 * (key.f64 ? 8 : 4);
-  int optin = 0, dev = 0;
-  if (e == cudaSuccess) e = cudaGetDevice(&dev);
-  if (e == cudaSuccess) e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-  se.mix_sw = std::min<int>(kMixWarps, (int)(optin / smem));
+  DeviceProps p;
+  if (e == cudaSuccess) e = device_props(p);
+  se.mix_sw = std::min<int>(kMixWarps, (int)(p.max_smem_optin / smem));
   if (e == cudaSuccess) e = cudaFuncSetAttribute((const void*)se.k_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e == cudaSuccess) e = cudaFuncSetAttribute((const void*)se.k_smem, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
   if (e == cudaSuccess && se.mix_sw > 0)
@@ -130,8 +110,7 @@ int spec_prepare(rbd_model* m, const SpecKey& key, bool load_on_device, std::str
   return RBD_OK;
 }
 
-int spec_try_launch(rbd_model* m, const SpecKey& key, const SpecLaunchArgs& a, cudaStream_t stream, bool& used,
-                    rbd_launch_info& li, const int** gate, std::string& err) {
+int spec_try_launch(rbd_model* m, const SpecKey& key, const SpecLaunchArgs& a, cudaStream_t stream, bool& used, const int** gate) {
   used = false;
   if (gate) *gate = nullptr;
   const Env& ev = env();
@@ -139,8 +118,8 @@ int spec_try_launch(rbd_model* m, const SpecKey& key, const SpecLaunchArgs& a, c
   if (a.ld * (key.f64 ? 8 : 4) >= (1ll << 32)) return RBD_OK;   // the generated code forms row offsets as 32 x 32 -> 64-bit products of the byte stride
   const int rows = spec_stash_rows(m->hm, key);
   if (rows > 256) return RBD_OK;                     // larger stashes leave too few warps per SM: the generic kernels serve
-  Props p;
-  if (cudaError_t e = props(p)) { err = cudaGetErrorString(e); return RBD_ECUDA; }
+  DeviceProps p;
+  RBD_CUDA_TRY(device_props(p));
   const size_t es = key.f64 ? 8 : 4;
   const size_t smem = (size_t)std::max(1, rows) * 32 * es;
   if (smem > (size_t)p.max_smem_optin) return RBD_OK;
@@ -170,11 +149,8 @@ int spec_try_launch(rbd_model* m, const SpecKey& key, const SpecLaunchArgs& a, c
   }
   const int64_t ngroups = (a.B + 31) / 32;
   int bps = 0;
-  if (cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, (const void*)se->k_smem, 32, smem)) {
-    err = cudaGetErrorString(e); return RBD_ECUDA;
-  }
+  RBD_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, (const void*)se->k_smem, 32, smem));
   if (bps < 1) return RBD_OK;
-  if (ev.smem_blocks > 0) bps = std::max(1, std::min(bps, ev.smem_blocks));
   // The mixed CTA (rbd_jit_kernels.cuh) is worth trying when it puts at least 15 % more warps on the SM than shared-memory blocks
   // alone and there is a group of samples for each of its warps; which of the two is faster depends on the program, so the first
   // call large enough to tell times both once and keeps the winner (not while capturing a graph).  RBD_JIT_VARIANT=1 / 2 forces one.
@@ -188,6 +164,7 @@ int spec_try_launch(rbd_model* m, const SpecKey& key, const SpecLaunchArgs& a, c
     void* l2_stash; int smem_warps;
   };
   int* last_flag = nullptr;
+  LaunchShape shape;
   auto run = [&](int variant) -> cudaError_t {        // 1 = shared-memory blocks, 2 = mixed CTA
     QueueCtx ctx;
     cudaError_t e = queue_begin(m, stream, ctx);
@@ -201,19 +178,19 @@ int spec_try_launch(rbd_model* m, const SpecKey& key, const SpecLaunchArgs& a, c
       e = cudaMallocAsync(&ka.l2_stash, (size_t)(mix_warps - mix_sw) * p.sms * smem, stream);
       if (e == cudaSuccess) e = cudaLaunchKernel((const void*)se->k_mix, dim3(p.sms), dim3(32 * mix_warps), params, smem * mix_sw, stream);
       if (ka.l2_stash) cudaFreeAsync(ka.l2_stash, stream);
-      li.grid = p.sms; li.block = 32 * mix_warps; li.blocks_per_sm = 1; li.smem_bytes = (int)(smem * mix_sw);
+      shape = {p.sms, 32 * mix_warps, (int)(smem * mix_sw), 1};
     } else {
       const int grid = (int)std::min<int64_t>(ngroups, (int64_t)bps * p.sms);
       e = cudaLaunchKernel((const void*)se->k_smem, dim3(grid), dim3(32), params, smem, stream);
-      li.grid = grid; li.block = 32; li.blocks_per_sm = bps; li.smem_bytes = (int)smem;
+      shape = {grid, 32, (int)smem, bps};
     }
     last_flag = ctx.flag;
     return e;
   };
   cudaError_t e = cudaSuccess;
   int variant = 1;
-  const char* force = getenv("RBD_JIT_VARIANT");
-  if (force && mix_ok) variant = atoi(force) == 2 ? 2 : 1;
+  const int force = jit_variant();
+  if (force && mix_ok) variant = force == 2 ? 2 : 1;
   else if (mix_ok) {
     variant = se->choice;
     cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
@@ -239,9 +216,9 @@ int spec_try_launch(rbd_model* m, const SpecKey& key, const SpecLaunchArgs& a, c
     if (variant == 0) variant = 1;
   }
   if (e == cudaSuccess) e = run(variant);
-  if (e != cudaSuccess) { err = std::string("specialised kernel launch: ") + cudaGetErrorString(e); return RBD_ECUDA; }
-  li.kernels_launched += 1;
-  if (gate && !key.f64 && !ev.no_gate) *gate = last_flag;
+  if (e != cudaSuccess) return api_fail_cuda(e, "specialised kernel launch");
+  api_note_launch(&shape, true);
+  if (gate && !key.f64) *gate = last_flag;
   used = true;
   return RBD_OK;
 }
