@@ -20,7 +20,7 @@
 namespace rbd {
 namespace {
 
-constexpr int kGeneratorVersion = 28;   // bump when the emitted code changes (part of the cubin cache key)
+constexpr int kGeneratorVersion = 29;   // bump when the emitted code changes (part of the cubin cache key)
 
 template <class F> const ModelDev<F>& devm(const HostModel& m);
 template <> const ModelDev<float>& devm<float>(const HostModel& m) { return m.dev32; }
@@ -118,6 +118,7 @@ struct Emitter {
   SpecStats stats;
 
   int split_every = 0;           // CUDA flavours: RBD_SPLIT() (a never-taken branch = basic-block boundary) every N statements
+  int split_folded = 0;          // the same for a program with folded chains
   std::vector<int32_t> uses;     // live uses of every node
   std::vector<uint8_t> fused;    // product folded into the FMA of its single consumer
 
@@ -541,7 +542,8 @@ struct Emitter {
     mark();
     plan_fma();
     if (fold) analyse_folds();
-    else { fold_at.assign(tr.nodes.size(), -1); in_fold.assign(tr.nodes.size(), -1); remat.assign(tr.nodes.size(), 0); }
+    if (!folds.empty()) split_every = split_folded;
+    if (!fold) { fold_at.assign(tr.nodes.size(), -1); in_fold.assign(tr.nodes.size(), -1); remat.assign(tr.nodes.size(), 0); }
     const auto& N = tr.nodes;
     stats.nodes_traced = (int)N.size();
     for (size_t i = 0; i < N.size(); ++i) if (live[i] && N[i].op != S_CONST && N[i].op != S_PARAM) ++stats.nodes_live;
@@ -596,8 +598,11 @@ bool spec_emit_function(const HostModel& hm, const SpecKey& key, int flavor, con
   if (flavor != FLAVOR_CPU) {
     // One basic block of 10^4 instructions lets ptxas stretch live ranges until it spills (Atlas: 128 registers + 350 B of
     // local memory, -10 % throughput); a never-taken branch every few hundred statements bounds its scheduling regions.
+    // A folded program's loops already end basic blocks every few hundred statements, and there the extra branches only cost
+    // (Atlas fp32 forward dynamics on H100 at 400 W: 800 M evals/s with a branch every 192 statements, 856 M without).
     em.split_every = 192;
-    if (const char* e = getenv("RBD_JIT_SPLIT")) em.split_every = atoi(e);
+    em.split_folded = 0;
+    if (const char* e = getenv("RBD_JIT_SPLIT")) em.split_every = em.split_folded = atoi(e);
   }
   em.emit();
   em.stats.stash_rows = rows;
