@@ -398,6 +398,29 @@ int32_t rbd_integrate_vjp(const rbd_model* model, int32_t dtype, int64_t B, cons
                           const void* q_traj_bar, const void* v_traj_bar,
                           void* q0_bar_tan, void* q0_bar_cfg, void* v0_bar, void* tau_bar, void* stream);
 
+/* simulate for a mechanism WITH contact points (DESIGN 4.14): rbd_integrate_schedule whose dynamics at every stage is dynamics! with
+ * contact -- contact_dynamics! (see rbd_contact_dynamics) and the forward dynamics on its wrenches, in one kernel -- and which also
+ * integrates the contact state s, the additional state of the reference's MechanismState, with the same RK4 tableau in plain
+ * Euclidean form (MuntheKaasIntegrator.step, src/ode_integrators.jl:233-300; simulate, src/simulate.jl:36-55):
+ *   stage i   s_i = s0 + dt a_i ṡ_{i-1},   step   s = s0 + dt sum_i b_i ṡ_i.
+ *   q [nq x B], v [nv x B], s [3*npoints*nhalfspaces x B] (layout of rbd_contact_dynamics' state; leading dimension ld) are advanced
+ *   IN PLACE; tau and its strides as in rbd_integrate_schedule; no external wrenches (simulate passes none).
+ * Reset semantics: the reference's contact_dynamics! resets the state of a pair that is out of contact, but its integrator
+ * overwrites the state with the stage value at every stage and with the step result at the end of the step, so within simulate a
+ * reset never survives.  This call therefore never resets: a pair out of contact has ṡ = 0, keeps its last integrated s (frozen,
+ * not zeroed) and resumes from it when it touches again.  s persists across calls exactly as the MechanismState's does, so
+ * consecutive calls equal one call of the summed steps, bit for bit.
+ * q_traj [(nsteps+1) x nq x B], v_traj [(nsteps+1) x nv x B], s_traj [(nsteps+1) x ns x B] (leading dimension B): all NULL, or all
+ * set (s_traj may be NULL when ns = 0) to record the trajectory as rbd_integrate_trajectory does; recording does not change the
+ * result.  Descriptor checks as rbd_contact_dynamics.  dtype other than fp32 / fp64: RBD_EUNSUPPORTED; nsteps < 0, dt <= 0, negative
+ * strides, s == NULL with ns > 0, or a partial set of trajectory pointers: RBD_EINVAL; B == 0: nothing to do.  Kernels per step:
+ * per stage the coordinate-map kernel(s) of rbd_integrate (1 or 2) and one forward-dynamics kernel, then the finishing kernel(s) of
+ * rbd_integrate (1 or 2) and, when ns > 0, one for s -- 15 for a floating-base robot when B >= 1024 and B and ld are multiples of
+ * 4 (fp32) / 2 (fp64) with 16-byte aligned q and v.  Mechanisms with loops are not supported (the Python layer refuses them with RBD_ELOOP). */
+int32_t rbd_integrate_contact(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau,
+                              int64_t tau_step_stride, int64_t tau_stage_stride, const rbd_contact_desc* contact, double dt, int32_t nsteps,
+                              void* q_traj, void* v_traj, void* s_traj, void* stream);
+
 /* Next row of the scope table (SURVEY 8(f) rank 2): kinematics by-products of the same outward sweep, all expressed in the
  * mechanism's root frame, 6-vectors as [angular; linear].  Every output pointer may be NULL (not computed).
  *   transforms_to_root  [12*nb x B]  rows 12 i .. 12 i + 11 = transform_to_root(state, successor of tree joint i):

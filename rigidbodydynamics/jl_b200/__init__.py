@@ -25,7 +25,8 @@ from .kinematics import (TreePath, center_of_mass, geometric_jacobian, geometric
                          momentum_matrix_, momentum_rate_bias, path, transforms_to_root, transforms_to_root_)
 from .contact import (ContactDesc, ContactPoint, HalfSpace3D, HuntCrossleyModel, SoftContactModel,  # noqa: F401
                       ViscoelasticCoulombModel, add_contact_point, add_environment_primitive, contact_desc, contact_dynamics_,
-                      contact_points, dynamics_contact_, environment, hunt_crossley_hertz, num_contact_states)
+                      contact_points, dynamics_contact_, environment, hunt_crossley_hertz, num_contact_states,
+                      simulate_contact_, simulate_contact_trajectory_)
 from .loops import (LoopDesc, PDGains, SE3PDGains, constraint_wrench_subspace, default_constraint_stabilization_gains,  # noqa: F401
                     dynamics_loops_, loop_desc, num_constraints)
 from .mechanism import maximal_coordinates  # noqa: F401

@@ -10,6 +10,8 @@
     contact_dynamics!(result, state)             mechanism_algorithms.jl:680-723     -> contact_dynamics_
     dynamics!(result, state, tau, wext) with contact points (contact wrenches added to the external ones, :850-856)
                                                                                       -> dynamics_contact_
+    simulate(state, final_time; Δt) with contact points (simulate.jl:36-55, ode_integrators.jl:233-300)
+                                                                                      -> simulate_contact_, simulate_contact_trajectory_
 
 The additional state ``s`` of a ``MechanismState`` (3 tangential-displacement entries per (contact point, half-space) pair, in
 body / point / half-space order, mechanism_state.jl:140-153) is a ``[num_contact_states, B]`` tensor here.  All compute is one
@@ -25,12 +27,12 @@ import numpy as np
 import torch
 
 from . import _cabi
-from .algorithms import DimensionMismatch, _call, _check, _ptr, _require_tree, _stream, dynamics_
+from .algorithms import DimensionMismatch, _call, _check, _ptr, _require_tree, _stream, _torque_schedule, dynamics_
 from .state import DynamicsResult, MechanismState, _DT
 
 __all__ = ["HuntCrossleyModel", "hunt_crossley_hertz", "ViscoelasticCoulombModel", "SoftContactModel", "ContactPoint", "HalfSpace3D",
            "add_contact_point", "contact_points", "add_environment_primitive", "environment", "num_contact_states", "ContactDesc",
-           "contact_desc", "contact_dynamics_", "dynamics_contact_"]
+           "contact_desc", "contact_dynamics_", "dynamics_contact_", "simulate_contact_", "simulate_contact_trajectory_"]
 
 
 @dataclass
@@ -196,3 +198,57 @@ def dynamics_contact_(result: DynamicsResult, state: MechanismState, torques: Op
         tw = cw
     result.totalwrenches = tw
     return dynamics_(result, state, torques, tw, want_qd=want_qd)
+
+
+def _integrate_contact(state: MechanismState, nsteps: int, contact_state: Optional[torch.Tensor], torques, dt: float,
+                       contact: Optional[ContactDesc], record: bool, what: str):
+    _require_tree(state, what)
+    state.check_modcount()
+    if nsteps < 0:
+        raise ValueError("nsteps must be >= 0")
+    lib = _cabi.load_library()
+    cd = contact if contact is not None else contact_desc(state.mechanism)
+    if contact_state is None and cd.nstates > 0:
+        raise ValueError(f"{what}: contact_state [{cd.nstates}, B] must be given (the mechanism has contact points)")
+    _check(contact_state, cd.nstates, state, "contact_state")
+    step = stage = 0
+    if torques is not None and torques.dim() in (3, 4):
+        step, stage = _torque_schedule(state, torques, nsteps)
+    else:
+        _check(torques, state.nv, state, "torques")
+    traj = (None, None, None)
+    if record:
+        new = lambda rows: torch.empty((nsteps + 1, rows, state.batch), dtype=state.dtype, device=state.q.device)   # noqa: E731
+        traj = (new(state.nq), new(state.nv), new(cd.nstates))
+    st, keep = cd.c_struct()
+    _call(lib.rbd_integrate_contact(state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q), _ptr(state.v),
+                                    _ptr(contact_state), _ptr(torques), step, stage, ctypes.byref(st), float(dt), nsteps,
+                                    *[_ptr(t) for t in traj], _stream()))
+    del keep
+    return traj
+
+
+def simulate_contact_trajectory_(state: MechanismState, nsteps: int, contact_state: Optional[torch.Tensor],
+                                 torques: Optional[torch.Tensor] = None, dt: float = 1e-4, contact: Optional[ContactDesc] = None):
+    """``nsteps`` steps of ``simulate_contact_``, recording the trajectory: returns ``(q_traj, v_traj, s_traj)``, [nsteps + 1, nq, B],
+    [nsteps + 1, nv, B] and [nsteps + 1, num_contact_states, B], block 0 the initial state and block s the state after step s.
+    ``state`` and ``contact_state`` are advanced in place exactly as ``simulate_contact_`` advances them."""
+    return _integrate_contact(state, nsteps, contact_state, torques, dt, contact, True, "simulate_contact_trajectory_")
+
+
+def simulate_contact_(state: MechanismState, final_time: float, contact_state: Optional[torch.Tensor],
+                      torques: Optional[torch.Tensor] = None, dt: float = 1e-4, contact: Optional[ContactDesc] = None) -> int:
+    """``simulate(state, final_time; Δt)`` for a mechanism with contact points (src/simulate.jl:36-55): Munthe-Kaas RK4 steps until
+    ``t >= final_time`` (the step count of ``simulate_``) of ``dynamics!`` with contact, integrating the contact state as well
+    (src/ode_integrators.jl:233-300), all on the GPU.  ``state.q``, ``state.v`` and ``contact_state`` ([num_contact_states, B], the
+    MechanismState's additional state, see ``contact_dynamics_``) are advanced in place; pass the same ``contact_state`` to the next
+    call to continue.  Within the rollout a pair out of contact keeps its state (ṡ = 0): the reference's resets never survive its
+    integrator (include/rbd_b200.h, rbd_integrate_contact).  ``torques``: None, constant [nv, B], per step [nsteps, nv, B] or per
+    stage [nsteps, 4, nv, B], as for ``simulate_trajectory_``.  ``contact``: the mechanism's ``contact_desc`` by default.  Returns
+    the number of steps taken."""
+    nsteps, t = 0, 0.0
+    while t < final_time:            # the reference's `while t < final_time` loop (ode_integrators.jl:311)
+        t += dt
+        nsteps += 1
+    _integrate_contact(state, nsteps, contact_state, torques, dt, contact, False, "simulate_contact_")
+    return nsteps

@@ -499,6 +499,52 @@ contact_kernel(const __grid_constant__ ModelDev<T> M, const __grid_constant__ Co
   }
 }
 
+// One RK4 stage of the contact rollout (rbd_integrate_contact): the EXT aba_kernel with the contact pass (contact_stage_pass,
+// rbd_kin.cuh) in place of ext_wrench_pass, and scratch rows only for the bodies that carry contact points (ContactScr).  Every
+// array has leading dimension B (the rollout's dense workspace).
+template <class T> struct ContactAbaArgs {
+  const T* q; const T* v; const T* tau;    // stage state, torques (NULL: zero)
+  const T* s0; const T* sdp;               // contact state at the start of the step, ṡ of the previous stage (NULL at stage 0)
+  T* vd; T* sd;                            // v̇_i, ṡ_i
+  T* scratch;                              // [6 * nw][grid threads] body-frame contact wrenches, one column per resident thread
+  T wa;                                    // dt * a_i
+  int64_t B;
+  int8_t wslot[kMaxBodies];                // scratch slot of each body (preorder), -1 = no contact points (ContactScr)
+};
+template <class T, int NT, bool GENERAL, int KINDS>
+__global__ void __launch_bounds__(NT, 1)
+aba_contact_kernel(const __grid_constant__ ModelDev<T> M, const __grid_constant__ ContactDev<T> C,
+                   const __grid_constant__ ContactAbaArgs<T> a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  using ST = Stash<T, NT>;
+  const ST st{reinterpret_cast<T*>(smem_raw) + threadIdx.x};
+  const int64_t nthreads = (int64_t)gridDim.x * NT;
+  const int64_t tid = (int64_t)blockIdx.x * NT + threadIdx.x;
+  const int64_t ngroups = (a.B + NT - 1) / NT;
+  for (int64_t g = blockIdx.x; g < ngroups; g += gridDim.x) {
+    const int64_t gn = g + gridDim.x;
+    if (gn < ngroups) {
+      const int64_t bn = gn * NT + (threadIdx.x & ~31);
+      prefetch_rows(a.q, M.nq, a.B, bn);
+      prefetch_rows(a.v, M.nv, a.B, bn);
+      prefetch_rows(a.tau, M.nv, a.B, bn);
+    }
+    const int64_t b = g * NT + threadIdx.x;
+    const bool active = b < a.B;
+    const int64_t bl = active ? b : a.B - 1;     // inactive lanes recompute the last sample, stores are masked
+    ContactAbaIO<T, KINDS> io;
+    io.q = {a.q + bl, a.B};
+    io.v = {a.v + bl, a.B};
+    io.tau = {a.tau ? a.tau + bl : nullptr, a.B};
+    io.vd = {a.vd + bl, a.B, active};
+    io.qd = {nullptr, a.B, active};
+    io.ext = {a.scratch ? a.scratch + tid : nullptr, nthreads, a.wslot};
+    const ContactStageIO<T> cs{a.s0 ? a.s0 + bl : nullptr, a.sdp ? a.sdp + bl : nullptr, a.sd ? a.sd + bl : nullptr, a.wa, a.B, active};
+    contact_stage_pass(M, C, io.q, io.v, cs, io.ext, st, M.slot_base, kSlotRowsAba);
+    aba_sample<T, ST, GENERAL>(M, io, st);
+  }
+}
+
 constexpr int kNT = 32;   // threads per block: one warp; warps never synchronise with each other
 
 // Launch `kernel` persistently with a stash of `rows` rows per thread in shared memory (plan_persistent).  `scratch_rows` > 0
@@ -885,21 +931,82 @@ __global__ void __launch_bounds__(128) integrate_finish_kernel(const __grid_cons
   }
 }
 
+// The contact rollout's finishing rows (ode_integrators.jl:283-296 on the additional state, in plain Euclidean form):
+// s = s0 + dt sum_i b_i ṡ_i into s (leading dimension ld), and into s0 as well when another step follows.
+template <class T> struct ContactFinishArgs {
+  T* s0; const T* sd[4];
+  T* s;
+  T w[4]; T dt;
+  int64_t B, ld, ns;
+  bool refresh;
+};
+template <class T>
+__global__ void __launch_bounds__(256) contact_finish_kernel(const ContactFinishArgs<T> a) {
+  const int64_t total = a.ns * a.B;
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = e / a.B, b = e - r * a.B;
+    const T x = a.s0[e] + a.dt * (a.w[0] * a.sd[0][e] + a.w[1] * a.sd[1][e] + a.w[2] * a.sd[2][e] + a.w[3] * a.sd[3][e]);
+    a.s[r * a.ld + b] = x;
+    if (a.refresh) a.s0[e] = x;
+  }
+}
+
+// rbd_integrate_contact: the contact descriptor in device form and the caller's contact state s [ns x B] (leading dimension ld) with
+// its optional trajectory [(nsteps + 1) x ns x B].
+template <class T> struct ContactRollout {
+  const ContactDev<T>* C;
+  int64_t ns;
+  T* s; T* traj_s;
+};
+
+// Forward dynamics of one stage of the contact rollout: aba_contact_kernel in the variant dynamics_t would pick for the EXT path.
+template <class T>
+int contact_stage_launch(const HostModel& hm, const ModelDev<T>& M, const ContactDev<T>& C, ContactAbaArgs<T> a, cudaStream_t stream,
+                         std::optional<LaunchPlan>& plan) {
+  const int nw = contact_wrench_slots(hm.nb, C, a.wslot);
+  bool other_kinds = false;
+  for (int i = 0; i < hm.nb; ++i) other_kinds |= (M.body[i].kind == K_PRIS || M.body[i].kind == K_FIXED);
+  auto kernel = hm.general ? aba_contact_kernel<T, kNT, true, kAllKinds>
+                           : (other_kinds ? aba_contact_kernel<T, kNT, false, kAllKinds> : aba_contact_kernel<T, kNT, false, 0>);
+  if (!plan) {        // one plan (grid and scratch) for every stage of the call
+    plan.emplace();
+    if (int rc = plan_persistent((const void*)kernel, kNT, (size_t)M.nrows * kNT * sizeof(T), (a.B + kNT - 1) / kNT, stream, *plan,
+                                 (size_t)6 * nw * sizeof(T))) return rc;
+  }
+  a.scratch = (T*)plan->work.p;
+  kernel<<<plan->grid, plan->block, plan->smem, stream>>>(M, C, a);
+  return api_launched(&*plan);
+}
+
 // traj_q / traj_v (rbd_integrate_trajectory): [(nsteps + 1) x rows x B] -- block 0 the initial state, block s + 1 written by the
 // finishing kernels of step s; q / v receive the final state as without them.  stages (rbd_integrate_vjp's recompute, nsteps = 1):
 // the four stages' (qs_i, vs_i, φ̇_i, v̇_i) are kept in [4 nq + 12 nv] x B rows (stage_rows) and the finishing step is skipped.
+// contact (rbd_integrate_contact): every stage's dynamics is aba_contact_kernel, which also writes ṡ_i, and the finishing step
+// also advances the contact state (contact_finish_kernel); the q / v kernels are the same.
 template <class T>
 int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v, const void* tau, int64_t step_stride,
                 int64_t stage_stride, double dt, int nsteps, cudaStream_t stream, T* traj_q = nullptr, T* traj_v = nullptr,
-                T* stages = nullptr) {
+                T* stages = nullptr, const ContactRollout<T>* contact = nullptr) {
   const HostModel& hm = model->hm;
   const ModelDev<T>& M = dev_model<T>(hm);
   DeviceProps p;
   RBD_CUDA_TRY(device_props(p));
   const size_t nq = hm.nq, nv = hm.nv;
+  const size_t ns = contact ? (size_t)contact->ns : 0;
   const size_t rows = 2 * nq + 10 * nv + (tau && ld != B ? nv : 0);
-  StreamAlloc work;
+  StreamAlloc work, swork;
   RBD_CUDA_TRY(work.alloc(rows * (size_t)B * sizeof(T), stream));
+  // contact state: s0 (the state at the start of the step, refreshed like q0 / v0) and the four stages' ṡ_i, [ns x B] each
+  T* s0 = nullptr;
+  T* sd[4] = {nullptr, nullptr, nullptr, nullptr};
+  std::optional<LaunchPlan> contact_plan;
+  if (ns) {
+    RBD_CUDA_TRY(swork.alloc(5 * ns * (size_t)B * sizeof(T), stream));
+    s0 = (T*)swork.p;
+    for (int i = 0; i < 4; ++i) sd[i] = s0 + (1 + (size_t)i) * ns * B;
+    RBD_CUDA_TRY(cudaMemcpy2DAsync(s0, B * sizeof(T), contact->s, ld * sizeof(T), B * sizeof(T), ns, cudaMemcpyDeviceToDevice, stream));
+    if (contact->traj_s) RBD_CUDA_TRY(cudaMemcpyAsync(contact->traj_s, s0, ns * B * sizeof(T), cudaMemcpyDeviceToDevice, stream));
+  }
   T* q0 = (T*)work.p; T* qs = q0 + nq * B; T* v0 = qs + nq * B; T* vs = v0 + nv * B;
   T* phid[4]; T* vd[4];
   for (int i = 0; i < 4; ++i) { phid[i] = vs + (size_t)(1 + i) * nv * B; vd[i] = vs + (size_t)(5 + i) * nv * B; }
@@ -958,7 +1065,12 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
         integrate_stage_kernel<T><<<dim3(grid, hm.nb), 128, 0, stream>>>(M, sa);
         if (int rc = api_launched()) return rc;
       }
-      if (int rc = dynamics_t<T>(model, B, B, qsi[i], vsi[i], tau_dense, nullptr, vd[i], nullptr, stream)) return rc;
+      if (contact) {
+        const ContactAbaArgs<T> ca{qsi[i], vsi[i], tau_dense, s0, i ? sd[i - 1] : nullptr, vd[i], sd[i], nullptr, (T)(dt * a[i]), B};
+        if (int rc = contact_stage_launch<T>(hm, M, *contact->C, ca, stream, contact_plan)) return rc;
+      } else if (int rc = dynamics_t<T>(model, B, B, qsi[i], vsi[i], tau_dense, nullptr, vd[i], nullptr, stream)) {
+        return rc;
+      }
     }
     if (stages) return RBD_OK;
     T* qo = traj_q ? traj_q + (size_t)(s + 1) * nq * B : (T*)q;
@@ -973,6 +1085,14 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
       integrate_finish_kernel<T><<<dim3(grid, hm.nb), 128, 0, stream>>>(M, fa);
       if (int rc = api_launched()) return rc;
     }
+    if (ns) {
+      const bool rec = contact->traj_s != nullptr;
+      const ContactFinishArgs<T> cf{s0, {sd[0], sd[1], sd[2], sd[3]}, rec ? contact->traj_s + (size_t)(s + 1) * ns * B : contact->s,
+                                    {(T)bw[0], (T)bw[1], (T)bw[2], (T)bw[3]}, (T)dt, B, rec ? B : ld, (int64_t)ns, s + 1 < nsteps};
+      const int grid_s = (int)std::min<int64_t>(((int64_t)ns * B + 255) / 256, (int64_t)p.sms * 8);
+      contact_finish_kernel<T><<<grid_s, 256, 0, stream>>>(cf);
+      if (int rc = api_launched()) return rc;
+    }
   }
   if (traj_q && nsteps > 0) {      // the final state into the caller's q / v, as rbd_integrate leaves it
     RBD_CUDA_TRY(cudaMemcpy2DAsync(q, ld * sizeof(T), traj_q + (size_t)nsteps * nq * B, B * sizeof(T), B * sizeof(T), nq,
@@ -980,6 +1100,9 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
     RBD_CUDA_TRY(cudaMemcpy2DAsync(v, ld * sizeof(T), traj_v + (size_t)nsteps * nv * B, B * sizeof(T), B * sizeof(T), nv,
                                    cudaMemcpyDeviceToDevice, stream));
   }
+  if (ns && contact->traj_s && nsteps > 0)
+    RBD_CUDA_TRY(cudaMemcpy2DAsync(contact->s, ld * sizeof(T), contact->traj_s + (size_t)nsteps * ns * B, B * sizeof(T), B * sizeof(T),
+                                   ns, cudaMemcpyDeviceToDevice, stream));
   return RBD_OK;
 }
 
@@ -1075,6 +1198,38 @@ int contact_t(const rbd_model* model, int64_t B, int64_t ld, const void* q, cons
                                stream, pl)) return rc;
   kernel<<<pl.grid, pl.block, pl.smem, stream>>>(M, C, a);
   return api_launched(&pl);
+}
+
+template <class T>
+int integrate_contact_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau, int64_t step_stride,
+                        int64_t stage_stride, const rbd_contact_desc& cd, double dt, int nsteps, void* q_traj, void* v_traj, void* s_traj,
+                        cudaStream_t stream) {
+  const HostModel& hm = model->hm;
+  std::unique_ptr<ContactDev<T>> C(new ContactDev<T>());     // passed by value to every stage's launch
+  build_contact_dev<T>(hm.nb, hm.pos.data(), hm.alignT.data(), cd, *C);
+  const ContactRollout<T> cr{C.get(), (int64_t)3 * cd.npoints * cd.nhalfspaces, (T*)s, (T*)s_traj};
+  return integrate_t<T>(model, B, ld, q, v, tau, step_stride, stage_stride, dt, nsteps, stream, (T*)q_traj, (T*)v_traj, nullptr, &cr);
+}
+
+// the descriptor checks of rbd_contact_dynamics and rbd_integrate_contact
+int check_contact(const rbd_model* model, const rbd_contact_desc* contact, const char* fn) {
+  const std::string f = fn;
+  if (!contact) return fail(RBD_EINVAL, f + ": contact must not be NULL");
+  if (contact->npoints < 0 || contact->nhalfspaces < 0) return fail(RBD_EINVAL, f + ": negative counts");
+  if (contact->npoints > kMaxContactPoints || contact->nhalfspaces > kMaxHalfSpaces)
+    return fail(RBD_EUNSUPPORTED, f + ": at most 32 contact points and 4 half-spaces");
+  if (contact->npoints && (!contact->body || !contact->location || !contact->normal_model || !contact->friction_model))
+    return fail(RBD_EINVAL, f + ": point arrays must not be NULL");
+  if (contact->nhalfspaces && !contact->halfspace) return fail(RBD_EINVAL, f + ": halfspace must not be NULL");
+  for (int p = 0; p < contact->npoints; ++p) {
+    if (contact->body[p] < 0 || contact->body[p] >= model->hm.nb) return fail(RBD_EINVAL, f + ": body index out of range");
+    if (!(contact->friction_model[3 * p + 2] > 0)) return fail(RBD_EINVAL, f + ": friction damping b must be > 0");
+  }
+  for (int h = 0; h < contact->nhalfspaces; ++h) {
+    const double* n = contact->halfspace + 6 * h + 3;
+    if (!(n[0] * n[0] + n[1] * n[1] + n[2] * n[2] > 0)) return fail(RBD_EINVAL, f + ": zero half-space normal");
+  }
+  return RBD_OK;
 }
 
 int check_common(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, bool allow_dual = false) {
@@ -1402,26 +1557,37 @@ int32_t rbd_contact_dynamics(const rbd_model* model, int32_t dtype, int64_t B, i
                              const rbd_contact_desc* contact, void* state, void* state_deriv_out, void* wrenches_out, void* stream) {
   if (int rc = check_common(model, dtype, B, ld)) return rc;
   const ApiCall call;
-  if (!contact) return fail(RBD_EINVAL, "rbd_contact_dynamics: contact must not be NULL");
-  if (contact->npoints < 0 || contact->nhalfspaces < 0) return fail(RBD_EINVAL, "rbd_contact_dynamics: negative counts");
-  if (contact->npoints > kMaxContactPoints || contact->nhalfspaces > kMaxHalfSpaces)
-    return fail(RBD_EUNSUPPORTED, "rbd_contact_dynamics: at most 32 contact points and 4 half-spaces");
-  if (contact->npoints && (!contact->body || !contact->location || !contact->normal_model || !contact->friction_model))
-    return fail(RBD_EINVAL, "rbd_contact_dynamics: point arrays must not be NULL");
-  if (contact->nhalfspaces && !contact->halfspace) return fail(RBD_EINVAL, "rbd_contact_dynamics: halfspace must not be NULL");
-  for (int p = 0; p < contact->npoints; ++p) {
-    if (contact->body[p] < 0 || contact->body[p] >= model->hm.nb) return fail(RBD_EINVAL, "rbd_contact_dynamics: body index out of range");
-    if (!(contact->friction_model[3 * p + 2] > 0)) return fail(RBD_EINVAL, "rbd_contact_dynamics: friction damping b must be > 0");
-  }
-  for (int h = 0; h < contact->nhalfspaces; ++h) {
-    const double* n = contact->halfspace + 6 * h + 3;
-    if (!(n[0] * n[0] + n[1] * n[1] + n[2] * n[2] > 0)) return fail(RBD_EINVAL, "rbd_contact_dynamics: zero half-space normal");
-  }
+  if (int rc = check_contact(model, contact, "rbd_contact_dynamics")) return rc;
   if (B == 0) return RBD_OK;
   if (!q || !v || !wrenches_out) return fail(RBD_EINVAL, "rbd_contact_dynamics: q, v and wrenches_out must not be NULL");
   cudaStream_t s = (cudaStream_t)stream;
   return dtype == RBD_F32 ? contact_t<float>(model, B, ld, q, v, *contact, state, state_deriv_out, wrenches_out, s)
                           : contact_t<double>(model, B, ld, q, v, *contact, state, state_deriv_out, wrenches_out, s);
+}
+
+int32_t rbd_integrate_contact(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau,
+                              int64_t tau_step_stride, int64_t tau_stage_stride, const rbd_contact_desc* contact, double dt, int32_t nsteps,
+                              void* q_traj, void* v_traj, void* s_traj, void* stream) {
+  if (!model) return fail(RBD_EINVAL, "model handle is NULL");
+  if (dtype != RBD_F32 && dtype != RBD_F64) return fail(RBD_EUNSUPPORTED, "rbd_integrate_contact: fp32 / fp64 only");
+  if (int rc = check_common(model, dtype, B, ld)) return rc;
+  if (nsteps < 0 || !(dt > 0)) return fail(RBD_EINVAL, "rbd_integrate_contact: need dt > 0 and nsteps >= 0");
+  if (tau_step_stride < 0 || tau_stage_stride < 0) return fail(RBD_EINVAL, "rbd_integrate_contact: torque strides must be >= 0");
+  if (int rc = check_contact(model, contact, "rbd_integrate_contact")) return rc;
+  const int64_t ns = (int64_t)3 * contact->npoints * contact->nhalfspaces;
+  const bool rec = q_traj || v_traj || s_traj;
+  if (rec && (!q_traj || !v_traj || (ns > 0 && !s_traj)))
+    return fail(RBD_EINVAL, "rbd_integrate_contact: q_traj, v_traj and s_traj must be all NULL or all set");
+  const ApiCall call;
+  if (B == 0) return RBD_OK;
+  if (!q || !v) return fail(RBD_EINVAL, "rbd_integrate_contact: q and v must not be NULL");
+  if (ns > 0 && !s) return fail(RBD_EINVAL, "rbd_integrate_contact: s must not be NULL when there are contact pairs");
+  if (nsteps == 0 && !rec) return RBD_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  return dtype == RBD_F32 ? integrate_contact_t<float>(model, B, ld, q, v, s, tau, tau_step_stride, tau_stage_stride, *contact, dt, nsteps,
+                                                       q_traj, v_traj, s_traj, st)
+                          : integrate_contact_t<double>(model, B, ld, q, v, s, tau, tau_step_stride, tau_stage_stride, *contact, dt, nsteps,
+                                                        q_traj, v_traj, s_traj, st);
 }
 
 int32_t rbd_dynamics_result(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,

@@ -626,6 +626,31 @@ inline void build_contact_dev(int nb, const int* pos, const double* alignT, cons
   }
 }
 
+// The force law of one (point pi, half-space with unit normal n) pair in contact: penetration z >= 0, point velocity vel (root
+// frame), tangential displacement xs(k), k = 0..2 (read inside, where the friction force needs it).  Out: the force on the body f
+// (root frame) and the state derivative xd.  Shared by contact_sample and the rollout's contact pass (contact_stage_pass).
+template <class T, class XS>
+RBD_HD void contact_force(const ContactDev<T>& C, int pi, const T* n, T z, const T* vel, const XS& xs, T* f, T* xd) {
+  const T zd = -(vel[0] * n[0] + vel[1] * n[1] + vel[2] * n[2]);
+  const T zn = contact_pow(z, C.hc[pi][2]);
+  T fn = C.hc[pi][1] * zn * zd + C.hc[pi][0] * zn;
+  fn = fn > T(0) ? fn : T(0);
+  const T mu = C.fr[pi][0], kf = C.fr[pi][1], bf = C.fr[pi][2];
+  T x[3], ft[3];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    x[k] = xs(k);
+    ft[k] = -kf * x[k] - bf * (vel[k] + zd * n[k]);          // f_stick; tangential velocity = velocity + zdot * normal
+  }
+  const T n2 = ft[0] * ft[0] + ft[1] * ft[1] + ft[2] * ft[2], m2 = (mu * fn) * (mu * fn);
+  if (n2 > m2) {
+    const T sc = contact_sqrt(m2 / n2);
+    ft[0] *= sc; ft[1] *= sc; ft[2] *= sc;
+  }
+#pragma unroll
+  for (int k = 0; k < 3; ++k) { f[k] = fn * n[k] + ft[k]; xd[k] = (-kf * x[k] - ft[k]) / bf; }
+}
+
 template <class T, class ST>
 RBD_HD void contact_sample(const ModelDev<T>& M, const ContactDev<T>& C, const ContactIO<T>& io, const ST& st) {
   const int nb = M.nb;
@@ -679,26 +704,8 @@ RBD_HD void contact_sample(const ModelDev<T>& M, const ContactDev<T>& C, const C
         const T sep = (pt[0] - C.hp[h][0]) * n[0] + (pt[1] - C.hp[h][1]) * n[1] + (pt[2] - C.hp[h][2]) * n[2];
         T xd[3] = {T(0), T(0), T(0)};
         if (sep <= T(0)) {
-          const T z = -sep;
-          const T zd = -(vel[0] * n[0] + vel[1] * n[1] + vel[2] * n[2]);
-          const T zn = contact_pow(z, C.hc[pi][2]);
-          T fn = C.hc[pi][1] * zn * zd + C.hc[pi][0] * zn;
-          fn = fn > T(0) ? fn : T(0);
-          const T mu = C.fr[pi][0], kf = C.fr[pi][1], bf = C.fr[pi][2];
-          T x[3], ft[3];
-#pragma unroll
-          for (int k = 0; k < 3; ++k) {
-            x[k] = io.s ? io.s[(srow + k) * io.ld] : T(0);
-            ft[k] = -kf * x[k] - bf * (vel[k] + zd * n[k]);          // f_stick; tangential velocity = velocity + zdot * normal
-          }
-          const T n2 = ft[0] * ft[0] + ft[1] * ft[1] + ft[2] * ft[2], m2 = (mu * fn) * (mu * fn);
-          if (n2 > m2) {
-            const T sc = contact_sqrt(m2 / n2);
-            ft[0] *= sc; ft[1] *= sc; ft[2] *= sc;
-          }
           T f[3];
-#pragma unroll
-          for (int k = 0; k < 3; ++k) { f[k] = fn * n[k] + ft[k]; xd[k] = (-kf * x[k] - ft[k]) / bf; }
+          contact_force(C, pi, n, -sep, vel, [&](int k) { return io.s ? io.s[(srow + k) * io.ld] : T(0); }, f, xd);
           T m[3];
           cross3(pt, f, m);                                   // Wrench(point, force)
 #pragma unroll
@@ -727,6 +734,144 @@ RBD_HD void contact_sample(const ModelDev<T>& M, const ContactDev<T>& C, const C
     }
     cur = w; twc = tw;
   }
+}
+
+// ==================================================================================================================
+// The contact pass of the contact rollout (rbd_integrate_contact, DESIGN 4.14): contact_dynamics! at one RK4 stage, as the
+// pre-pass of the forward-dynamics kernel.  It replaces ext_wrench_pass there: same outward sweep, with the twist tracked next to
+// the pose (branch nodes park both, 18 rows, in the ABA stash's pending slots), and the same output -- every body's wrench in its
+// own frame in the scratch rows aba_sample reads.  The stage's contact state  s_i = s0 + wa sd_prev  (wa = dt a_i, sd_prev = ṡ of
+// the previous stage, NULL at stage 0) is formed from two loads per pair in contact and never stored.  ṡ_i is written for every
+// pair, zero out of contact; nothing is reset: within the reference's integrator a reset does not survive the stage (DESIGN 4.14).
+// Only the bodies that carry contact points have scratch rows (ContactScr): 2 x 6 rows per sample for a biped instead of 6 nb.
+// ==================================================================================================================
+template <class T> struct ContactStageIO {
+  const T* s0; const T* sdp;    // [ns] rows of this sample's column (leading dimension ld)
+  T* sd;                        // ṡ_i out, same shape
+  T wa;
+  int64_t ld;
+  bool active;
+};
+static_assert(kSlotRowsAba >= 18, "the contact pass parks pose and twist in the ABA pending slots");
+
+// The scratch column of the body-frame contact wrenches: rows 6 slot[i] .. + 5 for body i (preorder) if it carries contact points
+// (slot[i] >= 0, in preorder), none otherwise.  get() is the view aba_sample reads, rows 6 i + k of every body: zero without rows.
+template <class T> struct ContactScr {
+  T* p;
+  int64_t ld;
+  const int8_t* slot;           // [nb]
+  RBD_HD T get(int row) const {
+    const int i = row / 6, c = slot[i];
+    return c < 0 ? T(0) : p[(int64_t)(6 * c + row - 6 * i) * ld];
+  }
+};
+// host side: slot[] of the bodies that carry points; returns their number
+template <class T> inline int contact_wrench_slots(int nb, const ContactDev<T>& C, int8_t* slot) {
+  int n = 0;
+  for (int i = 0; i < nb; ++i) slot[i] = (int8_t)(C.first[i + 1] > C.first[i] ? n++ : -1);
+  return n;
+}
+// aba_sample's IO for the contact rollout: AbaIO with the external wrenches read through ContactScr
+template <class T, int KINDS> struct ContactAbaIO {
+  static constexpr bool kExt = true;
+  static constexpr int kKinds = KINDS;
+  Col<T> q, v, tau;
+  ColOut<T> vd, qd;
+  ContactScr<T> ext;
+};
+
+template <class T, class ST>
+RBD_HD void contact_stage_pass(const ModelDev<T>& M, const ContactDev<T>& C, const Col<T>& q, const Col<T>& v,
+                               const ContactStageIO<T>& io, const ContactScr<T>& ext, const ST& st, int slot_base, int slot_rows) {
+  Pose<T> cur;
+  pose_identity(cur);
+  Mot<T> twc;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) twc.w[k] = twc.l[k] = T(0);
+  for (int i = 0; i < M.nb; ++i) {
+    const BodyDev<T>& bd = M.body[i];
+    Pose<T> pp;
+    Mot<T> twp;
+    if (bd.flags & F_ROOT_CHILD) {
+      pose_identity(pp);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) twp.w[k] = twp.l[k] = T(0);
+    } else if (bd.flags & F_FIRST_CHILD) {
+      pp = cur; twp = twc;
+    } else {
+      const int row = slot_base + bd.pslot * slot_rows;
+      T t[18];
+      st.fence_st();
+      st.template ldv<18>(row, t);
+#pragma unroll
+      for (int k = 0; k < 9; ++k) pp.R[k] = t[k];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) { pp.p[k] = t[9 + k]; twp.w[k] = t[12 + k]; twp.l[k] = t[15 + k]; }
+    }
+    T R[9], r[3], t[3];
+    frame_any(bd, q, R, r);
+    Pose<T> w;
+    mat_mul3(pp.R, R, w.R);
+    mat_vec(pp.R, r, t);
+    w.p[0] = pp.p[0] + t[0]; w.p[1] = pp.p[1] + t[1]; w.p[2] = pp.p[2] + t[2];
+    Mot<T> tw = twp;
+    const int nvj = kind_nv_dev(bd.kind);
+    for (int k = 0; k < nvj; ++k) {
+      Mot<T> S;
+      world_subspace(w, sub_comp(bd.kind, k), S);
+      const T x = v(bd.vrow + k);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) { tw.w[c] += x * S.w[c]; tw.l[c] += x * S.l[c]; }
+    }
+    T wn[3] = {T(0), T(0), T(0)}, wf[3] = {T(0), T(0), T(0)};      // root frame, as contact_sample sums them
+    for (int pi = C.first[i]; pi < C.first[i + 1]; ++pi) {
+      T pt[3], vel[3], tmp[3];
+      mat_vec(w.R, C.loc[pi], tmp);
+      pt[0] = w.p[0] + tmp[0]; pt[1] = w.p[1] + tmp[1]; pt[2] = w.p[2] + tmp[2];
+      cross3(tw.w, pt, vel);
+      vel[0] += tw.l[0]; vel[1] += tw.l[1]; vel[2] += tw.l[2];
+      for (int h = 0; h < C.nhalf; ++h) {
+        const int64_t srow = (int64_t)3 * (C.orig[pi] * C.nhalf + h);
+        const T* n = C.hn[h];
+        const T sep = (pt[0] - C.hp[h][0]) * n[0] + (pt[1] - C.hp[h][1]) * n[1] + (pt[2] - C.hp[h][2]) * n[2];
+        T xd[3] = {T(0), T(0), T(0)};
+        if (sep <= T(0)) {
+          T f[3], m[3];
+          contact_force(C, pi, n, -sep, vel, [&](int k) {        // s_i = s0 + wa sd_prev
+            const int64_t e = (srow + k) * io.ld;
+            return io.sdp ? io.s0[e] + io.wa * io.sdp[e] : io.s0[e];
+          }, f, xd);
+          cross3(pt, f, m);
+#pragma unroll
+          for (int k = 0; k < 3; ++k) { wn[k] += m[k]; wf[k] += f[k]; }
+        }
+        if (io.active) {
+#pragma unroll
+          for (int k = 0; k < 3; ++k) io.sd[(srow + k) * io.ld] = xd[k];
+        }
+      }
+    }
+    const int c = ext.slot[i];
+    if (c >= 0) {      // root frame -> body frame as ext_wrench_pass:  f_b = Rw^T f ,  n_b = Rw^T (n - pw x f)
+      T m[3], nb_[3], fb[3];
+      cross3(w.p, wf, m);
+      m[0] = wn[0] - m[0]; m[1] = wn[1] - m[1]; m[2] = wn[2] - m[2];
+      matT_vec(w.R, m, nb_);
+      matT_vec(w.R, wf, fb);
+      T* o = ext.p + (int64_t)6 * c * ext.ld;
+#pragma unroll
+      for (int k = 0; k < 3; ++k) { o[k * ext.ld] = nb_[k]; o[(3 + k) * ext.ld] = fb[k]; }
+    }
+    if (bd.flags & F_HAS_PENDING) {
+      const int row = slot_base + bd.oslot * slot_rows;
+#pragma unroll
+      for (int k = 0; k < 9; ++k) st.st(row + k, w.R[k]);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) { st.st(row + 9 + k, w.p[k]); st.st(row + 12 + k, tw.w[k]); st.st(row + 15 + k, tw.l[k]); }
+    }
+    cur = w; twc = tw;
+  }
+  st.fence_st();     // the slots are re-used by aba_sample
 }
 
 }  // namespace rbd
