@@ -421,6 +421,26 @@ int32_t rbd_integrate_contact(const rbd_model* model, int32_t dtype, int64_t B, 
                               int64_t tau_step_stride, int64_t tau_stage_stride, const rbd_contact_desc* contact, double dt, int32_t nsteps,
                               void* q_traj, void* v_traj, void* s_traj, void* stream);
 
+/* Reverse mode through a contact rollout (DESIGN 4.15): the gradient of
+ *   L = sum_s q_traj_bar[s] . q_traj[s] + v_traj_bar[s] . v_traj[s] + s_traj_bar[s] . s_traj[s]
+ * with respect to the initial state (q, v, s) and the torques, for the trajectory rbd_integrate_contact recorded with the same tau,
+ * strides, contact descriptor, dt and nsteps.  The conventions are rbd_integrate_vjp's: leading dimension B; s_traj / s_traj_bar
+ * [(nsteps+1) x ns x B] (ns = 3 npoints nhalfspaces); the *_bar inputs may be NULL (zero); outputs q0_bar_tan, q0_bar_cfg, v0_bar,
+ * s0_bar [ns x B] may be NULL; tau_bar is ADDED TO, so a rollout split into consecutive calls gives the gradients of one call, bit
+ * for bit; nsteps == 0 is the identity.  The contact force law is differentiated as implemented, on the branch each pair takes (in
+ * or out of contact, f_n clamped at 0, stick or slip); a point exactly on the surface gets the one-sided derivative of z^n; a pair
+ * out of contact passes its s adjoint through unchanged.  No gradient reaches the contact parameters or dt.  Descriptor checks as
+ * rbd_contact_dynamics; dtype other than fp32 / fp64: RBD_EUNSUPPORTED; the argument errors of rbd_integrate_vjp and s_traj == NULL
+ * with ns > 0: RBD_EINVAL; B == 0: nothing to do.  Kernels per step: the recompute of rbd_integrate_contact's step without its
+ * finishing kernels, 5 elementwise phases (1 or 2 kernels each, as rbd_integrate_vjp), 4 stage adjoints (one kernel each), and
+ * one configuration-covector kernel between steps.  Mechanisms with loops are not supported (the Python layer refuses them with
+ * RBD_ELOOP). */
+int32_t rbd_integrate_contact_vjp(const rbd_model* model, int32_t dtype, int64_t B, const void* q_traj, const void* v_traj,
+                                  const void* s_traj, const void* tau, int64_t tau_step_stride, int64_t tau_stage_stride,
+                                  const rbd_contact_desc* contact, double dt, int32_t nsteps, const void* q_traj_bar,
+                                  const void* v_traj_bar, const void* s_traj_bar, void* q0_bar_tan, void* q0_bar_cfg, void* v0_bar,
+                                  void* s0_bar, void* tau_bar, void* stream);
+
 /* Next row of the scope table (SURVEY 8(f) rank 2): kinematics by-products of the same outward sweep, all expressed in the
  * mechanism's root frame, 6-vectors as [angular; linear].  Every output pointer may be NULL (not computed).
  *   transforms_to_root  [12*nb x B]  rows 12 i .. 12 i + 11 = transform_to_root(state, successor of tree joint i):

@@ -3,9 +3,12 @@
     dynamics_vjp_          ν̄ᵀ ∂v̇/∂(q, v, τ, w_ext)        rbd_dynamics_vjp          (include/rbd_b200.h, csrc/rbd_adjoint.cuh)
     inverse_dynamics_vjp_  τ̄ᵀ ∂τ/∂(q, v, v̇, w_ext)         rbd_inverse_dynamics_vjp
     integrate_vjp_         gradient of a recorded rollout       rbd_integrate_vjp         (csrc/rbd_integrate_adjoint.cuh)
+    integrate_contact_vjp_ gradient of a recorded contact rollout  rbd_integrate_contact_vjp  (csrc/rbd_contact_adjoint.cuh)
     dynamics(mechanism, q, v, tau=None, externalwrenches=None)         differentiable v̇ = dynamics!(...)
     inverse_dynamics(mechanism, q, v, vd, externalwrenches=None)       differentiable τ = inverse_dynamics!(...)
     simulate(mechanism, q0, v0, torques=None, *, dt, nsteps, ...)     differentiable RK4 rollout (simulate)
+    simulate_contact(mechanism, q0, v0, s0, torques=None, *, contact, dt, nsteps, ...)
+                                                                       differentiable RK4 rollout with soft contact
 
 One product costs one Articulated-Body solve (forward dynamics only) plus one outward and one inward sweep: O(n) per sample, no
 nv x nv Jacobian is formed (``dynamics_derivatives_`` builds both full Jacobians instead).  Every tensor is ``[rows, B]``, contiguous,
@@ -30,7 +33,8 @@ from .algorithms import DimensionMismatch, _check, _ptr, _require_tree
 from .mechanism import Mechanism
 from .state import _DT, MechanismState, _model_handle
 
-__all__ = ["dynamics_vjp_", "inverse_dynamics_vjp_", "integrate_vjp_", "dynamics", "inverse_dynamics", "simulate"]
+__all__ = ["dynamics_vjp_", "inverse_dynamics_vjp_", "integrate_vjp_", "integrate_contact_vjp_", "dynamics", "inverse_dynamics", "simulate",
+           "simulate_contact"]
 
 
 def _stream(t: torch.Tensor):
@@ -325,3 +329,142 @@ def simulate(mechanism: Mechanism, q0: torch.Tensor, v0: torch.Tensor, torques: 
     segment of k steps before its VJP: peak memory O((nsteps / k + k) (nq + nv) B) instead of O(nsteps (nq + nv) B).  The gradients
     do not depend on k, bit for bit.  Not twice differentiable."""
     return _Simulate.apply(mechanism, q0, v0, torques, float(dt), int(nsteps), bool(trajectory), checkpoint_every)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# contact rollouts: rbd_integrate_contact (recording) / rbd_integrate_contact_vjp
+# ----------------------------------------------------------------------------------------------------------------------
+def _check_blocks(what: str, like: torch.Tensor, items):
+    for t, shape, name in items:
+        if t is None:
+            continue
+        if t.dtype != like.dtype or t.device != like.device or not t.is_contiguous():
+            raise TypeError(f"{what}: {name} must be contiguous, with the dtype and device of q_traj")
+        if shape is None or tuple(t.shape) != shape:
+            raise DimensionMismatch(f"{what}: {name} has wrong size: expected {shape}, got {tuple(t.shape)}")
+
+
+def integrate_contact_vjp_(mechanism: Mechanism, q_traj: torch.Tensor, v_traj: torch.Tensor, s_traj: torch.Tensor,
+                           torques: Optional[torch.Tensor] = None, *, contact, dt: float, q_traj_bar: Optional[torch.Tensor] = None,
+                           v_traj_bar: Optional[torch.Tensor] = None, s_traj_bar: Optional[torch.Tensor] = None,
+                           q0_bar_tan: Optional[torch.Tensor] = None, q0_bar_cfg: Optional[torch.Tensor] = None,
+                           v0_bar: Optional[torch.Tensor] = None, s0_bar: Optional[torch.Tensor] = None,
+                           tau_bar: Optional[torch.Tensor] = None):
+    """Gradient of ``L = sum_s q_traj_bar[s] . q_traj[s] + v_traj_bar[s] . v_traj[s] + s_traj_bar[s] . s_traj[s]`` over a trajectory
+    recorded by ``simulate_contact_trajectory_`` ([nsteps + 1, rows, B] each) with the same ``torques``, ``contact`` (a
+    ``ContactDesc``) and ``dt``.  Outputs (each optional, filled in place) as ``integrate_vjp_``, plus ``s0_bar`` [num_contact_states,
+    B]; ``tau_bar`` (shape of ``torques``) is ADDED TO."""
+    nsteps = q_traj.shape[0] - 1
+    h, B, step, stage = _rollout_inputs(mechanism, "integrate_contact_vjp_", q_traj[0], v_traj[0], torques, nsteps)
+    nq, nv, ns = h.info.nq, h.info.nv, contact.nstates
+    _check_blocks("integrate_contact_vjp_", q_traj, (
+        (q_traj, (nsteps + 1, nq, B), "q_traj"), (v_traj, (nsteps + 1, nv, B), "v_traj"), (s_traj, (nsteps + 1, ns, B), "s_traj"),
+        (q_traj_bar, (nsteps + 1, nq, B), "q_traj_bar"), (v_traj_bar, (nsteps + 1, nv, B), "v_traj_bar"),
+        (s_traj_bar, (nsteps + 1, ns, B), "s_traj_bar"), (q0_bar_tan, (nv, B), "q0_bar_tan"), (q0_bar_cfg, (nq, B), "q0_bar_cfg"),
+        (v0_bar, (nv, B), "v0_bar"), (s0_bar, (ns, B), "s0_bar"),
+        (tau_bar, None if torques is None else tuple(torques.shape), "tau_bar")))
+    _contact_vjp_call(h, q_traj, v_traj, s_traj, torques, step, stage, contact, dt, nsteps, q_traj_bar, v_traj_bar, s_traj_bar,
+                      q0_bar_tan, q0_bar_cfg, v0_bar, s0_bar, tau_bar)
+
+
+def _contact_vjp_call(h, qt, vt, st, tau, step, stage, contact, dt, n, qtb, vtb, stb, q0t, qc, vb, sb, tb):
+    import ctypes
+    B = qt.shape[2]
+    c, keep = contact.c_struct()
+    _cabi.check(_cabi.load_library().rbd_integrate_contact_vjp(
+        h.ptr, _DT[qt.dtype], B, _ptr(qt), _ptr(vt), _ptr(st), _ptr(tau), step, stage, ctypes.byref(c), float(dt), n, _ptr(qtb),
+        _ptr(vtb), _ptr(stb), _ptr(q0t), _ptr(qc), _ptr(vb), _ptr(sb), _ptr(tb), _stream(qt)))
+    del keep
+
+
+def _contact_trajectory(h, q0, v0, s0, tau, first, m, step, stage, contact, dt):
+    """rbd_integrate_contact recording steps first .. first + m from (q0, v0, s0) (not modified): [m + 1, rows, B] blocks."""
+    import ctypes
+    B = q0.shape[1]
+    q, v, s = q0.clone(), v0.clone(), s0.clone()
+    new = lambda x: torch.empty((m + 1,) + tuple(x.shape), dtype=x.dtype, device=x.device)   # noqa: E731
+    qt, vt, st = new(q0), new(v0), new(s0)
+    t = None if tau is None else (tau if tau.dim() == 2 else tau[first:])
+    c, keep = contact.c_struct()
+    _cabi.check(_cabi.load_library().rbd_integrate_contact(h.ptr, _DT[q0.dtype], B, B, _ptr(q), _ptr(v), _ptr(s), _ptr(t), step, stage,
+                                                           ctypes.byref(c), float(dt), m, _ptr(qt), _ptr(vt), _ptr(st), _stream(q0)))
+    del keep
+    return qt, vt, st
+
+
+class _SimulateContact(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, mechanism, q0, v0, s0, tau, contact, dt, nsteps, trajectory, every):
+        h, B, step, stage = _rollout_inputs(mechanism, "autodiff.simulate_contact", q0, v0, tau, nsteps)
+        ns = contact.nstates
+        if s0.dtype != q0.dtype or s0.device != q0.device or not s0.is_contiguous() or tuple(s0.shape) != (ns, B):
+            raise DimensionMismatch(f"autodiff.simulate_contact: s0 must be a contiguous [{ns}, {B}] tensor with the dtype and device of q0")
+        ctx.handle, ctx.contact, ctx.dt, ctx.nsteps, ctx.trajectory, ctx.step, ctx.stage = h, contact, dt, nsteps, trajectory, step, stage
+        if trajectory or B == 0:
+            qt, vt, st = _contact_trajectory(h, q0, v0, s0, tau, 0, nsteps, step, stage, contact, dt)
+            ctx.every = nsteps
+            ctx.save_for_backward(tau, qt, vt, st)
+            return (qt, vt, st) if trajectory else (qt[-1].clone(), vt[-1].clone(), st[-1].clone())
+        # checkpoints every `every` steps; backward re-records each segment before its VJP
+        every = max(1, min(every or nsteps, nsteps)) if nsteps else 1
+        ctx.every = every
+        q, v, s = q0, v0, s0
+        qs, vs, ss = [q0], [v0], [s0]
+        for first in range(0, nsteps, every):
+            qt, vt, st = _contact_trajectory(h, q, v, s, tau, first, min(every, nsteps - first), step, stage, contact, dt)
+            q, v, s = qt[-1].clone(), vt[-1].clone(), st[-1].clone()
+            qs.append(q); vs.append(v); ss.append(s)
+        ctx.save_for_backward(tau, torch.stack(qs[:-1]), torch.stack(vs[:-1]), torch.stack(ss[:-1]))
+        return q, v, s
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gq, gv, gs):
+        tau, qck, vck, sck = ctx.saved_tensors
+        h, dt, n, cd = ctx.handle, ctx.dt, ctx.nsteps, ctx.contact
+        need = ctx.needs_input_grad
+        q0, v0, s0 = qck[0], vck[0], sck[0]
+        tb = torch.zeros_like(tau) if (need[4] and tau is not None) else None
+        if q0.shape[1] == 0 or not (need[1] or need[2] or need[3] or tb is not None):
+            return (None, _out(need[1], q0, q0.shape[0]), _out(need[2], v0, v0.shape[0]), _out(need[3], s0, s0.shape[0]), tb,
+                    None, None, None, None, None)
+        if ctx.trajectory:
+            qa, va, sa = torch.empty_like(q0), torch.empty_like(v0), torch.empty_like(s0)
+            _contact_vjp_call(h, qck, vck, sck, tau, ctx.step, ctx.stage, cd, dt, n, gq.contiguous(), gv.contiguous(), gs.contiguous(),
+                              None, qa, va, sa, tb)
+        else:
+            # segments last to first; the adjoint of a segment's end state is its successor's q0_bar_cfg / v0_bar / s0_bar
+            k = ctx.every
+            qa, va, sa = gq.contiguous(), gv.contiguous(), gs.contiguous()
+            starts = list(range(0, n, k)) if n else []
+            if not starts:
+                qc_, vb_, sb_ = torch.empty_like(q0), torch.empty_like(v0), torch.empty_like(s0)
+                _contact_vjp_call(h, qck, vck, sck, tau, ctx.step, ctx.stage, cd, dt, 0, qa[None], va[None], sa[None], None, qc_, vb_,
+                                  sb_, tb)
+                qa, va, sa = qc_, vb_, sb_
+            for j in reversed(range(len(starts))):
+                first = starts[j]
+                m = min(k, n - first)
+                qt, vt, st = _contact_trajectory(h, qck[j], vck[j], sck[j], tau, first, m, ctx.step, ctx.stage, cd, dt)
+                qtb, vtb, stb = torch.zeros_like(qt), torch.zeros_like(vt), torch.zeros_like(st)
+                qtb[-1] = qa; vtb[-1] = va; stb[-1] = sa
+                t = None if tau is None else (tau if tau.dim() == 2 else tau[first:])
+                tbs = None if tb is None else (tb if tb.dim() == 2 else tb[first:])
+                qa, va, sa = torch.empty_like(q0), torch.empty_like(v0), torch.empty_like(s0)
+                _contact_vjp_call(h, qt, vt, st, t, ctx.step, ctx.stage, cd, dt, m, qtb, vtb, stb, None, qa, va, sa, tbs)
+        return (None, qa if need[1] else None, va if need[2] else None, sa if need[3] else None, tb, None, None, None, None, None)
+
+
+def simulate_contact(mechanism: Mechanism, q0: torch.Tensor, v0: torch.Tensor, s0: torch.Tensor, torques: Optional[torch.Tensor] = None, *,
+                     contact=None, dt: float, nsteps: int, trajectory: bool = True, checkpoint_every: Optional[int] = None):
+    """Differentiable ``nsteps`` steps of ``simulate_contact_`` from q0 [nq, B], v0 [nv, B] and the contact state s0
+    [num_contact_states, B].  ``contact``: a ``ContactDesc`` (the mechanism's ``contact_desc`` by default); ``torques`` as for
+    ``simulate``.  Returns ``(q_traj, v_traj, s_traj)`` ([nsteps + 1, rows, B], block 0 the initial state), or the final
+    ``(q, v, s)`` when ``trajectory=False``.  Gradients flow to q0 (as ``q_bar_cfg``), v0, s0 and the torques; backward runs
+    ``rbd_integrate_contact_vjp``, which differentiates the contact force law on the branch each pair takes.  ``checkpoint_every``
+    as for ``simulate``: the gradients do not depend on it, bit for bit.  Not twice differentiable."""
+    from .contact import contact_desc
+    if mechanism.has_loops():
+        raise _cabi.RbdError(_cabi.RBD_ELOOP, "autodiff.simulate_contact: This method can currently only handle tree Mechanisms.")
+    cd = contact if contact is not None else contact_desc(mechanism)
+    return _SimulateContact.apply(mechanism, q0, v0, s0, torques, cd, float(dt), int(nsteps), bool(trajectory), checkpoint_every)

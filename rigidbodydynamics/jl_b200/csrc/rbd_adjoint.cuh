@@ -59,8 +59,9 @@ constexpr int kAdjV = 12, kAdjA = 18, kAdjM = 24, kAdjP = 30, kAdjQ = 36, kAdjE 
 // Workspace rows per sample: the bodies, then (forward VJP) μ in reference velocity order.
 inline int adjoint_rows(int nb, int nv) { return kAdjBodyRows * nb + nv; }
 
-template <class T> struct AdjIO {
-  Col<T> q, v, vd, wext;           // wext may be invalid (no external wrenches)
+template <class T, class WX = Col<T>> struct AdjIO {
+  Col<T> q, v, vd;
+  WX wext;                         // may be invalid (no external wrenches); ColRW when this thread wrote it (rbd_contact_adjoint.cuh)
   ColOut<T> qt, qc, vb, vdb, wb;   // q̄_tan [nv], q̄_cfg [nq], v̄ [nv], v̇̄ [nv], w̄ [6 nb]; each may be invalid (not wanted)
   Scr<T> s;                        // this thread's workspace column
 };
@@ -166,8 +167,8 @@ template <class T> RBD_HD void cfg_adjoint(const BodyDev<T>& bd, const Col<T>& q
 
 // The reverse sweep of L = wt . ID(q, v, v̇, w_ext); weight k = wsign * W(row k).  g: gravity (the model's own; M.g is not read,
 // so the forward VJP can pass the zero-gravity copy of the model it solves with).
-template <class T, class W>
-RBD_HD void adjoint_sample(const ModelDev<T>& M, const T* g, const AdjIO<T>& io, const W& wt, T wsign) {
+template <class T, class W, class WX>
+RBD_HD void adjoint_sample(const ModelDev<T>& M, const T* g, const AdjIO<T, WX>& io, const W& wt, T wsign) {
   const int nb = M.nb;
   const Scr<T>& s = io.s;
   // ---- outward: pose, twist, acceleration, m; the body's own h, g, e, f ----
@@ -342,8 +343,8 @@ template <class T> using MinvIO = AbaIO<T, false, kAllKinds>;
 // Forward-dynamics VJP of one sample.  Mz: the model with ZERO gravity (the solve), g: the model's gravity (the sweep).
 // vd_bar: ν̄;  tau_bar: τ̄ = μ (may be invalid).  io.vdb must be invalid.  zero: one scalar 0 that is not written while the kernel
 // runs (the solve's velocity column reads it for every row, leading dimension 0).
-template <class T, class ST>
-RBD_HD void dynamics_vjp_sample(const ModelDev<T>& Mz, const T* g, const AdjIO<T>& io, const Col<T>& vd_bar,
+template <class T, class ST, class WX>
+RBD_HD void dynamics_vjp_sample(const ModelDev<T>& Mz, const T* g, const AdjIO<T, WX>& io, const Col<T>& vd_bar,
                                 const ColOut<T>& tau_bar, const T* zero, const ST& st) {
   const int mu0 = kAdjBodyRows * Mz.nb;
   MinvIO<T> a;

@@ -980,7 +980,8 @@ int contact_stage_launch(const HostModel& hm, const ModelDev<T>& M, const Contac
 
 // traj_q / traj_v (rbd_integrate_trajectory): [(nsteps + 1) x rows x B] -- block 0 the initial state, block s + 1 written by the
 // finishing kernels of step s; q / v receive the final state as without them.  stages (rbd_integrate_vjp's recompute, nsteps = 1):
-// the four stages' (qs_i, vs_i, φ̇_i, v̇_i) are kept in [4 nq + 12 nv] x B rows (stage_rows) and the finishing step is skipped.
+// the four stages' (qs_i, vs_i, φ̇_i, v̇_i) are kept in [4 nq + 12 nv] x B rows (stage_rows) and the finishing step is skipped; with
+// contact the four ṡ_i follow in 4 ns rows.
 // contact (rbd_integrate_contact): every stage's dynamics is aba_contact_kernel, which also writes ṡ_i, and the finishing step
 // also advances the contact state (contact_finish_kernel); the q / v kernels are the same.
 template <class T>
@@ -1017,6 +1018,7 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
     for (int i = 0; i < 4; ++i) {
       qsi[i] = stages + (size_t)i * nq * B; vsi[i] = stages + (4 * nq + (size_t)i * nv) * B;
       phid[i] = stages + (4 * nq + (4 + (size_t)i) * nv) * B; vd[i] = stages + (4 * nq + (8 + (size_t)i) * nv) * B;
+      if (ns) sd[i] = stages + ((size_t)stage_rows(nq, nv) + i * ns) * B;
     }
   T* qout = traj_q ? traj_q : (T*)q;       // the finishing kernels' target (block s + 1 of a trajectory)
   T* vout = traj_v ? traj_v : (T*)v;
@@ -1203,12 +1205,12 @@ int contact_t(const rbd_model* model, int64_t B, int64_t ld, const void* q, cons
 template <class T>
 int integrate_contact_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau, int64_t step_stride,
                         int64_t stage_stride, const rbd_contact_desc& cd, double dt, int nsteps, void* q_traj, void* v_traj, void* s_traj,
-                        cudaStream_t stream) {
+                        cudaStream_t stream, T* stages = nullptr) {
   const HostModel& hm = model->hm;
   std::unique_ptr<ContactDev<T>> C(new ContactDev<T>());     // passed by value to every stage's launch
   build_contact_dev<T>(hm.nb, hm.pos.data(), hm.alignT.data(), cd, *C);
   const ContactRollout<T> cr{C.get(), (int64_t)3 * cd.npoints * cd.nhalfspaces, (T*)s, (T*)s_traj};
-  return integrate_t<T>(model, B, ld, q, v, tau, step_stride, stage_stride, dt, nsteps, stream, (T*)q_traj, (T*)v_traj, nullptr, &cr);
+  return integrate_t<T>(model, B, ld, q, v, tau, step_stride, stage_stride, dt, nsteps, stream, (T*)q_traj, (T*)v_traj, stages, &cr);
 }
 
 // the descriptor checks of rbd_contact_dynamics and rbd_integrate_contact
@@ -1247,8 +1249,15 @@ int check_common(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, b
 // hooks for the other translation units of the library: argument checks, the RK4 driver
 namespace rbd {
 int api_check(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld) { return check_common(model, dtype, B, ld); }
+int api_check_contact(const rbd_model* model, const rbd_contact_desc* contact, const char* fn) { return check_contact(model, contact, fn); }
 int integrate_record(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, const void* tau, int64_t step_stride,
-                     int64_t stage_stride, double dt, int nsteps, void* q_traj, void* v_traj, void* stages, cudaStream_t stream) {
+                     int64_t stage_stride, double dt, int nsteps, void* q_traj, void* v_traj, void* stages, cudaStream_t stream,
+                     const rbd_contact_desc* contact, void* s) {
+  if (contact)
+    return dtype == RBD_F32 ? integrate_contact_t<float>(model, B, ld, q, v, s, tau, step_stride, stage_stride, *contact, dt, nsteps, q_traj,
+                                                         v_traj, nullptr, stream, (float*)stages)
+                            : integrate_contact_t<double>(model, B, ld, q, v, s, tau, step_stride, stage_stride, *contact, dt, nsteps, q_traj,
+                                                          v_traj, nullptr, stream, (double*)stages);
   return dtype == RBD_F32 ? integrate_t<float>(model, B, ld, q, v, tau, step_stride, stage_stride, dt, nsteps, stream, (float*)q_traj,
                                                (float*)v_traj, (float*)stages)
                           : integrate_t<double>(model, B, ld, q, v, tau, step_stride, stage_stride, dt, nsteps, stream, (double*)q_traj,

@@ -153,10 +153,14 @@ struct LaunchPlan : LaunchShape { StreamAlloc work; };
 int plan_persistent(const void* kernel, int block, size_t smem, int64_t ngroups, cudaStream_t stream, LaunchPlan& plan,
                     size_t work_per_thread = 0, size_t work_extra = 0, size_t work_cap = 0);
 // rbd_b200.cu's RK4 driver for rbd_integrate_trajectory (q_traj / v_traj) and rbd_integrate_vjp's recompute (stages: one step,
-// its four stages kept in stage_rows(nq, nv) x B rows, no finishing step).  fp32 / fp64, arguments checked by the caller.
+// its four stages kept in stage_rows(nq, nv) x B rows, no finishing step).  With `contact` it is the contact rollout from state s
+// (rbd_integrate_contact), and the recompute keeps the four ṡ_i in 4 ns more rows.  fp32 / fp64, arguments checked by the caller.
 inline int64_t stage_rows(int64_t nq, int64_t nv) { return 4 * nq + 12 * nv; }
 int integrate_record(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, const void* tau, int64_t step_stride,
-                     int64_t stage_stride, double dt, int nsteps, void* q_traj, void* v_traj, void* stages, cudaStream_t stream);
+                     int64_t stage_stride, double dt, int nsteps, void* q_traj, void* v_traj, void* stages, cudaStream_t stream,
+                     const rbd_contact_desc* contact = nullptr, void* s = nullptr);
+// rbd_b200.cu's descriptor checks of rbd_contact_dynamics (fn: the entry point named in the message)
+int api_check_contact(const rbd_model* model, const rbd_contact_desc* contact, const char* fn);
 // rbd_adjoint.cu's forward-dynamics VJP on dense [rows x B] arrays (no external wrenches); outputs may be NULL
 int dynamics_vjp_dense(const rbd_model* model, int32_t dtype, int64_t B, const void* q, const void* v, const void* vd, const void* vd_bar,
                        void* q_bar_cfg, void* v_bar, void* tau_bar, cudaStream_t stream);

@@ -7,16 +7,20 @@
 // An elementwise phase is one thread per (sample, joint) for the joints with non-linear maps (blockIdx.y = body) and, when the
 // batch allows, a vectorised kernel over the revolute / prismatic rows (16-byte accesses, like integrate_stage_linear_kernel).
 // Every launch, the recompute's and the VJPs' included, counts in the call's launch record (rbd_handle.h).
+// rbd_integrate_contact_vjp (rbd_contact_adjoint.cuh) is the same driver over rbd_integrate_contact's recompute, with
+// contact_vjp_kernel in place of each stage's forward-dynamics VJP; it also carries the contact state's adjoint.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
 #include <algorithm>
+#include <memory>
+#include <optional>
 #include <string>
 
 #include "../../../include/rbd_b200.h"
 #define sincos_slow sincos_slow_integrate_vjp_tu
+#include "rbd_contact_adjoint.cuh"
 #include "rbd_handle.h"
-#include "rbd_integrate_adjoint.cuh"
 
 using namespace rbd;
 
@@ -96,17 +100,66 @@ __global__ void __launch_bounds__(128) integrate_adjoint_out_kernel(const __grid
     adj_out(bd, a.q, a.qb, a.qt, a.qc, a.B, b);
 }
 
+// The contact rollout's stage adjoint (rbd_contact_adjoint.cuh): in place of the forward-dynamics VJP of a stage, one thread per
+// sample, persistent like dynamics_vjp_kernel (the solve's stash in shared memory, the workspace one column per resident thread).
+template <class T> struct ContactVjpArgs {
+  const T *q, *v, *vd, *vdb;          // stage l: (qs, vs, v̇), ν̄
+  T *qc, *vb, *taub;                  // q̄_cfg, v̄, τ̄ (NULL: not wanted)
+  const T *s0, *sdp, *stb;            // rbd_contact_adjoint.cuh's ContactVjpIO
+  T *sb1, *sacc, *sdc;
+  T* work;
+  const T* zero;
+  T g[3];
+  T wa, wdb;
+  int l;
+  int64_t B;
+};
+template <class T>
+__global__ void __launch_bounds__(32, 1) contact_vjp_kernel(const __grid_constant__ ModelDev<T> M, const __grid_constant__ ContactDev<T> C,
+                                                            const __grid_constant__ ContactVjpArgs<T> a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const Stash<T, 32> st{reinterpret_cast<T*>(smem_raw) + threadIdx.x};
+  const int64_t tid = (int64_t)blockIdx.x * 32 + threadIdx.x;
+  const int64_t ngroups = (a.B + 31) / 32;
+  for (int64_t g = blockIdx.x; g < ngroups; g += gridDim.x) {
+    const int64_t b = g * 32 + threadIdx.x;
+    const bool active = b < a.B;
+    const int64_t bl = active ? b : a.B - 1;      // inactive lanes recompute the last sample, stores are masked
+    ContactVjpIO<T> io;
+    io.q = {a.q + bl, a.B}; io.v = {a.v + bl, a.B}; io.vd = {a.vd + bl, a.B}; io.vdb = {a.vdb + bl, a.B};
+    io.qc = {a.qc + bl, a.B, active};
+    io.taub = {a.taub ? a.taub + bl : nullptr, a.B, active};
+    io.vb = a.vb + bl;
+    io.s0 = a.s0 + bl; io.sdp = a.sdp ? a.sdp + bl : nullptr; io.stb = a.stb ? a.stb + bl : nullptr;
+    io.sb1 = a.sb1 + bl; io.sacc = a.sacc + bl; io.sdc = a.sdc + bl;
+    io.ld = a.B; io.wa = a.wa; io.wdb = a.wdb; io.l = a.l;
+    io.s = {a.work + tid, (int64_t)gridDim.x * 32};
+    io.active = active;
+    contact_vjp_sample<T>(M, a.g, C, io, a.zero, st);
+  }
+}
+
+// the contact part of a rollout adjoint: the descriptor in device form, the recorded contact states and their adjoints
+template <class T> struct ContactVjp {
+  const rbd_contact_desc* cd;
+  const ContactDev<T>* C;
+  int64_t ns;
+  const T* s_traj; const T* stb;
+  T* s0b;
+};
+
 template <class T>
 int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q_traj, const T* v_traj, const T* tau, int64_t step_stride,
                     int64_t stage_stride, double dt, int nsteps, const T* qtb, const T* vtb, T* q0t, T* q0c, T* v0b, T* taub,
-                    cudaStream_t stream) {
+                    cudaStream_t stream, const ContactVjp<T>* contact = nullptr) {
   const HostModel& hm = model->hm;
   const ModelDev<T>& M = dev_model<T>(hm);
-  const int64_t nq = hm.nq, nv = hm.nv;
+  const int64_t nq = hm.nq, nv = hm.nv, ns = contact ? contact->ns : 0;
   DeviceProps p;
   RBD_CUDA_TRY(device_props(p));
-  // workspace: the four stages, then q̄_cfg / q̄ / q̄0 / q̄s (nq rows each), v̄ / τ̄ / v̄ / v̄0 / v̄s / v̇̄ / Φ̄ (nv rows each)
-  const int64_t srows = stage_rows(nq, nv), rows = srows + 4 * nq + 7 * nv;
+  // workspace: the four stages (with contact: and their ṡ_i), then q̄_cfg / q̄ / q̄0 / q̄s (nq rows each), v̄ / τ̄ / v̄ / v̄0 / v̄s / v̇̄ / Φ̄
+  // (nv rows each), then with contact s̄1 / s̄0 / the carried dt a_i s̄_i (ns rows each)
+  const int64_t srows = stage_rows(nq, nv) + 4 * ns, rows = srows + 4 * nq + 7 * nv + 3 * ns;
   StreamAlloc work;
   RBD_CUDA_TRY(work.alloc((size_t)rows * B * sizeof(T), stream));
   T* stages = (T*)work.p;
@@ -114,11 +167,32 @@ int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q
   auto take = [&](int64_t r) { T* o = next; next += r * B; return o; };
   T *qcb = take(nq), *qb = take(nq), *qb0 = take(nq), *qsb = take(nq);
   T *vvb = take(nv), *tb = take(nv), *vb = take(nv), *vb0 = take(nv), *vsb = take(nv), *vdb = take(nv), *phib = take(nv);
+  T *sb1 = take(ns), *sacc = take(ns), *sdc = take(ns);
   const size_t qbytes = (size_t)nq * B * sizeof(T), vbytes = (size_t)nv * B * sizeof(T);
   if (qtb) RBD_CUDA_TRY(cudaMemcpyAsync(qb, qtb + (size_t)nsteps * nq * B, qbytes, cudaMemcpyDeviceToDevice, stream));
   else RBD_CUDA_TRY(cudaMemsetAsync(qb, 0, qbytes, stream));
   if (vtb) RBD_CUDA_TRY(cudaMemcpyAsync(vb, vtb + (size_t)nsteps * nv * B, vbytes, cudaMemcpyDeviceToDevice, stream));
   else RBD_CUDA_TRY(cudaMemsetAsync(vb, 0, vbytes, stream));
+  const size_t sbytes = (size_t)ns * B * sizeof(T);
+  if (ns && contact->stb) RBD_CUDA_TRY(cudaMemcpyAsync(sb1, contact->stb + (size_t)nsteps * ns * B, sbytes, cudaMemcpyDeviceToDevice, stream));
+  else if (ns) RBD_CUDA_TRY(cudaMemsetAsync(sb1, 0, sbytes, stream));
+  // the contact stage adjoint: one plan (grid, workspace and the solve's zero) for the whole call
+  ContactVjpArgs<T> cva{};
+  std::optional<LaunchPlan> cplan;
+  ModelDev<T> Mz;
+  if (contact && nsteps > 0) {
+    Mz = M;
+    for (int k = 0; k < 3; ++k) { cva.g[k] = M.g[k]; Mz.g[k] = T(0); }
+    const size_t row_bytes = (size_t)contact_vjp_rows(hm.nb, hm.nv) * sizeof(T);
+    cplan.emplace();
+    if (int rc = plan_persistent((const void*)contact_vjp_kernel<T>, 32, (size_t)std::max(1, (int)M.nrows) * 32 * sizeof(T), (B + 31) / 32,
+                                 stream, *cplan, row_bytes, sizeof(T), size_t(512) << 20)) return rc;
+    cva.work = (T*)cplan->work.p;
+    cva.zero = cva.work + row_bytes / sizeof(T) * cplan->grid * 32;
+    RBD_CUDA_TRY(cudaMemsetAsync(const_cast<T*>(cva.zero), 0, sizeof(T), stream));
+    cva.vdb = vdb; cva.qc = qcb; cva.vb = vvb; cva.taub = taub ? tb : nullptr;
+    cva.sb1 = sb1; cva.sacc = sacc; cva.sdc = sdc; cva.B = B;
+  }
   bool has_other = false;
   for (int i = 0; i < hm.nb; ++i) has_other |= (M.body[i].kind != K_REV && M.body[i].kind != K_PRIS && M.body[i].kind != K_FIXED);
   constexpr int N = VecOf<T>::N;
@@ -143,8 +217,10 @@ int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q
   for (int s = nsteps - 1; s >= 0; --s) {
     const T* q0 = q_traj + (size_t)s * nq * B;
     const T* v0 = v_traj + (size_t)s * nv * B;
+    const T* s0 = contact ? contact->s_traj + (size_t)s * ns * B : nullptr;
     if (int rc = integrate_record(model, dtype, B, B, const_cast<T*>(q0), const_cast<T*>(v0), tau ? tau + s * step_stride : nullptr,
-                                  step_stride, stage_stride, dt, 1, nullptr, nullptr, stages, stream)) return rc;
+                                  step_stride, stage_stride, dt, 1, nullptr, nullptr, stages, stream, contact ? contact->cd : nullptr,
+                                  const_cast<T*>(s0))) return rc;
     a.q0 = q0;
     a.qtb = qtb ? qtb + (size_t)s * nq * B : nullptr;
     a.vtb = vtb ? vtb + (size_t)s * nv * B : nullptr;
@@ -166,7 +242,18 @@ int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q
         }
         continue;
       }
-      if (int rc = dynamics_vjp_dense(model, dtype, B, a.qs[a.l], a.vs[a.l], vd[a.l], vdb, qcb, vvb, taub ? tb : nullptr, stream)) return rc;
+      if (contact) {
+        const int l = a.l;
+        const T* sd = stages + (size_t)stage_rows(nq, nv) * B;
+        cva.q = a.qs[l]; cva.v = a.vs[l]; cva.vd = vd[l];
+        cva.s0 = s0; cva.sdp = l ? sd + (size_t)(l - 1) * ns * B : nullptr;
+        cva.stb = (l == 0 && contact->stb) ? contact->stb + (size_t)s * ns * B : nullptr;
+        cva.wa = a.wa[l]; cva.wdb = (T)dt * a.wb[l]; cva.l = l;
+        contact_vjp_kernel<T><<<cplan->grid, cplan->block, cplan->smem, stream>>>(Mz, *contact->C, cva);
+        if (int rc = api_launched(&*cplan)) return rc;
+      } else if (int rc = dynamics_vjp_dense(model, dtype, B, a.qs[a.l], a.vs[a.l], vd[a.l], vdb, qcb, vvb, taub ? tb : nullptr, stream)) {
+        return rc;
+      }
     }
   }
   if (q0t || q0c) {
@@ -174,7 +261,21 @@ int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q
     if (int rc = api_launched()) return rc;
   }
   if (v0b) RBD_CUDA_TRY(cudaMemcpyAsync(v0b, vb, vbytes, cudaMemcpyDeviceToDevice, stream));
+  if (ns && contact->s0b) RBD_CUDA_TRY(cudaMemcpyAsync(contact->s0b, sb1, sbytes, cudaMemcpyDeviceToDevice, stream));
   return RBD_OK;
+}
+
+template <class T>
+int integrate_contact_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const void* q_traj, const void* v_traj, const void* s_traj,
+                            const void* tau, int64_t step_stride, int64_t stage_stride, const rbd_contact_desc& cd, double dt, int nsteps,
+                            const void* qtb, const void* vtb, const void* stb, void* q0t, void* q0c, void* v0b, void* s0b, void* taub,
+                            cudaStream_t stream) {
+  const HostModel& hm = model->hm;
+  std::unique_ptr<ContactDev<T>> C(new ContactDev<T>());
+  build_contact_dev<T>(hm.nb, hm.pos.data(), hm.alignT.data(), cd, *C);
+  const ContactVjp<T> cv{&cd, C.get(), (int64_t)3 * cd.npoints * cd.nhalfspaces, (const T*)s_traj, (const T*)stb, (T*)s0b};
+  return integrate_vjp_t<T>(model, dtype, B, (const T*)q_traj, (const T*)v_traj, (const T*)tau, step_stride, stage_stride, dt, nsteps,
+                            (const T*)qtb, (const T*)vtb, (T*)q0t, (T*)q0c, (T*)v0b, (T*)taub, stream, &cv);
 }
 
 }  // namespace
@@ -199,4 +300,28 @@ extern "C" int32_t rbd_integrate_vjp(const rbd_model* model, int32_t dtype, int6
              : integrate_vjp_t<double>(model, dtype, B, (const double*)q_traj, (const double*)v_traj, (const double*)tau, tau_step_stride,
                                        tau_stage_stride, dt, nsteps, (const double*)q_traj_bar, (const double*)v_traj_bar,
                                        (double*)q0_bar_tan, (double*)q0_bar_cfg, (double*)v0_bar, (double*)tau_bar, s);
+}
+
+extern "C" int32_t rbd_integrate_contact_vjp(const rbd_model* model, int32_t dtype, int64_t B, const void* q_traj, const void* v_traj,
+                                             const void* s_traj, const void* tau, int64_t tau_step_stride, int64_t tau_stage_stride,
+                                             const rbd_contact_desc* contact, double dt, int32_t nsteps, const void* q_traj_bar,
+                                             const void* v_traj_bar, const void* s_traj_bar, void* q0_bar_tan, void* q0_bar_cfg,
+                                             void* v0_bar, void* s0_bar, void* tau_bar, void* stream) {
+  if (int rc = api_check(model, dtype, B, B)) return rc;
+  const ApiCall call;
+  if (dtype != RBD_F32 && dtype != RBD_F64) return api_fail(RBD_EUNSUPPORTED, "rbd_integrate_contact_vjp: fp32 and fp64 only");
+  if (nsteps < 0 || !(dt > 0)) return api_fail(RBD_EINVAL, "rbd_integrate_contact_vjp: need dt > 0 and nsteps >= 0");
+  if (tau_step_stride < 0 || tau_stage_stride < 0) return api_fail(RBD_EINVAL, "rbd_integrate_contact_vjp: torque strides must be >= 0");
+  if (!tau && tau_bar) return api_fail(RBD_EINVAL, "rbd_integrate_contact_vjp: tau_bar needs tau");
+  if (int rc = api_check_contact(model, contact, "rbd_integrate_contact_vjp")) return rc;
+  const int64_t ns = (int64_t)3 * contact->npoints * contact->nhalfspaces;
+  if (B == 0 || model->hm.nv == 0) return RBD_OK;
+  if (!q_traj || !v_traj) return api_fail(RBD_EINVAL, "rbd_integrate_contact_vjp: q_traj and v_traj must not be NULL");
+  if (ns > 0 && !s_traj) return api_fail(RBD_EINVAL, "rbd_integrate_contact_vjp: s_traj must not be NULL when there are contact pairs");
+  cudaStream_t s = (cudaStream_t)stream;
+  return dtype == RBD_F32
+             ? integrate_contact_vjp_t<float>(model, dtype, B, q_traj, v_traj, s_traj, tau, tau_step_stride, tau_stage_stride, *contact, dt,
+                                              nsteps, q_traj_bar, v_traj_bar, s_traj_bar, q0_bar_tan, q0_bar_cfg, v0_bar, s0_bar, tau_bar, s)
+             : integrate_contact_vjp_t<double>(model, dtype, B, q_traj, v_traj, s_traj, tau, tau_step_stride, tau_stage_stride, *contact, dt,
+                                               nsteps, q_traj_bar, v_traj_bar, s_traj_bar, q0_bar_tan, q0_bar_cfg, v0_bar, s0_bar, tau_bar, s);
 }

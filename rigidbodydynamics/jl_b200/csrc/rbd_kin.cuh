@@ -628,9 +628,10 @@ inline void build_contact_dev(int nb, const int* pos, const double* alignT, cons
 
 // The force law of one (point pi, half-space with unit normal n) pair in contact: penetration z >= 0, point velocity vel (root
 // frame), tangential displacement xs(k), k = 0..2 (read inside, where the friction force needs it).  Out: the force on the body f
-// (root frame) and the state derivative xd.  Shared by contact_sample and the rollout's contact pass (contact_stage_pass).
-template <class T, class XS>
-RBD_HD void contact_force(const ContactDev<T>& C, int pi, const T* n, T z, const T* vel, const XS& xs, T* f, T* xd) {
+// (root frame) and the state derivative xd.  Shared by contact_sample, the rollout's contact pass (contact_stage_pass) and, with
+// T = Dual1<P>, its adjoint (rbd_contact_adjoint.cuh): P is the scalar type of the descriptor.
+template <class T, class P, class XS>
+RBD_HD void contact_force(const ContactDev<P>& C, int pi, const P* n, T z, const T* vel, const XS& xs, T* f, T* xd) {
   const T zd = -(vel[0] * n[0] + vel[1] * n[1] + vel[2] * n[2]);
   const T zn = contact_pow(z, C.hc[pi][2]);
   T fn = C.hc[pi][1] * zn * zd + C.hc[pi][0] * zn;
