@@ -20,7 +20,10 @@
 namespace rbd {
 namespace {
 
-constexpr int kGeneratorVersion = 29;   // bump when the emitted code changes (part of the cubin cache key)
+constexpr int kGeneratorVersion = 30;   // bump when the emitted code changes (part of the cubin cache key)
+constexpr int kRegRowsAba = -1;         // register-resident stash rows of the fp32 forward-dynamics programs (-1: all eligible)
+constexpr int kSmemPerSm = 233472;      // H100: 228 KB of shared memory per SM ...
+constexpr int kSmemReservedPerBlock = 1024;   // ... of which each resident block takes 1 KB for the system
 
 template <class F> const ModelDev<F>& devm(const HostModel& m);
 template <> const ModelDev<float>& devm<float>(const HostModel& m) { return m.dev32; }
@@ -228,8 +231,14 @@ struct Emitter {
         ++stats.n_store;
         if (key.peers && n.arr == A_OUT0 && flavor != FLAVOR_CPU) return "RBD_STG_PEERS(" + row(i) + ", " + opnd(i, 0) + ");\n";
         return std::string("RBD_STG(") + arr_name(n.arr) + ", " + row(i) + ", " + opnd(i, 0) + ");\n";
-      case S_SLD: ++stats.n_sld; return v + "RBD_SLD(" + row(i) + ");\n";
-      case S_SST: ++stats.n_sst; return "RBD_SST(" + row(i) + ", " + opnd(i, 0) + ");\n";
+      case S_SLD:
+        ++stats.n_sld;
+        if (reg_row(n.row)) return v + rname(n.row) + ";\n";
+        return v + "RBD_SLD(" + row(i) + ");\n";
+      case S_SST:
+        ++stats.n_sst;
+        if (reg_row(n.row)) return rname(n.row) + " = " + opnd(i, 0) + ";\n";
+        return "RBD_SST(" + row(i) + ", " + opnd(i, 0) + ");\n";
       case S_SFENCE: return "RBD_SFENCE();\n";
       case S_XLD: return v + "RBD_XLD(" + row(i) + ");\n";
       case S_XST: return "RBD_XST(" + row(i) + ", " + opnd(i, 0) + ");\n";
@@ -270,6 +279,7 @@ struct Emitter {
     std::vector<int32_t> outs;                                       // nodes of A or B used after the loop
   };
   bool fold = true;
+  int total_rows = 0;            // stash rows of the algorithm's layout
   const HostModel* hm = nullptr;
   std::vector<Fold> folds;
   std::vector<int32_t> fold_at, in_fold;
@@ -465,9 +475,78 @@ struct Emitter {
     return ref(x);
   }
 
+  // ---- register-resident stash rows ------------------------------------------------------------------------------------
+  // A stash row that no statement addresses as row + rbd_it * Δ (Δ != 0) has one name in every statement that touches it, so it
+  // can be an ordinary variable instead of shared memory: the trunk bodies' rows and the pending slot of a folded program, any
+  // row of a straight-line one.  Up to `reg_budget` such rows (-1: all) become registers, chosen by accesses per statement of
+  // live range (a value is live from its store to the last load before the next store); the other rows are renumbered
+  // 0 .. shared_rows - 1 in their order.  The statements are the same either way, so the results are bit-identical.
+  int reg_budget = 0;
+  std::vector<int> rowmap;       // stash row -> shared-memory row, -1: register
+  std::vector<int> regs;         // register rows, ascending
+  int shared_rows = 0;
+
+  bool reg_row(int r) const { return r >= 0 && r < (int)rowmap.size() && rowmap[r] == -1; }
+  static std::string rname(int r) { return "rbd_r" + std::to_string(r); }
+  int srow(int r) const { return r < (int)rowmap.size() ? rowmap[r] : r; }
+  bool stash_op(int j) const { return tr.nodes[j].op == S_SLD || tr.nodes[j].op == S_SST; }
+  std::string row_text(int j) const { return std::to_string(stash_op(j) ? srow(tr.nodes[j].row) : tr.nodes[j].row); }
+
+  void plan_rows(int total_rows) {
+    const auto& N = tr.nodes;
+    int nrows = total_rows;
+    for (size_t i = 0; i < N.size(); ++i)
+      if (live[i] && (N[i].op == S_SLD || N[i].op == S_SST)) nrows = std::max(nrows, N[i].row + 1);
+    rowmap.resize(nrows);
+    for (int r = 0; r < nrows; ++r) rowmap[r] = r;
+    shared_rows = total_rows;
+    if (reg_budget == 0) return;
+    std::vector<uint8_t> indexed(nrows, 0), touched(nrows, 0);
+    for (const Fold& f : folds)
+      for (const auto& e : f.drow) {
+        const SymNode& n = N[e.first];
+        if (e.second == 0 || (n.op != S_SLD && n.op != S_SST) || fused[e.first]) continue;
+        indexed[n.row] = indexed[n.row + e.second] = 1;
+      }
+    std::vector<int64_t> acc(nrows, 0), span(nrows, 0), open(nrows, -1), last(nrows, -1);
+    for (size_t i = 0; i < N.size(); ++i) {
+      if (!live[i] || (N[i].op != S_SLD && N[i].op != S_SST)) continue;
+      const int r = N[i].row;
+      touched[r] = 1;
+      ++acc[r];
+      if (N[i].op == S_SST) {
+        if (open[r] >= 0 && last[r] > open[r]) span[r] += last[r] - open[r];
+        open[r] = (int64_t)i;
+      } else {
+        if (open[r] < 0) open[r] = (int64_t)i;
+        last[r] = (int64_t)i;
+      }
+    }
+    std::vector<int> cand;
+    for (int r = 0; r < nrows; ++r) {
+      if (open[r] >= 0 && last[r] > open[r]) span[r] += last[r] - open[r];
+      if (touched[r] && !indexed[r]) cand.push_back(r);
+    }
+    std::stable_sort(cand.begin(), cand.end(), [&](int x, int y) { return acc[x] * (span[y] + 1) > acc[y] * (span[x] + 1); });
+    if (reg_budget > 0 && (int)cand.size() > reg_budget) cand.resize(reg_budget);
+    regs = cand;
+    std::sort(regs.begin(), regs.end());
+    for (int r : regs) rowmap[r] = -1;
+    shared_rows = 0;
+    for (int r = 0; r < nrows; ++r)
+      if (rowmap[r] >= 0) rowmap[r] = touched[r] ? shared_rows++ : -2;    // -2: never accessed (no slot, never emitted)
+    stats.reg_rows = (int)regs.size();
+  }
+  std::string reg_decls() const {
+    std::string s;
+    for (int r : regs) s += "rbd_v " + rname(r) + " = RBD_K(" + lit(0.0) + ");\n";
+    return s;
+  }
+
   void emit_fold(const Fold& f, int& since) {
     const auto& N = tr.nodes;
     auto rowx = [](int row, int d) { return d ? "(" + std::to_string(row) + " + rbd_it * " + std::to_string(d) + ")" : std::to_string(row); };
+    auto srowx = [&](int row, int d) { return rowx(srow(row), d ? srow(row + d) - srow(row) : 0); };
     char hdr[160];
     snprintf(hdr, sizeof hdr, "// ABA pass %d: bodies %d..%d and their mirror images run one copy of the code\n", f.pass,
              std::min(f.first, f.first + (f.pass == 2 ? 1 - f.len : f.len - 1)), std::max(f.first, f.first + (f.pass == 2 ? 1 - f.len : f.len - 1)));
@@ -488,8 +567,12 @@ struct Emitter {
     const NameFn uname = [](int j) { return "u" + std::to_string(j); };
     const NameFn cname = [](int j) { return "c" + std::to_string(j); };
     const OpFn aop = [&](int j, int k) { return f.opa.at(j)[k]; };
-    const NameFn arow = [&](int j) { auto it = f.drow.find(j); return rowx(N[j].row, it == f.drow.end() ? 0 : it->second); };
-    const NameFn absrow = [&](int j) { return std::to_string(N[j].row); };
+    const NameFn arow = [&](int j) {
+      auto it = f.drow.find(j);
+      const int d = it == f.drow.end() ? 0 : it->second;
+      return stash_op(j) ? srowx(N[j].row, d) : rowx(N[j].row, d);
+    };
+    const NameFn absrow = [&](int j) { return row_text(j); };
     std::set<int32_t> outset(f.outs.begin(), f.outs.end());
     auto branches = [&](size_t at) {
       for (size_t k = 0; k < f.ca.size(); ++k) {
@@ -538,18 +621,23 @@ struct Emitter {
     stats.n_fold_bodies += f.len;
   }
 
-  void emit() {
+  void plan() {
     mark();
     plan_fma();
     if (fold) analyse_folds();
     if (!folds.empty()) split_every = split_folded;
     if (!fold) { fold_at.assign(tr.nodes.size(), -1); in_fold.assign(tr.nodes.size(), -1); remat.assign(tr.nodes.size(), 0); }
+    plan_rows(total_rows);
+  }
+
+  void emit() {
+    plan();
     const auto& N = tr.nodes;
     stats.nodes_traced = (int)N.size();
     for (size_t i = 0; i < N.size(); ++i) if (live[i] && N[i].op != S_CONST && N[i].op != S_PARAM) ++stats.nodes_live;
     const NameFn tname = [](int j) { return "t" + std::to_string(j); };
     const OpFn top = [&](int j, int k) { return outer_operand(k ? N[j].b : N[j].a); };
-    const NameFn trow = [&](int j) { return std::to_string(N[j].row); };
+    const NameFn trow = [&](int j) { return row_text(j); };
     int since = 0;
     for (size_t i = 0; i < N.size(); ++i) {
       if (fold_at[i] >= 0) {
@@ -595,6 +683,8 @@ bool spec_emit_function(const HostModel& hm, const SpecKey& key, int flavor, con
   Emitter em(tr, key, flavor);
   em.hm = &hm;
   em.fold = fold;
+  em.total_rows = rows;
+  em.reg_budget = spec_reg_rows(key);
   if (flavor != FLAVOR_CPU) {
     // One basic block of 10^4 instructions lets ptxas stretch live ranges until it spills (Atlas: 128 registers + 350 B of
     // local memory, -10 % throughput); a never-taken branch every few hundred statements bounds its scheduling regions.
@@ -606,6 +696,7 @@ bool spec_emit_function(const HostModel& hm, const SpecKey& key, int flavor, con
   }
   em.emit();
   em.stats.stash_rows = rows;
+  em.stats.shared_rows = em.shared_rows;
   if (stats) *stats = em.stats;
   out += em.param_table();
   const char* F = key.f64 ? "double" : "float";
@@ -621,6 +712,7 @@ bool spec_emit_function(const HostModel& hm, const SpecKey& key, int flavor, con
   out += sig + " {\n";
   if (flavor != FLAVOR_CPU) out += "RBD_FN_BEGIN\n";
   if (key.algo == SPEC_KIN) out += flavor == FLAVOR_CPU ? "RBD_KIN_BEGIN_CPU\n" : "RBD_KIN_BEGIN\n";
+  out += em.reg_decls();
   out += em.out;
   if (flavor != FLAVOR_CPU) out += "RBD_FN_END\n";
   out += "}\n";
@@ -635,13 +727,43 @@ int spec_stash_rows(const HostModel& hm, const SpecKey& key) {
   return key.algo == SPEC_ABA ? hm.dev64.nrows : (key.algo == SPEC_RNEA ? rnea_rows(hm) : std::max(1, crba_rows(hm)));
 }
 
+int spec_reg_rows(const SpecKey& key) {
+  if (key.algo != SPEC_ABA || key.f64) return 0;
+  if (const char* e = getenv("RBD_JIT_REG_ROWS")) return atoi(e);
+  return kRegRowsAba;
+}
+
+int spec_smem_blocks(const SpecKey& key, int shared_rows) {
+  if (const char* e = getenv("RBD_JIT_SMEM_BLOCKS")) return std::max(1, std::min(32, atoi(e)));
+  const int bytes = std::max(1, shared_rows) * 32 * (key.f64 ? 8 : 4);
+  // A program with register rows is compiled for at most 8 blocks, two warps per SM sub-partition and up to 255 registers each:
+  // Atlas fp32 forward dynamics runs 6 % faster that way than at the 11 blocks its 156 shared rows allow (168 registers, 128 B
+  // of spills; DESIGN.md section 7).
+  return std::max(1, std::min(spec_reg_rows(key) != 0 ? 8 : 16, kSmemPerSm / (bytes + kSmemReservedPerBlock)));
+}
+
+int spec_shared_rows(const HostModel& hm, const SpecKey& key) {
+  SymTrace tr;
+  int rows = 0;
+  std::string err;
+  if (spec_reg_rows(key) == 0 || !run_trace(hm, key, tr, rows, err)) return spec_stash_rows(hm, key);
+  Emitter em(tr, key, FLAVOR_SMEM);
+  em.hm = &hm;
+  em.total_rows = rows;
+  em.reg_budget = spec_reg_rows(key);
+  em.plan();
+  return em.shared_rows;
+}
+
 uint64_t spec_hash(const HostModel& hm, const SpecKey& key) {
   uint64_t h = 0xcbf29ce484222325ull;
   auto mix = [&](const void* p, size_t n) {
     const unsigned char* b = (const unsigned char*)p;
     for (size_t i = 0; i < n; ++i) { h ^= b[i]; h *= 0x100000001b3ull; }
   };
-  const int hdr[9] = {kGeneratorVersion, key.algo, key.f64, key.has_in2, key.has_out1, key.lower, hm.nb, hm.general, key.peers};
+  const char* blocks = getenv("RBD_JIT_SMEM_BLOCKS");
+  const int hdr[11] = {kGeneratorVersion, key.algo, key.f64, key.has_in2, key.has_out1, key.lower, hm.nb, hm.general, key.peers,
+                       spec_reg_rows(key), blocks ? atoi(blocks) : 0};
   mix(hdr, sizeof hdr);
   if (key.algo == SPEC_KIN) { mix(&key.kin_mask, sizeof key.kin_mask); mix(key.kin_sign, sizeof key.kin_sign); }
   if (key.f64) {
@@ -660,16 +782,17 @@ bool spec_emit_cuda_tu(const HostModel& hm, const SpecKey& key, std::string& out
   SpecStats st;
   if (!spec_emit_function(hm, key, FLAVOR_SMEM, "rbd_spec_smem", fn_smem, &st, err)) return false;
   if (stats) *stats = st;
-  char buf[768];
-  const int rows = spec_stash_rows(hm, key);
+  char buf[1024];
+  const int rows = st.reg_rows ? st.shared_rows : spec_stash_rows(hm, key);     // shared-memory rows
   snprintf(buf, sizeof buf,
            "// generated by librbd_b200.so (rbd_codegen.cpp) for one mechanism: %d live nodes (%d add/sub, %d mul, %d div, %d sincos, "
-           "%d global loads, %d stash loads, %d stash stores)\n"
+           "%d global loads, %d stash loads, %d stash stores; %d stash rows in registers)\n"
+           "#define RBD_SPEC_SMEM_BLOCKS %d\n"
            "#define RBD_SPEC_F64 %d\n#define RBD_SPEC_NQ %d\n#define RBD_SPEC_NV %d\n#define RBD_SPEC_ROWS %d\n"
            "#define RBD_SPEC_HAS_IN2 %d\n#define RBD_SPEC_HAS_OUT1 %d\n#define RBD_SPEC_OUT0_ROWS %d\n#define RBD_SPEC_OUT1_ROWS %d\n"
            "#define RBD_SPEC_ROW32 %d\n#define RBD_SPEC_KIN %d\n#define RBD_SPEC_USES_V %d\n#include \"rbd_jit_prelude.cuh\"\n",
-           st.nodes_live, st.n_add, st.n_mul, st.n_div, st.n_sincos, st.n_load, st.n_sld, st.n_sst,
-           key.f64 ? 1 : 0, hm.nq, hm.nv, rows, key.has_in2 ? 1 : 0, key.has_out1 ? 1 : 0, key.algo == SPEC_CRBA ? hm.nv * hm.nv : hm.nv, hm.nq,
+           st.nodes_live, st.n_add, st.n_mul, st.n_div, st.n_sincos, st.n_load, st.n_sld, st.n_sst, st.reg_rows,
+           spec_smem_blocks(key, rows), key.f64 ? 1 : 0, hm.nq, hm.nv, rows, key.has_in2 ? 1 : 0, key.has_out1 ? 1 : 0, key.algo == SPEC_CRBA ? hm.nv * hm.nv : hm.nv, hm.nq,
            key.algo == SPEC_CRBA ? 1 : 0, key.algo == SPEC_KIN ? 1 : 0, st.n_load_v > 0 ? 1 : 0);
   out += buf;
   out += "#define RBD_FLAVOR_SMEM 1\n#include \"rbd_jit_flavor.cuh\"\n" + fn_smem;

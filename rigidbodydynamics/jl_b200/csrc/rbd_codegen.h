@@ -28,6 +28,8 @@ struct SpecStats {
   int n_load_v = 0;      // global loads of the v array (0: the kernel shell does not prefetch it)
   int n_fold_loops = 0;  // (pass, chain pair) steps emitted once as a two-iteration loop for both mirror-image chains
   int n_fold_bodies = 0; // body steps whose code those loops share (summed over passes)
+  int reg_rows = 0;      // stash rows kept in registers (RBD_JIT_REG_ROWS)
+  int shared_rows = 0;   // stash rows left in shared memory (RBD_SPEC_ROWS of the CUDA flavour)
 };
 
 enum SpecFlavor : int { FLAVOR_CPU = 0, FLAVOR_SMEM = 1 };
@@ -40,7 +42,15 @@ bool spec_emit_function(const HostModel& hm, const SpecKey& key, int flavor, con
 
 // Whole NVRTC translation unit for `key`: defines + the per-sample function + the kernel shell of the prelude.
 bool spec_emit_cuda_tu(const HostModel& hm, const SpecKey& key, std::string& out, SpecStats* stats, std::string& err);
+// Rows of the algorithm's stash layout, and the rows of them the generated program keeps in shared memory (the others are
+// registers, see spec_reg_rows); the latter runs the tracer, it is meant for once per loaded program.
 int spec_stash_rows(const HostModel& hm, const SpecKey& key);
+int spec_shared_rows(const HostModel& hm, const SpecKey& key);
+// Budget of register-resident stash rows for `key` (-1: every eligible row); RBD_JIT_REG_ROWS overrides it for forward dynamics.
+int spec_reg_rows(const SpecKey& key);
+// Minimum resident single-warp blocks per SM rbd_jit_smem is compiled for (its register cap): as many as the shared stash
+// allows on a 228 KB SM, at most 16 (128 registers), at most 8 (255 registers) with register rows; RBD_JIT_SMEM_BLOCKS overrides it.
+int spec_smem_blocks(const SpecKey& key, int shared_rows);
 
 // Self-contained C++ translation unit (needs csrc/ on the include path) defining `extern "C" void name(q, v, in2, o0, o1, ld, sh)`
 // for ONE sample: column pointers with leading dimension ld, `sh` = stash_rows scalars of scratch.  Test tier only.

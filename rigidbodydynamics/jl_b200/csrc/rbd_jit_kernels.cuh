@@ -28,7 +28,9 @@
     g = gn;                                                                                         \
   }
 
-extern "C" __global__ void __launch_bounds__(32, RBD_SPEC_F64 ? 1 : 16) rbd_jit_smem(const RbdJitArgs a) {
+// Register cap of the single-warp blocks: as many blocks as the shared stash lets reside (RBD_SPEC_SMEM_BLOCKS, at most 16) share
+// the register file, so 8 resident Atlas warps get up to 255 registers each instead of 128.
+extern "C" __global__ void __launch_bounds__(32, RBD_SPEC_F64 ? 1 : RBD_SPEC_SMEM_BLOCKS) rbd_jit_smem(const RbdJitArgs a) {
   extern __shared__ __align__(16) unsigned char rbd_smem_raw[];
   volatile rbd_f* sh = reinterpret_cast<volatile rbd_f*>(rbd_smem_raw) + threadIdx.x;
 #define RBD_CALL_SMEM(q_, v_, i_, o0_, o1_, ld_, act_, fl_, pa_, pb_) rbd_spec_smem(q_, v_, i_, o0_, o1_, ld_, act_, fl_, pa_, pb_, sh)

@@ -88,7 +88,7 @@ int spec_prepare(rbd_model* m, const SpecKey& key, bool load_on_device, std::str
   cudaFuncAttributes fa{};
   if (e == cudaSuccess) { e = cudaFuncGetAttributes(&fa, (const void*)se.k_smem); se.regs_smem = fa.numRegs; }
   if (e == cudaSuccess) { e = cudaFuncGetAttributes(&fa, (const void*)se.k_mix); se.regs_mix = fa.numRegs; }
-  se.rows = spec_stash_rows(m->hm, key);
+  se.rows = spec_shared_rows(m->hm, key);       // the rows the program keeps in shared memory (the others are registers)
   const size_t smem = (size_t)std::max(1, se.rows) * 32 * (key.f64 ? 8 : 4);
   DeviceProps p;
   if (e == cudaSuccess) e = device_props(p);
@@ -121,8 +121,7 @@ int spec_try_launch(rbd_model* m, const SpecKey& key, const SpecLaunchArgs& a, c
   DeviceProps p;
   RBD_CUDA_TRY(device_props(p));
   const size_t es = key.f64 ? 8 : 4;
-  const size_t smem = (size_t)std::max(1, rows) * 32 * es;
-  if (smem > (size_t)p.max_smem_optin) return RBD_OK;
+  if ((size_t)std::max(1, rows) * 32 * es > (size_t)p.max_smem_optin) return RBD_OK;
   SpecEntry* se = nullptr;
   {
     std::lock_guard<std::mutex> lk(m->spec_mu);
@@ -148,8 +147,17 @@ int spec_try_launch(rbd_model* m, const SpecKey& key, const SpecLaunchArgs& a, c
     }
   }
   const int64_t ngroups = (a.B + 31) / 32;
+  const size_t smem = (size_t)std::max(1, se->rows) * 32 * es;      // shared-memory stash of one warp
+  // Experiments only (tools/time_stash.py): RBD_JIT_SMEM_PAD_BLOCKS=k pads the single-warp blocks' shared memory so that at most
+  // k of them fit on an SM, to measure throughput against resident warps with the program unchanged.
+  size_t smem_blk = smem;
+  if (const char* e = getenv("RBD_JIT_SMEM_PAD_BLOCKS")) {
+    const int k = atoi(e);
+    if (k > 0) smem_blk = std::max(smem, std::min((size_t)p.max_smem_optin, (size_t)(p.smem_per_sm / k) - 1024));
+    RBD_CUDA_TRY(cudaFuncSetAttribute((const void*)se->k_smem, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_blk));
+  }
   int bps = 0;
-  RBD_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, (const void*)se->k_smem, 32, smem));
+  RBD_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, (const void*)se->k_smem, 32, smem_blk));
   if (bps < 1) return RBD_OK;
   // The mixed CTA (rbd_jit_kernels.cuh) is worth trying when it puts at least 15 % more warps on the SM than shared-memory blocks
   // alone and there is a group of samples for each of its warps; which of the two is faster depends on the program, so the first
@@ -181,8 +189,8 @@ int spec_try_launch(rbd_model* m, const SpecKey& key, const SpecLaunchArgs& a, c
       shape = {p.sms, 32 * mix_warps, (int)(smem * mix_sw), 1};
     } else {
       const int grid = (int)std::min<int64_t>(ngroups, (int64_t)bps * p.sms);
-      e = cudaLaunchKernel((const void*)se->k_smem, dim3(grid), dim3(32), params, smem, stream);
-      shape = {grid, 32, (int)smem, bps};
+      e = cudaLaunchKernel((const void*)se->k_smem, dim3(grid), dim3(32), params, smem_blk, stream);
+      shape = {grid, 32, (int)smem_blk, bps};
     }
     last_flag = ctx.flag;
     return e;
