@@ -421,6 +421,25 @@ int32_t rbd_integrate_contact(const rbd_model* model, int32_t dtype, int64_t B, 
                               int64_t tau_step_stride, int64_t tau_stage_stride, const rbd_contact_desc* contact, double dt, int32_t nsteps,
                               void* q_traj, void* v_traj, void* s_traj, void* stream);
 
+/* simulate for a mechanism WITH kinematic loops (DESIGN 4.16): simulate(state, final_time; Δt, stabilization_gains) (src/simulate.jl:
+ * 36-55) -- the nsteps Munthe-Kaas RK4 steps of rbd_integrate_schedule, every stage evaluating dynamics! as the reference does
+ * (mechanism_algorithms.jl:845-864): contact_dynamics! first when `contact` is given, then the KKT solve of rbd_dynamics_loops with
+ * the contact wrenches as the external wrenches.  `loops` as rbd_dynamics_loops (gains NULL = stabilization_gains=nothing); nloops = 0
+ * is a tree rollout on the M^-1 (tau - c) path.  `contact` NULL = no contact; otherwise s is integrated, never reset and persists
+ * across calls exactly as in rbd_integrate_contact.  q, v, s (leading dimension ld) are advanced IN PLACE; tau and its strides as in
+ * rbd_integrate_schedule; the trajectory pointers as in rbd_integrate_contact (all NULL or all set, s_traj may be NULL when ns = 0;
+ * recording does not change the result); no external wrenches.  Descriptor checks as rbd_dynamics_loops and rbd_contact_dynamics;
+ * dtype other than fp32 / fp64: RBD_EUNSUPPORTED; loops == NULL, nsteps < 0, dt <= 0, negative strides, s == NULL with ns > 0, or a
+ * partial set of trajectory pointers: RBD_EINVAL; B == 0: nothing to do.  Kernels per step: per stage the coordinate-map kernel(s)
+ * of rbd_integrate (1 or 2) and one KKT forward-dynamics kernel (with the contact pass in it when ns > 0), then the finishing
+ * kernel(s) of rbd_integrate (1 or 2) and, when ns > 0, one for s -- 14 (15 with contact) for a floating-base robot when
+ * B >= 1024 and B and ld are multiples of 4 (fp32) / 2 (fp64) with 16-byte aligned q and v; 9 for an all-revolute linkage
+ * below that batch size. */
+int32_t rbd_integrate_loops(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, void* s,
+                            const void* tau, int64_t tau_step_stride, int64_t tau_stage_stride,
+                            const rbd_loop_desc* loops, const rbd_contact_desc* contact /* NULL = no contact */,
+                            double dt, int32_t nsteps, void* q_traj, void* v_traj, void* s_traj, void* stream);
+
 /* Reverse mode through a contact rollout (DESIGN 4.15): the gradient of
  *   L = sum_s q_traj_bar[s] . q_traj[s] + v_traj_bar[s] . v_traj[s] + s_traj_bar[s] . s_traj[s]
  * with respect to the initial state (q, v, s) and the torques, for the trajectory rbd_integrate_contact recorded with the same tau,

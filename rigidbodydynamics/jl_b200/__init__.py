@@ -28,7 +28,7 @@ from .contact import (ContactDesc, ContactPoint, HalfSpace3D, HuntCrossleyModel,
                       contact_points, dynamics_contact_, environment, hunt_crossley_hertz, num_contact_states,
                       simulate_contact_, simulate_contact_trajectory_)
 from .loops import (LoopDesc, PDGains, SE3PDGains, constraint_wrench_subspace, default_constraint_stabilization_gains,  # noqa: F401
-                    dynamics_loops_, loop_desc, num_constraints)
+                    dynamics_loops_, loop_desc, num_constraints, simulate_loops_, simulate_loops_trajectory_)
 from .mechanism import maximal_coordinates  # noqa: F401
 from . import autodiff  # noqa: F401  (rbd.autodiff.dynamics / inverse_dynamics: differentiable, kept out of this namespace)
 from .autodiff import dynamics_vjp_, integrate_contact_vjp_, integrate_vjp_, inverse_dynamics_vjp_  # noqa: F401

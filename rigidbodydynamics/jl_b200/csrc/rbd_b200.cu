@@ -954,9 +954,15 @@ __global__ void __launch_bounds__(256) contact_finish_kernel(const ContactFinish
 // rbd_integrate_contact: the contact descriptor in device form and the caller's contact state s [ns x B] (leading dimension ld) with
 // its optional trajectory [(nsteps + 1) x ns x B].
 template <class T> struct ContactRollout {
-  const ContactDev<T>* C;
+  const ContactDev<T>* C;         // NULL in the loop rollout (its stage kernel builds its own)
   int64_t ns;
   T* s; T* traj_s;
+};
+// rbd_integrate_loops: the loop descriptor and, with contact pairs, the contact descriptor, both in host form (rbd_loops.cu turns them
+// into device form once per call, loop_stage_launch).
+struct LoopRollout {
+  const rbd_loop_desc* desc;
+  const rbd_contact_desc* contact;
 };
 
 // Forward dynamics of one stage of the contact rollout: aba_contact_kernel in the variant dynamics_t would pick for the EXT path.
@@ -984,10 +990,12 @@ int contact_stage_launch(const HostModel& hm, const ModelDev<T>& M, const Contac
 // contact the four ṡ_i follow in 4 ns rows.
 // contact (rbd_integrate_contact): every stage's dynamics is aba_contact_kernel, which also writes ṡ_i, and the finishing step
 // also advances the contact state (contact_finish_kernel); the q / v kernels are the same.
+// loop (rbd_integrate_loops): every stage's dynamics is rbd_loops.cu's KKT kernel (loop_stage_launch), with the contact pass when
+// loop->contact is set -- then `contact` carries s and its trajectory, and the finishing step is as above.
 template <class T>
 int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v, const void* tau, int64_t step_stride,
                 int64_t stage_stride, double dt, int nsteps, cudaStream_t stream, T* traj_q = nullptr, T* traj_v = nullptr,
-                T* stages = nullptr, const ContactRollout<T>* contact = nullptr) {
+                T* stages = nullptr, const ContactRollout<T>* contact = nullptr, const LoopRollout* loop = nullptr) {
   const HostModel& hm = model->hm;
   const ModelDev<T>& M = dev_model<T>(hm);
   DeviceProps p;
@@ -1001,6 +1009,7 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
   T* s0 = nullptr;
   T* sd[4] = {nullptr, nullptr, nullptr, nullptr};
   std::optional<LaunchPlan> contact_plan;
+  std::shared_ptr<LoopStagePlan> loop_plan;      // one plan (descriptors, grid, workspace) for every stage of the call
   if (ns) {
     RBD_CUDA_TRY(swork.alloc(5 * ns * (size_t)B * sizeof(T), stream));
     s0 = (T*)swork.p;
@@ -1067,7 +1076,11 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
         integrate_stage_kernel<T><<<dim3(grid, hm.nb), 128, 0, stream>>>(M, sa);
         if (int rc = api_launched()) return rc;
       }
-      if (contact) {
+      if (loop) {
+        const LoopStageArgs la{qsi[i], vsi[i], tau_dense, s0, i ? sd[i - 1] : nullptr, sd[i], vd[i], dt * a[i], B};
+        if (int rc = loop_stage_launch(model, sizeof(T) == 8 ? RBD_F64 : RBD_F32, *loop->desc, loop->contact, la, loop_plan, stream))
+          return rc;
+      } else if (contact) {
         const ContactAbaArgs<T> ca{qsi[i], vsi[i], tau_dense, s0, i ? sd[i - 1] : nullptr, vd[i], sd[i], nullptr, (T)(dt * a[i]), B};
         if (int rc = contact_stage_launch<T>(hm, M, *contact->C, ca, stream, contact_plan)) return rc;
       } else if (int rc = dynamics_t<T>(model, B, B, qsi[i], vsi[i], tau_dense, nullptr, vd[i], nullptr, stream)) {
@@ -1262,6 +1275,23 @@ int integrate_record(const rbd_model* model, int32_t dtype, int64_t B, int64_t l
                                                (float*)v_traj, (float*)stages)
                           : integrate_t<double>(model, B, ld, q, v, tau, step_stride, stage_stride, dt, nsteps, stream, (double*)q_traj,
                                                 (double*)v_traj, (double*)stages);
+}
+template <class T>
+static int integrate_loops_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau, int64_t step_stride,
+                             int64_t stage_stride, const rbd_loop_desc& loops, const rbd_contact_desc* contact, double dt, int nsteps,
+                             void* q_traj, void* v_traj, void* s_traj, cudaStream_t stream) {
+  const LoopRollout lr{&loops, contact};
+  const ContactRollout<T> cr{nullptr, contact ? (int64_t)3 * contact->npoints * contact->nhalfspaces : 0, (T*)s, (T*)s_traj};
+  return integrate_t<T>(model, B, ld, q, v, tau, step_stride, stage_stride, dt, nsteps, stream, (T*)q_traj, (T*)v_traj, nullptr,
+                        contact ? &cr : nullptr, &lr);
+}
+int integrate_loops(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau,
+                    int64_t step_stride, int64_t stage_stride, const rbd_loop_desc& loops, const rbd_contact_desc* contact, double dt,
+                    int nsteps, void* q_traj, void* v_traj, void* s_traj, cudaStream_t stream) {
+  return dtype == RBD_F32 ? integrate_loops_t<float>(model, B, ld, q, v, s, tau, step_stride, stage_stride, loops, contact, dt, nsteps,
+                                                     q_traj, v_traj, s_traj, stream)
+                          : integrate_loops_t<double>(model, B, ld, q, v, s, tau, step_stride, stage_stride, loops, contact, dt, nsteps,
+                                                      q_traj, v_traj, s_traj, stream);
 }
 }  // namespace rbd
 

@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 
 #include <map>
+#include <memory>
 #include <mutex>
 #include <string>
 
@@ -159,6 +160,25 @@ inline int64_t stage_rows(int64_t nq, int64_t nv) { return 4 * nq + 12 * nv; }
 int integrate_record(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, const void* tau, int64_t step_stride,
                      int64_t stage_stride, double dt, int nsteps, void* q_traj, void* v_traj, void* stages, cudaStream_t stream,
                      const rbd_contact_desc* contact = nullptr, void* s = nullptr);
+// The same driver for rbd_integrate_loops (arguments checked by the caller; contact NULL or with ns > 0): every stage's dynamics is
+// loop_stage_launch, and with contact the finishing step also advances s as in rbd_integrate_contact.
+int integrate_loops(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau,
+                    int64_t step_stride, int64_t stage_stride, const rbd_loop_desc& loops, const rbd_contact_desc* contact, double dt,
+                    int nsteps, void* q_traj, void* v_traj, void* s_traj, cudaStream_t stream);
+// rbd_loops.cu's forward dynamics of one stage of the loop rollout: v̇ = the KKT solve of rbd_dynamics_loops at the stage state
+// (q, v) with torques tau (NULL: zero), every array [rows x B] dense.  With `contact` (ns > 0) the contact pass runs first in the
+// same kernel at the stage state s0 + wa ṡ_prev (ṡ_prev NULL at stage 0), writes ṡ and feeds its wrenches to the solve.  `plan`
+// starts empty; the first stage fills it (device descriptors, grid, workspace) and the caller keeps it for every stage of the call.
+struct LoopStagePlan;
+struct LoopStageArgs {
+  const void* q; const void* v; const void* tau;
+  const void* s0; const void* sdp; void* sd;     // contact state (contact only)
+  void* vd;
+  double wa;                                     // dt a_i
+  int64_t B;
+};
+int loop_stage_launch(const rbd_model* model, int32_t dtype, const rbd_loop_desc& loops, const rbd_contact_desc* contact,
+                      const LoopStageArgs& a, std::shared_ptr<LoopStagePlan>& plan, cudaStream_t stream);
 // rbd_b200.cu's descriptor checks of rbd_contact_dynamics (fn: the entry point named in the message)
 int api_check_contact(const rbd_model* model, const rbd_contact_desc* contact, const char* fn);
 // rbd_adjoint.cu's forward-dynamics VJP on dense [rows x B] arrays (no external wrenches); outputs may be NULL

@@ -65,8 +65,9 @@ inline LoopRows loop_rows(int nb, int nv, int nc, int nends, bool ext) {
   return r;
 }
 
-template <class T> struct LoopsIO {
-  Col<T> q, v, tau, wext;
+template <class T, class W = Col<T>> struct LoopsIO {
+  Col<T> q, v, tau;
+  W wext;                             // root-frame external wrenches (ext_wrench_pass)
   ColOut<T> vd, qd, lam, K, k;       // all but vd may be invalid (NULL = not wanted)
   Scr<T> w;                           // workspace column
   LoopRows r;
@@ -89,8 +90,8 @@ template <class T> RBD_HD void pose_mul(const T* Ra, const T* pa, const T* Rb, c
   p[0] = pa[0] + t[0]; p[1] = pa[1] + t[1]; p[2] = pa[2] + t[2];
 }
 
-template <class T, class ST, int KMAX>
-RBD_HD void loops_sample(const ModelDev<T>& M, const LoopDev<T>& L, const LoopsIO<T>& io, const ST& st) {
+template <class T, class ST, int KMAX, class W>
+RBD_HD void loops_sample(const ModelDev<T>& M, const LoopDev<T>& L, const LoopsIO<T, W>& io, const ST& st) {
   const int nb = M.nb, nv = M.nv, nc = L.nc;
   const Scr<T>& w = io.w;
   const LoopRows& r = io.r;
@@ -103,7 +104,7 @@ RBD_HD void loops_sample(const ModelDev<T>& M, const LoopDev<T>& L, const LoopsI
     crba_sample<T, ST, KMAX>(M, cio, st);
   }
   {
-    RneaIO<T> rio;
+    RneaIO<T, W> rio;
     rio.q = io.q; rio.v = io.v; rio.vd = {nullptr, io.q.ld}; rio.wext = io.wext;
     rio.tau = {w.p + (int64_t)r.z * w.ld, w.ld, true};
     rio.ext = {io.wext.valid() ? w.p + (int64_t)r.ext * w.ld : nullptr, w.ld};
@@ -429,6 +430,104 @@ RBD_HD void loops_sample(const ModelDev<T>& M, const LoopDev<T>& L, const LoopsI
     w.st(r.z + i, s);
     io.vd.st(i, s);
   }
+}
+
+// contact_dynamics! at one stage of the loop rollout (rbd_integrate_loops, DESIGN 4.16): contact_sample's sweep (root-frame pose and
+// twist, pending slots in the kin layout of the stash) with the stage semantics of contact_stage_pass -- the stage state
+// s_i = s0 + wa ṡ_{i-1} formed from two loads and never stored, ṡ_i written for every pair (zero out of contact), nothing reset --
+// and every body's ROOT-frame wrench (rows 6 refidx + c, as contact_sample writes them) into `wr`, the thread's own workspace rows,
+// by inactive lanes too.  A sibling rather than a variant of contact_sample, so that contact_kernel's code stays as it is.
+template <class T, class ST>
+RBD_HD void loops_contact_pass(const ModelDev<T>& M, const ContactDev<T>& C, const Col<T>& q, const Col<T>& v, const ContactStageIO<T>& io,
+                               const Scr<T>& wr, const ST& st) {
+  Pose<T> cur;
+  pose_identity(cur);
+  Mot<T> twc;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) twc.w[k] = twc.l[k] = T(0);
+  for (int i = 0; i < M.nb; ++i) {
+    const BodyDev<T>& bd = M.body[i];
+    Pose<T> pp;
+    Mot<T> twp;
+    if (bd.flags & F_ROOT_CHILD) {
+      pose_identity(pp);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) twp.w[k] = twp.l[k] = T(0);
+    } else if (bd.flags & F_FIRST_CHILD) {
+      pp = cur; twp = twc;
+    } else {
+      const int row = bd.pslot * kSlotRowsKin;
+#pragma unroll
+      for (int k = 0; k < 9; ++k) pp.R[k] = st.ld(row + k);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) { pp.p[k] = st.ld(row + 9 + k); twp.w[k] = st.ld(row + 12 + k); twp.l[k] = st.ld(row + 15 + k); }
+    }
+    T R[9], r[3];
+    frame_any(bd, q, R, r);
+    Pose<T> w;
+    pose_mul(pp.R, pp.p, R, r, w.R, w.p);
+    Mot<T> tw = twp;
+    const int nvj = kind_nv_dev(bd.kind);
+    for (int k = 0; k < nvj; ++k) {
+      Mot<T> S;
+      world_subspace(w, sub_comp(bd.kind, k), S);
+      const T x = v(bd.vrow + k);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) { tw.w[c] += x * S.w[c]; tw.l[c] += x * S.l[c]; }
+    }
+    T wn[3] = {T(0), T(0), T(0)}, wf[3] = {T(0), T(0), T(0)};
+    for (int pi = C.first[i]; pi < C.first[i + 1]; ++pi) {
+      T pt[3], vel[3], tmp[3];
+      mat_vec(w.R, C.loc[pi], tmp);
+      pt[0] = w.p[0] + tmp[0]; pt[1] = w.p[1] + tmp[1]; pt[2] = w.p[2] + tmp[2];
+      cross3(tw.w, pt, vel);                                   // point_velocity(twist, point)
+      vel[0] += tw.l[0]; vel[1] += tw.l[1]; vel[2] += tw.l[2];
+      for (int h = 0; h < C.nhalf; ++h) {
+        const int64_t srow = (int64_t)3 * (C.orig[pi] * C.nhalf + h);
+        const T* n = C.hn[h];
+        const T sep = (pt[0] - C.hp[h][0]) * n[0] + (pt[1] - C.hp[h][1]) * n[1] + (pt[2] - C.hp[h][2]) * n[2];
+        T xd[3] = {T(0), T(0), T(0)};
+        if (sep <= T(0)) {
+          T f[3], m[3];
+          contact_force(C, pi, n, -sep, vel, [&](int k) {        // s_i = s0 + wa sd_prev
+            const int64_t e = (srow + k) * io.ld;
+            return io.sdp ? io.s0[e] + io.wa * io.sdp[e] : io.s0[e];
+          }, f, xd);
+          cross3(pt, f, m);                                     // Wrench(point, force)
+#pragma unroll
+          for (int k = 0; k < 3; ++k) { wn[k] += m[k]; wf[k] += f[k]; }
+        }
+        if (io.active) {
+#pragma unroll
+          for (int k = 0; k < 3; ++k) io.sd[(srow + k) * io.ld] = xd[k];
+        }
+      }
+    }
+    const int orow = 6 * bd.refidx;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) { wr.st(orow + k, wn[k]); wr.st(orow + 3 + k, wf[k]); }
+    if (bd.flags & F_HAS_PENDING) {
+      const int row = bd.oslot * kSlotRowsKin;
+#pragma unroll
+      for (int k = 0; k < 9; ++k) st.st(row + k, w.R[k]);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) { st.st(row + 9 + k, w.p[k]); st.st(row + 12 + k, tw.w[k]); st.st(row + 15 + k, tw.l[k]); }
+    }
+    cur = w; twc = tw;
+  }
+}
+
+// One stage of the loop rollout with contact: dynamics! as mechanism_algorithms.jl:845-864 runs it -- loops_contact_pass into rows
+// wrow .. wrow + 6 nb - 1 of the workspace column (behind LoopRows::total), then loops_sample with them as the external wrenches.
+// io.r must be planned with ext = true.  The wrench rows are read back with plain loads (ColRW): the same thread wrote them in this
+// kernel, and the column is reused by the next sample the thread takes.
+template <class T, class ST, int KMAX>
+RBD_HD void loops_contact_sample(const ModelDev<T>& M, const LoopDev<T>& L, const ContactDev<T>& C, const ContactStageIO<T>& cs,
+                                 LoopsIO<T, ColRW<T>> io, int wrow, const ST& st) {
+  const Scr<T> wr{io.w.p + (int64_t)wrow * io.w.ld, io.w.ld};
+  loops_contact_pass(M, C, io.q, io.v, cs, wr, st);
+  io.wext = {wr.p, wr.ld};
+  loops_sample<T, ST, KMAX>(M, L, io, st);
 }
 
 // ------------------------------------------------------------------------------------------------------------------

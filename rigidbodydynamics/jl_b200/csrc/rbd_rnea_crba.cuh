@@ -43,9 +43,10 @@ template <class T> RBD_HD void frame_any(const BodyDev<T>& bd, const Col<T>& q, 
 // ------------------------------------------------------------------------------------------------------------------
 // Outward sweep that tracks each body's world pose in registers (branch nodes park theirs in their pending slot) and
 // writes  f_b = Rw^T f ,  n_b = Rw^T (n - pw x f)  for every body into the scratch column (rows 6 i .. 6 i + 5,
-// i = preorder position).  Wrench loads for body i+1 are issued while body i is processed.
-template <class T, class ST>
-RBD_HD void ext_wrench_pass(const ModelDev<T>& M, const Col<T>& q, const Col<T>& wext, const Scr<T>& ext,
+// i = preorder position).  Wrench loads for body i+1 are issued while body i is processed.  W: Col<T> for the caller's wrenches,
+// ColRW<T> for rows the same kernel wrote (the loop rollout's contact wrenches).
+template <class T, class ST, class W>
+RBD_HD void ext_wrench_pass(const ModelDev<T>& M, const Col<T>& q, const W& wext, const Scr<T>& ext,
                             const ST& stash, int slot_base, int slot_rows) {
   const auto st = stash.slots();     // only the pending slots are used here (world poses of branch nodes)
   Pose<T> cur;
@@ -103,16 +104,17 @@ RBD_HD void ext_wrench_pass(const ModelDev<T>& M, const Col<T>& q, const Col<T>&
 // ==================================================================================================================
 // Recursive Newton-Euler:  tau = M(q) v̇ + c(q, v, w_ext)      (vd invalid => v̇ = 0 => dynamics_bias)
 // ==================================================================================================================
-template <class T> struct RneaIO {
-  Col<T> q, v, vd, wext;
+template <class T, class W = Col<T>> struct RneaIO {
+  Col<T> q, v, vd;
+  W wext;                            // root-frame external wrenches (see ext_wrench_pass)
   ColOut<T> tau;
   Scr<T> ext;
 };
 
 // ST: Stash<T, STRIDE> (shared memory) or the symbolic stash of the code generator (rbd_sym.h); fence_st()
 // stands wherever a thread re-reads a word it wrote; it is a no-op for shared memory
-template <class T, class ST>
-RBD_HD void rnea_sample(const ModelDev<T>& M, const RneaIO<T>& io, const ST& st) {
+template <class T, class ST, class W>
+RBD_HD void rnea_sample(const ModelDev<T>& M, const RneaIO<T, W>& io, const ST& st) {
   const int nb = M.nb;
   const int slot_base = nb * kRneaRowsPerBody;
   if (io.ext.valid()) ext_wrench_pass(M, io.q, io.wext, io.ext, st, slot_base, kSlotRowsRnea);

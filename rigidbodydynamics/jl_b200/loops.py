@@ -6,9 +6,12 @@
                                                   quaternion_spherical.jl:60, sin_cos_revolute.jl:125; none for floating joints
     dynamics!(result, state, ...) with loops      mechanism_algorithms.jl:845-864 (constraint_jacobian! :574-598,
                                                   constraint_bias! :630-673, dynamics_solve! :747-822)   -> dynamics_loops_
+    simulate(state, final_time; Δt, stabilization_gains) with loops (simulate.jl:36-55), with or without contact points
+                                                  -> simulate_loops_, simulate_loops_trajectory_
 
 A ``Mechanism``'s spanning tree is its q / v order and its model handle; the non-tree joints travel with every call as an
-``rbd_loop_desc`` (include/rbd_b200.h).  All compute is one CUDA kernel behind ``rbd_dynamics_loops``; there is no CPU path.
+``rbd_loop_desc`` (include/rbd_b200.h).  All compute is one CUDA kernel behind ``rbd_dynamics_loops`` (per RK4 stage behind
+``rbd_integrate_loops``); there is no CPU path.
 """
 from __future__ import annotations
 
@@ -20,14 +23,15 @@ import numpy as np
 import torch
 
 from . import _cabi
-from .algorithms import _call, _check, _ptr, _stream
+from .algorithms import _call, _check, _ptr, _stream, _torque_schedule
+from .contact import ContactDesc, contact_desc
 from .joint_types import Fixed, Planar, Prismatic, QuaternionSpherical, Revolute
 from .mechanism import Mechanism
 from .spatial import rotation_between
 from .state import DynamicsResult, MechanismState, _DT
 
 __all__ = ["PDGains", "SE3PDGains", "default_constraint_stabilization_gains", "constraint_wrench_subspace", "num_constraints",
-           "LoopDesc", "loop_desc", "dynamics_loops_"]
+           "LoopDesc", "loop_desc", "dynamics_loops_", "simulate_loops_", "simulate_loops_trajectory_"]
 
 
 @dataclass
@@ -171,3 +175,62 @@ def dynamics_loops_(result: DynamicsResult, state: MechanismState, torques: Opti
                                  _ptr(result.qd) if want_qd else None, _ptr(lam), _ptr(K), _ptr(k), _stream()))
     del keep
     return result
+
+
+def _integrate_loops(state: MechanismState, nsteps: int, torques, dt: float, stabilization_gains, loops: Optional[LoopDesc],
+                     contact_state: Optional[torch.Tensor], contact: Optional[ContactDesc], record: bool, what: str):
+    state.check_modcount()
+    if nsteps < 0:
+        raise ValueError("nsteps must be >= 0")
+    lib = _cabi.load_library()
+    ld = loops if loops is not None else loop_desc(state.mechanism, stabilization_gains)
+    cd = contact if contact is not None else contact_desc(state.mechanism)
+    if contact_state is None and cd.nstates > 0:
+        raise ValueError(f"{what}: contact_state [{cd.nstates}, B] must be given (the mechanism has contact points)")
+    _check(contact_state, cd.nstates, state, "contact_state")
+    step = stage = 0
+    if torques is not None and torques.dim() in (3, 4):
+        step, stage = _torque_schedule(state, torques, nsteps)
+    else:
+        _check(torques, state.nv, state, "torques")
+    traj = (None, None, None)
+    if record:
+        new = lambda rows: torch.empty((nsteps + 1, rows, state.batch), dtype=state.dtype, device=state.q.device)   # noqa: E731
+        traj = (new(state.nq), new(state.nv), new(cd.nstates) if cd.nstates else None)
+    lst, keep = ld.c_struct()
+    cst, keep2 = cd.c_struct()
+    _call(lib.rbd_integrate_loops(state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q), _ptr(state.v),
+                                  _ptr(contact_state), _ptr(torques), step, stage, ctypes.byref(lst), ctypes.byref(cst), float(dt),
+                                  nsteps, *[_ptr(t) for t in traj], _stream()))
+    del keep, keep2
+    return traj
+
+
+def simulate_loops_trajectory_(state: MechanismState, nsteps: int, torques: Optional[torch.Tensor] = None, dt: float = 1e-4,
+                               stabilization_gains=_DEFAULT, loops: Optional[LoopDesc] = None,
+                               contact_state: Optional[torch.Tensor] = None, contact: Optional[ContactDesc] = None):
+    """``nsteps`` steps of ``simulate_loops_``, recording the trajectory: returns ``(q_traj, v_traj, s_traj)``, [nsteps + 1, nq, B],
+    [nsteps + 1, nv, B] and [nsteps + 1, num_contact_states, B] (None without contact states), block 0 the initial state and block s
+    the state after step s.  ``state`` and ``contact_state`` are advanced in place exactly as ``simulate_loops_`` advances them."""
+    return _integrate_loops(state, nsteps, torques, dt, stabilization_gains, loops, contact_state, contact, True,
+                            "simulate_loops_trajectory_")
+
+
+def simulate_loops_(state: MechanismState, final_time: float, torques: Optional[torch.Tensor] = None, dt: float = 1e-4,
+                    stabilization_gains=_DEFAULT, loops: Optional[LoopDesc] = None, contact_state: Optional[torch.Tensor] = None,
+                    contact: Optional[ContactDesc] = None) -> int:
+    """``simulate(state, final_time; Δt, stabilization_gains)`` (src/simulate.jl:36-55) for a mechanism with non-tree joints, all on
+    the GPU: Munthe-Kaas RK4 steps until ``t >= final_time`` (the step count of ``simulate_``) whose every stage runs ``dynamics!``
+    as ``dynamics_loops_`` does -- with contact points, contact_dynamics! first and its wrenches as the external wrenches
+    (mechanism_algorithms.jl:845-864).  ``state.q``, ``state.v`` and ``contact_state`` ([num_contact_states, B], required when the
+    mechanism has contact points) are advanced in place; the contact state follows ``simulate_contact_`` (integrated, never reset,
+    carried across calls).  ``torques``: None, constant [nv, B], per step [nsteps, nv, B] or per stage [nsteps, 4, nv, B].
+    ``stabilization_gains``: as ``loop_desc`` (default gains, None = off, or per joint); ``loops`` / ``contact``: prebuilt
+    descriptors (default: the mechanism's).  A tree mechanism is accepted (the KKT path without constraint rows).  Returns the number
+    of steps taken."""
+    nsteps, t = 0, 0.0
+    while t < final_time:            # the reference's `while t < final_time` loop (ode_integrators.jl:311)
+        t += dt
+        nsteps += 1
+    _integrate_loops(state, nsteps, torques, dt, stabilization_gains, loops, contact_state, contact, False, "simulate_loops_")
+    return nsteps
