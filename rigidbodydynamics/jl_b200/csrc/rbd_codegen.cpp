@@ -20,7 +20,7 @@
 namespace rbd {
 namespace {
 
-constexpr int kGeneratorVersion = 30;   // bump when the emitted code changes (part of the cubin cache key)
+constexpr int kGeneratorVersion = 31;   // bump when the emitted code changes (part of the cubin cache key)
 constexpr int kRegRowsAba = -1;         // register-resident stash rows of the fp32 forward-dynamics programs (-1: all eligible)
 constexpr int kSmemPerSm = 233472;      // H100: 228 KB of shared memory per SM ...
 constexpr int kSmemReservedPerBlock = 1024;   // ... of which each resident block takes 1 KB for the system
@@ -39,7 +39,7 @@ struct TraceScope {
 // triangle only, mechanism_algorithms.jl:248-272): a store to row i + j*nv with i < j is not recorded.
 struct LowerFilter { int nv; };
 
-bool run_trace(const HostModel& hm, const SpecKey& key, SymTrace& tr, int& stash_rows, std::string& err) {
+bool run_trace(const HostModel& hm, const SpecKey& key, bool trig, SymTrace& tr, int& stash_rows, std::string& err) {
   tr.single = !key.f64;
   TraceScope scope(&tr);
   std::unique_ptr<ModelDev<Sym>> M(new ModelDev<Sym>());
@@ -56,7 +56,8 @@ bool run_trace(const HostModel& hm, const SpecKey& key, SymTrace& tr, int& stash
         else if (a > 1) tr.fresh_steps.insert({pass, a - 1});
         else if (pass == 3) tr.fresh_steps.insert({2, -1});
       }
-  const SymStash st;
+  SymStash st;
+  st.trig = trig && key.algo == SPEC_ABA;
   if (key.algo == SPEC_ABA) {
     AbaIO<Sym, false, kAllKinds> io;
     io.q = {A_Q, true}; io.v = {A_V, true}; io.tau = {A_TAU, key.has_in2}; io.wext = {A_WEXT, false};
@@ -233,12 +234,12 @@ struct Emitter {
         return std::string("RBD_STG(") + arr_name(n.arr) + ", " + row(i) + ", " + opnd(i, 0) + ");\n";
       case S_SLD:
         ++stats.n_sld;
-        if (reg_row(n.row)) return v + rname(n.row) + ";\n";
-        return v + "RBD_SLD(" + row(i) + ");\n";
+        if (reg_row(n.arr, n.row)) return v + rname(n.arr, n.row) + ";\n";
+        return v + (n.arr == R_TRIG ? "RBD_TLD(" : "RBD_SLD(") + row(i) + ");\n";
       case S_SST:
         ++stats.n_sst;
-        if (reg_row(n.row)) return rname(n.row) + " = " + opnd(i, 0) + ";\n";
-        return "RBD_SST(" + row(i) + ", " + opnd(i, 0) + ");\n";
+        if (reg_row(n.arr, n.row)) return rname(n.arr, n.row) + " = " + opnd(i, 0) + ";\n";
+        return (n.arr == R_TRIG ? "RBD_TST(" : "RBD_SST(") + row(i) + ", " + opnd(i, 0) + ");\n";
       case S_SFENCE: return "RBD_SFENCE();\n";
       case S_XLD: return v + "RBD_XLD(" + row(i) + ");\n";
       case S_XST: return "RBD_XST(" + row(i) + ", " + opnd(i, 0) + ");\n";
@@ -403,9 +404,13 @@ struct Emitter {
           txt[0] = b0.txt;
           if (na.op == S_COS) { auto m = f.b2a.find(nb.b); if (m == f.b2a.end() || m->second != na.b) return false; }
           if (na.op == S_STORE && na.arr != nb.arr) return false;
+          if (na.op == S_SST && na.arr != nb.arr) return false;
           if (na.op == S_SST || na.op == S_STORE) f.drow[a] = nb.row - na.row;
           break;
-        case S_SLD: f.drow[a] = nb.row - na.row; break;
+        case S_SLD:
+          if (na.arr != nb.arr) return false;
+          f.drow[a] = nb.row - na.row;
+          break;
         case S_SFENCE: break;
         default: return false;
       }
@@ -481,36 +486,41 @@ struct Emitter {
   // row of a straight-line one.  Up to `reg_budget` such rows (-1: all) become registers, chosen by accesses per statement of
   // live range (a value is live from its store to the last load before the next store); the other rows are renumbered
   // 0 .. shared_rows - 1 in their order.  The statements are the same either way, so the results are bit-identical.
+  // The trig cache (region R_TRIG) is planned the same way on its own rows, every eligible one a register unless the budget is
+  // 0; its shared rows follow the stash's in each warp's shared memory (RBD_TLD / RBD_TST).
   int reg_budget = 0;
-  std::vector<int> rowmap;       // stash row -> shared-memory row, -1: register
-  std::vector<int> regs;         // register rows, ascending
-  int shared_rows = 0;
+  std::vector<int> rowmap[R_COUNT];   // row of a region -> shared-memory row of that region, -1: register
+  std::vector<int> regs[R_COUNT];     // register rows, ascending
+  int shared_rows = 0;                // shared rows of the stash
+  int trig_rows = 0;                  // shared rows of the trig cache
 
-  bool reg_row(int r) const { return r >= 0 && r < (int)rowmap.size() && rowmap[r] == -1; }
-  static std::string rname(int r) { return "rbd_r" + std::to_string(r); }
-  int srow(int r) const { return r < (int)rowmap.size() ? rowmap[r] : r; }
+  bool reg_row(int g, int r) const { return r >= 0 && r < (int)rowmap[g].size() && rowmap[g][r] == -1; }
+  static std::string rname(int g, int r) { return (g == R_TRIG ? "rbd_sc" : "rbd_r") + std::to_string(r); }
+  int srow(int g, int r) const { return r < (int)rowmap[g].size() ? rowmap[g][r] : r; }
   bool stash_op(int j) const { return tr.nodes[j].op == S_SLD || tr.nodes[j].op == S_SST; }
-  std::string row_text(int j) const { return std::to_string(stash_op(j) ? srow(tr.nodes[j].row) : tr.nodes[j].row); }
+  std::string row_text(int j) const { return std::to_string(stash_op(j) ? srow(tr.nodes[j].arr, tr.nodes[j].row) : tr.nodes[j].row); }
 
-  void plan_rows(int total_rows) {
+  // returns the number of shared rows of region g
+  int plan_region(int g, int total_rows, int budget) {
     const auto& N = tr.nodes;
+    auto in = [&](size_t i) { return live[i] && stash_op((int)i) && N[i].arr == g; };
+    std::vector<int>& map = rowmap[g];
     int nrows = total_rows;
     for (size_t i = 0; i < N.size(); ++i)
-      if (live[i] && (N[i].op == S_SLD || N[i].op == S_SST)) nrows = std::max(nrows, N[i].row + 1);
-    rowmap.resize(nrows);
-    for (int r = 0; r < nrows; ++r) rowmap[r] = r;
-    shared_rows = total_rows;
-    if (reg_budget == 0) return;
+      if (in(i)) nrows = std::max(nrows, N[i].row + 1);
+    map.resize(nrows);
+    for (int r = 0; r < nrows; ++r) map[r] = r;
+    if (g == R_STASH && budget == 0) return total_rows;
     std::vector<uint8_t> indexed(nrows, 0), touched(nrows, 0);
     for (const Fold& f : folds)
       for (const auto& e : f.drow) {
         const SymNode& n = N[e.first];
-        if (e.second == 0 || (n.op != S_SLD && n.op != S_SST) || fused[e.first]) continue;
+        if (e.second == 0 || !stash_op(e.first) || n.arr != g || fused[e.first]) continue;
         indexed[n.row] = indexed[n.row + e.second] = 1;
       }
     std::vector<int64_t> acc(nrows, 0), span(nrows, 0), open(nrows, -1), last(nrows, -1);
     for (size_t i = 0; i < N.size(); ++i) {
-      if (!live[i] || (N[i].op != S_SLD && N[i].op != S_SST)) continue;
+      if (!in(i)) continue;
       const int r = N[i].row;
       touched[r] = 1;
       ++acc[r];
@@ -528,25 +538,33 @@ struct Emitter {
       if (touched[r] && !indexed[r]) cand.push_back(r);
     }
     std::stable_sort(cand.begin(), cand.end(), [&](int x, int y) { return acc[x] * (span[y] + 1) > acc[y] * (span[x] + 1); });
-    if (reg_budget > 0 && (int)cand.size() > reg_budget) cand.resize(reg_budget);
-    regs = cand;
-    std::sort(regs.begin(), regs.end());
-    for (int r : regs) rowmap[r] = -1;
-    shared_rows = 0;
+    if (budget >= 0 && (int)cand.size() > budget) cand.resize(budget);
+    regs[g] = cand;
+    std::sort(regs[g].begin(), regs[g].end());
+    for (int r : regs[g]) map[r] = -1;
+    int shared = 0;
     for (int r = 0; r < nrows; ++r)
-      if (rowmap[r] >= 0) rowmap[r] = touched[r] ? shared_rows++ : -2;    // -2: never accessed (no slot, never emitted)
-    stats.reg_rows = (int)regs.size();
+      if (map[r] >= 0) map[r] = touched[r] ? shared++ : -2;    // -2: never accessed (no slot, never emitted)
+    return shared;
+  }
+  void plan_rows(int total_rows) {
+    shared_rows = plan_region(R_STASH, total_rows, reg_budget);
+    if (reg_budget != 0) stats.reg_rows = (int)regs[R_STASH].size();
+    trig_rows = plan_region(R_TRIG, 0, reg_budget == 0 ? 0 : -1);
+    stats.trig_rows = trig_rows;
+    stats.trig_reg_rows = (int)regs[R_TRIG].size();
   }
   std::string reg_decls() const {
     std::string s;
-    for (int r : regs) s += "rbd_v " + rname(r) + " = RBD_K(" + lit(0.0) + ");\n";
+    for (int g = 0; g < R_COUNT; ++g)
+      for (int r : regs[g]) s += "rbd_v " + rname(g, r) + " = RBD_K(" + lit(0.0) + ");\n";
     return s;
   }
 
   void emit_fold(const Fold& f, int& since) {
     const auto& N = tr.nodes;
     auto rowx = [](int row, int d) { return d ? "(" + std::to_string(row) + " + rbd_it * " + std::to_string(d) + ")" : std::to_string(row); };
-    auto srowx = [&](int row, int d) { return rowx(srow(row), d ? srow(row + d) - srow(row) : 0); };
+    auto srowx = [&](int g, int row, int d) { return rowx(srow(g, row), d ? srow(g, row + d) - srow(g, row) : 0); };
     char hdr[160];
     snprintf(hdr, sizeof hdr, "// ABA pass %d: bodies %d..%d and their mirror images run one copy of the code\n", f.pass,
              std::min(f.first, f.first + (f.pass == 2 ? 1 - f.len : f.len - 1)), std::max(f.first, f.first + (f.pass == 2 ? 1 - f.len : f.len - 1)));
@@ -570,7 +588,7 @@ struct Emitter {
     const NameFn arow = [&](int j) {
       auto it = f.drow.find(j);
       const int d = it == f.drow.end() ? 0 : it->second;
-      return stash_op(j) ? srowx(N[j].row, d) : rowx(N[j].row, d);
+      return stash_op(j) ? srowx(N[j].arr, N[j].row, d) : rowx(N[j].row, d);
     };
     const NameFn absrow = [&](int j) { return row_text(j); };
     std::set<int32_t> outset(f.outs.begin(), f.outs.end());
@@ -630,8 +648,7 @@ struct Emitter {
     plan_rows(total_rows);
   }
 
-  void emit() {
-    plan();
+  void emit() {      // after plan()
     const auto& N = tr.nodes;
     stats.nodes_traced = (int)N.size();
     for (size_t i = 0; i < N.size(); ++i) if (live[i] && N[i].op != S_CONST && N[i].op != S_PARAM) ++stats.nodes_live;
@@ -675,27 +692,53 @@ struct Emitter {
 
 }  // namespace
 
+namespace {
+
+// Shared-memory rows of a planned program's stash (RBD_SPEC_ROWS): the compacted rows when some are registers, else the
+// algorithm's layout.
+int smem_stash_rows(const HostModel& hm, const SpecKey& key, const Emitter& em) {
+  return em.stats.reg_rows ? em.shared_rows : spec_stash_rows(hm, key);
+}
+
+// Traces `key` and plans its program (`em`, over `tr`).  The trig cache (spec_trig) is kept only if its shared rows cost no
+// resident single-warp blocks; otherwise the program is traced again without it (the cache only saves recomputation).
+bool plan_program(const HostModel& hm, const SpecKey& key, int flavor, bool fold, SymTrace& tr, std::unique_ptr<Emitter>& em,
+                  std::string& err) {
+  for (bool trig = spec_trig(key);; trig = false) {
+    em.reset();
+    tr = SymTrace();
+    int rows = 0;
+    if (!run_trace(hm, key, trig, tr, rows, err)) return false;
+    em.reset(new Emitter(tr, key, flavor));
+    em->hm = &hm;
+    em->fold = fold;
+    em->total_rows = rows;
+    em->reg_budget = spec_reg_rows(key);
+    if (flavor != FLAVOR_CPU) {
+      // One basic block of 10^4 instructions lets ptxas stretch live ranges until it spills (Atlas: 128 registers + 350 B of
+      // local memory, -10 % throughput); a never-taken branch every few hundred statements bounds its scheduling regions.
+      // A folded program's loops already end basic blocks every few hundred statements, and there the extra branches only cost
+      // (Atlas fp32 forward dynamics on H100 at 400 W: 800 M evals/s with a branch every 192 statements, 856 M without).
+      em->split_every = 192;
+      em->split_folded = 0;
+      if (const char* e = getenv("RBD_JIT_SPLIT")) em->split_every = em->split_folded = atoi(e);
+    }
+    em->plan();
+    const int stash = smem_stash_rows(hm, key, *em);
+    if (!trig || spec_smem_blocks(key, stash + em->trig_rows) >= spec_smem_blocks(key, stash)) return true;
+  }
+}
+
+}  // namespace
+
 bool spec_emit_function(const HostModel& hm, const SpecKey& key, int flavor, const std::string& name, std::string& out,
                         SpecStats* stats, std::string& err, bool fold) {
   SymTrace tr;
-  int rows = 0;
-  if (!run_trace(hm, key, tr, rows, err)) return false;
-  Emitter em(tr, key, flavor);
-  em.hm = &hm;
-  em.fold = fold;
-  em.total_rows = rows;
-  em.reg_budget = spec_reg_rows(key);
-  if (flavor != FLAVOR_CPU) {
-    // One basic block of 10^4 instructions lets ptxas stretch live ranges until it spills (Atlas: 128 registers + 350 B of
-    // local memory, -10 % throughput); a never-taken branch every few hundred statements bounds its scheduling regions.
-    // A folded program's loops already end basic blocks every few hundred statements, and there the extra branches only cost
-    // (Atlas fp32 forward dynamics on H100 at 400 W: 800 M evals/s with a branch every 192 statements, 856 M without).
-    em.split_every = 192;
-    em.split_folded = 0;
-    if (const char* e = getenv("RBD_JIT_SPLIT")) em.split_every = em.split_folded = atoi(e);
-  }
+  std::unique_ptr<Emitter> pem;
+  if (!plan_program(hm, key, flavor, fold, tr, pem, err)) return false;
+  Emitter& em = *pem;
   em.emit();
-  em.stats.stash_rows = rows;
+  em.stats.stash_rows = em.total_rows;
   em.stats.shared_rows = em.shared_rows;
   if (stats) *stats = em.stats;
   out += em.param_table();
@@ -712,6 +755,7 @@ bool spec_emit_function(const HostModel& hm, const SpecKey& key, int flavor, con
   out += sig + " {\n";
   if (flavor != FLAVOR_CPU) out += "RBD_FN_BEGIN\n";
   if (key.algo == SPEC_KIN) out += flavor == FLAVOR_CPU ? "RBD_KIN_BEGIN_CPU\n" : "RBD_KIN_BEGIN\n";
+  if (flavor == FLAVOR_CPU && em.trig_rows) out += "rbd_v rbd_trig[" + std::to_string(em.trig_rows) + "];\n";
   out += em.reg_decls();
   out += em.out;
   if (flavor != FLAVOR_CPU) out += "RBD_FN_END\n";
@@ -742,17 +786,19 @@ int spec_smem_blocks(const SpecKey& key, int shared_rows) {
   return std::max(1, std::min(spec_reg_rows(key) != 0 ? 8 : 16, kSmemPerSm / (bytes + kSmemReservedPerBlock)));
 }
 
+bool spec_trig(const SpecKey& key) {
+  if (key.algo != SPEC_ABA || key.f64) return false;
+  const char* e = getenv("RBD_JIT_TRIG");
+  return !e || e[0] != '0';
+}
+
 int spec_shared_rows(const HostModel& hm, const SpecKey& key) {
+  if (spec_reg_rows(key) == 0 && !spec_trig(key)) return spec_stash_rows(hm, key);
   SymTrace tr;
-  int rows = 0;
+  std::unique_ptr<Emitter> em;
   std::string err;
-  if (spec_reg_rows(key) == 0 || !run_trace(hm, key, tr, rows, err)) return spec_stash_rows(hm, key);
-  Emitter em(tr, key, FLAVOR_SMEM);
-  em.hm = &hm;
-  em.total_rows = rows;
-  em.reg_budget = spec_reg_rows(key);
-  em.plan();
-  return em.shared_rows;
+  if (!plan_program(hm, key, FLAVOR_SMEM, true, tr, em, err)) return spec_stash_rows(hm, key);
+  return smem_stash_rows(hm, key, *em) + em->trig_rows;
 }
 
 uint64_t spec_hash(const HostModel& hm, const SpecKey& key) {
@@ -762,8 +808,8 @@ uint64_t spec_hash(const HostModel& hm, const SpecKey& key) {
     for (size_t i = 0; i < n; ++i) { h ^= b[i]; h *= 0x100000001b3ull; }
   };
   const char* blocks = getenv("RBD_JIT_SMEM_BLOCKS");
-  const int hdr[11] = {kGeneratorVersion, key.algo, key.f64, key.has_in2, key.has_out1, key.lower, hm.nb, hm.general, key.peers,
-                       spec_reg_rows(key), blocks ? atoi(blocks) : 0};
+  const int hdr[12] = {kGeneratorVersion, key.algo, key.f64, key.has_in2, key.has_out1, key.lower, hm.nb, hm.general, key.peers,
+                       spec_reg_rows(key), blocks ? atoi(blocks) : 0, spec_trig(key)};
   mix(hdr, sizeof hdr);
   if (key.algo == SPEC_KIN) { mix(&key.kin_mask, sizeof key.kin_mask); mix(key.kin_sign, sizeof key.kin_sign); }
   if (key.f64) {
@@ -783,16 +829,17 @@ bool spec_emit_cuda_tu(const HostModel& hm, const SpecKey& key, std::string& out
   if (!spec_emit_function(hm, key, FLAVOR_SMEM, "rbd_spec_smem", fn_smem, &st, err)) return false;
   if (stats) *stats = st;
   char buf[1024];
-  const int rows = st.reg_rows ? st.shared_rows : spec_stash_rows(hm, key);     // shared-memory rows
+  const int rows = st.reg_rows ? st.shared_rows : spec_stash_rows(hm, key);     // shared-memory rows of the stash (smem_stash_rows)
   snprintf(buf, sizeof buf,
            "// generated by librbd_b200.so (rbd_codegen.cpp) for one mechanism: %d live nodes (%d add/sub, %d mul, %d div, %d sincos, "
-           "%d global loads, %d stash loads, %d stash stores; %d stash rows in registers)\n"
+           "%d global loads, %d stash loads, %d stash stores; %d stash rows in registers; trig cache: %d rows in shared memory, "
+           "%d in registers)\n"
            "#define RBD_SPEC_SMEM_BLOCKS %d\n"
-           "#define RBD_SPEC_F64 %d\n#define RBD_SPEC_NQ %d\n#define RBD_SPEC_NV %d\n#define RBD_SPEC_ROWS %d\n"
+           "#define RBD_SPEC_F64 %d\n#define RBD_SPEC_NQ %d\n#define RBD_SPEC_NV %d\n#define RBD_SPEC_ROWS %d\n#define RBD_SPEC_TRIG_ROWS %d\n"
            "#define RBD_SPEC_HAS_IN2 %d\n#define RBD_SPEC_HAS_OUT1 %d\n#define RBD_SPEC_OUT0_ROWS %d\n#define RBD_SPEC_OUT1_ROWS %d\n"
            "#define RBD_SPEC_ROW32 %d\n#define RBD_SPEC_KIN %d\n#define RBD_SPEC_USES_V %d\n#include \"rbd_jit_prelude.cuh\"\n",
-           st.nodes_live, st.n_add, st.n_mul, st.n_div, st.n_sincos, st.n_load, st.n_sld, st.n_sst, st.reg_rows,
-           spec_smem_blocks(key, rows), key.f64 ? 1 : 0, hm.nq, hm.nv, rows, key.has_in2 ? 1 : 0, key.has_out1 ? 1 : 0, key.algo == SPEC_CRBA ? hm.nv * hm.nv : hm.nv, hm.nq,
+           st.nodes_live, st.n_add, st.n_mul, st.n_div, st.n_sincos, st.n_load, st.n_sld, st.n_sst, st.reg_rows, st.trig_rows,
+           st.trig_reg_rows, spec_smem_blocks(key, rows + st.trig_rows), key.f64 ? 1 : 0, hm.nq, hm.nv, rows, st.trig_rows, key.has_in2 ? 1 : 0, key.has_out1 ? 1 : 0, key.algo == SPEC_CRBA ? hm.nv * hm.nv : hm.nv, hm.nq,
            key.algo == SPEC_CRBA ? 1 : 0, key.algo == SPEC_KIN ? 1 : 0, st.n_load_v > 0 ? 1 : 0);
   out += buf;
   out += "#define RBD_FLAVOR_SMEM 1\n#include \"rbd_jit_flavor.cuh\"\n" + fn_smem;
@@ -806,6 +853,7 @@ bool spec_emit_cpu_tu(const HostModel& hm, const SpecKey& key, const std::string
          "#include \"rbd_device.cuh\"\n"
          "#define RBD_LDG(p, r) p[(long long)(r) * ld]\n#define RBD_STG(p, r, x) p[(long long)(r) * ld] = (x)\n"
          "#define RBD_SLD(r) sh[r]\n#define RBD_SST(r, x) sh[r] = (x)\n#define RBD_SFENCE()\n"
+         "#define RBD_TLD(r) rbd_trig[r]\n#define RBD_TST(r, x) rbd_trig[r] = (x)\n"
          "#define RBD_RCP(x) (1 / (x))\n#define RBD_DIV(a, b) ((a) / (b))\n#define RBD_SINCOS(x, s, c) rbd::sincos_t(x, s, c)\n"
          "#define RBD_K(x) (x)\n#define RBD_ADD(a, b) ((a) + (b))\n#define RBD_SUB(a, b) ((a) - (b))\n#define RBD_MUL(a, b) ((a) * (b))\n"
          "#define RBD_KIN_BEGIN_CPU rbd_v *ko0 = ko[0], *ko1 = ko[1], *ko2 = ko[2], *ko3 = ko[3], *ko4 = ko[4], *ko5 = ko[5], *ko6 = ko[6], *ko7 = ko[7]; (void)ko0; (void)ko1; (void)ko2; (void)ko3; (void)ko4; (void)ko5; (void)ko6; (void)ko7;\n"

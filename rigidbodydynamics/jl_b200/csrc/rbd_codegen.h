@@ -30,6 +30,8 @@ struct SpecStats {
   int n_fold_bodies = 0; // body steps whose code those loops share (summed over passes)
   int reg_rows = 0;      // stash rows kept in registers (RBD_JIT_REG_ROWS)
   int shared_rows = 0;   // stash rows left in shared memory (RBD_SPEC_ROWS of the CUDA flavour)
+  int trig_rows = 0;     // trig cache rows in shared memory, after the stash's (RBD_SPEC_TRIG_ROWS; spec_trig)
+  int trig_reg_rows = 0; // trig cache rows in registers
 };
 
 enum SpecFlavor : int { FLAVOR_CPU = 0, FLAVOR_SMEM = 1 };
@@ -42,10 +44,15 @@ bool spec_emit_function(const HostModel& hm, const SpecKey& key, int flavor, con
 
 // Whole NVRTC translation unit for `key`: defines + the per-sample function + the kernel shell of the prelude.
 bool spec_emit_cuda_tu(const HostModel& hm, const SpecKey& key, std::string& out, SpecStats* stats, std::string& err);
-// Rows of the algorithm's stash layout, and the rows of them the generated program keeps in shared memory (the others are
-// registers, see spec_reg_rows); the latter runs the tracer, it is meant for once per loaded program.
+// Rows of the algorithm's stash layout, and the rows of one warp's shared memory in the generated program: the stash rows it
+// keeps there (the others are registers, see spec_reg_rows) plus those of its trig cache (spec_trig).  The latter runs the
+// tracer, it is meant for once per loaded program.
 int spec_stash_rows(const HostModel& hm, const SpecKey& key);
 int spec_shared_rows(const HostModel& hm, const SpecKey& key);
+// Whether the program keeps a trig cache: (sin, cos) of every revolute joint computed once in the first ABA pass and read back in
+// the other two (trig_keep, rbd_device.cuh).  fp32 forward dynamics only, and only where its shared rows cost no resident
+// blocks; RBD_JIT_TRIG=0 turns it off.
+bool spec_trig(const SpecKey& key);
 // Budget of register-resident stash rows for `key` (-1: every eligible row); RBD_JIT_REG_ROWS overrides it for forward dynamics.
 int spec_reg_rows(const SpecKey& key);
 // Minimum resident single-warp blocks per SM rbd_jit_smem is compiled for (its register cap): as many as the shared stash

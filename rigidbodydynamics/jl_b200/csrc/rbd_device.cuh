@@ -42,6 +42,7 @@ namespace rbd {
 
 // Per-thread view of the shared-memory stash: row k of this sample is p[k * STRIDE].
 template <class T, int STRIDE> struct Stash {
+  static constexpr bool kTrig = false;   // no (sin, cos) cache of the revolute joints (see trig_keep)
   T* p;
   RBD_HD T ld(int row) const { return p[row * STRIDE]; }
   RBD_HD void st(int row, T v) const { p[row * STRIDE] = v; }
@@ -706,8 +707,11 @@ RBD_HD void prefetch_body(const ModelDev<T>& M, int i, const IO& io, Pre<T>& p) 
     for (int k = 0; k < 6; ++k) p.w[k] = io.ext.get(6 * i + k);
   }
   if (kind == K_REV || kind == K_PRIS || kind == K_SINCOS) {     // multi-DoF bodies read their rows directly
-    p.q0 = io.q(bd.qrow);                 // the joint angle is re-read (and sin/cos recomputed) in every pass:
-    if (kind == K_SINCOS) p.q1 = io.q(bd.qrow + 1);   // two stash rows per body buy ~40 % more resident warps
+    // The joint angle is re-read (and sin/cos recomputed) in every pass unless the stash keeps a trig cache (trig_keep): in the
+    // generic kernels two more stash rows per body would cost ~40 % of the resident warps; in the model-specialised fp32
+    // forward-dynamics program the angle loads of passes 2 and 3 are then dead code the generator drops.
+    p.q0 = io.q(bd.qrow);
+    if (kind == K_SINCOS) p.q1 = io.q(bd.qrow + 1);
     p.qd = io.v(bd.vrow);
     if (PASS == 2 && io.tau.valid()) p.tau = io.tau(bd.vrow);
   }
@@ -721,6 +725,22 @@ template <class T> RBD_HD void joint_scd(int kind, const Pre<T>& pre, T& s, T& c
   if (kind == K_REV) sincos_t(pre.q0 + qoff, s, c);
   else if (kind == K_SINCOS) { s = pre.q0; c = pre.q1; }
   else if (kind == K_PRIS) d = pre.q0;
+}
+
+// Trig cache (ST::kTrig): pass 1 keeps the (sin, cos) of every revolute joint, passes 2 and 3 read them back instead of
+// evaluating sin / cos of the same angle again.  Only the code generator's stash has one (SymStash, rbd_sym.h: a separate region
+// of the specialised program's shared memory, or registers); the generic kernels' Stash has none and compiles as before.
+template <class T, class ST> RBD_HD void trig_keep(const ST& st, int kind, int i, const T& s, const T& c) {
+  if constexpr (ST::kTrig) {
+    if (kind == K_REV) st.trig_st(i, s, c);
+  }
+}
+// joint_scd of passes 2 and 3, from the cache where there is one
+template <class T, class ST> RBD_HD void joint_scd_cached(const ST& st, int kind, int i, const Pre<T>& pre, T& s, T& c, T& d) {
+  if constexpr (ST::kTrig) {
+    if (kind == K_REV && st.trig_ld(i, s, c)) { d = T(0); return; }
+  }
+  joint_scd(kind, pre, s, c, d, pre.qoff);
 }
 
 // ---- pass 1 (outward): velocities ---------------------------------------------------------------------------------
@@ -751,12 +771,14 @@ RBD_HD void aba_pass1_body(const ModelDev<T>& M, int i, const IO& io, const ST& 
   if (pre.zflags) {                                  // revolute, E = [P] Rz(q + qoff)
     T s, c;
     sincos_t(pre.q0 + pre.qoff, s, c);
+    trig_keep(st, K_REV, i, s, c);
     if (pre.zflags & F_ZPERP) motion_to_child_z<T, 1>(s, c, bd.pt, vp, v);
     else motion_to_child_z<T, 0>(s, c, bd.pt, vp, v);
     v.w[2] += pre.qd;
   } else if (!ANY || kind == K_REV || kind == K_PRIS || kind == K_SINCOS || kind == K_FIXED) {
     T s, c, d, qd = T(0);
     joint_scd(kind, pre, s, c, d);
+    trig_keep(st, kind, i, s, c);          // (qoff is 0 outside the fast classes: the same angle as passes 2 and 3)
     if (!(IO::kKinds & kHasFixed) || kind != K_FIXED) qd = pre.qd;
     frame_1dof(bd, s, c, d, R, r);
     motion_to_child(R, r, vp, v);
@@ -849,7 +871,7 @@ RBD_HD void aba_pass2_1dof(const ModelDev<T>& M, int i, const IO& io, const ST& 
     return;
   }
   T sn, c, dd;
-  joint_scd(kind, pre, sn, c, dd, pre.qoff);
+  joint_scd_cached(st, kind, i, pre, sn, c, dd);
   const T qd = pre.qd;
   const T tau = pre.tau;
   if (!(IO::kKinds & kHasPris) || kind != K_PRIS) {
@@ -1078,7 +1100,7 @@ RBD_HD void aba_pass3_1dof(const ModelDev<T>& M, int i, const IO& io, const ST& 
     return;
   }
   T sn, c, dd;
-  joint_scd(kind, pre, sn, c, dd, pre.qoff);
+  joint_scd_cached(st, kind, i, pre, sn, c, dd);
   const T qd = pre.qd;
   T tt[6];
   st.template ldv<6>(bd.row0, tt);

@@ -39,7 +39,7 @@ extern "C" __global__ void __launch_bounds__(32, RBD_SPEC_F64 ? 1 : RBD_SPEC_SME
 
 // All warps run the same program through a generic stash pointer, so the SM fetches ONE instruction stream (two kernels side by
 // side starve each other's instruction supply, DESIGN.md 4.8).
-#define RBD_STASH_ROWS (RBD_SPEC_ROWS > 0 ? RBD_SPEC_ROWS : 1)
+#define RBD_STASH_ROWS (RBD_SPEC_ROWS + RBD_SPEC_TRIG_ROWS > 0 ? RBD_SPEC_ROWS + RBD_SPEC_TRIG_ROWS : 1)   /* + the trig cache */
 extern "C" __global__ void __launch_bounds__(512, 1) rbd_jit_mix(const RbdJitArgs a) {
   extern __shared__ __align__(16) unsigned char rbd_smem_raw[];
   const unsigned w = threadIdx.x >> 5;

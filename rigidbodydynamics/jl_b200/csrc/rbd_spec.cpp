@@ -88,7 +88,7 @@ int spec_prepare(rbd_model* m, const SpecKey& key, bool load_on_device, std::str
   cudaFuncAttributes fa{};
   if (e == cudaSuccess) { e = cudaFuncGetAttributes(&fa, (const void*)se.k_smem); se.regs_smem = fa.numRegs; }
   if (e == cudaSuccess) { e = cudaFuncGetAttributes(&fa, (const void*)se.k_mix); se.regs_mix = fa.numRegs; }
-  se.rows = spec_shared_rows(m->hm, key);       // the rows the program keeps in shared memory (the others are registers)
+  se.rows = spec_shared_rows(m->hm, key);       // one warp's shared rows: stash (the others are registers) and trig cache
   const size_t smem = (size_t)std::max(1, se.rows) * 32 * (key.f64 ? 8 : 4);
   DeviceProps p;
   if (e == cudaSuccess) e = device_props(p);

@@ -34,8 +34,8 @@ enum SymOp : int32_t {
   S_SIN, S_COS,          // the two results of one sincos_t(a): always created as a pair (cos node id = sin node id + 1)
   S_LOAD,                // global input:  arr = which array, row
   S_STORE,               // global output: arr, row, a = value
-  S_SLD,                 // stash load:  row; grp = id of the first load of its ldv<N> batch
-  S_SST,                 // stash store: row, a = value
+  S_SLD,                 // stash load:  row; grp = id of the first load of its ldv<N> batch; arr = region (R_STASH / R_TRIG)
+  S_SST,                 // stash store: row, a = value; arr = region
   S_SFENCE,              // stash store fence: where a thread re-reads its own stash writes (a no-op in shared memory)
   S_XLD, S_XST,          // per-thread global scratch (body-frame external wrenches): row[, a]
   S_PARAM,               // model constant of one instance of a folded chain pair: row = slot, arr = instance (0 left, 1 right), c = value
@@ -45,6 +45,8 @@ enum SymOp : int32_t {
 enum SymArr : int32_t { A_Q = 0, A_V, A_TAU, A_VD_IN, A_WEXT, A_OUT0, A_OUT1,
                         A_K0, A_K1, A_K2, A_K3, A_K4, A_K5, A_K6, A_K7,      // the eight outputs of rbd_kinematics, in rbd_kinematics_out order
                         A_COUNT };
+// rows of stash loads / stores: the algorithm's stash, or the trig cache (SymStash::trig), which has its own row numbering
+enum SymRegion : int32_t { R_STASH = 0, R_TRIG = 1, R_COUNT };
 
 struct SymNode {
   int32_t op;
@@ -204,8 +206,8 @@ struct SymTrace {
     return id;
   }
   void store(int32_t arr, int32_t row, int32_t v) { push({S_STORE, v, -1, arr, row, 0, 0.0}); }
-  int32_t sld(int32_t row, int32_t grp) { const int32_t id = push({S_SLD, -1, -1, 0, row, grp, 0.0}); return id; }
-  void sst(int32_t row, int32_t v) { push({S_SST, v, -1, 0, row, 0, 0.0}); }
+  int32_t sld(int32_t row, int32_t grp, int32_t region = R_STASH) { return push({S_SLD, -1, -1, region, row, grp, 0.0}); }
+  void sst(int32_t row, int32_t v, int32_t region = R_STASH) { push({S_SST, v, -1, region, row, 0, 0.0}); }
   void sfence() { if (!nodes.empty() && nodes.back().op == S_SFENCE) return; push({S_SFENCE, -1, -1, 0, 0, 0, 0.0}); }
   int32_t xld(int32_t row) { return push({S_XLD, -1, -1, 0, row, 0, 0.0}); }
   void xst(int32_t row, int32_t v) { push({S_XST, v, -1, 0, row, 0, 0.0}); }
@@ -281,6 +283,23 @@ template <> struct Scr<Sym> {
   bool valid() const { return present; }
 };
 struct SymStash {
+  // Trig cache of the ABA passes (trig_keep, rbd_device.cuh), when `trig`: the (sin, cos) of the revolute joint of body i (preorder)
+  // in rows 2i, 2i + 1 of region R_TRIG, so the two chains of a folded pair address theirs a constant offset apart.
+  static constexpr bool kTrig = true;
+  bool trig = false;
+  void trig_st(int i, const Sym& s, const Sym& c) const {
+    if (!trig) return;
+    sym_trace()->sst(2 * i, s.id, R_TRIG);
+    sym_trace()->sst(2 * i + 1, c.id, R_TRIG);
+  }
+  bool trig_ld(int i, Sym& s, Sym& c) const {
+    if (!trig) return false;
+    SymTrace* t = sym_trace();
+    const int32_t first = (int32_t)t->nodes.size();
+    s = mk(t->sld(2 * i, first, R_TRIG));
+    c = mk(t->sld(2 * i + 1, first, R_TRIG));
+    return true;
+  }
   Sym ld(int row) const {
     SymTrace* t = sym_trace();
     const int32_t id = (int32_t)t->nodes.size();
