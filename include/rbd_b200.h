@@ -492,6 +492,62 @@ typedef struct rbd_kinematics_out {
 int32_t rbd_kinematics(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                        const int8_t* path_sign, const rbd_kinematics_out* out, void* stream);
 
+/* Task-space kinematics (DESIGN 4.17): point Jacobians, relative transforms, twists and accelerations of chosen bodies, in any
+ * body frame, for up to RBD_MAX_TASKS tasks from ONE launch.  A task is a body of interest, a base body, a point fixed in the body
+ * and a frame to express results in.  The descriptor holds plain HOST arrays, read at call time like rbd_contact_desc:
+ *   body[t]   tree-joint index whose successor is the target body, -1 = the root body
+ *   base[t]   the source body, same encoding; the path is path(mechanism, base, body)
+ *   frame[t]  body whose default frame results are expressed in, -1 = the root frame; frame == NULL: the root frame for all tasks
+ *   point[t]  [3] point fixed in `body`, in the frame after its joint (the frame of rbd_model_desc.inertia, as in
+ *             rbd_contact_desc.location); point == NULL: every task uses its body's origin */
+#define RBD_MAX_TASKS 32
+typedef struct rbd_task_desc {
+  int32_t ntasks;          /* 0 .. RBD_MAX_TASKS */
+  const int32_t* body;     /* [ntasks] */
+  const int32_t* base;     /* [ntasks] */
+  const int32_t* frame;    /* [ntasks] or NULL */
+  const double* point;     /* [ntasks][3] or NULL */
+} rbd_task_desc;
+
+/* Every output may be NULL (not computed).  Task t owns rows [t*R, (t+1)*R) of each array (R = the per-task row count below), K =
+ * ntasks; 6-vectors are [angular; linear].  With F the task's frame, T_X = transform_to_root(state, X) (mechanism_state.jl:687-714):
+ *   transform           [12 K x B]    relative_transform(state, frame(body), frame(base)) = inv(T_base) T_body: rotation row-major
+ *                                     (9), translation (3); independent of `frame`                 mechanism_state.jl:1011-1014
+ *   point               [3 K x B]     the point in F: transform(state, point, F)
+ *   twist               [6 K x B]     relative_twist(state, body, base) expressed in F              mechanism_state.jl:1016-1038
+ *   point_velocity      [3 K x B]     velocity of the point w.r.t. base, in F = point_velocity(twist, point) = point_jacobian * v
+ *   geometric_jacobian  [6 nv K x B]  geometric_jacobian!(J, state, path) with J.frame = F: column k at rows 6k .. 6k+5 of the task's
+ *                                     block; joints off the path give zero columns                 mechanism_algorithms.jl:101-132
+ *   point_jacobian      [3 nv K x B]  point_jacobian!(Jp, state, path, point) in F: column k at rows 3k .. 3k+2
+ *                                                                                                   mechanism_algorithms.jl:154-224
+ *   acceleration        [6 K x B]     relative_acceleration(accels, body, base) with accels = spatial_accelerations!(state, v̇), then
+ *                                     transform(state, accel, F)          mechanism_algorithms.jl:421-426, mechanism_state.jl:1049-1056
+ *   point_acceleration  [3 K x B]     point_acceleration(twist, accel, point), all three in F       spatial/spatialmotion.jl:351-363
+ * The point Jacobian takes the point in the BODY's frame, constant over the batch; the reference's point_jacobian! takes it in
+ * Jp.frame.  Both give the same matrix for the same physical point. */
+typedef struct rbd_task_out {
+  void* transform;
+  void* point;
+  void* twist;
+  void* point_velocity;
+  void* geometric_jacobian;
+  void* point_jacobian;
+  void* acceleration;
+  void* point_acceleration;
+} rbd_task_out;
+
+/* q [nq x B]; v [nv x B], may be NULL only when none of twist / point_velocity / acceleration / point_acceleration is requested
+ * (RBD_EINVAL otherwise); vd [nv x B] or NULL = zero joint accelerations.  With vd == NULL, acceleration and point_acceleration are
+ * exactly the velocity-product terms J̇ v that task-space controllers need (ẍ = J v̇ + J̇ v).  Gravity is in no output: the root's
+ * acceleration -g of spatial_accelerations! is common to body and base and cancels.  body == base is allowed (identity transform;
+ * zero twist, Jacobians and acceleration).  Errors, all decided on the host before any CUDA call: NULL model / q / tasks / out, an
+ * index outside -1 .. nb-1 or ntasks < 0: RBD_EINVAL; ntasks > RBD_MAX_TASKS or a dtype other than fp32 / fp64: RBD_EUNSUPPORTED;
+ * ld < B: RBD_EDIM.  B == 0 or ntasks == 0: RBD_OK, nothing written.  One kernel launch per call.  The per-sample working set
+ * (the outward sweep's pending slots plus 12 to 24 rows for every distinct body the tasks name) lives in shared memory; if it does
+ * not fit a block (fp64 with several dozen distinct bodies), the call returns RBD_EUNSUPPORTED: split the tasks over two calls. */
+int32_t rbd_task_kinematics(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
+                            const void* vd, const rbd_task_desc* tasks, const rbd_task_out* out, void* stream);
+
 /* Host-pointer variants: same semantics, host buffers in, host buffers out, copies inside the call. */
 int32_t rbd_dynamics_host(rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                           const void* tau, const void* wext, void* vd_out, void* qd_out);

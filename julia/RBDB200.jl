@@ -325,6 +325,72 @@ RigidBodyDynamics.momentum_matrix!(A::AbstractMatrix, state::BatchedState) = (ki
 RigidBodyDynamics.geometric_jacobian!(J::AbstractMatrix, state::BatchedState, p::RigidBodyDynamics.TreePath) =
     (kinematics!(state; path = p, geometric_jacobian = J); J)
 
+"Mirror of `rbd_task_desc` (include/rbd_b200.h): host arrays, read during the call."
+struct rbd_task_desc
+    ntasks::Int32
+    body::Ptr{Int32}
+    base::Ptr{Int32}
+    frame::Ptr{Int32}
+    point::Ptr{Float64}
+end
+
+"Mirror of `rbd_task_out`: eight device pointers, C_NULL = not requested."
+struct rbd_task_out
+    transform::Ptr{Cvoid}
+    point::Ptr{Cvoid}
+    twist::Ptr{Cvoid}
+    point_velocity::Ptr{Cvoid}
+    geometric_jacobian::Ptr{Cvoid}
+    point_jacobian::Ptr{Cvoid}
+    acceleration::Ptr{Cvoid}
+    point_acceleration::Ptr{Cvoid}
+end
+
+"Tree-joint index whose successor is `body`, -1 for the root body (the encoding of `rbd_task_desc`)."
+function body_index(model::Model, body::RigidBody)
+    body == root_body(model.mechanism) && return Int32(-1)
+    for (i, j) in enumerate(tree_joints(model.mechanism))
+        successor(j, model.mechanism) == body && return Int32(i - 1)
+    end
+    throw(ArgumentError("body $(body) is not part of the mechanism"))
+end
+
+"""
+    task_kinematics!(state, tasks; vd = nothing, outs...)
+
+One launch of `rbd_task_kinematics` for up to 32 tasks `(body, base, point, frame)`: `body`, `base` are `RigidBody`s, `point` is a
+3-vector in the frame after `body`'s joint (`nothing` = its origin), `frame` is the `RigidBody` whose default frame results are
+expressed in (`nothing` = the root frame).  Every keyword is an optional B x rows device matrix, task t owning rows
+t*R+1 .. (t+1)*R: `transform` (12, `relative_transform`), `point` (3), `twist` (6, `relative_twist`), `point_velocity` (3),
+`geometric_jacobian` (6 nv, `geometric_jacobian!` with J.frame = frame), `point_jacobian` (3 nv, `point_jacobian!`),
+`acceleration` (6, `relative_acceleration` transformed to the frame) and `point_acceleration` (3).  `vd = nothing` gives the
+velocity-product terms J̇ v.  src/mechanism_algorithms.jl:101-224, 421-426; src/mechanism_state.jl:1011-1056;
+src/spatial/spatialmotion.jl:346-401.
+"""
+function task_kinematics!(state::BatchedState{T}, tasks; vd = nothing, outs...) where {T <: Union{Float32, Float64}}
+    checkstate(state)
+    B = size(state.q, 1)
+    model = state.model
+    body = Int32[body_index(model, t[1]) for t in tasks]
+    base = Int32[body_index(model, t[2]) for t in tasks]
+    frame = Int32[t[4] === nothing ? Int32(-1) : body_index(model, t[4]) for t in tasks]
+    point = zeros(Float64, 3, length(tasks))
+    for (k, t) in enumerate(tasks)
+        t[3] === nothing || (point[:, k] .= t[3])
+    end
+    ptr(name) = haskey(outs, name) ? devptr(outs[name]) : C_NULL
+    to = rbd_task_out(ptr(:transform), ptr(:point), ptr(:twist), ptr(:point_velocity), ptr(:geometric_jacobian),
+                      ptr(:point_jacobian), ptr(:acceleration), ptr(:point_acceleration))
+    GC.@preserve state outs vd body base frame point begin
+        td = rbd_task_desc(Int32(length(tasks)), pointer(body), pointer(base), pointer(frame), pointer(point))
+        check(ccall((:rbd_task_kinematics, librbd), Int32,
+                    (Ptr{Cvoid}, Int32, Int64, Int64, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ref{rbd_task_desc}, Ref{rbd_task_out}, Ptr{Cvoid}),
+                    model.handle, dtype_code(T), B, B, devptr(state.q), devptr(state.v),
+                    vd === nothing ? C_NULL : devptr(vd), td, to, stream_ptr()))
+    end
+    outs
+end
+
 # ---- SURVEY 8(f) rank 3: Jacobians of forward dynamics ----------------------------------------------------------------------
 
 """

@@ -23,6 +23,8 @@ from .algorithms import (DimensionMismatch, dynamics_, dynamics_derivatives_, dy
 from .kinematics import (TreePath, center_of_mass, geometric_jacobian, geometric_jacobian_,  # noqa: F401
                          gravitational_potential_energy, kinematics_, kinetic_energy, momentum, momentum_matrix,
                          momentum_matrix_, momentum_rate_bias, path, transforms_to_root, transforms_to_root_)
+from .kinematics import (TaskFrame, point_acceleration, point_jacobian, point_velocity, relative_acceleration,  # noqa: F401
+                         relative_transform, relative_twist, task_kinematics_)
 from .contact import (ContactDesc, ContactPoint, HalfSpace3D, HuntCrossleyModel, SoftContactModel,  # noqa: F401
                       ViscoelasticCoulombModel, add_contact_point, add_environment_primitive, contact_desc, contact_dynamics_,
                       contact_points, dynamics_contact_, environment, hunt_crossley_hertz, num_contact_states,

@@ -13,6 +13,7 @@ import numpy as np
 
 RBD_MAX_BODIES = 64
 RBD_MAX_LOOP_JOINTS, RBD_MAX_CONSTRAINTS = 16, 96
+RBD_MAX_TASKS = 32
 
 RBD_OK, RBD_EINVAL, RBD_EDIM, RBD_ELOOP, RBD_ESTALE, RBD_ECUDA, RBD_EUNSUPPORTED, RBD_ENOMEM = range(8)
 RBD_F32, RBD_F64, RBD_DUAL64X6 = 0, 1, 2
@@ -61,6 +62,19 @@ class RbdKinematicsOut(Structure):
     _fields_ = [(n, c_void_p) for n in ("transforms_to_root", "center_of_mass", "kinetic_energy",
                                         "gravitational_potential_energy", "momentum", "momentum_rate_bias",
                                         "momentum_matrix", "geometric_jacobian")]
+
+
+TASK_OUTPUTS = ("transform", "point", "twist", "point_velocity", "geometric_jacobian", "point_jacobian", "acceleration",
+                "point_acceleration")
+
+
+class RbdTaskDesc(Structure):
+    _fields_ = [("ntasks", c_int32), ("body", POINTER(c_int32)), ("base", POINTER(c_int32)), ("frame", POINTER(c_int32)),
+                ("point", POINTER(c_double))]
+
+
+class RbdTaskOut(Structure):
+    _fields_ = [(n, c_void_p) for n in TASK_OUTPUTS]
 
 
 class RbdError(RuntimeError):
@@ -129,6 +143,7 @@ SYMBOLS = {
     "rbd_integrate_loops": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, c_double, _i32, _vp, _vp, _vp, _vp]),
     "rbd_integrate_contact_vjp":(c_int32, [_vp, _i32, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _vp, c_double, _i32] + [_vp] * 9),
     "rbd_kinematics": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, POINTER(RbdKinematicsOut), _vp]),
+    "rbd_task_kinematics": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, POINTER(RbdTaskDesc), POINTER(RbdTaskOut), _vp]),
     "rbd_dynamics_host": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rbd_inverse_dynamics_host": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp]),
     "rbd_dynamics_bias_host": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp]),

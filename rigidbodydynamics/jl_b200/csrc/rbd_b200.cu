@@ -29,6 +29,7 @@
 #include "../../../include/rbd_b200.h"
 #include "rbd_rnea_crba.cuh"
 #include "rbd_kin.cuh"
+#include "rbd_task.cuh"
 #include "rbd_dual.cuh"
 #include "rbd_integrate.cuh"
 #include "rbd_model.h"
@@ -496,6 +497,41 @@ contact_kernel(const __grid_constant__ ModelDev<T> M, const __grid_constant__ Co
     io.ld = a.ld;
     io.active = active;
     contact_sample<T>(M, C, io, st);
+  }
+}
+
+// Task-space kinematics (task_sample, rbd_task.cuh): one thread per sample, stash = pending slots + named-body slots.
+template <class T> struct TaskArgs {
+  const T *q, *v, *vd;
+  T *tr, *pt, *tw, *pv, *J, *Jp, *acc, *pacc;
+  int64_t ld, B;
+};
+static_assert(sizeof(ModelDev<double>) + sizeof(TaskDev<double>) + sizeof(TaskArgs<double>) <= 32764,
+              "task_kernel's parameters exceed the kernel-parameter limit");
+template <class T, int NT>
+__global__ void __launch_bounds__(NT, sizeof(T) == 4 ? 16 : 8)
+task_kernel(const __grid_constant__ ModelDev<T> M, const __grid_constant__ TaskDev<T> D, const TaskArgs<T> a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const Stash<T, NT> st{reinterpret_cast<T*>(smem_raw) + threadIdx.x};
+  const int64_t ngroups = (a.B + NT - 1) / NT;
+  for (int64_t g = blockIdx.x; g < ngroups; g += gridDim.x) {
+    const int64_t gn = g + gridDim.x;
+    if (gn < ngroups) {
+      const int64_t bn = gn * NT + (threadIdx.x & ~31);
+      prefetch_rows(a.q, M.nq, a.ld, bn);
+      if (a.v) prefetch_rows(a.v, M.nv, a.ld, bn);
+    }
+    const int64_t b = g * NT + threadIdx.x;
+    const bool active = b < a.B;
+    const int64_t bl = active ? b : a.B - 1;
+    TaskIO<T> io;
+    io.q = {a.q + bl, a.ld};
+    io.v = {a.v ? a.v + bl : nullptr, a.ld};
+    io.vd = {a.vd ? a.vd + bl : nullptr, a.ld};
+    auto out = [&](T* p) { return ColOut<T>{p ? p + bl : nullptr, a.ld, active}; };
+    io.tr = out(a.tr); io.pt = out(a.pt); io.tw = out(a.tw); io.pv = out(a.pv);
+    io.J = out(a.J); io.Jp = out(a.Jp); io.acc = out(a.acc); io.pacc = out(a.pacc);
+    task_sample<T>(M, D, io, st);
   }
 }
 
@@ -1216,6 +1252,25 @@ int contact_t(const rbd_model* model, int64_t B, int64_t ld, const void* q, cons
 }
 
 template <class T>
+int task_t(const rbd_model* model, int64_t B, int64_t ld, const void* q, const void* v, const void* vd, const rbd_task_desc& d,
+           const rbd_task_out& o, cudaStream_t stream) {
+  const HostModel& hm = model->hm;
+  const ModelDev<T>& M = dev_model<T>(hm);
+  const bool want_acc = o.acceleration || o.point_acceleration;
+  const bool want_vel = want_acc || o.twist || o.point_velocity;
+  std::unique_ptr<TaskDev<T>> D(new TaskDev<T>());
+  const int nnamed = build_task_dev<T>(hm, d, want_vel, want_acc, *D);
+  TaskArgs<T> a{(const T*)q, (const T*)v, (const T*)vd, (T*)o.transform, (T*)o.point, (T*)o.twist, (T*)o.point_velocity,
+                (T*)o.geometric_jacobian, (T*)o.point_jacobian, (T*)o.acceleration, (T*)o.point_acceleration, ld, B};
+  auto kernel = task_kernel<T, kNT>;
+  const int rows = std::max(1, D->named_base + nnamed * D->slot_rows);
+  LaunchPlan pl;
+  if (int rc = plan_persistent((const void*)kernel, kNT, (size_t)rows * kNT * sizeof(T), (B + kNT - 1) / kNT, stream, pl)) return rc;
+  kernel<<<pl.grid, pl.block, pl.smem, stream>>>(M, *D, a);
+  return api_launched(&pl);
+}
+
+template <class T>
 int integrate_contact_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau, int64_t step_stride,
                         int64_t stage_stride, const rbd_contact_desc& cd, double dt, int nsteps, void* q_traj, void* v_traj, void* s_traj,
                         cudaStream_t stream, T* stages = nullptr) {
@@ -1317,6 +1372,23 @@ int32_t rbd_kinematics(const rbd_model* model, int32_t dtype, int64_t B, int64_t
   cudaStream_t s = (cudaStream_t)stream;
   return dtype == RBD_F32 ? kinematics_t<float>(model, B, ld, q, v, path_sign, *out, s)
                           : kinematics_t<double>(model, B, ld, q, v, path_sign, *out, s);
+}
+
+int32_t rbd_task_kinematics(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
+                            const void* vd, const rbd_task_desc* tasks, const rbd_task_out* out, void* stream) {
+  const ApiCall call;
+  if (!model) return fail(RBD_EINVAL, "rbd_task_kinematics: model handle is NULL");
+  if (dtype != RBD_F32 && dtype != RBD_F64) return fail(RBD_EUNSUPPORTED, "rbd_task_kinematics: fp32 and fp64 only");
+  if (B < 0 || ld < B) return fail(RBD_EDIM, "rbd_task_kinematics: batch size / leading dimension mismatch (need ld >= B >= 0)");
+  if (!q || !out) return fail(RBD_EINVAL, "rbd_task_kinematics: q and out must not be NULL");
+  std::string err;
+  if (int rc = check_task_desc(model->hm.nb, tasks, err)) return fail(rc, "rbd_task_kinematics: " + err);
+  if (!v && (out->twist || out->point_velocity || out->acceleration || out->point_acceleration))
+    return fail(RBD_EINVAL, "rbd_task_kinematics: twist / point_velocity / acceleration / point_acceleration need v");
+  if (B == 0 || tasks->ntasks == 0) return RBD_OK;
+  cudaStream_t s = (cudaStream_t)stream;
+  return dtype == RBD_F32 ? task_t<float>(model, B, ld, q, v, vd, *tasks, *out, s)
+                          : task_t<double>(model, B, ld, q, v, vd, *tasks, *out, s);
 }
 
 // ---- host-pointer variants: chunked H2D -> kernel -> D2H pipeline over three internal streams ----

@@ -11,12 +11,22 @@ reference, every quantity in the mechanism's root frame, 6-vectors as [angular; 
 
 All are one call of ``rbd_kinematics`` (include/rbd_b200.h) on the current CUDA stream; ``kinematics_`` exposes the fused
 form (any subset of outputs from a single launch).  There is no CPU path.
+
+Task-space kinematics -- quantities of chosen bodies relative to other bodies, in any body frame -- are one call of
+``rbd_task_kinematics`` (DESIGN 4.17); ``task_kinematics_`` is its fused form for up to 32 ``TaskFrame``s:
+
+    relative_transform(state, from, to)            -> relative_transform       src/mechanism_state.jl:1011-1014
+    relative_twist(state, body, base)              -> relative_twist           src/mechanism_state.jl:1016-1038
+    relative_acceleration(result, body, base)      -> relative_acceleration    src/mechanism_algorithms.jl:421-426
+    point_jacobian!(Jp, state, path, point)        -> point_jacobian           src/mechanism_algorithms.jl:154-224
+    point_velocity / point_acceleration            -> point_velocity, point_acceleration   src/spatial/spatialmotion.jl:346-363
+    geometric_jacobian!(J, state, path), J.frame   -> geometric_jacobian(..., frame=)      src/mechanism_algorithms.jl:101-132
 """
 from __future__ import annotations
 
 import ctypes
 from dataclasses import dataclass
-from typing import Dict, Optional
+from typing import Dict, Optional, Sequence
 
 import numpy as np
 import torch
@@ -28,7 +38,8 @@ from .state import MechanismState, _DT
 
 __all__ = ["TreePath", "path", "kinematics_", "transforms_to_root", "transforms_to_root_", "center_of_mass", "kinetic_energy",
            "gravitational_potential_energy", "momentum", "momentum_rate_bias", "momentum_matrix", "momentum_matrix_",
-           "geometric_jacobian", "geometric_jacobian_"]
+           "geometric_jacobian", "geometric_jacobian_", "TaskFrame", "task_desc", "task_kinematics_", "relative_transform",
+           "relative_twist", "relative_acceleration", "point_jacobian", "point_velocity", "point_acceleration"]
 
 _ROWS = {"transforms_to_root": lambda s: 12 * len(s.mechanism.joints), "center_of_mass": lambda s: 3,
          "kinetic_energy": lambda s: 1, "gravitational_potential_energy": lambda s: 1, "momentum": lambda s: 6,
@@ -151,10 +162,145 @@ def momentum_matrix(state: MechanismState):
     return _one(state, "momentum_matrix")
 
 
-def geometric_jacobian_(out: torch.Tensor, state: MechanismState, path_: TreePath):
-    """``geometric_jacobian!(J, state, path)`` in the root frame: [6 nv, B], column k at rows 6 k .. 6 k + 5."""
-    return _one(state, "geometric_jacobian", out, path_)
+def geometric_jacobian_(out: torch.Tensor, state: MechanismState, path_: TreePath, frame: Optional[RigidBody] = None):
+    """``geometric_jacobian!(J, state, path)``: [6 nv, B], column k at rows 6 k .. 6 k + 5, in the root frame (``rbd_kinematics``)
+    or, with ``frame``, in that body's default frame (``rbd_task_kinematics``)."""
+    if frame is None:
+        return _one(state, "geometric_jacobian", out, path_)
+    task_kinematics_(state, [TaskFrame(path_.target, path_.source, None, frame)], geometric_jacobian=out)
+    return out
 
 
-def geometric_jacobian(state: MechanismState, path_: TreePath):
-    return _one(state, "geometric_jacobian", None, path_)
+def geometric_jacobian(state: MechanismState, path_: TreePath, frame: Optional[RigidBody] = None):
+    if frame is None:
+        return _one(state, "geometric_jacobian", None, path_)
+    return geometric_jacobian_(_task_alloc(state, "geometric_jacobian", 1), state, path_, frame)
+
+
+# ---- task-space kinematics -------------------------------------------------------------------------------------------------
+@dataclass
+class TaskFrame:
+    """One task of ``rbd_task_kinematics``: ``body`` relative to ``base`` (None = the root body), the point ``point`` fixed in
+    ``body`` and given in its frame (None = its origin), results expressed in the default frame of ``frame`` (None = the root
+    frame)."""
+    body: RigidBody
+    base: Optional[RigidBody] = None
+    point: Optional[Sequence[float]] = None
+    frame: Optional[RigidBody] = None
+
+
+_TASK_ROWS = {"transform": lambda s: 12, "point": lambda s: 3, "twist": lambda s: 6, "point_velocity": lambda s: 3,
+              "geometric_jacobian": lambda s: 6 * s.nv, "point_jacobian": lambda s: 3 * s.nv, "acceleration": lambda s: 6,
+              "point_acceleration": lambda s: 3}
+_TASK_NEEDS_V = ("twist", "point_velocity", "acceleration", "point_acceleration")
+
+
+def task_desc(mechanism: Mechanism, tasks: Sequence[TaskFrame]):
+    """The C struct ``rbd_task_desc`` for ``tasks``; returns (struct, keepalive arrays)."""
+    index = {id(j.successor): i for i, j in enumerate(mechanism.joints)}
+
+    def idx(body):
+        if body is None or body is mechanism.root_body:
+            return -1
+        if id(body) not in index:
+            raise ValueError(f"body {getattr(body, 'name', body)!r} does not belong to this mechanism")
+        return index[id(body)]
+    if len(tasks) > _cabi.RBD_MAX_TASKS:
+        raise ValueError(f"at most {_cabi.RBD_MAX_TASKS} tasks per call")
+    body = np.array([idx(t.body) for t in tasks], np.int32)
+    base = np.array([idx(t.base) for t in tasks], np.int32)
+    frame = np.array([idx(t.frame) for t in tasks], np.int32)
+    point = np.zeros((len(tasks), 3))
+    for k, t in enumerate(tasks):
+        if t.point is not None:
+            point[k] = np.asarray(t.point, np.float64).reshape(3)
+    d = _cabi.RbdTaskDesc()
+    d.ntasks = len(tasks)
+    i32, f64 = ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_double)
+    d.body, d.base, d.frame = (a.ctypes.data_as(i32) for a in (body, base, frame))
+    d.point = point.ctypes.data_as(f64)
+    return d, (body, base, frame, point)
+
+
+def task_kinematics_(state: MechanismState, tasks: Sequence[TaskFrame], vd: Optional[torch.Tensor] = None,
+                     **outs: Optional[torch.Tensor]) -> Dict[str, torch.Tensor]:
+    """Fused form: fill any subset of {transform, point, twist, point_velocity, geometric_jacobian, point_jacobian, acceleration,
+    point_acceleration} ([rows * len(tasks), B] tensors of the state's dtype and device; task t owns rows t*rows .. (t+1)*rows - 1)
+    with one kernel launch.  ``vd`` ([nv, B]) or None = zero joint accelerations: acceleration / point_acceleration are then the
+    velocity-product terms J̇ v.  Gravity is in no output."""
+    state.check_modcount()
+    lib = _cabi.load_library()
+    to = _cabi.RbdTaskOut()
+    K = len(tasks)
+    for name, t in outs.items():
+        if name not in _TASK_ROWS:
+            raise TypeError(f"unknown task kinematics output {name!r}")
+        if t is None:
+            continue
+        rows = _TASK_ROWS[name](state) * K
+        if t.dtype != state.dtype or t.device != state.q.device:
+            raise TypeError(f"{name}: dtype/device must match the state")
+        if t.dim() != 2 or t.shape[0] != rows or t.shape[1] != state.batch:
+            raise DimensionMismatch(f"{name} has wrong size: expected ({rows}, {state.batch}), got {tuple(t.shape)}")
+        if not t.is_contiguous():
+            raise ValueError(f"{name} must be [rows, B] contiguous (batch index fastest)")
+        setattr(to, name, t.data_ptr())
+    if vd is not None:
+        if vd.dtype != state.dtype or vd.device != state.q.device:
+            raise TypeError("vd: dtype/device must match the state")
+        if tuple(vd.shape) != (state.nv, state.batch):
+            raise DimensionMismatch(f"vd has wrong size: expected ({state.nv}, {state.batch}), got {tuple(vd.shape)}")
+        if not vd.is_contiguous():
+            raise ValueError("vd must be [nv, B] contiguous (batch index fastest)")
+    d, keep = task_desc(state.mechanism, tasks)
+    _cabi.check(lib.rbd_task_kinematics(state.handle.ptr, _DT[state.dtype], state.batch, state.batch, state.q.data_ptr(),
+                                        state.v.data_ptr(), None if vd is None else vd.data_ptr(), ctypes.byref(d),
+                                        ctypes.byref(to), _stream()))
+    return {k: t for k, t in outs.items() if t is not None}
+
+
+def _task_alloc(state: MechanismState, name: str, ntasks: int) -> torch.Tensor:
+    return torch.empty((_TASK_ROWS[name](state) * ntasks, state.batch), dtype=state.dtype, device=state.q.device)
+
+
+def _task_one(state: MechanismState, name: str, task: TaskFrame, vd: Optional[torch.Tensor] = None) -> torch.Tensor:
+    out = _task_alloc(state, name, 1)
+    task_kinematics_(state, [task], vd, **{name: out})
+    return out
+
+
+def relative_transform(state: MechanismState, body: RigidBody, base: Optional[RigidBody] = None) -> torch.Tensor:
+    """``relative_transform(state, default_frame(body), default_frame(base))`` = inv(T_base) T_body: [12, B], rotation
+    row-major (9) then translation (3)."""
+    return _task_one(state, "transform", TaskFrame(body, base))
+
+
+def relative_twist(state: MechanismState, body: RigidBody, base: Optional[RigidBody] = None,
+                   frame: Optional[RigidBody] = None) -> torch.Tensor:
+    """``relative_twist(state, body, base)`` expressed in ``frame`` (None = root frame): [6, B], [angular; linear]."""
+    return _task_one(state, "twist", TaskFrame(body, base, None, frame))
+
+
+def relative_acceleration(state: MechanismState, body: RigidBody, base: Optional[RigidBody] = None,
+                          vd: Optional[torch.Tensor] = None, frame: Optional[RigidBody] = None) -> torch.Tensor:
+    """``relative_acceleration`` of the spatial accelerations at joint accelerations ``vd`` (None = zero), transformed to
+    ``frame`` like ``transform(state, accel, frame)``: [6, B]."""
+    return _task_one(state, "acceleration", TaskFrame(body, base, None, frame), vd)
+
+
+def point_jacobian(state: MechanismState, path_: TreePath, point: Sequence[float], frame: Optional[RigidBody] = None) -> torch.Tensor:
+    """``point_jacobian!(Jp, state, path, point)`` for a point fixed in ``path_.target`` and given in its frame, expressed in
+    ``frame``: [3 nv, B], column k at rows 3 k .. 3 k + 2."""
+    return _task_one(state, "point_jacobian", TaskFrame(path_.target, path_.source, point, frame))
+
+
+def point_velocity(state: MechanismState, path_: TreePath, point: Sequence[float], frame: Optional[RigidBody] = None) -> torch.Tensor:
+    """Velocity of the point (fixed in ``path_.target``, given in its frame) with respect to ``path_.source``, in ``frame``: [3, B]."""
+    return _task_one(state, "point_velocity", TaskFrame(path_.target, path_.source, point, frame))
+
+
+def point_acceleration(state: MechanismState, path_: TreePath, point: Sequence[float], vd: Optional[torch.Tensor] = None,
+                       frame: Optional[RigidBody] = None) -> torch.Tensor:
+    """``point_acceleration(twist, accel, point)`` of the point with respect to ``path_.source`` at joint accelerations ``vd``
+    (None = zero: the velocity-product term J̇ v), all in ``frame``: [3, B]."""
+    return _task_one(state, "point_acceleration", TaskFrame(path_.target, path_.source, point, frame), vd)
