@@ -20,7 +20,9 @@
 namespace rbd {
 namespace {
 
-constexpr int kGeneratorVersion = 31;   // bump when the emitted code changes (part of the cubin cache key)
+constexpr int kGeneratorVersion = 34;   // bump when the emitted code changes (part of the cubin cache key)
+constexpr int kChainReach = 256;        // nodes a sum tree may span outside fold segments (plan_chains)
+constexpr int kFmaCap = 0;              // terms above which a sum is split into two FMA chains (0: never; spec_fma_cap)
 constexpr int kRegRowsAba = -1;         // register-resident stash rows of the fp32 forward-dynamics programs (-1: all eligible)
 constexpr int kSmemPerSm = 233472;      // H100: 228 KB of shared memory per SM ...
 constexpr int kSmemReservedPerBlock = 1024;   // ... of which each resident block takes 1 KB for the system
@@ -152,6 +154,120 @@ struct Emitter {
   }
   std::unordered_map<size_t, int32_t> fma_of;   // add / sub node -> the product folded into it
 
+  using NameFn = std::function<std::string(int)>;
+  using OpFn = std::function<std::string(int, int)>;
+
+  // Sums as FMA chains (spec_fma_chain; replaces plan_fma).  A sum tree is an add / sub node (its root) together with every
+  // add / sub operand that has exactly one use, recursively; its leaves are the other operands, a "product" when it is a
+  // single-use multiplication.  The tree is emitted as ONE statement, a chain: a start value (a non-product leaf, else the
+  // product of one), then one RBD_FMA / RBD_FNMA per product, then one RBD_ADD / RBD_SUB per other leaf.  `(a b - c d) + (e f +
+  // g h)` costs 1 FMUL + 3 FFMA instead of 2 FMUL + 2 FFMA + 1 FADD: the unit is compiled with --fmad=false and IEEE adds, so
+  // ptxas never reassociates it itself.  The leaf order is a function of the tree's structure only (products in the order they
+  // were traced, then the other leaves by consumer, literals last), so the two chains of a folded pair plan alike.  A tree never
+  // crosses a region (`region`): the segments of a foldable chain pair and their connection brackets are regions of their own.
+  // Outside those regions a partial sum is not absorbed into a consumer more than kChainReach nodes after the earliest value its
+  // own tree keeps live: the chain is emitted at its root, so a sum accumulated over the whole program (the momentum or energy
+  // of every body in a kinematics program) would keep every leaf live to the end (Atlas centre of mass + energies + momentum:
+  // 3.5 KB of spills without the limit).  Not in forward-dynamics programs: their sums over bodies go through the stash, and
+  // their planning must not depend on node distances, which the trig cache (kept or not, spec_trig) shifts -- the program is
+  // bit-identical with and without it.
+  // Above `chain_cap` terms (0: no limit) a sum is split into two chains of half the terms each, joined by one add.
+  struct Term { int32_t owner; int8_t k; bool prod, neg; };    // operand k of tree node `owner`; sign of the term in the sum
+  bool chain = false;
+  int chain_cap = 0;
+  std::unordered_map<int32_t, std::vector<Term>> chain_of;     // root -> terms in emission order (two chains: see chain_split)
+  std::unordered_map<int32_t, int> chain_split;                // root -> terms of the first of two chains
+  std::vector<int32_t> region;
+
+  bool is_sum(int i) const { return live[i] && (tr.nodes[i].op == S_ADD || tr.nodes[i].op == S_SUB); }
+  int32_t operand(const Term& t) const { return t.k ? tr.nodes[t.owner].b : tr.nodes[t.owner].a; }
+
+  void plan_chains() {
+    const auto& N = tr.nodes;
+    uses.assign(N.size(), 0);
+    fused.assign(N.size(), 0);
+    for (size_t i = 0; i < N.size(); ++i) {
+      if (!live[i] || N[i].op == S_COS) continue;
+      if (N[i].a >= 0) ++uses[N[i].a];
+      if (N[i].b >= 0) ++uses[N[i].b];
+    }
+    plan_regions();
+    // interior nodes; first[i] = the earliest value a tree rooted at i keeps live (literals are immediates and do not count)
+    std::vector<int32_t> first(N.size(), INT32_MAX);
+    auto held = [&](int o) {
+      if (tr.is_lit(o)) return INT32_MAX;
+      if (N[o].op != S_MUL || uses[o] != 1) return o;
+      int32_t f = INT32_MAX;                           // a product multiplied out in the chain keeps its operands live
+      for (int x : {N[o].a, N[o].b}) if (!tr.is_lit(x)) f = std::min(f, x);
+      return f;
+    };
+    for (size_t i = 0; i < N.size(); ++i) {
+      if (!is_sum((int)i)) continue;
+      for (int o : {N[i].a, N[i].b}) {
+        const bool in = is_sum(o) && uses[o] == 1 && region[o] == region[i] &&
+                        (region[i] != 0 || key.algo == SPEC_ABA || (int)i - first[o] <= kChainReach);
+        if (in) fused[o] = 1;
+        first[i] = std::min(first[i], in ? first[o] : held(o));
+      }
+    }
+    for (size_t i = 0; i < N.size(); ++i) {
+      if (!is_sum((int)i) || fused[i]) continue;
+      std::vector<Term> P, Q;                          // product leaves, other leaves
+      std::function<void(int, bool)> walk = [&](int j, bool neg) {
+        for (int k = 0; k < 2; ++k) {
+          const int o = k ? N[j].b : N[j].a;
+          const bool s = neg != (k == 1 && N[j].op == S_SUB);
+          if (is_sum(o) && fused[o]) walk(o, s);
+          else if (N[o].op == S_MUL && uses[o] == 1 && region[o] == region[j]) { fused[o] = 1; P.push_back({j, (int8_t)k, true, s}); }
+          else Q.push_back({j, (int8_t)k, false, s});
+        }
+      };
+      walk((int)i, false);
+      std::sort(P.begin(), P.end(), [&](const Term& x, const Term& y) { return operand(x) < operand(y); });
+      // (a literal after the other operand: constants are shared by the whole trace, so their node ids -- which order the operands
+      // of an add -- differ between the two chains of a pair)
+      auto qkey = [&](const Term& x) { return std::make_tuple(x.owner, tr.is_lit(operand(x)), x.k); };
+      std::sort(Q.begin(), Q.end(), [&](const Term& x, const Term& y) { return qkey(x) < qkey(y); });
+      std::vector<Term> all(P);
+      all.insert(all.end(), Q.begin(), Q.end());
+      const size_t n = all.size(), h = chain_cap > 0 && (int)n > chain_cap && n >= 4 ? n / 2 : n;
+      std::vector<Term>& out = chain_of[(int32_t)i];
+      order_chain(all.begin(), all.begin() + h, out);
+      order_chain(all.begin() + h, all.end(), out);
+      if (h < n) chain_split[(int32_t)i] = (int)h;
+    }
+  }
+  // One chain of the terms [b, e) (products first): the start -- the first positive non-product, else the first non-product,
+  // else the first positive product, else the first product -- then the products, then the other leaves.
+  template <class It> static void order_chain(It b, It e, std::vector<Term>& out) {
+    if (b == e) return;
+    It start = e;
+    for (int pass = 0; pass < 4 && start == e; ++pass)
+      for (It t = b; t != e; ++t)
+        if (t->prod == (pass >= 2) && (!t->neg || pass % 2 == 1)) { start = t; break; }
+    out.push_back(*start);
+    for (It t = b; t != e; ++t) if (t != start && t->prod) out.push_back(*t);
+    for (It t = b; t != e; ++t) if (t != start && !t->prod) out.push_back(*t);
+  }
+  std::string chain_expr(const Term* t, size_t n, const OpFn& opnd) {
+    auto leaf = [&](const Term& x) { return opnd(x.owner, x.k); };
+    auto fac = [&](const Term& x, int q) { return opnd(operand(x), q); };
+    std::string e;
+    if (t[0].prod) e = "RBD_MUL(" + (t[0].neg ? "RBD_NEG(" + fac(t[0], 0) + ")" : fac(t[0], 0)) + ", " + fac(t[0], 1) + ")";
+    else e = t[0].neg ? "RBD_NEG(" + leaf(t[0]) + ")" : leaf(t[0]);
+    for (size_t j = 1; j < n; ++j)
+      e = t[j].prod ? std::string(t[j].neg ? "RBD_FNMA(" : "RBD_FMA(") + fac(t[j], 0) + ", " + fac(t[j], 1) + ", " + e + ")"
+                    : std::string(t[j].neg ? "RBD_SUB(" : "RBD_ADD(") + e + ", " + leaf(t[j]) + ")";
+    return e;
+  }
+  std::string chain_text(int i, const OpFn& opnd) {
+    const std::vector<Term>& t = chain_of.at(i);
+    auto sp = chain_split.find(i);
+    if (sp == chain_split.end()) return chain_expr(t.data(), t.size(), opnd);
+    const std::string e0 = chain_expr(t.data(), sp->second, opnd);
+    return "RBD_ADD(" + e0 + ", " + chain_expr(t.data() + sp->second, t.size() - sp->second, opnd) + ")";
+  }
+
   Emitter(const SymTrace& t, const SpecKey& k, int f) : tr(t), key(k), flavor(f), live(t.nodes.size(), 0) {}
 
   void mark() {      // nodes are in topological order: one backward sweep
@@ -200,14 +316,19 @@ struct Emitter {
   }
 
   // Text of statement i: name(j) = variable of node j, opnd(j, k) = operand k (0: a, 1: b) of node j, row(j) = its row expression.
-  using NameFn = std::function<std::string(int)>;
-  using OpFn = std::function<std::string(int, int)>;
   std::string stmt(int i, const NameFn& name, const OpFn& opnd, const NameFn& row) {
     const SymNode& n = tr.nodes[i];
     const std::string v = "const rbd_v " + name(i) + " = ";
     switch (n.op) {
       case S_ADD:
       case S_SUB: {
+        if (chain) {      // the statistics count the tree's add / sub nodes and the products it multiplies out on their own
+          const std::vector<Term>& t = chain_of.at(i);
+          auto sp = chain_split.find(i);
+          stats.n_add += (int)t.size() - 1;
+          stats.n_mul += t[0].prod + (sp != chain_split.end() && t[sp->second].prod);
+          return v + chain_text(i, opnd) + ";\n";
+        }
         ++stats.n_add;
         auto it = fma_of.find(i);
         if (it == fma_of.end()) return v + (n.op == S_ADD ? "RBD_ADD(" : "RBD_SUB(") + opnd(i, 0) + ", " + opnd(i, 1) + ");\n";
@@ -278,6 +399,7 @@ struct Emitter {
     std::vector<std::array<int32_t, 3>> pv;                          // per-instance values: A node, B node, connection k (-1: none)
     std::set<std::pair<int32_t, int32_t>> pvs;
     std::vector<int32_t> outs;                                       // nodes of A or B used after the loop
+    std::unordered_set<int32_t> swapped;                             // A's commutative statements bound to B's operands crosswise
   };
   bool fold = true;
   int total_rows = 0;            // stash rows of the algorithm's layout
@@ -340,6 +462,27 @@ struct Emitter {
     return "";
   }
 
+  // B's sum chain rooted at b is A's rooted at a, term by term: the same operation on the twin operand of the twin consumer
+  bool same_chain(const Fold& f, int a, int b) const {
+    auto ia = chain_of.find(a), ib = chain_of.find(b);
+    if ((ia == chain_of.end()) != (ib == chain_of.end())) return false;
+    if (ia == chain_of.end()) return true;
+    auto sa = chain_split.find(a), sb = chain_split.find(b);
+    if ((sa == chain_split.end() ? 0 : sa->second) != (sb == chain_split.end() ? 0 : sb->second)) return false;
+    const std::vector<Term>& ta = ia->second;
+    const std::vector<Term>& tb = ib->second;
+    if (ta.size() != tb.size()) return false;
+    auto twin = [&](int32_t y, int32_t x) { auto m = f.b2a.find(y); return m != f.b2a.end() && m->second == x; };
+    for (size_t j = 0; j < ta.size(); ++j) {
+      const Term& x = ta[j];
+      const Term& y = tb[j];
+      if (x.prod != y.prod || x.neg != y.neg || !twin(y.owner, x.owner)) return false;
+      if (y.k != (f.swapped.count(x.owner) ? 1 - x.k : x.k)) return false;
+      if (x.prod && !twin(operand(y), operand(x))) return false;
+    }
+    return true;
+  }
+
   bool try_fold(Fold& f, const std::vector<int>& sa, const std::vector<int>& sb, const std::map<int, std::vector<int>>& conn_of_step) {
     const auto& N = tr.nodes;
     const int L = (int)sa.size();
@@ -391,7 +534,10 @@ struct Emitter {
       switch (na.op) {
         case S_ADD: case S_MUL: case S_SUB: case S_DIV: {
           bool ok = bind(f, na.a, nb.a, b0) && bind(f, na.b, nb.b, b1);
-          if (!ok && (na.op == S_ADD || na.op == S_MUL)) ok = bind(f, na.a, nb.b, b0) && bind(f, na.b, nb.a, b1);
+          if (!ok && (na.op == S_ADD || na.op == S_MUL)) {
+            ok = bind(f, na.a, nb.b, b0) && bind(f, na.b, nb.a, b1);
+            if (ok) f.swapped.insert(a);
+          }
           if (!ok) return false;
           if (b0.kind == 1 && b1.kind == 1 && b0.x == b1.x && b0.d != b1.d) return false;
           commit(f, b0); commit(f, b1);
@@ -414,6 +560,7 @@ struct Emitter {
         case S_SFENCE: break;
         default: return false;
       }
+      if (chain && !same_chain(f, a, b)) return false;
     }
     for (int k = 0; k < L; ++k) {
       for (int x : f.ca[k]) for (int o : {N[x].a, N[x].b}) if (o >= 0 && N[x].op != S_COS && conn_ref(f, 0, o).empty()) return false;
@@ -436,38 +583,69 @@ struct Emitter {
     return true;
   }
 
-  void analyse_folds() {
-    const auto& N = tr.nodes;
-    fold_at.assign(N.size(), -1);
-    in_fold.assign(N.size(), -1);
-    remat.assign(N.size(), 0);
-    if (!hm || hm->pairs.empty() || tr.steps.empty()) return;
+  // (pass, chain pair) segments that may fold: the steps of segment A and of segment B
+  struct Seg { int pass; FoldPair fp; std::vector<int> sa, sb; };
+  std::vector<Seg> pair_segments() const {
+    std::vector<Seg> segs;
+    if (!hm || hm->pairs.empty() || tr.steps.empty()) return segs;
     std::map<std::pair<int, int>, int> sidx;
     for (size_t s = 0; s < tr.steps.size(); ++s) sidx[{tr.steps[s].pass, tr.steps[s].body}] = (int)s;
-    std::map<int, std::vector<int>> conn_of_step;
-    for (size_t c = 0; c < tr.conns.size(); ++c) conn_of_step[tr.conns[c].step].push_back((int)c);
     for (int pass = 1; pass <= 3; ++pass)
       for (const FoldPair& fp : hm->pairs) {
         if (fp.l0 < 1) continue;
-        std::vector<int> sa, sb;
+        Seg g{pass, fp, {}, {}};
         bool ok = true;
         for (int k = 0; k < fp.len && ok; ++k) {
           const int a = pass == 2 ? fp.l0 + 2 * fp.len - 1 - k : fp.l0 + k;
           const int b = pass == 2 ? fp.l0 + fp.len - 1 - k : fp.l0 + fp.len + k;
           auto ia = sidx.find({pass, a}), ib = sidx.find({pass, b});
           ok = ia != sidx.end() && ib != sidx.end();
-          if (ok) { sa.push_back(ia->second); sb.push_back(ib->second); }
+          if (ok) { g.sa.push_back(ia->second); g.sb.push_back(ib->second); }
         }
-        if (!ok || sb.back() + 1 >= (int)tr.steps.size()) continue;
-        Fold f;
-        f.pass = pass; f.len = fp.len; f.instA = pass == 2 ? 1 : 0;
-        f.first = pass == 2 ? fp.l0 + 2 * fp.len - 1 : fp.l0;
-        f.a0 = tr.steps[sa[0]].node; f.mid = tr.steps[sb[0]].node; f.b1 = tr.steps[sb.back() + 1].node;
-        if (!try_fold(f, sa, sb, conn_of_step)) continue;
-        fold_at[f.a0] = (int)folds.size();
-        for (int i = f.a0; i < f.b1; ++i) in_fold[i] = (int)folds.size();
-        folds.push_back(std::move(f));
+        if (!ok || g.sb.back() + 1 >= (int)tr.steps.size()) continue;
+        segs.push_back(std::move(g));
       }
+    return segs;
+  }
+  // Regions sum trees stay inside (plan_chains): each segment of a pair that may fold, and each connection bracket in one, is a
+  // region of its own; everything else is region 0.  Planned the same with and without folding, so both emit the same arithmetic.
+  void plan_regions() {
+    const auto& N = tr.nodes;
+    region.assign(N.size(), 0);
+    int next = 1;
+    for (const Seg& g : pair_segments()) {
+      const int a0 = tr.steps[g.sa[0]].node, mid = tr.steps[g.sb[0]].node, b1 = tr.steps[g.sb.back() + 1].node;
+      for (int i = a0; i < mid; ++i) region[i] = next;
+      for (int i = mid; i < b1; ++i) region[i] = next + 1;
+      next += 2;
+    }
+    for (size_t c = 0; c + 1 < tr.conns.size(); ++c) {
+      const int n0 = tr.conns[c].node, n1 = tr.conns[c + 1].node;
+      if (!tr.conns[c].begin || tr.conns[c + 1].begin || n0 >= (int)N.size() || region[n0] == 0) continue;
+      for (int i = n0; i < n1 && i < (int)N.size(); ++i) region[i] = next;
+      ++next;
+    }
+  }
+
+  void analyse_folds() {
+    const auto& N = tr.nodes;
+    fold_at.assign(N.size(), -1);
+    in_fold.assign(N.size(), -1);
+    remat.assign(N.size(), 0);
+    std::map<int, std::vector<int>> conn_of_step;
+    for (size_t c = 0; c < tr.conns.size(); ++c) conn_of_step[tr.conns[c].step].push_back((int)c);
+    for (const Seg& g : pair_segments()) {
+      const int pass = g.pass;
+      const FoldPair& fp = g.fp;
+      Fold f;
+      f.pass = pass; f.len = fp.len; f.instA = pass == 2 ? 1 : 0;
+      f.first = pass == 2 ? fp.l0 + 2 * fp.len - 1 : fp.l0;
+      f.a0 = tr.steps[g.sa[0]].node; f.mid = tr.steps[g.sb[0]].node; f.b1 = tr.steps[g.sb.back() + 1].node;
+      if (!try_fold(f, g.sa, g.sb, conn_of_step)) continue;
+      fold_at[f.a0] = (int)folds.size();
+      for (int i = f.a0; i < f.b1; ++i) in_fold[i] = (int)folds.size();
+      folds.push_back(std::move(f));
+    }
   }
 
   std::string outer_operand(int x) {
@@ -641,7 +819,7 @@ struct Emitter {
 
   void plan() {
     mark();
-    plan_fma();
+    if (chain) plan_chains(); else plan_fma();
     if (fold) analyse_folds();
     if (!folds.empty()) split_every = split_folded;
     if (!fold) { fold_at.assign(tr.nodes.size(), -1); in_fold.assign(tr.nodes.size(), -1); remat.assign(tr.nodes.size(), 0); }
@@ -714,6 +892,8 @@ bool plan_program(const HostModel& hm, const SpecKey& key, int flavor, bool fold
     em->fold = fold;
     em->total_rows = rows;
     em->reg_budget = spec_reg_rows(key);
+    em->chain = spec_fma_chain(key);
+    em->chain_cap = spec_fma_cap();
     if (flavor != FLAVOR_CPU) {
       // One basic block of 10^4 instructions lets ptxas stretch live ranges until it spills (Atlas: 128 registers + 350 B of
       // local memory, -10 % throughput); a never-taken branch every few hundred statements bounds its scheduling regions.
@@ -786,6 +966,25 @@ int spec_smem_blocks(const SpecKey& key, int shared_rows) {
   return std::max(1, std::min(spec_reg_rows(key) != 0 ? 8 : 16, kSmemPerSm / (bytes + kSmemReservedPerBlock)));
 }
 
+bool spec_fma_chain(const SpecKey& key) {
+  if (const char* e = getenv("RBD_JIT_FMA_CHAIN")) return e[0] != '0';
+  // Measured on H100 (DESIGN.md section 7): faster for forward dynamics and kinematics; slower for the 7-DoF arm's mass matrix
+  // (+5.9 %) and Atlas inverse dynamics (+2 %), small latency-bound programs where the longer dependency chains cost more
+  // than the instructions they save.
+  return key.algo == SPEC_ABA || key.algo == SPEC_KIN;
+}
+
+int spec_fma_cap() {
+  const char* e = getenv("RBD_JIT_FMA_CAP");
+  return e ? std::max(0, atoi(e)) : kFmaCap;
+}
+
+bool spec_rcp_gate(const SpecKey& key) {
+  if (key.f64) return false;
+  const char* e = getenv("RBD_JIT_RCP");
+  return !e || e[0] != '0';
+}
+
 bool spec_trig(const SpecKey& key) {
   if (key.algo != SPEC_ABA || key.f64) return false;
   const char* e = getenv("RBD_JIT_TRIG");
@@ -808,8 +1007,9 @@ uint64_t spec_hash(const HostModel& hm, const SpecKey& key) {
     for (size_t i = 0; i < n; ++i) { h ^= b[i]; h *= 0x100000001b3ull; }
   };
   const char* blocks = getenv("RBD_JIT_SMEM_BLOCKS");
-  const int hdr[12] = {kGeneratorVersion, key.algo, key.f64, key.has_in2, key.has_out1, key.lower, hm.nb, hm.general, key.peers,
-                       spec_reg_rows(key), blocks ? atoi(blocks) : 0, spec_trig(key)};
+  const int hdr[15] = {kGeneratorVersion, key.algo, key.f64, key.has_in2, key.has_out1, key.lower, hm.nb, hm.general, key.peers,
+                       spec_reg_rows(key), blocks ? atoi(blocks) : 0, spec_trig(key), spec_fma_chain(key),
+                       spec_fma_chain(key) ? spec_fma_cap() : 0, spec_rcp_gate(key)};
   mix(hdr, sizeof hdr);
   if (key.algo == SPEC_KIN) { mix(&key.kin_mask, sizeof key.kin_mask); mix(key.kin_sign, sizeof key.kin_sign); }
   if (key.f64) {
@@ -837,11 +1037,13 @@ bool spec_emit_cuda_tu(const HostModel& hm, const SpecKey& key, std::string& out
            "#define RBD_SPEC_SMEM_BLOCKS %d\n"
            "#define RBD_SPEC_F64 %d\n#define RBD_SPEC_NQ %d\n#define RBD_SPEC_NV %d\n#define RBD_SPEC_ROWS %d\n#define RBD_SPEC_TRIG_ROWS %d\n"
            "#define RBD_SPEC_HAS_IN2 %d\n#define RBD_SPEC_HAS_OUT1 %d\n#define RBD_SPEC_OUT0_ROWS %d\n#define RBD_SPEC_OUT1_ROWS %d\n"
-           "#define RBD_SPEC_ROW32 %d\n#define RBD_SPEC_KIN %d\n#define RBD_SPEC_USES_V %d\n#include \"rbd_jit_prelude.cuh\"\n",
+           "#define RBD_SPEC_ROW32 %d\n#define RBD_SPEC_KIN %d\n#define RBD_SPEC_USES_V %d\n",
            st.nodes_live, st.n_add, st.n_mul, st.n_div, st.n_sincos, st.n_load, st.n_sld, st.n_sst, st.reg_rows, st.trig_rows,
            st.trig_reg_rows, spec_smem_blocks(key, rows + st.trig_rows), key.f64 ? 1 : 0, hm.nq, hm.nv, rows, st.trig_rows, key.has_in2 ? 1 : 0, key.has_out1 ? 1 : 0, key.algo == SPEC_CRBA ? hm.nv * hm.nv : hm.nv, hm.nq,
            key.algo == SPEC_CRBA ? 1 : 0, key.algo == SPEC_KIN ? 1 : 0, st.n_load_v > 0 ? 1 : 0);
   out += buf;
+  if (!key.f64 && !spec_rcp_gate(key)) out += "#define RBD_SPEC_RCP_LIB 1\n";
+  out += "#include \"rbd_jit_prelude.cuh\"\n";
   out += "#define RBD_FLAVOR_SMEM 1\n#include \"rbd_jit_flavor.cuh\"\n" + fn_smem;
   out += "#include \"rbd_jit_kernels.cuh\"\n";
   return true;

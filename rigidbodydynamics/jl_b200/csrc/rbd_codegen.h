@@ -53,6 +53,14 @@ int spec_shared_rows(const HostModel& hm, const SpecKey& key);
 // the other two (trig_keep, rbd_device.cuh).  fp32 forward dynamics only, and only where its shared rows cost no resident
 // blocks; RBD_JIT_TRIG=0 turns it off.
 bool spec_trig(const SpecKey& key);
+// Whether sums are planned as FMA chains (Emitter::plan_chains): by default in forward-dynamics and kinematics programs;
+// RBD_JIT_FMA_CHAIN=0 / 1 turns them off / on for every program (off: one product per add, the planning before them).  And the
+// number of terms above which a sum is split into two chains joined by one add (RBD_JIT_FMA_CAP; 0: never).
+bool spec_fma_chain(const SpecKey& key);
+int spec_fma_cap();
+// Whether an fp32 program's reciprocals are the branch-free fast path under the range gate (rbd_jit_prelude.cuh, RBD_RCP);
+// RBD_JIT_RCP=0 keeps the library's __frcp_rn.
+bool spec_rcp_gate(const SpecKey& key);
 // Budget of register-resident stash rows for `key` (-1: every eligible row); RBD_JIT_REG_ROWS overrides it for forward dynamics.
 int spec_reg_rows(const SpecKey& key);
 // Minimum resident single-warp blocks per SM rbd_jit_smem is compiled for (its register cap): as many as the shared stash
