@@ -440,6 +440,49 @@ int32_t rbd_integrate_loops(const rbd_model* model, int32_t dtype, int64_t B, in
                             const rbd_loop_desc* loops, const rbd_contact_desc* contact /* NULL = no contact */,
                             double dt, int32_t nsteps, void* q_traj, void* v_traj, void* s_traj, void* stream);
 
+/* Closed-loop rollouts (DESIGN 4.18): any of the three rollouts above -- the tree (rbd_integrate_schedule / _trajectory), contact
+ * (`contact` set, rbd_integrate_contact) or loop rollout (`loops` set, rbd_integrate_loops; with `contact` too, its contact
+ * variant) -- with joint-space feedback evaluated at EVERY RK4 stage on that stage's state (q_s, v_s), as the reference's
+ * simulate calls control!(τ, t, state) at every stage (src/simulate.jl:36-55).  Per DoF, with e = local_coordinates!(q_ref, q_s)
+ * (q_s - q_ref for Revolute, Prismatic, Planar, SPQuatFloating; the angle difference for SinCosRevolute; the rotation vector of
+ * q_ref^-1 q_s for QuaternionSpherical; the SE(3) log of q_ref^-1 q_s for QuaternionFloating) and the reference's pd(gains, e, ė)
+ * = -k e - d ė (src/pdcontrol.jl:35):
+ *   RBD_PD_TORQUE            τ = τ_ff - Kp e - Kd (v_s - v_ref)
+ *   RBD_PD_COMPUTED_TORQUE   v̇_des = v̇_ref - Kp e - Kd (v_s - v_ref),  τ = inverse_dynamics!(q_s, v_s, v̇_des) + τ_ff
+ *                            (no contact wrenches in the inverse dynamics, as in the reference's PD tests' control!)
+ * then, when effort bounds are given, τ_k is clamped to [lo_k, hi_k].  τ_ff is tau with its strides, exactly as in
+ * rbd_integrate_schedule (NULL = 0).  The quaternions of q_ref must be unit quaternions (they are not normalised).
+ * Every device array has the dtype of the call and leading dimension ld (kp / kd with gain_ld); q_ref of step s starts at
+ * s * q_ref_step_stride elements, v_ref / vd_ref at s * v_ref_step_stride (0 = held over the call).  effort_lo / effort_hi are host
+ * arrays, copied to the device on every call from pageable memory: that copy is not allowed during CUDA-graph stream capture, so a
+ * captured rollout must pass them as NULL.
+ * Everything else -- state, contact state, trajectories, return codes -- is as in the rollout the call runs.
+ * Argument errors (before any CUDA call): pd, kp, kd or q_ref NULL, an unknown mode, vd_ref in RBD_PD_TORQUE mode, negative strides,
+ * gain_ld other than 0 / ld, only one of effort_lo / effort_hi, or lo > hi: RBD_EINVAL; RBD_PD_COMPUTED_TORQUE with loops (nloops
+ * > 0): RBD_ELOOP (inverse_dynamics! has no kinematic loops).  Kernels per stage: PD mode launches exactly the rollout's kernels
+ * (the law runs in its coordinate-map kernels, which write the stage torques the dynamics reads); computed-torque mode adds the
+ * inverse dynamics (1 kernel, 2 when the fp32 specialised kernel hands samples beyond its sin / cos range to the generic one) and
+ * one elementwise kernel (τ_ff, clamp). */
+#define RBD_PD_TORQUE 0
+#define RBD_PD_COMPUTED_TORQUE 1
+typedef struct rbd_pd_desc {
+  int32_t mode;                          /* RBD_PD_TORQUE or RBD_PD_COMPUTED_TORQUE */
+  const void* kp; const void* kd;        /* device [nv] (gain_ld = 0, shared by the batch) or [nv x B] (gain_ld = ld) */
+  int64_t gain_ld;
+  const void* q_ref;                     /* device [nq x B] block per step */
+  const void* v_ref;                     /* device [nv x B] block per step, NULL = 0 */
+  const void* vd_ref;                    /* device [nv x B] block per step, computed-torque mode only, NULL = 0 */
+  int64_t q_ref_step_stride;             /* elements between the q_ref blocks of consecutive steps; 0 = held over the call */
+  int64_t v_ref_step_stride;             /* the same for v_ref and vd_ref */
+  const double* effort_lo;               /* host [nv], NULL = unbounded */
+  const double* effort_hi;               /* host [nv], NULL = unbounded */
+} rbd_pd_desc;
+int32_t rbd_integrate_pd(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau,
+                         int64_t tau_step_stride, int64_t tau_stage_stride, const rbd_pd_desc* pd,
+                         const rbd_loop_desc* loops /* NULL = tree or contact rollout */,
+                         const rbd_contact_desc* contact /* NULL = no contact */, double dt, int32_t nsteps, void* q_traj, void* v_traj,
+                         void* s_traj, void* stream);
+
 /* Reverse mode through a contact rollout (DESIGN 4.15): the gradient of
  *   L = sum_s q_traj_bar[s] . q_traj[s] + v_traj_bar[s] . v_traj[s] + s_traj_bar[s] . s_traj[s]
  * with respect to the initial state (q, v, s) and the torques, for the trajectory rbd_integrate_contact recorded with the same tau,

@@ -275,6 +275,50 @@ function RigidBodyDynamics.simulate(state::BatchedState{T}, final_time, torques 
     nsteps
 end
 
+"Mirror of `rbd_pd_desc` (include/rbd_b200.h)."
+struct rbd_pd_desc
+    mode::Int32
+    kp::Ptr{Cvoid}
+    kd::Ptr{Cvoid}
+    gain_ld::Int64
+    q_ref::Ptr{Cvoid}
+    v_ref::Ptr{Cvoid}
+    vd_ref::Ptr{Cvoid}
+    q_ref_step_stride::Int64
+    v_ref_step_stride::Int64
+    effort_lo::Ptr{Float64}
+    effort_hi::Ptr{Float64}
+end
+
+"""
+`simulate` with joint-space feedback evaluated at every RK4 stage (rbd_integrate_pd, DESIGN 4.18): the `control!` of the
+reference's PD tests, batched.  `kp`, `kd`: gains per velocity DoF, a vector (shared) or a B × nv matrix (per sample); `q_ref`
+(B × nq, unit quaternions), `v_ref` / `v̇_ref` (B × nv, `nothing` = 0) held over the call; `computed_torque = true` gives
+τ = inverse_dynamics!(q, v, v̇_ref - kp e - kd (v - v_ref)) + torques, otherwise τ = torques - kp e - kd (v - v_ref); `effort_bounds`
+(a pair of nv-vectors, e.g. from `effort_bounds(joint)` of every tree joint) clamps τ.  Tree mechanisms without contact points.
+(Not run here: no Julia installation is available to the project's tests; the Python binding exercises the same entry point.)
+"""
+function simulate_pd(state::BatchedState{T}, final_time, kp, kd, q_ref; v_ref = nothing, v̇_ref = nothing,
+                     computed_torque::Bool = false, effort_bounds = nothing, torques = nothing, Δt = 1e-4) where {T <: Union{Float32, Float64}}
+    checkstate(state)
+    B = size(state.q, 1)
+    nsteps = 0; t = 0.0
+    while t < final_time; t += Δt; nsteps += 1; end            # the reference's `while t < final_time` (ode_integrators.jl:311)
+    lo, hi = effort_bounds === nothing ? (nothing, nothing) : (Vector{Float64}(effort_bounds[1]), Vector{Float64}(effort_bounds[2]))
+    ptr(x) = x === nothing ? C_NULL : devptr(x)
+    GC.@preserve state kp kd q_ref v_ref v̇_ref torques lo hi begin
+        desc = rbd_pd_desc(Int32(computed_torque ? 1 : 0), devptr(kp), devptr(kd), ndims(kp) == 2 ? Int64(B) : Int64(0),
+                           devptr(q_ref), ptr(v_ref), ptr(v̇_ref), 0, 0,
+                           lo === nothing ? Ptr{Float64}(C_NULL) : pointer(lo), hi === nothing ? Ptr{Float64}(C_NULL) : pointer(hi))
+        check(ccall((:rbd_integrate_pd, librbd), Int32,
+                    (Ptr{Cvoid}, Int32, Int64, Int64, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Int64, Int64, Ref{rbd_pd_desc},
+                     Ptr{Cvoid}, Ptr{Cvoid}, Float64, Int32, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
+                    state.model.handle, dtype_code(T), B, B, devptr(state.q), devptr(state.v), C_NULL, ptr(torques), 0, 0, desc,
+                    C_NULL, C_NULL, Float64(Δt), Int32(nsteps), C_NULL, C_NULL, C_NULL, stream_ptr()))
+    end
+    nsteps
+end
+
 "Mirror of `rbd_kinematics_out` (include/rbd_b200.h): eight device pointers, C_NULL = not requested."
 struct rbd_kinematics_out
     transforms_to_root::Ptr{Cvoid}

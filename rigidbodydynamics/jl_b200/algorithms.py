@@ -17,6 +17,7 @@ import torch
 
 from . import _cabi
 from .state import DynamicsResult, MechanismState, _DT
+from .pd import integrate_pd
 
 __all__ = ["dynamics_", "dynamics_dual_", "dynamics_derivatives_", "dynamics_ode_", "simulate_", "simulate_trajectory_", "inverse_dynamics_", "inverse_dynamics", "mass_matrix_", "mass_matrix",
            "dynamics_bias_", "dynamics_bias", "DimensionMismatch"]
@@ -168,11 +169,13 @@ def _torque_schedule(state: MechanismState, torques: torch.Tensor, nsteps: int):
     return (4 * blk, blk) if torques.dim() == 4 else (blk, 0)
 
 
-def simulate_trajectory_(state: MechanismState, nsteps: int, torques: Optional[torch.Tensor] = None, dt: float = 1e-4):
+def simulate_trajectory_(state: MechanismState, nsteps: int, torques: Optional[torch.Tensor] = None, dt: float = 1e-4, *,
+                         controller=None):
     """``nsteps`` Munthe-Kaas RK4 steps like ``simulate_``, recording the trajectory: returns ``(q_traj, v_traj)``,
     [nsteps + 1, nq, B] and [nsteps + 1, nv, B], block 0 the initial state and block s the state after step s.  ``state`` is advanced
     in place exactly as ``simulate_`` advances it.  ``torques``: None, constant [nv, B], per step [nsteps, nv, B] or per stage
-    [nsteps, 4, nv, B].  The recorded trajectory is what ``autodiff.integrate_vjp_`` differentiates."""
+    [nsteps, 4, nv, B].  ``controller``: a ``JointPD`` evaluated at every stage (``torques`` is then its feedforward), as in
+    ``simulate_``.  The recorded trajectory of an open-loop rollout is what ``autodiff.integrate_vjp_`` differentiates."""
     _require_tree(state, "simulate_trajectory_")
     state.check_modcount()
     if nsteps < 0:
@@ -185,16 +188,22 @@ def simulate_trajectory_(state: MechanismState, nsteps: int, torques: Optional[t
         _check(torques, state.nv, state, "torques")
     q_traj = torch.empty((nsteps + 1, state.nq, state.batch), dtype=state.dtype, device=state.q.device)
     v_traj = torch.empty((nsteps + 1, state.nv, state.batch), dtype=state.dtype, device=state.q.device)
+    if controller is not None:
+        integrate_pd(state, controller, nsteps, torques, step, stage, dt, traj=(q_traj, v_traj, None), what="simulate_trajectory_")
+        return q_traj, v_traj
     _call(lib.rbd_integrate_trajectory(state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q), _ptr(state.v),
                                        _ptr(torques), step, stage, float(dt), nsteps, _ptr(q_traj), _ptr(v_traj), _stream()))
     return q_traj, v_traj
 
 
-def simulate_(state: MechanismState, final_time: float, torques: Optional[torch.Tensor] = None, dt: float = 1e-4) -> int:
+def simulate_(state: MechanismState, final_time: float, torques: Optional[torch.Tensor] = None, dt: float = 1e-4, *,
+              controller=None) -> int:
     """``simulate(state0, final_time, control!; Δt)`` (src/simulate.jl:36-55) for the whole batch, on the GPU: Munthe-Kaas RK4
     steps (src/ode_integrators.jl:233-300) until ``t >= final_time``; ``state.q`` / ``state.v`` are advanced in place.  The
-    control is the default passive one (``torques=None``) or a constant torque array [nv, B] (zero-order hold over the call);
-    a time-varying controller calls this once per control interval.  Returns the number of steps taken."""
+    control is the default passive one (``torques=None``), a constant torque array [nv, B] (zero-order hold over the call) or an
+    open-loop schedule ([nsteps, nv, B] or [nsteps, 4, nv, B]).  ``controller``: a ``JointPD`` (joint-space PD or computed-torque
+    feedback) evaluated at every RK4 stage on that stage's state, with ``torques`` as its feedforward.  Returns the number of steps
+    taken."""
     _require_tree(state, "simulate_")
     state.check_modcount()
     lib = _cabi.load_library()
@@ -202,6 +211,14 @@ def simulate_(state: MechanismState, final_time: float, torques: Optional[torch.
     while t < final_time:            # the reference's `while t < final_time` loop (ode_integrators.jl:311)
         t += dt
         nsteps += 1
+    if controller is not None:
+        step = stage = 0
+        if torques is not None and torques.dim() in (3, 4):
+            step, stage = _torque_schedule(state, torques, nsteps)
+        else:
+            _check(torques, state.nv, state, "torques")
+        integrate_pd(state, controller, nsteps, torques, step, stage, dt, what="simulate_")
+        return nsteps
     if torques is not None and torques.dim() in (3, 4):
         step, stage = _torque_schedule(state, torques, nsteps)
         _call(lib.rbd_integrate_schedule(state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q), _ptr(state.v),

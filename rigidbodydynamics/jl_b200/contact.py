@@ -28,6 +28,7 @@ import torch
 
 from . import _cabi
 from .algorithms import DimensionMismatch, _call, _check, _ptr, _require_tree, _stream, _torque_schedule, dynamics_
+from .pd import integrate_pd
 from .state import DynamicsResult, MechanismState, _DT
 
 __all__ = ["HuntCrossleyModel", "hunt_crossley_hertz", "ViscoelasticCoulombModel", "SoftContactModel", "ContactPoint", "HalfSpace3D",
@@ -201,7 +202,7 @@ def dynamics_contact_(result: DynamicsResult, state: MechanismState, torques: Op
 
 
 def _integrate_contact(state: MechanismState, nsteps: int, contact_state: Optional[torch.Tensor], torques, dt: float,
-                       contact: Optional[ContactDesc], record: bool, what: str):
+                       contact: Optional[ContactDesc], record: bool, what: str, controller=None):
     _require_tree(state, what)
     state.check_modcount()
     if nsteps < 0:
@@ -220,6 +221,9 @@ def _integrate_contact(state: MechanismState, nsteps: int, contact_state: Option
     if record:
         new = lambda rows: torch.empty((nsteps + 1, rows, state.batch), dtype=state.dtype, device=state.q.device)   # noqa: E731
         traj = (new(state.nq), new(state.nv), new(cd.nstates))
+    if controller is not None:
+        integrate_pd(state, controller, nsteps, torques, step, stage, dt, contact=cd, contact_state=contact_state, traj=traj, what=what)
+        return traj
     st, keep = cd.c_struct()
     _call(lib.rbd_integrate_contact(state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q), _ptr(state.v),
                                     _ptr(contact_state), _ptr(torques), step, stage, ctypes.byref(st), float(dt), nsteps,
@@ -229,26 +233,30 @@ def _integrate_contact(state: MechanismState, nsteps: int, contact_state: Option
 
 
 def simulate_contact_trajectory_(state: MechanismState, nsteps: int, contact_state: Optional[torch.Tensor],
-                                 torques: Optional[torch.Tensor] = None, dt: float = 1e-4, contact: Optional[ContactDesc] = None):
+                                 torques: Optional[torch.Tensor] = None, dt: float = 1e-4, contact: Optional[ContactDesc] = None, *,
+                                 controller=None):
     """``nsteps`` steps of ``simulate_contact_``, recording the trajectory: returns ``(q_traj, v_traj, s_traj)``, [nsteps + 1, nq, B],
     [nsteps + 1, nv, B] and [nsteps + 1, num_contact_states, B], block 0 the initial state and block s the state after step s.
-    ``state`` and ``contact_state`` are advanced in place exactly as ``simulate_contact_`` advances them."""
-    return _integrate_contact(state, nsteps, contact_state, torques, dt, contact, True, "simulate_contact_trajectory_")
+    ``state`` and ``contact_state`` are advanced in place exactly as ``simulate_contact_`` advances them.  ``controller``: a
+    ``JointPD`` evaluated at every stage, as in ``simulate_contact_`` (``torques`` is then its feedforward)."""
+    return _integrate_contact(state, nsteps, contact_state, torques, dt, contact, True, "simulate_contact_trajectory_", controller)
 
 
 def simulate_contact_(state: MechanismState, final_time: float, contact_state: Optional[torch.Tensor],
-                      torques: Optional[torch.Tensor] = None, dt: float = 1e-4, contact: Optional[ContactDesc] = None) -> int:
+                      torques: Optional[torch.Tensor] = None, dt: float = 1e-4, contact: Optional[ContactDesc] = None, *,
+                      controller=None) -> int:
     """``simulate(state, final_time; Δt)`` for a mechanism with contact points (src/simulate.jl:36-55): Munthe-Kaas RK4 steps until
     ``t >= final_time`` (the step count of ``simulate_``) of ``dynamics!`` with contact, integrating the contact state as well
     (src/ode_integrators.jl:233-300), all on the GPU.  ``state.q``, ``state.v`` and ``contact_state`` ([num_contact_states, B], the
     MechanismState's additional state, see ``contact_dynamics_``) are advanced in place; pass the same ``contact_state`` to the next
     call to continue.  Within the rollout a pair out of contact keeps its state (ṡ = 0): the reference's resets never survive its
     integrator (include/rbd_b200.h, rbd_integrate_contact).  ``torques``: None, constant [nv, B], per step [nsteps, nv, B] or per
-    stage [nsteps, 4, nv, B], as for ``simulate_trajectory_``.  ``contact``: the mechanism's ``contact_desc`` by default.  Returns
-    the number of steps taken."""
+    stage [nsteps, 4, nv, B], as for ``simulate_trajectory_``.  ``contact``: the mechanism's ``contact_desc`` by default.
+    ``controller``: a ``JointPD`` evaluated at every stage, as in ``simulate_`` (its inverse dynamics, in computed-torque mode, sees
+    no contact wrenches).  Returns the number of steps taken."""
     nsteps, t = 0, 0.0
     while t < final_time:            # the reference's `while t < final_time` loop (ode_integrators.jl:311)
         t += dt
         nsteps += 1
-    _integrate_contact(state, nsteps, contact_state, torques, dt, contact, False, "simulate_contact_")
+    _integrate_contact(state, nsteps, contact_state, torques, dt, contact, False, "simulate_contact_", controller)
     return nsteps

@@ -32,6 +32,7 @@
 #include "rbd_task.cuh"
 #include "rbd_dual.cuh"
 #include "rbd_integrate.cuh"
+#include "rbd_pd.cuh"
 #include "rbd_model.h"
 
 using namespace rbd;
@@ -831,6 +832,15 @@ template <class T> struct OffsetRow {      // base[row] + wa * p[row]
     return p ? b + wa * p[(int64_t)row * ld] : b;
   }
 };
+// rbd_integrate_pd: the feedback law of this (step, stage) on the stage state (rbd_pd.cuh), written to out [nv x B] -- the torques
+// (PD mode), or v̇_des (computed-torque mode: ff = v̇_ref, no saturation here).  out == NULL: open loop.
+template <class T> struct PdStage {
+  const T* qref; const T* vref; const T* ff;   // caller arrays at this (step, stage), leading dimension ld; vref / ff NULL = 0
+  const T* kp; const T* kd; int64_t g_ld;      // [nv] (g_ld = 0) or [nv x ld] (g_ld = ld)
+  const T* lo; const T* hi;                    // device [nv] or NULL (no saturation)
+  T* out;
+  int64_t ld;
+};
 template <class T> struct StageArgs {
   const T* q0; const T* v0;               // state at the start of the step
   const T* phid_prev; const T* vd_prev;   // rates of the previous stage (NULL for stage 0)
@@ -838,6 +848,7 @@ template <class T> struct StageArgs {
   T wa;                                   // dt * a_i
   int64_t B;
   bool skip_linear;                       // revolute / prismatic joints are done by the vectorised kernel below
+  PdStage<T> pd;
 };
 template <class T>
 __global__ void __launch_bounds__(128) integrate_stage_kernel(const __grid_constant__ ModelDev<T> M, const StageArgs<T> a) {
@@ -852,6 +863,13 @@ __global__ void __launch_bounds__(128) integrate_stage_kernel(const __grid_const
     for (int k = k0; k < k1; ++k) a.vs[(int64_t)k * a.B + b] = vs(k);
     const ColOut<T> qs{a.qs + b, a.B, true}, phid{a.phid + b, a.B, true};
     joint_stage(bd, q0, phi, vs, qs, phid);
+    if (a.pd.out) {        // reads back the stage rows this thread has just written
+      const PdStage<T>& p = a.pd;
+      const int64_t gc = p.g_ld ? b : 0;
+      const PdSample<T> ps{a.qs + b, a.vs + b, a.B, p.qref + b, p.vref ? p.vref + b : nullptr, p.ff ? p.ff + b : nullptr, p.ld,
+                           p.kp + gc, p.kd + gc, p.g_ld ? p.g_ld : 1, p.lo, p.hi};
+      pd_joint(bd, ps, ColOut<T>{p.out + b, a.B, true});
+    }
   }
 }
 // Revolute / prismatic joints (the bulk of a robot): q_s = q0 + wa phid_prev, v_s = v0 + wa vd_prev, phid = v_s -- plain row
@@ -902,6 +920,44 @@ __global__ void __launch_bounds__(256) integrate_stage_linear_kernel(const __gri
     reinterpret_cast<V*>(a.qs + qo)[i] = qs;
     reinterpret_cast<V*>(a.vs + vo)[i] = vs;
     reinterpret_cast<V*>(a.phid + vo)[i] = vs;
+    if (a.pd.out) {        // the feedback law on the same rows (rbd_pd.cuh): e = q_s - q_ref
+      const PdStage<T>& p = a.pd;
+      const int64_t qc = (int64_t)bd.qrow * p.ld, vc = (int64_t)bd.vrow * p.ld;
+      alignas(sizeof(V)) T x[N], w[N], qr[N], vr[N], ff[N], kp[N], kd[N], u[N];
+      *reinterpret_cast<V*>(x) = qs;
+      *reinterpret_cast<V*>(w) = vs;
+      *reinterpret_cast<V*>(qr) = reinterpret_cast<const V*>(p.qref + qc)[i];
+      if (p.vref) *reinterpret_cast<V*>(vr) = reinterpret_cast<const V*>(p.vref + vc)[i];
+      if (p.ff) *reinterpret_cast<V*>(ff) = reinterpret_cast<const V*>(p.ff + vc)[i];
+      if (p.g_ld) {
+        *reinterpret_cast<V*>(kp) = reinterpret_cast<const V*>(p.kp + (int64_t)bd.vrow * p.g_ld)[i];
+        *reinterpret_cast<V*>(kd) = reinterpret_cast<const V*>(p.kd + (int64_t)bd.vrow * p.g_ld)[i];
+      }
+      const T kp0 = p.g_ld ? T(0) : p.kp[bd.vrow], kd0 = p.g_ld ? T(0) : p.kd[bd.vrow];
+#pragma unroll
+      for (int k = 0; k < N; ++k) {
+        u[k] = pd_law(x[k] - qr[k], w[k], p.vref ? vr[k] : T(0), p.ff ? ff[k] : T(0), p.g_ld ? kp[k] : kp0, p.g_ld ? kd[k] : kd0);
+        if (p.lo) u[k] = clamp_t(u[k], p.lo[bd.vrow], p.hi[bd.vrow]);
+      }
+      reinterpret_cast<V*>(p.out + vo)[i] = *reinterpret_cast<const V*>(u);
+    }
+  }
+}
+// computed-torque mode, after the inverse dynamics of the stage: tau = clamp(ID(q_s, v_s, v̇_des) + τ_ff, lo, hi), in place
+template <class T> struct PdFinishArgs {
+  T* tau; const T* ff; int64_t ld;        // tau [nv x B]; ff (caller leading dimension ld) or NULL
+  const T* lo; const T* hi;               // device [nv] or NULL
+  int64_t nv, B;
+};
+template <class T>
+__global__ void __launch_bounds__(256) pd_finish_kernel(const PdFinishArgs<T> a) {
+  const int64_t total = a.nv * a.B;
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t k = e / a.B, b = e - k * a.B;
+    T x = a.tau[e];
+    if (a.ff) x += a.ff[k * a.ld + b];
+    if (a.lo) x = clamp_t(x, a.lo[k], a.hi[k]);
+    a.tau[e] = x;
   }
 }
 // v = v0 + dt sum_i b_i vd_i ,  q = global(q0, dt sum_i b_i phid_i)        (ode_integrators.jl:283-296)
@@ -1020,6 +1076,15 @@ int contact_stage_launch(const HostModel& hm, const ModelDev<T>& M, const Contac
   return api_launched(&*plan);
 }
 
+// rbd_integrate_pd: the controller over the call (arguments checked by the caller).  Gains and references are caller arrays with
+// leading dimension ld; the references of step s start at s * qref_stride (q_ref) / s * vref_stride (v_ref, v̇_ref) elements.
+template <class T> struct PdRollout {
+  bool computed_torque;
+  const T* kp; const T* kd; int64_t g_ld;
+  const T* qref; const T* vref; const T* vdref; int64_t qref_stride, vref_stride;
+  const double* lo; const double* hi;      // host [nv] or NULL
+};
+
 // traj_q / traj_v (rbd_integrate_trajectory): [(nsteps + 1) x rows x B] -- block 0 the initial state, block s + 1 written by the
 // finishing kernels of step s; q / v receive the final state as without them.  stages (rbd_integrate_vjp's recompute, nsteps = 1):
 // the four stages' (qs_i, vs_i, φ̇_i, v̇_i) are kept in [4 nq + 12 nv] x B rows (stage_rows) and the finishing step is skipped; with
@@ -1028,19 +1093,24 @@ int contact_stage_launch(const HostModel& hm, const ModelDev<T>& M, const Contac
 // also advances the contact state (contact_finish_kernel); the q / v kernels are the same.
 // loop (rbd_integrate_loops): every stage's dynamics is rbd_loops.cu's KKT kernel (loop_stage_launch), with the contact pass when
 // loop->contact is set -- then `contact` carries s and its trajectory, and the finishing step is as above.
+// pd (rbd_integrate_pd): the stage kernels also evaluate the feedback law on the stage state and write the stage's torques into the
+// taud rows, which the stage's dynamics (any of the three) reads in place of tau; τ_ff (tau and its strides) is read by the law.  In
+// computed-torque mode they write v̇_des into vd[i] instead (the dynamics overwrites it), and inverse_dynamics_t plus
+// pd_finish_kernel turn it into the torques.
 template <class T>
 int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v, const void* tau, int64_t step_stride,
                 int64_t stage_stride, double dt, int nsteps, cudaStream_t stream, T* traj_q = nullptr, T* traj_v = nullptr,
-                T* stages = nullptr, const ContactRollout<T>* contact = nullptr, const LoopRollout* loop = nullptr) {
+                T* stages = nullptr, const ContactRollout<T>* contact = nullptr, const LoopRollout* loop = nullptr,
+                const PdRollout<T>* pd = nullptr) {
   const HostModel& hm = model->hm;
   const ModelDev<T>& M = dev_model<T>(hm);
   DeviceProps p;
   RBD_CUDA_TRY(device_props(p));
   const size_t nq = hm.nq, nv = hm.nv;
   const size_t ns = contact ? (size_t)contact->ns : 0;
-  const size_t rows = 2 * nq + 10 * nv + (tau && ld != B ? nv : 0);
+  const size_t rows = 2 * nq + 10 * nv + (pd || (tau && ld != B) ? nv : 0);
   StreamAlloc work, swork;
-  RBD_CUDA_TRY(work.alloc(rows * (size_t)B * sizeof(T), stream));
+  RBD_CUDA_TRY(work.alloc((rows * (size_t)B + (pd ? 2 * nv : 0)) * sizeof(T), stream));
   // contact state: s0 (the state at the start of the step, refreshed like q0 / v0) and the four stages' ṡ_i, [ns x B] each
   T* s0 = nullptr;
   T* sd[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -1073,7 +1143,18 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
   const bool varying = step_stride != 0 || stage_stride != 0;
   auto tau_at = [&](int s_, int i_) -> const T* { return tau ? (const T*)tau + (size_t)s_ * step_stride + (size_t)i_ * stage_stride : nullptr; };
   const T* tau_dense = (const T*)tau;
-  if (tau && ld != B && !varying) {
+  // the controller's saturation bounds on the device, behind the workspace rows (copied from pageable memory: staged before return)
+  const T* pd_lo = nullptr;
+  const T* pd_hi = nullptr;
+  if (pd && pd->lo) {
+    std::vector<T> bounds(2 * nv);
+    for (size_t k = 0; k < nv; ++k) { bounds[k] = (T)pd->lo[k]; bounds[nv + k] = (T)pd->hi[k]; }
+    T* dev = (T*)work.p + rows * (size_t)B;
+    RBD_CUDA_TRY(cudaMemcpyAsync(dev, bounds.data(), 2 * nv * sizeof(T), cudaMemcpyHostToDevice, stream));
+    pd_lo = dev; pd_hi = dev + nv;
+  }
+  if (pd) tau_dense = taud;
+  else if (tau && ld != B && !varying) {
     RBD_CUDA_TRY(cudaMemcpy2DAsync(taud, B * sizeof(T), tau, ld * sizeof(T), B * sizeof(T), nv, cudaMemcpyDeviceToDevice, stream));
     tau_dense = taud;
   }
@@ -1081,6 +1162,14 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
   // the vectorised kernel needs whole vectors per row (workspace rows are B long and 256-byte aligned)
   const bool vec_ok = B % VecOf<T>::N == 0 && B >= 1024;
   const int grid_lin = (int)std::min<int64_t>((B / VecOf<T>::N + 255) / 256, (int64_t)p.sms * 4);
+  // ... and, for the feedback law in it, vector-aligned rows of the controller's caller arrays at every (step, stage)
+  auto vec_aligned = [&](const void* a, int64_t stride) {
+    return !a || (((uintptr_t)a % sizeof(typename VecOf<T>::type)) == 0 && stride % VecOf<T>::N == 0);
+  };
+  const bool vec_stage = vec_ok && (!pd || (ld % VecOf<T>::N == 0 && vec_aligned(pd->qref, pd->qref_stride) &&
+                                            vec_aligned(pd->vref, pd->vref_stride) && vec_aligned(pd->vdref, pd->vref_stride) &&
+                                            (pd->g_ld == 0 || (vec_aligned(pd->kp, 0) && vec_aligned(pd->kd, 0))) &&
+                                            vec_aligned(tau, step_stride) && vec_aligned(tau, stage_stride)));
   // ... and, for the finishing kernel, vector-aligned rows of the caller's arrays too
   const bool vec_user = vec_ok && ldo % VecOf<T>::N == 0 && ((uintptr_t)qout % sizeof(typename VecOf<T>::type)) == 0 &&
                         ((uintptr_t)vout % sizeof(typename VecOf<T>::type)) == 0;
@@ -1096,20 +1185,34 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
   }
   for (int s = 0; s < nsteps; ++s) {
     for (int i = 0; i < 4; ++i) {
-      if (varying) {
+      if (varying && !pd) {
         tau_dense = tau_at(s, i);
         if (tau && ld != B) {
           RBD_CUDA_TRY(cudaMemcpy2DAsync(taud, B * sizeof(T), tau_dense, ld * sizeof(T), B * sizeof(T), nv, cudaMemcpyDeviceToDevice, stream));
           tau_dense = taud;
         }
       }
-      StageArgs<T> sa{q0, v0, i ? phid[i - 1] : nullptr, i ? vd[i - 1] : nullptr, phid[i], qsi[i], vsi[i], (T)(dt * a[i]), B, vec_ok};
-      if (vec_ok) {        // revolute / prismatic rows, VEC samples per thread
+      StageArgs<T> sa{q0, v0, i ? phid[i - 1] : nullptr, i ? vd[i - 1] : nullptr, phid[i], qsi[i], vsi[i], (T)(dt * a[i]), B, vec_stage};
+      if (pd) {
+        const T* qref = pd->qref + (size_t)s * pd->qref_stride;
+        const size_t r = (size_t)s * pd->vref_stride;
+        const T* vref = pd->vref ? pd->vref + r : nullptr;
+        sa.pd = pd->computed_torque ? PdStage<T>{qref, vref, pd->vdref ? pd->vdref + r : nullptr, pd->kp, pd->kd, pd->g_ld, nullptr,
+                                                 nullptr, vd[i], ld}
+                                    : PdStage<T>{qref, vref, tau_at(s, i), pd->kp, pd->kd, pd->g_ld, pd_lo, pd_hi, taud, ld};
+      }
+      if (vec_stage) {     // revolute / prismatic rows, VEC samples per thread
         integrate_stage_linear_kernel<T><<<dim3(grid_lin, hm.nb), 256, 0, stream>>>(M, sa);
         if (int rc = api_launched()) return rc;
       }
-      if (!vec_ok || has_other) {
+      if (!vec_stage || has_other) {
         integrate_stage_kernel<T><<<dim3(grid, hm.nb), 128, 0, stream>>>(M, sa);
+        if (int rc = api_launched()) return rc;
+      }
+      if (pd && pd->computed_torque) {     // tau = clamp(ID(q_s, v_s, v̇_des) + τ_ff), without contact wrenches
+        if (int rc = inverse_dynamics_t<T>(model, B, B, qsi[i], vsi[i], vd[i], nullptr, taud, stream)) return rc;
+        const PdFinishArgs<T> pf{taud, tau_at(s, i), ld, pd_lo, pd_hi, (int64_t)nv, B};
+        pd_finish_kernel<T><<<(int)std::min<int64_t>(((int64_t)nv * B + 255) / 256, (int64_t)p.sms * 8), 256, 0, stream>>>(pf);
         if (int rc = api_launched()) return rc;
       }
       if (loop) {
@@ -1349,6 +1452,32 @@ int integrate_loops(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld
                                                       q_traj, v_traj, s_traj, stream);
 }
 }  // namespace rbd
+
+namespace {
+template <class T>
+int integrate_pd_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau, int64_t step_stride,
+                   int64_t stage_stride, const rbd_pd_desc& d, const rbd_loop_desc* loops, const rbd_contact_desc* contact, double dt,
+                   int nsteps, void* q_traj, void* v_traj, void* s_traj, cudaStream_t stream) {
+  const PdRollout<T> pd{d.mode == RBD_PD_COMPUTED_TORQUE, (const T*)d.kp, (const T*)d.kd, d.gain_ld, (const T*)d.q_ref,
+                        (const T*)d.v_ref, (const T*)d.vd_ref, d.q_ref_step_stride, d.v_ref_step_stride, d.effort_lo, d.effort_hi};
+  const int64_t ns = contact ? (int64_t)3 * contact->npoints * contact->nhalfspaces : 0;
+  if (loops) {
+    const LoopRollout lr{loops, contact};
+    const ContactRollout<T> cr{nullptr, ns, (T*)s, (T*)s_traj};
+    return integrate_t<T>(model, B, ld, q, v, tau, step_stride, stage_stride, dt, nsteps, stream, (T*)q_traj, (T*)v_traj, nullptr,
+                          contact ? &cr : nullptr, &lr, &pd);
+  }
+  if (contact) {
+    std::unique_ptr<ContactDev<T>> C(new ContactDev<T>());
+    build_contact_dev<T>(model->hm.nb, model->hm.pos.data(), model->hm.alignT.data(), *contact, *C);
+    const ContactRollout<T> cr{C.get(), ns, (T*)s, (T*)s_traj};
+    return integrate_t<T>(model, B, ld, q, v, tau, step_stride, stage_stride, dt, nsteps, stream, (T*)q_traj, (T*)v_traj, nullptr, &cr,
+                          nullptr, &pd);
+  }
+  return integrate_t<T>(model, B, ld, q, v, tau, step_stride, stage_stride, dt, nsteps, stream, (T*)q_traj, (T*)v_traj, nullptr, nullptr,
+                        nullptr, &pd);
+}
+}  // namespace
 
 // ------------------------------------------------------------------------------------------------------------------
 // C ABI
@@ -1699,6 +1828,49 @@ int32_t rbd_integrate_contact(const rbd_model* model, int32_t dtype, int64_t B, 
                                                        q_traj, v_traj, s_traj, st)
                           : integrate_contact_t<double>(model, B, ld, q, v, s, tau, tau_step_stride, tau_stage_stride, *contact, dt, nsteps,
                                                         q_traj, v_traj, s_traj, st);
+}
+
+int32_t rbd_integrate_pd(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau,
+                         int64_t tau_step_stride, int64_t tau_stage_stride, const rbd_pd_desc* pd, const rbd_loop_desc* loops,
+                         const rbd_contact_desc* contact, double dt, int32_t nsteps, void* q_traj, void* v_traj, void* s_traj,
+                         void* stream) {
+  if (!model) return fail(RBD_EINVAL, "model handle is NULL");
+  if (dtype != RBD_F32 && dtype != RBD_F64) return fail(RBD_EUNSUPPORTED, "rbd_integrate_pd: fp32 / fp64 only");
+  if (int rc = check_common(model, dtype, B, ld)) return rc;
+  if (nsteps < 0 || !(dt > 0)) return fail(RBD_EINVAL, "rbd_integrate_pd: need dt > 0 and nsteps >= 0");
+  if (tau_step_stride < 0 || tau_stage_stride < 0) return fail(RBD_EINVAL, "rbd_integrate_pd: torque strides must be >= 0");
+  if (!pd) return fail(RBD_EINVAL, "rbd_integrate_pd: pd must not be NULL");
+  if (!pd->kp || !pd->kd || !pd->q_ref) return fail(RBD_EINVAL, "rbd_integrate_pd: kp, kd and q_ref must not be NULL");
+  if (pd->mode != RBD_PD_TORQUE && pd->mode != RBD_PD_COMPUTED_TORQUE) return fail(RBD_EINVAL, "rbd_integrate_pd: unknown mode");
+  if (pd->q_ref_step_stride < 0 || pd->v_ref_step_stride < 0) return fail(RBD_EINVAL, "rbd_integrate_pd: reference strides must be >= 0");
+  if (pd->gain_ld != 0 && pd->gain_ld != ld) return fail(RBD_EINVAL, "rbd_integrate_pd: gain_ld must be 0 or ld");
+  if (pd->mode == RBD_PD_TORQUE && pd->vd_ref) return fail(RBD_EINVAL, "rbd_integrate_pd: vd_ref is for computed-torque mode only");
+  if (!pd->effort_lo != !pd->effort_hi) return fail(RBD_EINVAL, "rbd_integrate_pd: effort_lo and effort_hi must be both NULL or both set");
+  if (pd->effort_lo)
+    for (int k = 0; k < model->hm.nv; ++k)
+      if (!(pd->effort_lo[k] <= pd->effort_hi[k])) return fail(RBD_EINVAL, "rbd_integrate_pd: effort bounds need lo <= hi");
+  if (loops) {
+    if (int rc = api_check_loops(model, loops)) return rc;
+    if (pd->mode == RBD_PD_COMPUTED_TORQUE && loops->nloops > 0)
+      return fail(RBD_ELOOP, "rbd_integrate_pd: computed-torque mode needs inverse_dynamics!, which has no kinematic loops");
+  }
+  if (contact)
+    if (int rc = check_contact(model, contact, "rbd_integrate_pd")) return rc;
+  const int64_t ns = contact ? (int64_t)3 * contact->npoints * contact->nhalfspaces : 0;
+  const bool rec = q_traj || v_traj || s_traj;
+  if (rec && (!q_traj || !v_traj || (ns > 0 && !s_traj)))
+    return fail(RBD_EINVAL, "rbd_integrate_pd: q_traj, v_traj and s_traj must be all NULL or all set");
+  const ApiCall call;
+  if (B == 0) return RBD_OK;
+  if (!q || !v) return fail(RBD_EINVAL, "rbd_integrate_pd: q and v must not be NULL");
+  if (ns > 0 && !s) return fail(RBD_EINVAL, "rbd_integrate_pd: s must not be NULL when there are contact pairs");
+  if (nsteps == 0 && !rec) return RBD_OK;
+  const rbd_contact_desc* c = ns > 0 || !loops ? contact : nullptr;     // the loop rollout takes contact only with pairs
+  cudaStream_t st = (cudaStream_t)stream;
+  return dtype == RBD_F32 ? integrate_pd_t<float>(model, B, ld, q, v, s, tau, tau_step_stride, tau_stage_stride, *pd, loops, c, dt, nsteps,
+                                                  q_traj, v_traj, s_traj, st)
+                          : integrate_pd_t<double>(model, B, ld, q, v, s, tau, tau_step_stride, tau_stage_stride, *pd, loops, c, dt,
+                                                   nsteps, q_traj, v_traj, s_traj, st);
 }
 
 int32_t rbd_dynamics_result(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,

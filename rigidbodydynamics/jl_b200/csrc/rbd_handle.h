@@ -181,6 +181,8 @@ int loop_stage_launch(const rbd_model* model, int32_t dtype, const rbd_loop_desc
                       const LoopStageArgs& a, std::shared_ptr<LoopStagePlan>& plan, cudaStream_t stream);
 // rbd_b200.cu's descriptor checks of rbd_contact_dynamics (fn: the entry point named in the message)
 int api_check_contact(const rbd_model* model, const rbd_contact_desc* contact, const char* fn);
+// rbd_loops.cu's descriptor checks of rbd_dynamics_loops
+int api_check_loops(const rbd_model* model, const rbd_loop_desc* loops);
 // rbd_adjoint.cu's forward-dynamics VJP on dense [rows x B] arrays (no external wrenches); outputs may be NULL
 int dynamics_vjp_dense(const rbd_model* model, int32_t dtype, int64_t B, const void* q, const void* v, const void* vd, const void* vd_bar,
                        void* q_bar_cfg, void* v_bar, void* tau_bar, cudaStream_t stream);

@@ -122,23 +122,29 @@ template <class T> RBD_HD void qfloat_global(const T* q0, const T* phi, T* q) {
   mat_vec(R0, tr, t);
   q[4] = q0[4] + t[0]; q[5] = q0[5] + t[1]; q[6] = q0[6] + t[2];
 }
-// local_coordinates!: (phi, phi_dot) = log_with_time_derivative(q0^-1 q, twist v)   (quaternion_floating.jl:205-231)
-template <class T> RBD_HD void qfloat_local_rate(const T* q0, const T* q, const T* v, T* phid) {
+// log(q0^-1 q): the exponential coordinates (psi, qq) of the relative transform, and the dexp^-1 coefficients A, B at psi
+// (_log, spatialmotion.jl:226-252) -- local_coordinates! of QuaternionFloating (quaternion_floating.jl:205-231)
+template <class T> RBD_HD void qfloat_log(const T* q0, const T* q, T* psi, T* qq, T& A, T& B) {
   const T q0c[4] = {q0[0], -q0[1], -q0[2], -q0[3]};
   T dq[4];
   quat_mul(q0c, q, dq);
   T R0[9], d[3] = {q[4] - q0[4], q[5] - q0[5], q[6] - q0[6]}, p[3];
   rot_quat(q0[0], q0[1], q0[2], q0[3], R0);
   matT_vec(R0, d, p);
-  T psi[3], t2;
+  T t2;
   rotvec_from_quat(dq, psi, t2);
-  T g, A, B;
+  T g;
   dexpinv_coeffs(t2, g, A, B);
-  // X = (psi, qq): qq = p - psi x p / 2 + g psi x (psi x p)     (_log, spatialmotion.jl:226-252)
-  T c1[3], c2[3], qq[3];
+  // qq = p - psi x p / 2 + g psi x (psi x p)
+  T c1[3], c2[3];
   cross3(psi, p, c1);
   cross3(psi, c1, c2);
   qq[0] = p[0] - T(0.5) * c1[0] + g * c2[0]; qq[1] = p[1] - T(0.5) * c1[1] + g * c2[1]; qq[2] = p[2] - T(0.5) * c1[2] + g * c2[2];
+}
+// local_coordinates!: (phi, phi_dot) = log_with_time_derivative(q0^-1 q, twist v)   (quaternion_floating.jl:205-231)
+template <class T> RBD_HD void qfloat_local_rate(const T* q0, const T* q, const T* v, T* phid) {
+  T psi[3], qq[3], A, B;
+  qfloat_log(q0, q, psi, qq, A, B);
   // X_dot = V + ad_X V / 2 + A ad_X^2 V + B ad_X^4 V            (Lemma 4, spatialmotion.jl:272-296)
   const T* w = v; const T* vl = v + 3;
   T a1w[3], a1v[3], a2w[3], a2v[3], a3w[3], a3v[3], a4w[3], a4v[3];
@@ -159,14 +165,19 @@ template <class T> RBD_HD void qsph_global(const T* q0, const T* phi, T* q) {
   quat_from_rotvec(phi, dq);
   quat_mul(q0, dq, q);
 }
-template <class T> RBD_HD void qsph_local_rate(const T* q0, const T* q, const T* w, T* phid) {
+// the rotation vector phi of q0^-1 q (local_coordinates!) and g of dexp^-1 at it
+template <class T> RBD_HD void qsph_log(const T* q0, const T* q, T* phi, T& g) {
   const T q0c[4] = {q0[0], -q0[1], -q0[2], -q0[3]};
-  T dq[4], phi[3], t2;
+  T dq[4], t2;
   quat_mul(q0c, q, dq);
   rotvec_from_quat(dq, phi, t2);
-  // phi_dot = w + phi x w / 2 + 1/theta^2 (1 - theta s / (2 (1 - c))) phi x (phi x w);  the bracket / theta^2 equals g above
-  T g, A, B;
+  T A, B;
   dexpinv_coeffs(t2, g, A, B);
+}
+template <class T> RBD_HD void qsph_local_rate(const T* q0, const T* q, const T* w, T* phid) {
+  T phi[3], g;
+  qsph_log(q0, q, phi, g);
+  // phi_dot = w + phi x w / 2 + 1/theta^2 (1 - theta s / (2 (1 - c))) phi x (phi x w);  the bracket / theta^2 equals g above
   T c1[3], c2[3];
   cross3(phi, w, c1);
   cross3(phi, c1, c2);

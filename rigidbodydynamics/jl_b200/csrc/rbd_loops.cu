@@ -178,6 +178,11 @@ int loop_stage_t(const rbd_model* model, const rbd_loop_desc& loops, const rbd_c
 }  // namespace
 
 namespace rbd {
+int api_check_loops(const rbd_model* model, const rbd_loop_desc* loops) {
+  std::string err;
+  if (int rc = check_loop_desc(model->hm, loops, err)) return api_fail(rc, err);
+  return RBD_OK;
+}
 int loop_stage_launch(const rbd_model* model, int32_t dtype, const rbd_loop_desc& loops, const rbd_contact_desc* contact,
                       const LoopStageArgs& a, std::shared_ptr<LoopStagePlan>& plan, cudaStream_t stream) {
   return dtype == RBD_F32 ? loop_stage_t<float>(model, loops, contact, a, plan, stream)

@@ -27,6 +27,7 @@ from .algorithms import _call, _check, _ptr, _stream, _torque_schedule
 from .contact import ContactDesc, contact_desc
 from .joint_types import Fixed, Planar, Prismatic, QuaternionSpherical, Revolute
 from .mechanism import Mechanism
+from .pd import integrate_pd
 from .spatial import rotation_between
 from .state import DynamicsResult, MechanismState, _DT
 
@@ -178,7 +179,7 @@ def dynamics_loops_(result: DynamicsResult, state: MechanismState, torques: Opti
 
 
 def _integrate_loops(state: MechanismState, nsteps: int, torques, dt: float, stabilization_gains, loops: Optional[LoopDesc],
-                     contact_state: Optional[torch.Tensor], contact: Optional[ContactDesc], record: bool, what: str):
+                     contact_state: Optional[torch.Tensor], contact: Optional[ContactDesc], record: bool, what: str, controller=None):
     state.check_modcount()
     if nsteps < 0:
         raise ValueError("nsteps must be >= 0")
@@ -197,6 +198,10 @@ def _integrate_loops(state: MechanismState, nsteps: int, torques, dt: float, sta
     if record:
         new = lambda rows: torch.empty((nsteps + 1, rows, state.batch), dtype=state.dtype, device=state.q.device)   # noqa: E731
         traj = (new(state.nq), new(state.nv), new(cd.nstates) if cd.nstates else None)
+    if controller is not None:
+        integrate_pd(state, controller, nsteps, torques, step, stage, dt, loops=ld, contact=cd, contact_state=contact_state, traj=traj,
+                     what=what)
+        return traj
     lst, keep = ld.c_struct()
     cst, keep2 = cd.c_struct()
     _call(lib.rbd_integrate_loops(state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q), _ptr(state.v),
@@ -208,17 +213,20 @@ def _integrate_loops(state: MechanismState, nsteps: int, torques, dt: float, sta
 
 def simulate_loops_trajectory_(state: MechanismState, nsteps: int, torques: Optional[torch.Tensor] = None, dt: float = 1e-4,
                                stabilization_gains=_DEFAULT, loops: Optional[LoopDesc] = None,
-                               contact_state: Optional[torch.Tensor] = None, contact: Optional[ContactDesc] = None):
+                               contact_state: Optional[torch.Tensor] = None, contact: Optional[ContactDesc] = None, *,
+                               controller=None):
     """``nsteps`` steps of ``simulate_loops_``, recording the trajectory: returns ``(q_traj, v_traj, s_traj)``, [nsteps + 1, nq, B],
     [nsteps + 1, nv, B] and [nsteps + 1, num_contact_states, B] (None without contact states), block 0 the initial state and block s
-    the state after step s.  ``state`` and ``contact_state`` are advanced in place exactly as ``simulate_loops_`` advances them."""
+    the state after step s.  ``state`` and ``contact_state`` are advanced in place exactly as ``simulate_loops_`` advances them.
+    ``controller``: a ``JointPD`` evaluated at every stage, as in ``simulate_loops_`` (``torques`` is then its feedforward; PD mode
+    only when the mechanism has loops)."""
     return _integrate_loops(state, nsteps, torques, dt, stabilization_gains, loops, contact_state, contact, True,
-                            "simulate_loops_trajectory_")
+                            "simulate_loops_trajectory_", controller)
 
 
 def simulate_loops_(state: MechanismState, final_time: float, torques: Optional[torch.Tensor] = None, dt: float = 1e-4,
                     stabilization_gains=_DEFAULT, loops: Optional[LoopDesc] = None, contact_state: Optional[torch.Tensor] = None,
-                    contact: Optional[ContactDesc] = None) -> int:
+                    contact: Optional[ContactDesc] = None, *, controller=None) -> int:
     """``simulate(state, final_time; Δt, stabilization_gains)`` (src/simulate.jl:36-55) for a mechanism with non-tree joints, all on
     the GPU: Munthe-Kaas RK4 steps until ``t >= final_time`` (the step count of ``simulate_``) whose every stage runs ``dynamics!``
     as ``dynamics_loops_`` does -- with contact points, contact_dynamics! first and its wrenches as the external wrenches
@@ -226,11 +234,13 @@ def simulate_loops_(state: MechanismState, final_time: float, torques: Optional[
     mechanism has contact points) are advanced in place; the contact state follows ``simulate_contact_`` (integrated, never reset,
     carried across calls).  ``torques``: None, constant [nv, B], per step [nsteps, nv, B] or per stage [nsteps, 4, nv, B].
     ``stabilization_gains``: as ``loop_desc`` (default gains, None = off, or per joint); ``loops`` / ``contact``: prebuilt
-    descriptors (default: the mechanism's).  A tree mechanism is accepted (the KKT path without constraint rows).  Returns the number
-    of steps taken."""
+    descriptors (default: the mechanism's).  A tree mechanism is accepted (the KKT path without constraint rows).  ``controller``: a
+    ``JointPD`` evaluated at every stage, as in ``simulate_`` (PD mode only when the mechanism has loops: computed-torque mode needs
+    inverse_dynamics!, which refuses loops with RBD_ELOOP).  Returns the number of steps taken."""
     nsteps, t = 0, 0.0
     while t < final_time:            # the reference's `while t < final_time` loop (ode_integrators.jl:311)
         t += dt
         nsteps += 1
-    _integrate_loops(state, nsteps, torques, dt, stabilization_gains, loops, contact_state, contact, False, "simulate_loops_")
+    _integrate_loops(state, nsteps, torques, dt, stabilization_gains, loops, contact_state, contact, False, "simulate_loops_",
+                     controller)
     return nsteps

@@ -45,12 +45,27 @@ class RigidBody:
         return f"RigidBody({self.name!r})"
 
 
-class Joint:
-    """joint.jl:43-67."""
+@dataclass(frozen=True)
+class Bounds:
+    """Bounds{T} (src/bounds.jl): a closed interval, (-inf, inf) by default."""
+    lower: float = -np.inf
+    upper: float = np.inf
 
-    def __init__(self, name: str, joint_type: JointType):
+
+class Joint:
+    """joint.jl:43-67.  ``position_bounds`` ([nq]), ``velocity_bounds`` and ``effort_bounds`` ([nv]): lists of ``Bounds``, infinite
+    unless given (joint.jl:51-58, parsed from URDF <limit> by parse_urdf)."""
+
+    def __init__(self, name: str, joint_type: JointType, *, position_bounds: Optional[Sequence[Bounds]] = None,
+                 velocity_bounds: Optional[Sequence[Bounds]] = None, effort_bounds: Optional[Sequence[Bounds]] = None):
         self.name = name
         self.joint_type = joint_type
+        self.position_bounds = list(position_bounds) if position_bounds is not None else [Bounds()] * joint_type.nq
+        self.velocity_bounds = list(velocity_bounds) if velocity_bounds is not None else [Bounds()] * joint_type.nv
+        self.effort_bounds = list(effort_bounds) if effort_bounds is not None else [Bounds()] * joint_type.nv
+        if len(self.position_bounds) != joint_type.nq or len(self.velocity_bounds) != joint_type.nv or \
+                len(self.effort_bounds) != joint_type.nv:
+            raise ValueError("joint bounds: nq position bounds and nv velocity / effort bounds")
         self.joint_to_predecessor = Transform3D.identity()   # frame before joint -> predecessor body frame
         # frame after joint -> successor body frame: the identity for tree joints (the body frame IS the frame after the joint),
         # inv(successor_pose) for non-tree joints (mechanism_modification.jl:34)
@@ -254,7 +269,8 @@ def maximal_coordinates(mechanism: Mechanism, floating_joint_type: type = Quater
         body = bodymap[src] = RigidBody(src.name, src.inertia.copy())
         ret.attach(root, body, Joint(str(src.name), floating_joint_type()))
     for src in mechanism.joints + mechanism.non_tree_joints:             # _copyjoint! (:48-63)
-        joint = jointmap[src] = Joint(src.name, copy.deepcopy(src.joint_type))
+        joint = jointmap[src] = Joint(src.name, copy.deepcopy(src.joint_type), position_bounds=src.position_bounds,
+                                      velocity_bounds=src.velocity_bounds, effort_bounds=src.effort_bounds)
         ret.attach(bodymap[src.predecessor], bodymap[src.successor], joint, joint_pose=src.joint_to_predecessor,
                    successor_pose=src.joint_to_successor.inv())
     return ret
@@ -287,3 +303,9 @@ def rand_floating_tree_mechanism(rng, nonfloating_joint_types: Sequence[type]) -
         nr = m.non_root_bodies()
         return m.root_body if not nr else nr[int(r.integers(len(nr)))]
     return rand_tree_mechanism(rng, [QuaternionFloating, *nonfloating_joint_types], sel)
+
+
+def effort_bounds(mechanism: "Mechanism"):
+    """The tree joints' effort bounds in velocity order: ``(lo, hi)``, two float64 arrays [nv] -- the saturation of a ``JointPD``."""
+    b = [e for j in mechanism.joints for e in j.effort_bounds]
+    return np.array([x.lower for x in b], float), np.array([x.upper for x in b], float)

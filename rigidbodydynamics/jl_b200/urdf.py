@@ -10,7 +10,8 @@ Rules that decide the q/v/τ index order (get one wrong and every batched array 
   * fixed tree joints are then removed, the others keep their relative order (parse.jl:216-218);
   * <origin rpy> -> Rz(yaw) Ry(pitch) Rx(roll) (parse.jl:46-51); <inertia> is about the COM in the
     <inertial><origin> frame and is transformed into the link frame (parse.jl:104-112);
-  * <dynamics damping>, <limit>, <mimic> do not enter the dynamics (parse.jl:74-95).
+  * <dynamics damping>, <limit>, <mimic> do not enter the dynamics (parse.jl:74-95); <limit> gives the joint bounds
+    (parse.jl:75-91): lower / upper the position bounds, velocity="v" / effort="e" the bounds (-v, v) / (-e, e).
 """
 from __future__ import annotations
 
@@ -21,7 +22,7 @@ from typing import Dict, Optional
 import numpy as np
 
 from .joint_types import (Fixed, JointType, Planar, Prismatic, QuaternionFloating, Revolute)
-from .mechanism import DEFAULT_GRAVITATIONAL_ACCELERATION, Joint, Mechanism, RigidBody
+from .mechanism import DEFAULT_GRAVITATIONAL_ACCELERATION, Bounds, Joint, Mechanism, RigidBody
 from .spatial import SpatialInertia, Transform3D, rot_rpy, rotation_between
 
 
@@ -58,7 +59,8 @@ def _pose_dict(xml_pose: Optional[ET.Element]):
 def read_urdf(filename: str) -> dict:
     """URDF file -> plain "robot description" dict holding exactly what the reference's parser reads:
     links (name, optional inertial: mass / origin / 6 inertia entries) and joints (name, type, parent, child, origin,
-    axis) in DOCUMENT order, direct children of <robot> only (parse.jl:184-185)."""
+    axis, limit: the attributes lower / upper / velocity / effort present on its <limit> elements) in DOCUMENT order, direct
+    children of <robot> only (parse.jl:184-185)."""
     xroot = ET.parse(filename).getroot()
     if xroot.tag != "robot":
         raise ValueError("URDF root element must be <robot>")
@@ -76,7 +78,11 @@ def read_urdf(filename: str) -> dict:
         links.append({"name": xl.get("name"), "inertial": inertial})
     for xj in xroot.findall("joint"):
         ax = xj.find("axis")
+        limit = {}
+        for xlim in xj.findall("limit"):          # later elements override earlier ones, attribute by attribute (parse.jl:78-91)
+            limit.update({k: float(xlim.get(k)) for k in ("lower", "upper", "velocity", "effort") if xlim.get(k) is not None})
         joints.append({
+            "limit": limit,
             "name": xj.get("name"), "type": xj.get("type"),
             "parent": xj.find("parent").get("link"), "child": xj.find("child").get("link"),
             "origin": _pose_dict(xj.find("origin")),
@@ -114,6 +120,15 @@ def _joint_type_from(j: dict, joint_types: Dict[str, type]) -> JointType:
         R = rotation_between([0.0, 0.0, 1.0], axis)          # plane perpendicular to the URDF axis
         return cls(R @ np.array([1.0, 0, 0]), R @ np.array([0, 1.0, 0]))
     raise ValueError(f"joint type {t} not recognized")
+
+
+def _joint_bounds(j: dict, jt: JointType):
+    """parse_joint_bounds (parse.jl:75-91): (position, velocity, effort) bounds; descriptions without <limit> get infinite ones."""
+    lim = j.get("limit") or {}
+    pos = Bounds(lim.get("lower", -np.inf), lim.get("upper", np.inf))
+    vel = Bounds(-lim["velocity"], lim["velocity"]) if "velocity" in lim else Bounds()
+    eff = Bounds(-lim["effort"], lim["effort"]) if "effort" in lim else Bounds()
+    return dict(position_bounds=[pos] * jt.nq, velocity_bounds=[vel] * jt.nv, effort_bounds=[eff] * jt.nv)
 
 
 def _body_from(link: dict) -> RigidBody:
@@ -171,7 +186,8 @@ def mechanism_from_description(desc: dict, *, floating: bool = False, joint_type
     mech.attach(mech.root_body, body, Joint(f"{body.name}_to_world", root_joint_type))   # parse.jl:121-127
     for e in tree_edges:
         parent = bodies[e["parent"]]
-        joint = Joint(e["name"], _joint_type_from(e, jt))
+        joint_type = _joint_type_from(e, jt)
+        joint = Joint(e["name"], joint_type, **_joint_bounds(e, joint_type))
         rot, trans = _pose(e.get("origin"))
         body = _body_from(name_to_link[e["child"]])
         bodies[e["child"]] = body
