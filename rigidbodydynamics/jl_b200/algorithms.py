@@ -11,13 +11,14 @@ without the built library or without a GPU these raise.
 """
 from __future__ import annotations
 
+import ctypes
 from typing import Optional
 
 import torch
 
 from . import _cabi
+from .pd import JointPD
 from .state import DynamicsResult, MechanismState, _DT
-from .pd import integrate_pd
 
 __all__ = ["dynamics_", "dynamics_dual_", "dynamics_derivatives_", "dynamics_ode_", "simulate_", "simulate_trajectory_", "inverse_dynamics_", "inverse_dynamics", "mass_matrix_", "mass_matrix",
            "dynamics_bias_", "dynamics_bias", "DimensionMismatch"]
@@ -169,6 +170,62 @@ def _torque_schedule(state: MechanismState, torques: torch.Tensor, nsteps: int):
     return (4 * blk, blk) if torques.dim() == 4 else (blk, 0)
 
 
+def _steps(final_time: float, dt: float) -> int:
+    """The step count of the reference's `while t < final_time` loop (ode_integrators.jl:311)."""
+    nsteps, t = 0, 0.0
+    while t < final_time:
+        t += dt
+        nsteps += 1
+    return nsteps
+
+
+def _rollout(state: MechanismState, nsteps: int, torques: Optional[torch.Tensor], dt: float, what: str, record: bool = False,
+             controller=None, loops=None, contact=None, contact_state: Optional[torch.Tensor] = None):
+    """``nsteps`` RK4 steps of the state (leading dimension B) in one call of the library's rollout: the tree rollout, or with the
+    prebuilt descriptors ``loops`` / ``contact`` the loop / contact rollout, with ``controller`` evaluated at every stage.  Returns
+    ``(q_traj, v_traj, s_traj)`` when ``record`` (s_traj None without contact, and for the loop rollout without contact states),
+    else three Nones."""
+    state.check_modcount()
+    if nsteps < 0:
+        raise ValueError("nsteps must be >= 0")
+    lib = _cabi.load_library()
+    ns = contact.nstates if contact is not None else 0
+    if contact_state is None and ns > 0:
+        raise ValueError(f"{what}: contact_state [{ns}, B] must be given (the mechanism has contact points)")
+    _check(contact_state, ns, state, "contact_state")
+    step = stage = 0
+    if torques is not None and torques.dim() in (3, 4):
+        step, stage = _torque_schedule(state, torques, nsteps)
+    else:
+        _check(torques, state.nv, state, "torques")
+    traj = (None, None, None)
+    if record:
+        new = lambda rows: torch.empty((nsteps + 1, rows, state.batch), dtype=state.dtype, device=state.q.device)   # noqa: E731
+        traj = (new(state.nq), new(state.nv), None if contact is None or (loops is not None and ns == 0) else new(ns))
+    lst, keep_l = loops.c_struct() if loops is not None else (None, None)          # keep_*: arrays alive over the call
+    cst, keep_c = contact.c_struct() if contact is not None else (None, None)
+    ref = lambda st: None if st is None else ctypes.byref(st)                     # noqa: E731
+    head = (state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q), _ptr(state.v))
+    steps = (float(dt), nsteps)
+    out = tuple(_ptr(t) for t in traj)
+    if controller is not None:
+        if not isinstance(controller, JointPD):
+            raise TypeError(f"{what}: controller must be a JointPD")
+        pd, keep_pd = controller._c_struct(state, nsteps, what)
+        _call(lib.rbd_integrate_pd(*head, _ptr(contact_state), _ptr(torques), step, stage, ctypes.byref(pd), ref(lst), ref(cst),
+                                   *steps, *out, _stream()))
+    elif loops is not None:
+        _call(lib.rbd_integrate_loops(*head, _ptr(contact_state), _ptr(torques), step, stage, ref(lst), ref(cst), *steps, *out,
+                                      _stream()))
+    elif contact is not None:
+        _call(lib.rbd_integrate_contact(*head, _ptr(contact_state), _ptr(torques), step, stage, ref(cst), *steps, *out, _stream()))
+    elif record:
+        _call(lib.rbd_integrate_trajectory(*head, _ptr(torques), step, stage, *steps, *out[:2], _stream()))
+    else:
+        _call(lib.rbd_integrate_schedule(*head, _ptr(torques), step, stage, *steps, _stream()))
+    return traj
+
+
 def simulate_trajectory_(state: MechanismState, nsteps: int, torques: Optional[torch.Tensor] = None, dt: float = 1e-4, *,
                          controller=None):
     """``nsteps`` Munthe-Kaas RK4 steps like ``simulate_``, recording the trajectory: returns ``(q_traj, v_traj)``,
@@ -177,23 +234,7 @@ def simulate_trajectory_(state: MechanismState, nsteps: int, torques: Optional[t
     [nsteps, 4, nv, B].  ``controller``: a ``JointPD`` evaluated at every stage (``torques`` is then its feedforward), as in
     ``simulate_``.  The recorded trajectory of an open-loop rollout is what ``autodiff.integrate_vjp_`` differentiates."""
     _require_tree(state, "simulate_trajectory_")
-    state.check_modcount()
-    if nsteps < 0:
-        raise ValueError("nsteps must be >= 0")
-    lib = _cabi.load_library()
-    step = stage = 0
-    if torques is not None and torques.dim() in (3, 4):
-        step, stage = _torque_schedule(state, torques, nsteps)
-    else:
-        _check(torques, state.nv, state, "torques")
-    q_traj = torch.empty((nsteps + 1, state.nq, state.batch), dtype=state.dtype, device=state.q.device)
-    v_traj = torch.empty((nsteps + 1, state.nv, state.batch), dtype=state.dtype, device=state.q.device)
-    if controller is not None:
-        integrate_pd(state, controller, nsteps, torques, step, stage, dt, traj=(q_traj, v_traj, None), what="simulate_trajectory_")
-        return q_traj, v_traj
-    _call(lib.rbd_integrate_trajectory(state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q), _ptr(state.v),
-                                       _ptr(torques), step, stage, float(dt), nsteps, _ptr(q_traj), _ptr(v_traj), _stream()))
-    return q_traj, v_traj
+    return _rollout(state, nsteps, torques, dt, "simulate_trajectory_", record=True, controller=controller)[:2]
 
 
 def simulate_(state: MechanismState, final_time: float, torques: Optional[torch.Tensor] = None, dt: float = 1e-4, *,
@@ -205,28 +246,8 @@ def simulate_(state: MechanismState, final_time: float, torques: Optional[torch.
     feedback) evaluated at every RK4 stage on that stage's state, with ``torques`` as its feedforward.  Returns the number of steps
     taken."""
     _require_tree(state, "simulate_")
-    state.check_modcount()
-    lib = _cabi.load_library()
-    nsteps, t = 0, 0.0
-    while t < final_time:            # the reference's `while t < final_time` loop (ode_integrators.jl:311)
-        t += dt
-        nsteps += 1
-    if controller is not None:
-        step = stage = 0
-        if torques is not None and torques.dim() in (3, 4):
-            step, stage = _torque_schedule(state, torques, nsteps)
-        else:
-            _check(torques, state.nv, state, "torques")
-        integrate_pd(state, controller, nsteps, torques, step, stage, dt, what="simulate_")
-        return nsteps
-    if torques is not None and torques.dim() in (3, 4):
-        step, stage = _torque_schedule(state, torques, nsteps)
-        _call(lib.rbd_integrate_schedule(state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q), _ptr(state.v),
-                                         _ptr(torques), step, stage, float(dt), nsteps, _stream()))
-        return nsteps
-    _check(torques, state.nv, state, "torques")
-    _call(lib.rbd_integrate(state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q), _ptr(state.v),
-                            _ptr(torques), float(dt), nsteps, _stream()))
+    nsteps = _steps(final_time, dt)
+    _rollout(state, nsteps, torques, dt, "simulate_", controller=controller)
     return nsteps
 
 

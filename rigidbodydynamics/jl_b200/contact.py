@@ -27,8 +27,7 @@ import numpy as np
 import torch
 
 from . import _cabi
-from .algorithms import DimensionMismatch, _call, _check, _ptr, _require_tree, _stream, _torque_schedule, dynamics_
-from .pd import integrate_pd
+from .algorithms import DimensionMismatch, _call, _check, _ptr, _require_tree, _rollout, _steps, _stream, dynamics_
 from .state import DynamicsResult, MechanismState, _DT
 
 __all__ = ["HuntCrossleyModel", "hunt_crossley_hertz", "ViscoelasticCoulombModel", "SoftContactModel", "ContactPoint", "HalfSpace3D",
@@ -201,37 +200,6 @@ def dynamics_contact_(result: DynamicsResult, state: MechanismState, torques: Op
     return dynamics_(result, state, torques, tw, want_qd=want_qd)
 
 
-def _integrate_contact(state: MechanismState, nsteps: int, contact_state: Optional[torch.Tensor], torques, dt: float,
-                       contact: Optional[ContactDesc], record: bool, what: str, controller=None):
-    _require_tree(state, what)
-    state.check_modcount()
-    if nsteps < 0:
-        raise ValueError("nsteps must be >= 0")
-    lib = _cabi.load_library()
-    cd = contact if contact is not None else contact_desc(state.mechanism)
-    if contact_state is None and cd.nstates > 0:
-        raise ValueError(f"{what}: contact_state [{cd.nstates}, B] must be given (the mechanism has contact points)")
-    _check(contact_state, cd.nstates, state, "contact_state")
-    step = stage = 0
-    if torques is not None and torques.dim() in (3, 4):
-        step, stage = _torque_schedule(state, torques, nsteps)
-    else:
-        _check(torques, state.nv, state, "torques")
-    traj = (None, None, None)
-    if record:
-        new = lambda rows: torch.empty((nsteps + 1, rows, state.batch), dtype=state.dtype, device=state.q.device)   # noqa: E731
-        traj = (new(state.nq), new(state.nv), new(cd.nstates))
-    if controller is not None:
-        integrate_pd(state, controller, nsteps, torques, step, stage, dt, contact=cd, contact_state=contact_state, traj=traj, what=what)
-        return traj
-    st, keep = cd.c_struct()
-    _call(lib.rbd_integrate_contact(state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q), _ptr(state.v),
-                                    _ptr(contact_state), _ptr(torques), step, stage, ctypes.byref(st), float(dt), nsteps,
-                                    *[_ptr(t) for t in traj], _stream()))
-    del keep
-    return traj
-
-
 def simulate_contact_trajectory_(state: MechanismState, nsteps: int, contact_state: Optional[torch.Tensor],
                                  torques: Optional[torch.Tensor] = None, dt: float = 1e-4, contact: Optional[ContactDesc] = None, *,
                                  controller=None):
@@ -239,7 +207,10 @@ def simulate_contact_trajectory_(state: MechanismState, nsteps: int, contact_sta
     [nsteps + 1, nv, B] and [nsteps + 1, num_contact_states, B], block 0 the initial state and block s the state after step s.
     ``state`` and ``contact_state`` are advanced in place exactly as ``simulate_contact_`` advances them.  ``controller``: a
     ``JointPD`` evaluated at every stage, as in ``simulate_contact_`` (``torques`` is then its feedforward)."""
-    return _integrate_contact(state, nsteps, contact_state, torques, dt, contact, True, "simulate_contact_trajectory_", controller)
+    _require_tree(state, "simulate_contact_trajectory_")
+    cd = contact if contact is not None else contact_desc(state.mechanism)
+    return _rollout(state, nsteps, torques, dt, "simulate_contact_trajectory_", record=True, controller=controller, contact=cd,
+                    contact_state=contact_state)
 
 
 def simulate_contact_(state: MechanismState, final_time: float, contact_state: Optional[torch.Tensor],
@@ -254,9 +225,8 @@ def simulate_contact_(state: MechanismState, final_time: float, contact_state: O
     stage [nsteps, 4, nv, B], as for ``simulate_trajectory_``.  ``contact``: the mechanism's ``contact_desc`` by default.
     ``controller``: a ``JointPD`` evaluated at every stage, as in ``simulate_`` (its inverse dynamics, in computed-torque mode, sees
     no contact wrenches).  Returns the number of steps taken."""
-    nsteps, t = 0, 0.0
-    while t < final_time:            # the reference's `while t < final_time` loop (ode_integrators.jl:311)
-        t += dt
-        nsteps += 1
-    _integrate_contact(state, nsteps, contact_state, torques, dt, contact, False, "simulate_contact_", controller)
+    _require_tree(state, "simulate_contact_")
+    nsteps = _steps(final_time, dt)
+    cd = contact if contact is not None else contact_desc(state.mechanism)
+    _rollout(state, nsteps, torques, dt, "simulate_contact_", controller=controller, contact=cd, contact_state=contact_state)
     return nsteps

@@ -1043,20 +1043,6 @@ __global__ void __launch_bounds__(256) contact_finish_kernel(const ContactFinish
   }
 }
 
-// rbd_integrate_contact: the contact descriptor in device form and the caller's contact state s [ns x B] (leading dimension ld) with
-// its optional trajectory [(nsteps + 1) x ns x B].
-template <class T> struct ContactRollout {
-  const ContactDev<T>* C;         // NULL in the loop rollout (its stage kernel builds its own)
-  int64_t ns;
-  T* s; T* traj_s;
-};
-// rbd_integrate_loops: the loop descriptor and, with contact pairs, the contact descriptor, both in host form (rbd_loops.cu turns them
-// into device form once per call, loop_stage_launch).
-struct LoopRollout {
-  const rbd_loop_desc* desc;
-  const rbd_contact_desc* contact;
-};
-
 // Forward dynamics of one stage of the contact rollout: aba_contact_kernel in the variant dynamics_t would pick for the EXT path.
 template <class T>
 int contact_stage_launch(const HostModel& hm, const ModelDev<T>& M, const ContactDev<T>& C, ContactAbaArgs<T> a, cudaStream_t stream,
@@ -1076,38 +1062,42 @@ int contact_stage_launch(const HostModel& hm, const ModelDev<T>& M, const Contac
   return api_launched(&*plan);
 }
 
-// rbd_integrate_pd: the controller over the call (arguments checked by the caller).  Gains and references are caller arrays with
-// leading dimension ld; the references of step s start at s * qref_stride (q_ref) / s * vref_stride (v_ref, v̇_ref) elements.
-template <class T> struct PdRollout {
-  bool computed_torque;
-  const T* kp; const T* kd; int64_t g_ld;
-  const T* qref; const T* vref; const T* vdref; int64_t qref_stride, vref_stride;
-  const double* lo; const double* hi;      // host [nv] or NULL
-};
-
-// traj_q / traj_v (rbd_integrate_trajectory): [(nsteps + 1) x rows x B] -- block 0 the initial state, block s + 1 written by the
-// finishing kernels of step s; q / v receive the final state as without them.  stages (rbd_integrate_vjp's recompute, nsteps = 1):
-// the four stages' (qs_i, vs_i, φ̇_i, v̇_i) are kept in [4 nq + 12 nv] x B rows (stage_rows) and the finishing step is skipped; with
-// contact the four ṡ_i follow in 4 ns rows.
+// The RK4 driver of every rollout (rbd::integrate, rbd_handle.h).
+// Trajectories: block 0 the initial state, block s + 1 written by the finishing kernels of step s; q / v / s receive the final
+// state as without them.  stages (rbd_integrate_vjp's recompute, nsteps = 1): the four stages' (qs_i, vs_i, φ̇_i, v̇_i) are kept in
+// [4 nq + 12 nv] x B rows (stage_rows) and the finishing step is skipped; with contact the four ṡ_i follow in 4 ns rows.
 // contact (rbd_integrate_contact): every stage's dynamics is aba_contact_kernel, which also writes ṡ_i, and the finishing step
 // also advances the contact state (contact_finish_kernel); the q / v kernels are the same.
-// loop (rbd_integrate_loops): every stage's dynamics is rbd_loops.cu's KKT kernel (loop_stage_launch), with the contact pass when
-// loop->contact is set -- then `contact` carries s and its trajectory, and the finishing step is as above.
+// loops (rbd_integrate_loops): every stage's dynamics is rbd_loops.cu's KKT kernel (loop_stage_launch), with the contact pass when
+// there is contact, and the finishing step is as above.
 // pd (rbd_integrate_pd): the stage kernels also evaluate the feedback law on the stage state and write the stage's torques into the
 // taud rows, which the stage's dynamics (any of the three) reads in place of tau; τ_ff (tau and its strides) is read by the law.  In
 // computed-torque mode they write v̇_des into vd[i] instead (the dynamics overwrites it), and inverse_dynamics_t plus
-// pd_finish_kernel turn it into the torques.
+// pd_finish_kernel turn it into the torques.  Gains and references are caller arrays with leading dimension ld.
 template <class T>
-int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v, const void* tau, int64_t step_stride,
-                int64_t stage_stride, double dt, int nsteps, cudaStream_t stream, T* traj_q = nullptr, T* traj_v = nullptr,
-                T* stages = nullptr, const ContactRollout<T>* contact = nullptr, const LoopRollout* loop = nullptr,
-                const PdRollout<T>* pd = nullptr) {
+int integrate_t(const rbd_model* model, int64_t B, int64_t ld, const Rollout& r, cudaStream_t stream) {
   const HostModel& hm = model->hm;
   const ModelDev<T>& M = dev_model<T>(hm);
   DeviceProps p;
   RBD_CUDA_TRY(device_props(p));
   const size_t nq = hm.nq, nv = hm.nv;
-  const size_t ns = contact ? (size_t)contact->ns : 0;
+  void* const q = r.q; void* const v = r.v;
+  const void* tau = r.tau;
+  const int64_t step_stride = r.tau_step_stride, stage_stride = r.tau_stage_stride;
+  const double dt = r.dt;
+  const int nsteps = r.nsteps;
+  T *traj_q = (T*)r.q_traj, *traj_v = (T*)r.v_traj, *traj_s = (T*)r.s_traj, *stages = (T*)r.stages;
+  const rbd_pd_desc* pd = r.pd;
+  const bool computed_torque = pd && pd->mode == RBD_PD_COMPUTED_TORQUE;
+  const rbd_contact_desc* cd = r.contact;
+  const size_t ns = cd ? (size_t)3 * cd->npoints * cd->nhalfspaces : 0;
+  // the contact rollout's descriptor in device form, passed by value to every stage's launch (the loop rollout's stage kernel
+  // builds its own)
+  std::unique_ptr<ContactDev<T>> C;
+  if (cd && !r.loops) {
+    C.reset(new ContactDev<T>());
+    build_contact_dev<T>(hm.nb, hm.pos.data(), hm.alignT.data(), *cd, *C);
+  }
   const size_t rows = 2 * nq + 10 * nv + (pd || (tau && ld != B) ? nv : 0);
   StreamAlloc work, swork;
   RBD_CUDA_TRY(work.alloc((rows * (size_t)B + (pd ? 2 * nv : 0)) * sizeof(T), stream));
@@ -1120,8 +1110,8 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
     RBD_CUDA_TRY(swork.alloc(5 * ns * (size_t)B * sizeof(T), stream));
     s0 = (T*)swork.p;
     for (int i = 0; i < 4; ++i) sd[i] = s0 + (1 + (size_t)i) * ns * B;
-    RBD_CUDA_TRY(cudaMemcpy2DAsync(s0, B * sizeof(T), contact->s, ld * sizeof(T), B * sizeof(T), ns, cudaMemcpyDeviceToDevice, stream));
-    if (contact->traj_s) RBD_CUDA_TRY(cudaMemcpyAsync(contact->traj_s, s0, ns * B * sizeof(T), cudaMemcpyDeviceToDevice, stream));
+    RBD_CUDA_TRY(cudaMemcpy2DAsync(s0, B * sizeof(T), r.s, ld * sizeof(T), B * sizeof(T), ns, cudaMemcpyDeviceToDevice, stream));
+    if (traj_s) RBD_CUDA_TRY(cudaMemcpyAsync(traj_s, s0, ns * B * sizeof(T), cudaMemcpyDeviceToDevice, stream));
   }
   T* q0 = (T*)work.p; T* qs = q0 + nq * B; T* v0 = qs + nq * B; T* vs = v0 + nv * B;
   T* phid[4]; T* vd[4];
@@ -1146,9 +1136,9 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
   // the controller's saturation bounds on the device, behind the workspace rows (copied from pageable memory: staged before return)
   const T* pd_lo = nullptr;
   const T* pd_hi = nullptr;
-  if (pd && pd->lo) {
+  if (pd && pd->effort_lo) {
     std::vector<T> bounds(2 * nv);
-    for (size_t k = 0; k < nv; ++k) { bounds[k] = (T)pd->lo[k]; bounds[nv + k] = (T)pd->hi[k]; }
+    for (size_t k = 0; k < nv; ++k) { bounds[k] = (T)pd->effort_lo[k]; bounds[nv + k] = (T)pd->effort_hi[k]; }
     T* dev = (T*)work.p + rows * (size_t)B;
     RBD_CUDA_TRY(cudaMemcpyAsync(dev, bounds.data(), 2 * nv * sizeof(T), cudaMemcpyHostToDevice, stream));
     pd_lo = dev; pd_hi = dev + nv;
@@ -1166,9 +1156,9 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
   auto vec_aligned = [&](const void* a, int64_t stride) {
     return !a || (((uintptr_t)a % sizeof(typename VecOf<T>::type)) == 0 && stride % VecOf<T>::N == 0);
   };
-  const bool vec_stage = vec_ok && (!pd || (ld % VecOf<T>::N == 0 && vec_aligned(pd->qref, pd->qref_stride) &&
-                                            vec_aligned(pd->vref, pd->vref_stride) && vec_aligned(pd->vdref, pd->vref_stride) &&
-                                            (pd->g_ld == 0 || (vec_aligned(pd->kp, 0) && vec_aligned(pd->kd, 0))) &&
+  const bool vec_stage = vec_ok && (!pd || (ld % VecOf<T>::N == 0 && vec_aligned(pd->q_ref, pd->q_ref_step_stride) &&
+                                            vec_aligned(pd->v_ref, pd->v_ref_step_stride) && vec_aligned(pd->vd_ref, pd->v_ref_step_stride) &&
+                                            (pd->gain_ld == 0 || (vec_aligned(pd->kp, 0) && vec_aligned(pd->kd, 0))) &&
                                             vec_aligned(tau, step_stride) && vec_aligned(tau, stage_stride)));
   // ... and, for the finishing kernel, vector-aligned rows of the caller's arrays too
   const bool vec_user = vec_ok && ldo % VecOf<T>::N == 0 && ((uintptr_t)qout % sizeof(typename VecOf<T>::type)) == 0 &&
@@ -1193,13 +1183,14 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
         }
       }
       StageArgs<T> sa{q0, v0, i ? phid[i - 1] : nullptr, i ? vd[i - 1] : nullptr, phid[i], qsi[i], vsi[i], (T)(dt * a[i]), B, vec_stage};
-      if (pd) {
-        const T* qref = pd->qref + (size_t)s * pd->qref_stride;
-        const size_t r = (size_t)s * pd->vref_stride;
-        const T* vref = pd->vref ? pd->vref + r : nullptr;
-        sa.pd = pd->computed_torque ? PdStage<T>{qref, vref, pd->vdref ? pd->vdref + r : nullptr, pd->kp, pd->kd, pd->g_ld, nullptr,
-                                                 nullptr, vd[i], ld}
-                                    : PdStage<T>{qref, vref, tau_at(s, i), pd->kp, pd->kd, pd->g_ld, pd_lo, pd_hi, taud, ld};
+      if (pd) {     // the references of step s start at s * q_ref_step_stride (q_ref) / s * v_ref_step_stride (v_ref, v̇_ref)
+        const T* qref = (const T*)pd->q_ref + (size_t)s * pd->q_ref_step_stride;
+        const size_t o = (size_t)s * pd->v_ref_step_stride;
+        const T* vref = pd->v_ref ? (const T*)pd->v_ref + o : nullptr;
+        const T *kp = (const T*)pd->kp, *kd = (const T*)pd->kd;
+        sa.pd = computed_torque ? PdStage<T>{qref, vref, pd->vd_ref ? (const T*)pd->vd_ref + o : nullptr, kp, kd, pd->gain_ld, nullptr,
+                                             nullptr, vd[i], ld}
+                                : PdStage<T>{qref, vref, tau_at(s, i), kp, kd, pd->gain_ld, pd_lo, pd_hi, taud, ld};
       }
       if (vec_stage) {     // revolute / prismatic rows, VEC samples per thread
         integrate_stage_linear_kernel<T><<<dim3(grid_lin, hm.nb), 256, 0, stream>>>(M, sa);
@@ -1209,19 +1200,18 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
         integrate_stage_kernel<T><<<dim3(grid, hm.nb), 128, 0, stream>>>(M, sa);
         if (int rc = api_launched()) return rc;
       }
-      if (pd && pd->computed_torque) {     // tau = clamp(ID(q_s, v_s, v̇_des) + τ_ff), without contact wrenches
+      if (computed_torque) {     // tau = clamp(ID(q_s, v_s, v̇_des) + τ_ff), without contact wrenches
         if (int rc = inverse_dynamics_t<T>(model, B, B, qsi[i], vsi[i], vd[i], nullptr, taud, stream)) return rc;
         const PdFinishArgs<T> pf{taud, tau_at(s, i), ld, pd_lo, pd_hi, (int64_t)nv, B};
         pd_finish_kernel<T><<<(int)std::min<int64_t>(((int64_t)nv * B + 255) / 256, (int64_t)p.sms * 8), 256, 0, stream>>>(pf);
         if (int rc = api_launched()) return rc;
       }
-      if (loop) {
+      if (r.loops) {
         const LoopStageArgs la{qsi[i], vsi[i], tau_dense, s0, i ? sd[i - 1] : nullptr, sd[i], vd[i], dt * a[i], B};
-        if (int rc = loop_stage_launch(model, sizeof(T) == 8 ? RBD_F64 : RBD_F32, *loop->desc, loop->contact, la, loop_plan, stream))
-          return rc;
-      } else if (contact) {
+        if (int rc = loop_stage_launch(model, sizeof(T) == 8 ? RBD_F64 : RBD_F32, *r.loops, cd, la, loop_plan, stream)) return rc;
+      } else if (C) {
         const ContactAbaArgs<T> ca{qsi[i], vsi[i], tau_dense, s0, i ? sd[i - 1] : nullptr, vd[i], sd[i], nullptr, (T)(dt * a[i]), B};
-        if (int rc = contact_stage_launch<T>(hm, M, *contact->C, ca, stream, contact_plan)) return rc;
+        if (int rc = contact_stage_launch<T>(hm, M, *C, ca, stream, contact_plan)) return rc;
       } else if (int rc = dynamics_t<T>(model, B, B, qsi[i], vsi[i], tau_dense, nullptr, vd[i], nullptr, stream)) {
         return rc;
       }
@@ -1240,8 +1230,8 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
       if (int rc = api_launched()) return rc;
     }
     if (ns) {
-      const bool rec = contact->traj_s != nullptr;
-      const ContactFinishArgs<T> cf{s0, {sd[0], sd[1], sd[2], sd[3]}, rec ? contact->traj_s + (size_t)(s + 1) * ns * B : contact->s,
+      const bool rec = traj_s != nullptr;
+      const ContactFinishArgs<T> cf{s0, {sd[0], sd[1], sd[2], sd[3]}, rec ? traj_s + (size_t)(s + 1) * ns * B : (T*)r.s,
                                     {(T)bw[0], (T)bw[1], (T)bw[2], (T)bw[3]}, (T)dt, B, rec ? B : ld, (int64_t)ns, s + 1 < nsteps};
       const int grid_s = (int)std::min<int64_t>(((int64_t)ns * B + 255) / 256, (int64_t)p.sms * 8);
       contact_finish_kernel<T><<<grid_s, 256, 0, stream>>>(cf);
@@ -1254,9 +1244,9 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v,
     RBD_CUDA_TRY(cudaMemcpy2DAsync(v, ld * sizeof(T), traj_v + (size_t)nsteps * nv * B, B * sizeof(T), B * sizeof(T), nv,
                                    cudaMemcpyDeviceToDevice, stream));
   }
-  if (ns && contact->traj_s && nsteps > 0)
-    RBD_CUDA_TRY(cudaMemcpy2DAsync(contact->s, ld * sizeof(T), contact->traj_s + (size_t)nsteps * ns * B, B * sizeof(T), B * sizeof(T),
-                                   ns, cudaMemcpyDeviceToDevice, stream));
+  if (ns && traj_s && nsteps > 0)
+    RBD_CUDA_TRY(cudaMemcpy2DAsync(r.s, ld * sizeof(T), traj_s + (size_t)nsteps * ns * B, B * sizeof(T), B * sizeof(T), ns,
+                                   cudaMemcpyDeviceToDevice, stream));
   return RBD_OK;
 }
 
@@ -1373,17 +1363,6 @@ int task_t(const rbd_model* model, int64_t B, int64_t ld, const void* q, const v
   return api_launched(&pl);
 }
 
-template <class T>
-int integrate_contact_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau, int64_t step_stride,
-                        int64_t stage_stride, const rbd_contact_desc& cd, double dt, int nsteps, void* q_traj, void* v_traj, void* s_traj,
-                        cudaStream_t stream, T* stages = nullptr) {
-  const HostModel& hm = model->hm;
-  std::unique_ptr<ContactDev<T>> C(new ContactDev<T>());     // passed by value to every stage's launch
-  build_contact_dev<T>(hm.nb, hm.pos.data(), hm.alignT.data(), cd, *C);
-  const ContactRollout<T> cr{C.get(), (int64_t)3 * cd.npoints * cd.nhalfspaces, (T*)s, (T*)s_traj};
-  return integrate_t<T>(model, B, ld, q, v, tau, step_stride, stage_stride, dt, nsteps, stream, (T*)q_traj, (T*)v_traj, stages, &cr);
-}
-
 // the descriptor checks of rbd_contact_dynamics and rbd_integrate_contact
 int check_contact(const rbd_model* model, const rbd_contact_desc* contact, const char* fn) {
   const std::string f = fn;
@@ -1415,69 +1394,44 @@ int check_common(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, b
   return RBD_OK;
 }
 
+// The argument checks of the rollout entry points (fn: the entry point named in the messages); each entry point adds the checks
+// of the argument that names it.  RBD_OK also when there is nothing to compute.  The rollouts with a descriptor (contact, loops,
+// controller) report every dtype but fp32 / fp64 as unsupported, and check q, v and s even when they take no step.
+int check_rollout(const char* fn, const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const Rollout& r) {
+  const std::string f = fn;
+  const bool described = r.contact || r.loops || r.pd;
+  if (!model) return fail(RBD_EINVAL, "model handle is NULL");
+  if (described && dtype != RBD_F32 && dtype != RBD_F64) return fail(RBD_EUNSUPPORTED, f + ": fp32 / fp64 only");
+  if (int rc = check_common(model, dtype, B, ld)) return rc;
+  if (r.nsteps < 0 || !(r.dt > 0)) return fail(RBD_EINVAL, f + ": need dt > 0 and nsteps >= 0");
+  if (r.tau_step_stride < 0 || r.tau_stage_stride < 0) return fail(RBD_EINVAL, f + ": torque strides must be >= 0");
+  if (r.loops)
+    if (int rc = api_check_loops(model, r.loops)) return rc;
+  if (r.contact)
+    if (int rc = check_contact(model, r.contact, fn)) return rc;
+  const int64_t ns = r.contact ? (int64_t)3 * r.contact->npoints * r.contact->nhalfspaces : 0;
+  const bool rec = r.q_traj || r.v_traj || r.s_traj;
+  if (rec && (!r.q_traj || !r.v_traj || (ns > 0 && !r.s_traj)))
+    return fail(RBD_EINVAL, f + ": q_traj, v_traj and s_traj must be all NULL or all set");
+  if (B == 0 || (r.nsteps == 0 && !rec && !described)) return RBD_OK;
+  if (!r.q || !r.v) return fail(RBD_EINVAL, f + ": q and v must not be NULL");
+  if (ns > 0 && !r.s) return fail(RBD_EINVAL, f + ": s must not be NULL when there are contact pairs");
+  return RBD_OK;
+}
+
 }  // namespace
 
 // hooks for the other translation units of the library: argument checks, the RK4 driver
 namespace rbd {
 int api_check(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld) { return check_common(model, dtype, B, ld); }
 int api_check_contact(const rbd_model* model, const rbd_contact_desc* contact, const char* fn) { return check_contact(model, contact, fn); }
-int integrate_record(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, const void* tau, int64_t step_stride,
-                     int64_t stage_stride, double dt, int nsteps, void* q_traj, void* v_traj, void* stages, cudaStream_t stream,
-                     const rbd_contact_desc* contact, void* s) {
-  if (contact)
-    return dtype == RBD_F32 ? integrate_contact_t<float>(model, B, ld, q, v, s, tau, step_stride, stage_stride, *contact, dt, nsteps, q_traj,
-                                                         v_traj, nullptr, stream, (float*)stages)
-                            : integrate_contact_t<double>(model, B, ld, q, v, s, tau, step_stride, stage_stride, *contact, dt, nsteps, q_traj,
-                                                          v_traj, nullptr, stream, (double*)stages);
-  return dtype == RBD_F32 ? integrate_t<float>(model, B, ld, q, v, tau, step_stride, stage_stride, dt, nsteps, stream, (float*)q_traj,
-                                               (float*)v_traj, (float*)stages)
-                          : integrate_t<double>(model, B, ld, q, v, tau, step_stride, stage_stride, dt, nsteps, stream, (double*)q_traj,
-                                                (double*)v_traj, (double*)stages);
-}
-template <class T>
-static int integrate_loops_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau, int64_t step_stride,
-                             int64_t stage_stride, const rbd_loop_desc& loops, const rbd_contact_desc* contact, double dt, int nsteps,
-                             void* q_traj, void* v_traj, void* s_traj, cudaStream_t stream) {
-  const LoopRollout lr{&loops, contact};
-  const ContactRollout<T> cr{nullptr, contact ? (int64_t)3 * contact->npoints * contact->nhalfspaces : 0, (T*)s, (T*)s_traj};
-  return integrate_t<T>(model, B, ld, q, v, tau, step_stride, stage_stride, dt, nsteps, stream, (T*)q_traj, (T*)v_traj, nullptr,
-                        contact ? &cr : nullptr, &lr);
-}
-int integrate_loops(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau,
-                    int64_t step_stride, int64_t stage_stride, const rbd_loop_desc& loops, const rbd_contact_desc* contact, double dt,
-                    int nsteps, void* q_traj, void* v_traj, void* s_traj, cudaStream_t stream) {
-  return dtype == RBD_F32 ? integrate_loops_t<float>(model, B, ld, q, v, s, tau, step_stride, stage_stride, loops, contact, dt, nsteps,
-                                                     q_traj, v_traj, s_traj, stream)
-                          : integrate_loops_t<double>(model, B, ld, q, v, s, tau, step_stride, stage_stride, loops, contact, dt, nsteps,
-                                                      q_traj, v_traj, s_traj, stream);
+int integrate(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const Rollout& r, cudaStream_t stream) {
+  if (B == 0 || (r.nsteps == 0 && !r.q_traj)) return RBD_OK;
+  Rollout n = r;
+  if (n.loops && n.contact && n.contact->npoints * n.contact->nhalfspaces == 0) n.contact = nullptr;
+  return dtype == RBD_F32 ? integrate_t<float>(model, B, ld, n, stream) : integrate_t<double>(model, B, ld, n, stream);
 }
 }  // namespace rbd
-
-namespace {
-template <class T>
-int integrate_pd_t(const rbd_model* model, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau, int64_t step_stride,
-                   int64_t stage_stride, const rbd_pd_desc& d, const rbd_loop_desc* loops, const rbd_contact_desc* contact, double dt,
-                   int nsteps, void* q_traj, void* v_traj, void* s_traj, cudaStream_t stream) {
-  const PdRollout<T> pd{d.mode == RBD_PD_COMPUTED_TORQUE, (const T*)d.kp, (const T*)d.kd, d.gain_ld, (const T*)d.q_ref,
-                        (const T*)d.v_ref, (const T*)d.vd_ref, d.q_ref_step_stride, d.v_ref_step_stride, d.effort_lo, d.effort_hi};
-  const int64_t ns = contact ? (int64_t)3 * contact->npoints * contact->nhalfspaces : 0;
-  if (loops) {
-    const LoopRollout lr{loops, contact};
-    const ContactRollout<T> cr{nullptr, ns, (T*)s, (T*)s_traj};
-    return integrate_t<T>(model, B, ld, q, v, tau, step_stride, stage_stride, dt, nsteps, stream, (T*)q_traj, (T*)v_traj, nullptr,
-                          contact ? &cr : nullptr, &lr, &pd);
-  }
-  if (contact) {
-    std::unique_ptr<ContactDev<T>> C(new ContactDev<T>());
-    build_contact_dev<T>(model->hm.nb, model->hm.pos.data(), model->hm.alignT.data(), *contact, *C);
-    const ContactRollout<T> cr{C.get(), ns, (T*)s, (T*)s_traj};
-    return integrate_t<T>(model, B, ld, q, v, tau, step_stride, stage_stride, dt, nsteps, stream, (T*)q_traj, (T*)v_traj, nullptr, &cr,
-                          nullptr, &pd);
-  }
-  return integrate_t<T>(model, B, ld, q, v, tau, step_stride, stage_stride, dt, nsteps, stream, (T*)q_traj, (T*)v_traj, nullptr, nullptr,
-                        nullptr, &pd);
-}
-}  // namespace
 
 // ------------------------------------------------------------------------------------------------------------------
 // C ABI
@@ -1742,15 +1696,10 @@ int32_t rbd_dynamics_gather(const rbd_model* model, int32_t dtype, int64_t B, in
 
 int32_t rbd_integrate_schedule(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, const void* tau,
                                int64_t tau_step_stride, int64_t tau_stage_stride, double dt, int32_t nsteps, void* stream) {
-  if (int rc = check_common(model, dtype, B, ld)) return rc;
-  if (nsteps < 0 || !(dt > 0)) return fail(RBD_EINVAL, "rbd_integrate: need dt > 0 and nsteps >= 0");
-  if (tau_step_stride < 0 || tau_stage_stride < 0) return fail(RBD_EINVAL, "rbd_integrate: torque strides must be >= 0");
+  const Rollout r{q, v, nullptr, tau, tau_step_stride, tau_stage_stride, dt, nsteps};
+  if (int rc = check_rollout("rbd_integrate", model, dtype, B, ld, r)) return rc;
   const ApiCall call;
-  if (B == 0 || nsteps == 0) return RBD_OK;
-  if (!q || !v) return fail(RBD_EINVAL, "rbd_integrate: q and v must not be NULL");
-  cudaStream_t s = (cudaStream_t)stream;
-  return dtype == RBD_F32 ? integrate_t<float>(model, B, ld, q, v, tau, tau_step_stride, tau_stage_stride, dt, nsteps, s)
-                          : integrate_t<double>(model, B, ld, q, v, tau, tau_step_stride, tau_stage_stride, dt, nsteps, s);
+  return rbd::integrate(model, dtype, B, ld, r, (cudaStream_t)stream);
 }
 
 int32_t rbd_integrate(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, const void* tau,
@@ -1761,14 +1710,13 @@ int32_t rbd_integrate(const rbd_model* model, int32_t dtype, int64_t B, int64_t 
 int32_t rbd_integrate_trajectory(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, const void* tau,
                                  int64_t tau_step_stride, int64_t tau_stage_stride, double dt, int32_t nsteps, void* q_traj,
                                  void* v_traj, void* stream) {
-  if (int rc = check_common(model, dtype, B, ld)) return rc;
-  if (nsteps < 0 || !(dt > 0)) return fail(RBD_EINVAL, "rbd_integrate_trajectory: need dt > 0 and nsteps >= 0");
-  if (tau_step_stride < 0 || tau_stage_stride < 0) return fail(RBD_EINVAL, "rbd_integrate_trajectory: torque strides must be >= 0");
+  // both trajectories are required, except by an empty batch: only a full set goes to the shared checks
+  const bool rec = q_traj && v_traj;
+  const Rollout r{q, v, nullptr, tau, tau_step_stride, tau_stage_stride, dt, nsteps, rec ? q_traj : nullptr, rec ? v_traj : nullptr};
+  if (int rc = check_rollout("rbd_integrate_trajectory", model, dtype, B, ld, r)) return rc;
+  if (B > 0 && !rec) return fail(RBD_EINVAL, "rbd_integrate_trajectory: q_traj and v_traj must not be NULL");
   const ApiCall call;
-  if (B == 0) return RBD_OK;
-  if (!q || !v || !q_traj || !v_traj) return fail(RBD_EINVAL, "rbd_integrate_trajectory: q, v, q_traj and v_traj must not be NULL");
-  return rbd::integrate_record(model, dtype, B, ld, q, v, tau, tau_step_stride, tau_stage_stride, dt, nsteps, q_traj, v_traj, nullptr,
-                               (cudaStream_t)stream);
+  return rbd::integrate(model, dtype, B, ld, r, (cudaStream_t)stream);
 }
 
 int32_t rbd_inverse_dynamics(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q,
@@ -1808,37 +1756,29 @@ int32_t rbd_contact_dynamics(const rbd_model* model, int32_t dtype, int64_t B, i
 int32_t rbd_integrate_contact(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau,
                               int64_t tau_step_stride, int64_t tau_stage_stride, const rbd_contact_desc* contact, double dt, int32_t nsteps,
                               void* q_traj, void* v_traj, void* s_traj, void* stream) {
-  if (!model) return fail(RBD_EINVAL, "model handle is NULL");
-  if (dtype != RBD_F32 && dtype != RBD_F64) return fail(RBD_EUNSUPPORTED, "rbd_integrate_contact: fp32 / fp64 only");
-  if (int rc = check_common(model, dtype, B, ld)) return rc;
-  if (nsteps < 0 || !(dt > 0)) return fail(RBD_EINVAL, "rbd_integrate_contact: need dt > 0 and nsteps >= 0");
-  if (tau_step_stride < 0 || tau_stage_stride < 0) return fail(RBD_EINVAL, "rbd_integrate_contact: torque strides must be >= 0");
-  if (int rc = check_contact(model, contact, "rbd_integrate_contact")) return rc;
-  const int64_t ns = (int64_t)3 * contact->npoints * contact->nhalfspaces;
-  const bool rec = q_traj || v_traj || s_traj;
-  if (rec && (!q_traj || !v_traj || (ns > 0 && !s_traj)))
-    return fail(RBD_EINVAL, "rbd_integrate_contact: q_traj, v_traj and s_traj must be all NULL or all set");
+  const Rollout r{q, v, s, tau, tau_step_stride, tau_stage_stride, dt, nsteps, q_traj, v_traj, s_traj, nullptr, contact};
+  if (int rc = check_rollout("rbd_integrate_contact", model, dtype, B, ld, r)) return rc;
+  if (!contact) return fail(RBD_EINVAL, "rbd_integrate_contact: contact must not be NULL");
   const ApiCall call;
-  if (B == 0) return RBD_OK;
-  if (!q || !v) return fail(RBD_EINVAL, "rbd_integrate_contact: q and v must not be NULL");
-  if (ns > 0 && !s) return fail(RBD_EINVAL, "rbd_integrate_contact: s must not be NULL when there are contact pairs");
-  if (nsteps == 0 && !rec) return RBD_OK;
-  cudaStream_t st = (cudaStream_t)stream;
-  return dtype == RBD_F32 ? integrate_contact_t<float>(model, B, ld, q, v, s, tau, tau_step_stride, tau_stage_stride, *contact, dt, nsteps,
-                                                       q_traj, v_traj, s_traj, st)
-                          : integrate_contact_t<double>(model, B, ld, q, v, s, tau, tau_step_stride, tau_stage_stride, *contact, dt, nsteps,
-                                                        q_traj, v_traj, s_traj, st);
+  return rbd::integrate(model, dtype, B, ld, r, (cudaStream_t)stream);
+}
+
+int32_t rbd_integrate_loops(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau,
+                            int64_t tau_step_stride, int64_t tau_stage_stride, const rbd_loop_desc* loops, const rbd_contact_desc* contact,
+                            double dt, int32_t nsteps, void* q_traj, void* v_traj, void* s_traj, void* stream) {
+  const Rollout r{q, v, s, tau, tau_step_stride, tau_stage_stride, dt, nsteps, q_traj, v_traj, s_traj, nullptr, contact, loops};
+  if (int rc = check_rollout("rbd_integrate_loops", model, dtype, B, ld, r)) return rc;
+  if (!loops) return fail(RBD_EINVAL, "rbd_integrate_loops: loops must not be NULL");
+  const ApiCall call;
+  return rbd::integrate(model, dtype, B, ld, r, (cudaStream_t)stream);
 }
 
 int32_t rbd_integrate_pd(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau,
                          int64_t tau_step_stride, int64_t tau_stage_stride, const rbd_pd_desc* pd, const rbd_loop_desc* loops,
                          const rbd_contact_desc* contact, double dt, int32_t nsteps, void* q_traj, void* v_traj, void* s_traj,
                          void* stream) {
-  if (!model) return fail(RBD_EINVAL, "model handle is NULL");
-  if (dtype != RBD_F32 && dtype != RBD_F64) return fail(RBD_EUNSUPPORTED, "rbd_integrate_pd: fp32 / fp64 only");
-  if (int rc = check_common(model, dtype, B, ld)) return rc;
-  if (nsteps < 0 || !(dt > 0)) return fail(RBD_EINVAL, "rbd_integrate_pd: need dt > 0 and nsteps >= 0");
-  if (tau_step_stride < 0 || tau_stage_stride < 0) return fail(RBD_EINVAL, "rbd_integrate_pd: torque strides must be >= 0");
+  const Rollout r{q, v, s, tau, tau_step_stride, tau_stage_stride, dt, nsteps, q_traj, v_traj, s_traj, nullptr, contact, loops, pd};
+  if (int rc = check_rollout("rbd_integrate_pd", model, dtype, B, ld, r)) return rc;
   if (!pd) return fail(RBD_EINVAL, "rbd_integrate_pd: pd must not be NULL");
   if (!pd->kp || !pd->kd || !pd->q_ref) return fail(RBD_EINVAL, "rbd_integrate_pd: kp, kd and q_ref must not be NULL");
   if (pd->mode != RBD_PD_TORQUE && pd->mode != RBD_PD_COMPUTED_TORQUE) return fail(RBD_EINVAL, "rbd_integrate_pd: unknown mode");
@@ -1849,28 +1789,10 @@ int32_t rbd_integrate_pd(const rbd_model* model, int32_t dtype, int64_t B, int64
   if (pd->effort_lo)
     for (int k = 0; k < model->hm.nv; ++k)
       if (!(pd->effort_lo[k] <= pd->effort_hi[k])) return fail(RBD_EINVAL, "rbd_integrate_pd: effort bounds need lo <= hi");
-  if (loops) {
-    if (int rc = api_check_loops(model, loops)) return rc;
-    if (pd->mode == RBD_PD_COMPUTED_TORQUE && loops->nloops > 0)
-      return fail(RBD_ELOOP, "rbd_integrate_pd: computed-torque mode needs inverse_dynamics!, which has no kinematic loops");
-  }
-  if (contact)
-    if (int rc = check_contact(model, contact, "rbd_integrate_pd")) return rc;
-  const int64_t ns = contact ? (int64_t)3 * contact->npoints * contact->nhalfspaces : 0;
-  const bool rec = q_traj || v_traj || s_traj;
-  if (rec && (!q_traj || !v_traj || (ns > 0 && !s_traj)))
-    return fail(RBD_EINVAL, "rbd_integrate_pd: q_traj, v_traj and s_traj must be all NULL or all set");
+  if (pd->mode == RBD_PD_COMPUTED_TORQUE && loops && loops->nloops > 0)
+    return fail(RBD_ELOOP, "rbd_integrate_pd: computed-torque mode needs inverse_dynamics!, which has no kinematic loops");
   const ApiCall call;
-  if (B == 0) return RBD_OK;
-  if (!q || !v) return fail(RBD_EINVAL, "rbd_integrate_pd: q and v must not be NULL");
-  if (ns > 0 && !s) return fail(RBD_EINVAL, "rbd_integrate_pd: s must not be NULL when there are contact pairs");
-  if (nsteps == 0 && !rec) return RBD_OK;
-  const rbd_contact_desc* c = ns > 0 || !loops ? contact : nullptr;     // the loop rollout takes contact only with pairs
-  cudaStream_t st = (cudaStream_t)stream;
-  return dtype == RBD_F32 ? integrate_pd_t<float>(model, B, ld, q, v, s, tau, tau_step_stride, tau_stage_stride, *pd, loops, c, dt, nsteps,
-                                                  q_traj, v_traj, s_traj, st)
-                          : integrate_pd_t<double>(model, B, ld, q, v, s, tau, tau_step_stride, tau_stage_stride, *pd, loops, c, dt,
-                                                   nsteps, q_traj, v_traj, s_traj, st);
+  return rbd::integrate(model, dtype, B, ld, r, (cudaStream_t)stream);
 }
 
 int32_t rbd_dynamics_result(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,

@@ -153,18 +153,27 @@ struct KeepLaunchRecord {
 struct LaunchPlan : LaunchShape { StreamAlloc work; };
 int plan_persistent(const void* kernel, int block, size_t smem, int64_t ngroups, cudaStream_t stream, LaunchPlan& plan,
                     size_t work_per_thread = 0, size_t work_extra = 0, size_t work_cap = 0);
-// rbd_b200.cu's RK4 driver for rbd_integrate_trajectory (q_traj / v_traj) and rbd_integrate_vjp's recompute (stages: one step,
-// its four stages kept in stage_rows(nq, nv) x B rows, no finishing step).  With `contact` it is the contact rollout from state s
-// (rbd_integrate_contact), and the recompute keeps the four ṡ_i in 4 ns more rows.  fp32 / fp64, arguments checked by the caller.
+// One request to rbd_b200.cu's RK4 driver, in the form the C entry points receive it (include/rbd_b200.h).  q, v and the contact
+// state s are [rows x B] with leading dimension ld; the torques of (step s, stage i) start at tau + s * tau_step_stride +
+// i * tau_stage_stride (NULL: zero).
+struct Rollout {
+  void* q; void* v; void* s;
+  const void* tau;
+  int64_t tau_step_stride, tau_stage_stride;
+  double dt;
+  int nsteps;
+  void* q_traj = nullptr; void* v_traj = nullptr; void* s_traj = nullptr;   // [(nsteps + 1) x rows x B] each, or all NULL
+  void* stages = nullptr;                      // rbd_integrate_vjp's recompute, see stage_rows
+  const rbd_contact_desc* contact = nullptr;   // the contact rollout, or the loop rollout's contact pass
+  const rbd_loop_desc* loops = nullptr;        // every stage's dynamics is the KKT solve (loop_stage_launch)
+  const rbd_pd_desc* pd = nullptr;             // feedback evaluated at every stage
+};
+// The recompute of one step (nsteps = 1, ld = B) keeps its four stages in stage_rows(nq, nv) x B rows of `stages` (4 ns more with
+// contact, for the ṡ_i) and skips the finishing step.
 inline int64_t stage_rows(int64_t nq, int64_t nv) { return 4 * nq + 12 * nv; }
-int integrate_record(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, const void* tau, int64_t step_stride,
-                     int64_t stage_stride, double dt, int nsteps, void* q_traj, void* v_traj, void* stages, cudaStream_t stream,
-                     const rbd_contact_desc* contact = nullptr, void* s = nullptr);
-// The same driver for rbd_integrate_loops (arguments checked by the caller; contact NULL or with ns > 0): every stage's dynamics is
-// loop_stage_launch, and with contact the finishing step also advances s as in rbd_integrate_contact.
-int integrate_loops(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau,
-                    int64_t step_stride, int64_t stage_stride, const rbd_loop_desc& loops, const rbd_contact_desc* contact, double dt,
-                    int nsteps, void* q_traj, void* v_traj, void* s_traj, cudaStream_t stream);
+// Runs the rollout (fp32 / fp64, arguments checked by the caller).  RBD_OK at once when B == 0, or when nsteps == 0 and nothing is
+// recorded.  The loop rollout takes its contact pass only when there are contact pairs.
+int integrate(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const Rollout& r, cudaStream_t stream);
 // rbd_loops.cu's forward dynamics of one stage of the loop rollout: v̇ = the KKT solve of rbd_dynamics_loops at the stage state
 // (q, v) with torques tau (NULL: zero), every array [rows x B] dense.  With `contact` (ns > 0) the contact pass runs first in the
 // same kernel at the stage state s0 + wa ṡ_prev (ṡ_prev NULL at stage 0), writes ṡ and feeds its wrenches to the solve.  `plan`

@@ -218,9 +218,11 @@ int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q
     const T* q0 = q_traj + (size_t)s * nq * B;
     const T* v0 = v_traj + (size_t)s * nv * B;
     const T* s0 = contact ? contact->s_traj + (size_t)s * ns * B : nullptr;
-    if (int rc = integrate_record(model, dtype, B, B, const_cast<T*>(q0), const_cast<T*>(v0), tau ? tau + s * step_stride : nullptr,
-                                  step_stride, stage_stride, dt, 1, nullptr, nullptr, stages, stream, contact ? contact->cd : nullptr,
-                                  const_cast<T*>(s0))) return rc;
+    Rollout r{const_cast<T*>(q0), const_cast<T*>(v0), const_cast<T*>(s0), tau ? tau + s * step_stride : nullptr, step_stride,
+              stage_stride, dt, 1};
+    r.stages = stages;
+    r.contact = contact ? contact->cd : nullptr;
+    if (int rc = integrate(model, dtype, B, B, r, stream)) return rc;
     a.q0 = q0;
     a.qtb = qtb ? qtb + (size_t)s * nq * B : nullptr;
     a.vtb = vtb ? vtb + (size_t)s * nv * B : nullptr;

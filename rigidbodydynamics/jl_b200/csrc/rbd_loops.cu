@@ -1,5 +1,5 @@
 // rbd_dynamics_loops: dynamics! for mechanisms with kinematic loops (csrc/rbd_loops.cuh has the mathematics), and the stage
-// dynamics of the loop rollout rbd_integrate_loops (its RK4 driver is rbd_b200.cu's integrate_t).
+// dynamics of the loop rollout rbd_integrate_loops (its RK4 driver and entry point are in rbd_b200.cu).
 //
 // One generic persistent kernel, one thread per sample, one launch per call: CRBA, RNEA bias, q̇, the constraint Jacobian / bias
 // sweep and the KKT solve run back to back in the same thread, so no intermediate crosses a launch boundary.  The per-sample
@@ -202,30 +202,4 @@ extern "C" int32_t rbd_dynamics_loops(const rbd_model* model, int32_t dtype, int
   cudaStream_t s = (cudaStream_t)stream;
   return dtype == RBD_F32 ? loops_t<float>(model, B, ld, q, v, tau, wext, *loops, vd_out, qd_out, lambda_out, K_out, k_out, s)
                           : loops_t<double>(model, B, ld, q, v, tau, wext, *loops, vd_out, qd_out, lambda_out, K_out, k_out, s);
-}
-
-extern "C" int32_t rbd_integrate_loops(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, void* s,
-                                       const void* tau, int64_t tau_step_stride, int64_t tau_stage_stride, const rbd_loop_desc* loops,
-                                       const rbd_contact_desc* contact, double dt, int32_t nsteps, void* q_traj, void* v_traj,
-                                       void* s_traj, void* stream) {
-  if (!model) return api_fail(RBD_EINVAL, "model handle is NULL");
-  if (dtype != RBD_F32 && dtype != RBD_F64) return api_fail(RBD_EUNSUPPORTED, "rbd_integrate_loops: fp32 / fp64 only");
-  if (int rc = api_check(model, dtype, B, ld)) return rc;
-  if (nsteps < 0 || !(dt > 0)) return api_fail(RBD_EINVAL, "rbd_integrate_loops: need dt > 0 and nsteps >= 0");
-  if (tau_step_stride < 0 || tau_stage_stride < 0) return api_fail(RBD_EINVAL, "rbd_integrate_loops: torque strides must be >= 0");
-  std::string err;
-  if (int rc = check_loop_desc(model->hm, loops, err)) return api_fail(rc, err);
-  if (contact)
-    if (int rc = api_check_contact(model, contact, "rbd_integrate_loops")) return rc;
-  const int64_t ns = contact ? (int64_t)3 * contact->npoints * contact->nhalfspaces : 0;
-  const bool rec = q_traj || v_traj || s_traj;
-  if (rec && (!q_traj || !v_traj || (ns > 0 && !s_traj)))
-    return api_fail(RBD_EINVAL, "rbd_integrate_loops: q_traj, v_traj and s_traj must be all NULL or all set");
-  const ApiCall call;
-  if (B == 0) return RBD_OK;
-  if (!q || !v) return api_fail(RBD_EINVAL, "rbd_integrate_loops: q and v must not be NULL");
-  if (ns > 0 && !s) return api_fail(RBD_EINVAL, "rbd_integrate_loops: s must not be NULL when there are contact pairs");
-  if (nsteps == 0 && !rec) return RBD_OK;
-  return integrate_loops(model, dtype, B, ld, q, v, s, tau, tau_step_stride, tau_stage_stride, *loops, ns > 0 ? contact : nullptr, dt,
-                         nsteps, q_traj, v_traj, s_traj, (cudaStream_t)stream);
 }

@@ -23,11 +23,10 @@ import numpy as np
 import torch
 
 from . import _cabi
-from .algorithms import _call, _check, _ptr, _stream, _torque_schedule
+from .algorithms import _call, _check, _ptr, _rollout, _steps, _stream
 from .contact import ContactDesc, contact_desc
 from .joint_types import Fixed, Planar, Prismatic, QuaternionSpherical, Revolute
 from .mechanism import Mechanism
-from .pd import integrate_pd
 from .spatial import rotation_between
 from .state import DynamicsResult, MechanismState, _DT
 
@@ -178,39 +177,6 @@ def dynamics_loops_(result: DynamicsResult, state: MechanismState, torques: Opti
     return result
 
 
-def _integrate_loops(state: MechanismState, nsteps: int, torques, dt: float, stabilization_gains, loops: Optional[LoopDesc],
-                     contact_state: Optional[torch.Tensor], contact: Optional[ContactDesc], record: bool, what: str, controller=None):
-    state.check_modcount()
-    if nsteps < 0:
-        raise ValueError("nsteps must be >= 0")
-    lib = _cabi.load_library()
-    ld = loops if loops is not None else loop_desc(state.mechanism, stabilization_gains)
-    cd = contact if contact is not None else contact_desc(state.mechanism)
-    if contact_state is None and cd.nstates > 0:
-        raise ValueError(f"{what}: contact_state [{cd.nstates}, B] must be given (the mechanism has contact points)")
-    _check(contact_state, cd.nstates, state, "contact_state")
-    step = stage = 0
-    if torques is not None and torques.dim() in (3, 4):
-        step, stage = _torque_schedule(state, torques, nsteps)
-    else:
-        _check(torques, state.nv, state, "torques")
-    traj = (None, None, None)
-    if record:
-        new = lambda rows: torch.empty((nsteps + 1, rows, state.batch), dtype=state.dtype, device=state.q.device)   # noqa: E731
-        traj = (new(state.nq), new(state.nv), new(cd.nstates) if cd.nstates else None)
-    if controller is not None:
-        integrate_pd(state, controller, nsteps, torques, step, stage, dt, loops=ld, contact=cd, contact_state=contact_state, traj=traj,
-                     what=what)
-        return traj
-    lst, keep = ld.c_struct()
-    cst, keep2 = cd.c_struct()
-    _call(lib.rbd_integrate_loops(state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q), _ptr(state.v),
-                                  _ptr(contact_state), _ptr(torques), step, stage, ctypes.byref(lst), ctypes.byref(cst), float(dt),
-                                  nsteps, *[_ptr(t) for t in traj], _stream()))
-    del keep, keep2
-    return traj
-
-
 def simulate_loops_trajectory_(state: MechanismState, nsteps: int, torques: Optional[torch.Tensor] = None, dt: float = 1e-4,
                                stabilization_gains=_DEFAULT, loops: Optional[LoopDesc] = None,
                                contact_state: Optional[torch.Tensor] = None, contact: Optional[ContactDesc] = None, *,
@@ -220,8 +186,10 @@ def simulate_loops_trajectory_(state: MechanismState, nsteps: int, torques: Opti
     the state after step s.  ``state`` and ``contact_state`` are advanced in place exactly as ``simulate_loops_`` advances them.
     ``controller``: a ``JointPD`` evaluated at every stage, as in ``simulate_loops_`` (``torques`` is then its feedforward; PD mode
     only when the mechanism has loops)."""
-    return _integrate_loops(state, nsteps, torques, dt, stabilization_gains, loops, contact_state, contact, True,
-                            "simulate_loops_trajectory_", controller)
+    ld = loops if loops is not None else loop_desc(state.mechanism, stabilization_gains)
+    cd = contact if contact is not None else contact_desc(state.mechanism)
+    return _rollout(state, nsteps, torques, dt, "simulate_loops_trajectory_", record=True, controller=controller, loops=ld, contact=cd,
+                    contact_state=contact_state)
 
 
 def simulate_loops_(state: MechanismState, final_time: float, torques: Optional[torch.Tensor] = None, dt: float = 1e-4,
@@ -237,10 +205,8 @@ def simulate_loops_(state: MechanismState, final_time: float, torques: Optional[
     descriptors (default: the mechanism's).  A tree mechanism is accepted (the KKT path without constraint rows).  ``controller``: a
     ``JointPD`` evaluated at every stage, as in ``simulate_`` (PD mode only when the mechanism has loops: computed-torque mode needs
     inverse_dynamics!, which refuses loops with RBD_ELOOP).  Returns the number of steps taken."""
-    nsteps, t = 0, 0.0
-    while t < final_time:            # the reference's `while t < final_time` loop (ode_integrators.jl:311)
-        t += dt
-        nsteps += 1
-    _integrate_loops(state, nsteps, torques, dt, stabilization_gains, loops, contact_state, contact, False, "simulate_loops_",
-                     controller)
+    nsteps = _steps(final_time, dt)
+    ld = loops if loops is not None else loop_desc(state.mechanism, stabilization_gains)
+    cd = contact if contact is not None else contact_desc(state.mechanism)
+    _rollout(state, nsteps, torques, dt, "simulate_loops_", controller=controller, loops=ld, contact=cd, contact_state=contact_state)
     return nsteps

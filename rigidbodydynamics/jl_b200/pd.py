@@ -13,13 +13,11 @@ each clamped to the effort bounds when they are given.  Pass one as ``controller
 from __future__ import annotations
 
 import ctypes
-from typing import Optional
 
 import numpy as np
 import torch
 
-from . import _cabi
-from .state import MechanismState, _DT
+from .state import MechanismState
 
 __all__ = ["JointPD"]
 
@@ -95,19 +93,3 @@ class JointPD:
                        ptr(vd_ref), qs, vs or vds, None if lo is None else lo.ctypes.data_as(dp),
                        None if hi is None else hi.ctypes.data_as(dp))
         return d, keep
-
-
-def integrate_pd(state: MechanismState, controller: JointPD, nsteps: int, torques, step: int, stage: int, dt: float,
-                 loops=None, contact=None, contact_state: Optional[torch.Tensor] = None, traj=(None, None, None), what: str = ""):
-    """rbd_integrate_pd on the state (leading dimension B); loops / contact: prebuilt descriptors or None."""
-    from .algorithms import _ptr, _stream
-    if not isinstance(controller, JointPD):
-        raise TypeError(f"{what}: controller must be a JointPD")
-    d, keep = controller._c_struct(state, nsteps, what)
-    lst, keep2 = loops.c_struct() if loops is not None else (None, None)
-    cst, keep3 = contact.c_struct() if contact is not None else (None, None)
-    _cabi.check(_cabi.load_library().rbd_integrate_pd(
-        state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q),
-        _ptr(state.v), _ptr(contact_state), _ptr(torques), step, stage, ctypes.byref(d), None if lst is None else ctypes.byref(lst),
-        None if cst is None else ctypes.byref(cst), float(dt), nsteps, *[_ptr(t) for t in traj], _stream()))
-    del keep, keep2, keep3
