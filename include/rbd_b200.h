@@ -503,6 +503,37 @@ int32_t rbd_integrate_contact_vjp(const rbd_model* model, int32_t dtype, int64_t
                                   const void* v_traj_bar, const void* s_traj_bar, void* q0_bar_tan, void* q0_bar_cfg, void* v0_bar,
                                   void* s0_bar, void* tau_bar, void* stream);
 
+/* Reverse mode through a closed-loop rollout (DESIGN 4.19): the gradient of
+ *   L = sum_s q_traj_bar[s] . q_traj[s] + v_traj_bar[s] . v_traj[s] (+ s_traj_bar[s] . s_traj[s] with contact)
+ * for the trajectory rbd_integrate_pd recorded with the same controller `pd`, tau and strides, contact descriptor (NULL: the tree
+ * rollout), dt and nsteps, leading dimension B (gain_ld 0 or B).  Gradients reach the initial state and τ_ff (the outputs of
+ * rbd_integrate_vjp / rbd_integrate_contact_vjp, same shapes and conventions, tau_bar ADDED TO) and the controller's device arrays
+ * through `pd_bar` (each ADDED TO, NULL = not wanted; pd_bar NULL: none):
+ *   kp, kd          [nv x B]: per-sample contributions, also for shared gains (gain_ld = 0: the caller sums over the batch, so that a
+ *                   rollout split into consecutive calls gives the gradients of one call, bit for bit)
+ *   q_ref           the shape of pd->q_ref ([nq x B] held, or a block per step at q_ref_step_stride); the derivative with respect
+ *                   to the nq coordinates as given (the law does not normalise q_ref)
+ *   v_ref, vd_ref   the shapes of pd->v_ref / pd->vd_ref
+ * The saturation's derivative is zero wherever the APPLIED torque equals a bound (1[lo < τ < hi]; torch.clamp's inclusive mask
+ * differs from it only where τ is exactly on a bound).  Nothing reaches the effort bounds, dt or the contact parameters.
+ * Argument errors (before any CUDA call): rbd_integrate_pd's controller checks, those of rbd_integrate_vjp /
+ * rbd_integrate_contact_vjp, pd == NULL, and pd_bar->v_ref / vd_ref without pd->v_ref / vd_ref: RBD_EINVAL; in computed-torque
+ * mode the model limits of rbd_inverse_dynamics_vjp: RBD_EUNSUPPORTED.  There is no loop rollout here.  Kernels per step: the
+ * recompute of rbd_integrate_pd's step without its finishing kernels, then as rbd_integrate_vjp (or rbd_integrate_contact_vjp)
+ * -- PD mode launches exactly their kernels; computed-torque mode adds per stage one inverse-dynamics VJP and, with effort bounds,
+ * one elementwise mask kernel.  The effort bounds are copied to the device once per call (from pageable memory, so a call captured
+ * in a CUDA graph must have none, as in rbd_integrate_pd); the per-step recompute reuses that copy. */
+typedef struct rbd_pd_bar {
+  void* kp; void* kd;                    /* [nv x B] */
+  void* q_ref;                           /* the shape of pd->q_ref */
+  void* v_ref; void* vd_ref;             /* the shapes of pd->v_ref / pd->vd_ref */
+} rbd_pd_bar;
+int32_t rbd_integrate_pd_vjp(const rbd_model* model, int32_t dtype, int64_t B, const void* q_traj, const void* v_traj,
+                             const void* s_traj, const void* tau, int64_t tau_step_stride, int64_t tau_stage_stride,
+                             const rbd_pd_desc* pd, const rbd_contact_desc* contact /* NULL = tree rollout */, double dt,
+                             int32_t nsteps, const void* q_traj_bar, const void* v_traj_bar, const void* s_traj_bar, void* q0_bar_tan,
+                             void* q0_bar_cfg, void* v0_bar, void* s0_bar, void* tau_bar, const rbd_pd_bar* pd_bar, void* stream);
+
 /* Next row of the scope table (SURVEY 8(f) rank 2): kinematics by-products of the same outward sweep, all expressed in the
  * mechanism's root frame, 6-vectors as [angular; linear].  Every output pointer may be NULL (not computed).
  *   transforms_to_root  [12*nb x B]  rows 12 i .. 12 i + 11 = transform_to_root(state, successor of tree joint i):

@@ -4,11 +4,13 @@
     inverse_dynamics_vjp_  τ̄ᵀ ∂τ/∂(q, v, v̇, w_ext)         rbd_inverse_dynamics_vjp
     integrate_vjp_         gradient of a recorded rollout       rbd_integrate_vjp         (csrc/rbd_integrate_adjoint.cuh)
     integrate_contact_vjp_ gradient of a recorded contact rollout  rbd_integrate_contact_vjp  (csrc/rbd_contact_adjoint.cuh)
+    integrate_pd_vjp_      gradient of a recorded closed-loop rollout  rbd_integrate_pd_vjp  (csrc/rbd_integrate_adjoint.cuh)
     dynamics(mechanism, q, v, tau=None, externalwrenches=None)         differentiable v̇ = dynamics!(...)
     inverse_dynamics(mechanism, q, v, vd, externalwrenches=None)       differentiable τ = inverse_dynamics!(...)
     simulate(mechanism, q0, v0, torques=None, *, dt, nsteps, ...)     differentiable RK4 rollout (simulate)
     simulate_contact(mechanism, q0, v0, s0, torques=None, *, contact, dt, nsteps, ...)
                                                                        differentiable RK4 rollout with soft contact
+    both with controller=JointPD(...): closed loop, gradients also to the controller's gains and references
 
 One product costs one Articulated-Body solve (forward dynamics only) plus one outward and one inward sweep: O(n) per sample, no
 nv x nv Jacobian is formed (``dynamics_derivatives_`` builds both full Jacobians instead).  Every tensor is ``[rows, B]``, contiguous,
@@ -33,8 +35,8 @@ from .algorithms import DimensionMismatch, _check, _ptr, _require_tree
 from .mechanism import Mechanism
 from .state import _DT, MechanismState, _model_handle
 
-__all__ = ["dynamics_vjp_", "inverse_dynamics_vjp_", "integrate_vjp_", "integrate_contact_vjp_", "dynamics", "inverse_dynamics", "simulate",
-           "simulate_contact"]
+__all__ = ["dynamics_vjp_", "inverse_dynamics_vjp_", "integrate_vjp_", "integrate_contact_vjp_", "integrate_pd_vjp_", "dynamics",
+           "inverse_dynamics", "simulate", "simulate_contact"]
 
 
 def _stream(t: torch.Tensor):
@@ -320,14 +322,21 @@ def _vjp_call(h, qt, vt, tau, step, stage, dt, n, qtb, vtb, qc, vb, tb):
 
 
 def simulate(mechanism: Mechanism, q0: torch.Tensor, v0: torch.Tensor, torques: Optional[torch.Tensor] = None, *, dt: float,
-             nsteps: int, trajectory: bool = True, checkpoint_every: Optional[int] = None):
+             nsteps: int, trajectory: bool = True, checkpoint_every: Optional[int] = None, controller=None):
     """Differentiable ``nsteps`` Munthe-Kaas RK4 steps of ``simulate`` from q0 [nq, B], v0 [nv, B].  ``torques``: None (zero),
     constant [nv, B], per step [nsteps, nv, B] or per stage [nsteps, 4, nv, B].  Returns ``(q_traj, v_traj)`` ([nsteps + 1, rows, B],
     block 0 the initial state), or ``(q_final, v_final)`` when ``trajectory=False``.  Gradients flow to q0 (as ``q_bar_cfg``, see the
     module docstring), v0 and the torques; backward runs ``rbd_integrate_vjp``, which recomputes each step's stages from the recorded
     states.  With ``trajectory=False`` and ``checkpoint_every=k`` only every k-th state is kept, and backward re-records each
     segment of k steps before its VJP: peak memory O((nsteps / k + k) (nq + nv) B) instead of O(nsteps (nq + nv) B).  The gradients
-    do not depend on k, bit for bit.  Not twice differentiable."""
+    do not depend on k, bit for bit.  Not twice differentiable.
+
+    ``controller``: a ``JointPD`` evaluated at every stage (``torques`` is then τ_ff), as ``simulate_(..., controller=)``.  Gradients
+    then also flow to those of its ``kp``, ``kd``, ``q_ref``, ``v_ref`` and ``vd_ref`` that require grad (shared gains: summed over
+    the batch); backward runs ``rbd_integrate_pd_vjp``."""
+    if controller is not None:
+        return _simulate_pd(mechanism, q0, v0, None, torques, controller, None, dt, nsteps, trajectory, checkpoint_every,
+                            "autodiff.simulate")
     return _Simulate.apply(mechanism, q0, v0, torques, float(dt), int(nsteps), bool(trajectory), checkpoint_every)
 
 
@@ -456,15 +465,215 @@ class _SimulateContact(torch.autograd.Function):
 
 
 def simulate_contact(mechanism: Mechanism, q0: torch.Tensor, v0: torch.Tensor, s0: torch.Tensor, torques: Optional[torch.Tensor] = None, *,
-                     contact=None, dt: float, nsteps: int, trajectory: bool = True, checkpoint_every: Optional[int] = None):
+                     contact=None, dt: float, nsteps: int, trajectory: bool = True, checkpoint_every: Optional[int] = None,
+                     controller=None):
     """Differentiable ``nsteps`` steps of ``simulate_contact_`` from q0 [nq, B], v0 [nv, B] and the contact state s0
     [num_contact_states, B].  ``contact``: a ``ContactDesc`` (the mechanism's ``contact_desc`` by default); ``torques`` as for
     ``simulate``.  Returns ``(q_traj, v_traj, s_traj)`` ([nsteps + 1, rows, B], block 0 the initial state), or the final
     ``(q, v, s)`` when ``trajectory=False``.  Gradients flow to q0 (as ``q_bar_cfg``), v0, s0 and the torques; backward runs
     ``rbd_integrate_contact_vjp``, which differentiates the contact force law on the branch each pair takes.  ``checkpoint_every``
-    as for ``simulate``: the gradients do not depend on it, bit for bit.  Not twice differentiable."""
+    as for ``simulate``: the gradients do not depend on it, bit for bit.  ``controller`` as for ``simulate``.  Not twice
+    differentiable."""
     from .contact import contact_desc
     if mechanism.has_loops():
         raise _cabi.RbdError(_cabi.RBD_ELOOP, "autodiff.simulate_contact: This method can currently only handle tree Mechanisms.")
     cd = contact if contact is not None else contact_desc(mechanism)
+    if controller is not None:
+        return _simulate_pd(mechanism, q0, v0, s0, torques, controller, cd, dt, nsteps, trajectory, checkpoint_every,
+                            "autodiff.simulate_contact")
     return _SimulateContact.apply(mechanism, q0, v0, s0, torques, cd, float(dt), int(nsteps), bool(trajectory), checkpoint_every)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# closed-loop rollouts: rbd_integrate_pd (recording) / rbd_integrate_pd_vjp
+# ----------------------------------------------------------------------------------------------------------------------
+class _Batch:
+    """What JointPD._c_struct reads from a state: sizes, dtype and device of a rollout's initial q0."""
+
+    def __init__(self, h, q0: torch.Tensor):
+        self.nq, self.nv, self.batch, self.dtype, self.q = h.info.nq, h.info.nv, q0.shape[1], q0.dtype, q0
+
+
+def _pd_struct(controller, h, q0, nsteps, what):
+    from .pd import JointPD
+    if not isinstance(controller, JointPD):
+        raise TypeError(f"{what}: controller must be a JointPD")
+    return controller._c_struct(_Batch(h, q0), nsteps, what)
+
+
+def integrate_pd_vjp_(mechanism: Mechanism, q_traj: torch.Tensor, v_traj: torch.Tensor, torques: Optional[torch.Tensor] = None, *,
+                      controller, dt: float, contact=None, s_traj: Optional[torch.Tensor] = None,
+                      q_traj_bar: Optional[torch.Tensor] = None, v_traj_bar: Optional[torch.Tensor] = None,
+                      s_traj_bar: Optional[torch.Tensor] = None, q0_bar_tan: Optional[torch.Tensor] = None,
+                      q0_bar_cfg: Optional[torch.Tensor] = None, v0_bar: Optional[torch.Tensor] = None,
+                      s0_bar: Optional[torch.Tensor] = None, tau_bar: Optional[torch.Tensor] = None,
+                      kp_bar: Optional[torch.Tensor] = None, kd_bar: Optional[torch.Tensor] = None,
+                      q_ref_bar: Optional[torch.Tensor] = None, v_ref_bar: Optional[torch.Tensor] = None,
+                      vd_ref_bar: Optional[torch.Tensor] = None):
+    """Gradient of ``L = sum_s q_traj_bar[s] . q_traj[s] + v_traj_bar[s] . v_traj[s] (+ s_traj_bar[s] . s_traj[s])`` over a
+    trajectory recorded with ``controller`` (a ``JointPD``) by ``simulate_trajectory_`` or, with ``contact`` (a ``ContactDesc``)
+    and ``s_traj``, by ``simulate_contact_trajectory_``, with the same ``torques`` (τ_ff) and ``dt``.  State and torque outputs as
+    ``integrate_vjp_`` / ``integrate_contact_vjp_``.  Controller outputs, each optional and ADDED TO: ``kp_bar`` / ``kd_bar`` [nv, B]
+    (per sample, also for shared gains: sum over the batch for theirs), ``q_ref_bar`` / ``v_ref_bar`` / ``vd_ref_bar`` with the shapes
+    of ``q_ref`` / ``v_ref`` / ``vd_ref``.  Mechanisms with loops are refused (RBD_ELOOP)."""
+    what = "integrate_pd_vjp_"
+    nsteps = q_traj.shape[0] - 1
+    h, B, step, stage = _rollout_inputs(mechanism, what, q_traj[0], v_traj[0], torques, nsteps)
+    nq, nv = h.info.nq, h.info.nv
+    ns = 0 if contact is None else contact.nstates
+    pd, keep = _pd_struct(controller, h, q_traj[0], nsteps, what)
+    shape = lambda t: None if t is None else tuple(t.shape)      # noqa: E731
+    for bar, ref, name in ((v_ref_bar, controller.v_ref, "v_ref"), (vd_ref_bar, controller.vd_ref, "vd_ref")):
+        if bar is not None and ref is None:
+            raise ValueError(f"{what}: {name}_bar needs the controller's {name}")
+    if contact is None and (s_traj is not None or s_traj_bar is not None or s0_bar is not None):
+        raise ValueError(f"{what}: s_traj, s_traj_bar and s0_bar need contact")
+    _check_blocks(what, q_traj, (
+        (q_traj, (nsteps + 1, nq, B), "q_traj"), (v_traj, (nsteps + 1, nv, B), "v_traj"),
+        (s_traj, (nsteps + 1, ns, B), "s_traj"), (q_traj_bar, (nsteps + 1, nq, B), "q_traj_bar"),
+        (v_traj_bar, (nsteps + 1, nv, B), "v_traj_bar"), (s_traj_bar, (nsteps + 1, ns, B), "s_traj_bar"),
+        (q0_bar_tan, (nv, B), "q0_bar_tan"), (q0_bar_cfg, (nq, B), "q0_bar_cfg"), (v0_bar, (nv, B), "v0_bar"), (s0_bar, (ns, B), "s0_bar"),
+        (tau_bar, shape(torques), "tau_bar"), (kp_bar, (nv, B), "kp_bar"), (kd_bar, (nv, B), "kd_bar"),
+        (q_ref_bar, shape(controller.q_ref), "q_ref_bar"), (v_ref_bar, shape(controller.v_ref), "v_ref_bar"),
+        (vd_ref_bar, shape(controller.vd_ref), "vd_ref_bar")))
+    if contact is not None and ns > 0 and s_traj is None:
+        raise ValueError(f"{what}: s_traj is needed with contact pairs")
+    _pd_vjp_call(h, q_traj, v_traj, s_traj, torques, step, stage, pd, contact, dt, nsteps, q_traj_bar, v_traj_bar, s_traj_bar,
+                 q0_bar_tan, q0_bar_cfg, v0_bar, s0_bar, tau_bar, (kp_bar, kd_bar, q_ref_bar, v_ref_bar, vd_ref_bar))
+    del keep
+
+
+def _pd_vjp_call(h, qt, vt, st, tau, step, stage, pd, contact, dt, n, qtb, vtb, stb, q0t, qc, vb, sb, tb, bars):
+    import ctypes
+    from .pd import _RbdPdBar
+    B = qt.shape[2]
+    c, keep = contact.c_struct() if contact is not None else (None, None)
+    pb = _RbdPdBar(*[_ptr(t) for t in bars])
+    _cabi.check(_cabi.load_library().rbd_integrate_pd_vjp(
+        h.ptr, _DT[qt.dtype], B, _ptr(qt), _ptr(vt), _ptr(st), _ptr(tau), step, stage, ctypes.byref(pd),
+        None if c is None else ctypes.byref(c), float(dt), n, _ptr(qtb), _ptr(vtb), _ptr(stb), _ptr(q0t), _ptr(qc), _ptr(vb), _ptr(sb),
+        _ptr(tb), ctypes.byref(pb), _stream(qt)))
+    del keep
+
+
+def _pd_trajectory(h, q0, v0, s0, tau, first, m, step, stage, ctl, contact, dt, what):
+    """rbd_integrate_pd recording steps first .. first + m from (q0, v0[, s0]) (not modified): [m + 1, rows, B] blocks."""
+    import ctypes
+    B = q0.shape[1]
+    q, v = q0.clone(), v0.clone()
+    s = None if s0 is None else s0.clone()
+    new = lambda x: torch.empty((m + 1,) + tuple(x.shape), dtype=x.dtype, device=x.device)   # noqa: E731
+    qt, vt = new(q0), new(v0)
+    st = None if s0 is None else new(s0)
+    t = None if tau is None else (tau if tau.dim() == 2 else tau[first:])
+    pd, keep = _pd_struct(ctl._steps_from(first), h, q0, m, what)
+    c, keep2 = contact.c_struct() if contact is not None else (None, None)
+    _cabi.check(_cabi.load_library().rbd_integrate_pd(
+        h.ptr, _DT[q0.dtype], B, B, _ptr(q), _ptr(v), _ptr(s), _ptr(t), step, stage, ctypes.byref(pd), None,
+        None if c is None else ctypes.byref(c), float(dt), m, _ptr(qt), _ptr(vt), _ptr(st), _stream(q0)))
+    del keep, keep2
+    return qt, vt, st
+
+
+class _SimulatePD(torch.autograd.Function):
+    """The closed-loop rollout; the controller's tensors are inputs (kp, kd, q_ref, v_ref, vd_ref), `spec` = (computed_torque,
+    effort_bounds).  s0 / contact are None for the tree rollout."""
+
+    @staticmethod
+    def forward(ctx, mechanism, q0, v0, s0, tau, kp, kd, q_ref, v_ref, vd_ref, spec, contact, dt, nsteps, trajectory, every):
+        from .pd import JointPD
+        what = "autodiff.simulate" if contact is None else "autodiff.simulate_contact"
+        h, B, step, stage = _rollout_inputs(mechanism, what, q0, v0, tau, nsteps)
+        ctl = JointPD(kp, kd, q_ref, v_ref, vd_ref=vd_ref, computed_torque=spec[0], effort_bounds=spec[1])
+        _pd_struct(ctl, h, q0, nsteps, what)          # the controller's checks, before any call
+        if contact is not None:
+            ns = contact.nstates
+            if s0.dtype != q0.dtype or s0.device != q0.device or not s0.is_contiguous() or tuple(s0.shape) != (ns, B):
+                raise DimensionMismatch(f"{what}: s0 must be a contiguous [{ns}, {B}] tensor with the dtype and device of q0")
+        ctx.handle, ctx.ctl, ctx.contact, ctx.dt, ctx.nsteps, ctx.trajectory = h, ctl, contact, dt, nsteps, trajectory
+        ctx.step, ctx.stage, ctx.what = step, stage, what
+        if trajectory or B == 0:
+            every = nsteps
+        else:       # checkpoints every `every` steps; backward re-records each segment before its VJP
+            every = max(1, min(every or nsteps, nsteps)) if nsteps else 1
+        ctx.every = every
+        q, v, s = q0, v0, s0
+        qs, vs, ss = [q0], [v0], [s0]
+        for first in range(0, max(nsteps, 1), every):
+            m = min(every, nsteps - first)
+            qt, vt, st = _pd_trajectory(h, q, v, s, tau, first, m, step, stage, ctl, contact, dt, what)
+            if trajectory or B == 0:
+                break
+            q, v, s = qt[-1].clone(), vt[-1].clone(), None if st is None else st[-1].clone()
+            qs.append(q); vs.append(v); ss.append(s)
+        if trajectory or B == 0:
+            ctx.save_for_backward(tau, qt, vt, st, kp, kd, q_ref, v_ref, vd_ref)
+            out = (qt, vt) if contact is None else (qt, vt, st)
+            return out if trajectory else tuple(x[-1].clone() for x in out)
+        ctx.save_for_backward(tau, torch.stack(qs[:-1]), torch.stack(vs[:-1]), None if s0 is None else torch.stack(ss[:-1]), kp, kd,
+                              q_ref, v_ref, vd_ref)
+        return (q, v) if contact is None else (q, v, s)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, *grads):
+        tau, qck, vck, sck, kp, kd, q_ref, v_ref, vd_ref = ctx.saved_tensors
+        h, dt, n, cd, ctl = ctx.handle, ctx.dt, ctx.nsteps, ctx.contact, ctx.ctl
+        need = ctx.needs_input_grad
+        gq, gv = grads[0].contiguous(), grads[1].contiguous()
+        gs = grads[2].contiguous() if cd is not None else None
+        q0, v0 = qck[0], vck[0]
+        s0 = None if sck is None else sck[0]
+        B = q0.shape[1]
+        zero = lambda want, like: torch.zeros_like(like) if (want and like is not None) else None       # noqa: E731
+        tb = zero(need[4], tau)
+        kpb = torch.zeros_like(v0) if need[5] else None
+        kdb = torch.zeros_like(v0) if need[6] else None
+        qrb, vrb, vdrb = zero(need[7], q_ref), zero(need[8], v_ref), zero(need[9], vd_ref)
+        qa, va = torch.zeros_like(q0), torch.zeros_like(v0)
+        sa = None if s0 is None else torch.zeros_like(s0)
+        nothing = (None,) * 6
+        if B and any(need[1:10]):
+            pd, keep = _pd_struct(ctl, h, q0, n, ctx.what)
+            if ctx.trajectory:
+                _pd_vjp_call(h, qck, vck, sck, tau, ctx.step, ctx.stage, pd, cd, dt, n, gq, gv, gs, None, qa, va, sa, tb,
+                             (kpb, kdb, qrb, vrb, vdrb))
+            else:
+                # segments last to first; the adjoint of a segment's end state is its successor's q0_bar_cfg / v0_bar (/ s0_bar)
+                k = ctx.every
+                starts = list(range(0, n, k)) if n else [0]
+                qa, va, sa = gq, gv, gs
+                for j in reversed(range(len(starts))):
+                    first = starts[j]
+                    m = min(k, n - first)
+                    qt, vt, st = _pd_trajectory(h, qck[j], vck[j], None if sck is None else sck[j], tau, first, m, ctx.step, ctx.stage,
+                                                ctl, cd, dt, ctx.what)
+                    bars = lambda x: torch.zeros_like(x)                      # noqa: E731
+                    qtb, vtb = bars(qt), bars(vt)
+                    qtb[-1] = qa; vtb[-1] = va
+                    stb = None
+                    if st is not None:
+                        stb = bars(st)
+                        stb[-1] = sa
+                    seg = lambda t: t if t is None or t.dim() == 2 else t[first:]      # noqa: E731
+                    pds, keep2 = _pd_struct(ctl._steps_from(first), h, q0, m, ctx.what)
+                    qa, va = torch.empty_like(q0), torch.empty_like(v0)
+                    sa = None if s0 is None else torch.empty_like(s0)
+                    _pd_vjp_call(h, qt, vt, st, seg(tau), ctx.step, ctx.stage, pds, cd, dt, m, qtb, vtb, stb, None, qa, va, sa, seg(tb),
+                                 (kpb, kdb, seg(qrb), seg(vrb), seg(vdrb)))
+            del keep
+        if kpb is not None and kp.dim() == 1:
+            kpb = kpb.sum(1)
+        if kdb is not None and kd.dim() == 1:
+            kdb = kdb.sum(1)
+        return (None, qa if need[1] else None, va if need[2] else None, sa if (need[3] and sa is not None) else None, tb, kpb, kdb, qrb,
+                vrb, vdrb) + nothing
+
+
+def _simulate_pd(mechanism, q0, v0, s0, torques, controller, contact, dt, nsteps, trajectory, every, what):
+    from .pd import JointPD
+    if not isinstance(controller, JointPD):
+        raise TypeError(f"{what}: controller must be a JointPD")
+    c = controller
+    return _SimulatePD.apply(mechanism, q0, v0, s0, torques, c.kp, c.kd, c.q_ref, c.v_ref, c.vd_ref, (c.computed_torque, c.effort_bounds),
+                             contact, float(dt), int(nsteps), bool(trajectory), every)

@@ -80,15 +80,6 @@ __global__ void __launch_bounds__(kNT, 1) inverse_dynamics_vjp_kernel(const __gr
   }
 }
 
-// Same model limits as rbd_dynamics_derivatives
-int check_limits(const HostModel& hm, const char* who) {
-  DerivDev D;
-  DerivAnc A;
-  if (!build_deriv_dev(hm.dev64, D, A))
-    return api_fail(RBD_EUNSUPPORTED, std::string(who) + ": more than 128 velocity coordinates or 4096 mass-matrix entries");
-  return RBD_OK;
-}
-
 template <class T>
 int vjp_t(const rbd_model* model, bool fd, int64_t B, int64_t ld, VjpArgs<T> a, cudaStream_t stream) {
   const HostModel& hm = model->hm;
@@ -121,6 +112,22 @@ VjpArgs<T> args(int64_t B, int64_t ld, const void* q, const void* v, const void*
 
 }  // namespace
 
+// Same model limits as rbd_dynamics_derivatives
+int rbd::check_vjp_limits(const HostModel& hm, const char* who) {
+  DerivDev D;
+  DerivAnc A;
+  if (!build_deriv_dev(hm.dev64, D, A))
+    return api_fail(RBD_EUNSUPPORTED, std::string(who) + ": more than 128 velocity coordinates or 4096 mass-matrix entries");
+  return RBD_OK;
+}
+
+int rbd::inverse_dynamics_vjp_dense(const rbd_model* model, int32_t dtype, int64_t B, const void* q, const void* v, const void* vd,
+                                    const void* tau_bar, void* q_bar_cfg, void* v_bar, void* vd_bar, cudaStream_t s) {
+  return dtype == RBD_F32
+             ? vjp_t<float>(model, false, B, B, args<float>(B, B, q, v, vd, nullptr, tau_bar, nullptr, q_bar_cfg, v_bar, vd_bar, nullptr, nullptr), s)
+             : vjp_t<double>(model, false, B, B, args<double>(B, B, q, v, vd, nullptr, tau_bar, nullptr, q_bar_cfg, v_bar, vd_bar, nullptr, nullptr), s);
+}
+
 int rbd::dynamics_vjp_dense(const rbd_model* model, int32_t dtype, int64_t B, const void* q, const void* v, const void* vd,
                             const void* vd_bar, void* q_bar_cfg, void* v_bar, void* tau_bar, cudaStream_t s) {
   return dtype == RBD_F32
@@ -135,7 +142,7 @@ extern "C" int32_t rbd_dynamics_vjp(const rbd_model* model, int32_t dtype, int64
   const ApiCall call;
   if (B == 0 || model->hm.nv == 0) return RBD_OK;
   if (!q || !v || !vd || !vd_bar) return api_fail(RBD_EINVAL, "rbd_dynamics_vjp: q, v, vd and vd_bar must not be NULL");
-  if (int rc = check_limits(model->hm, "rbd_dynamics_vjp")) return rc;
+  if (int rc = check_vjp_limits(model->hm, "rbd_dynamics_vjp")) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   (void)tau;     // tau enters only through v̇, which is given: accepted so that the call mirrors rbd_dynamics
   return dtype == RBD_F32
@@ -150,7 +157,7 @@ extern "C" int32_t rbd_inverse_dynamics_vjp(const rbd_model* model, int32_t dtyp
   const ApiCall call;
   if (B == 0 || model->hm.nv == 0) return RBD_OK;
   if (!q || !v || !vd || !tau_bar) return api_fail(RBD_EINVAL, "rbd_inverse_dynamics_vjp: q, v, vd and tau_bar must not be NULL");
-  if (int rc = check_limits(model->hm, "rbd_inverse_dynamics_vjp")) return rc;
+  if (int rc = check_vjp_limits(model->hm, "rbd_inverse_dynamics_vjp")) return rc;
   cudaStream_t s = (cudaStream_t)stream;
   return dtype == RBD_F32
              ? vjp_t<float>(model, false, B, ld, args<float>(B, ld, q, v, vd, wext, tau_bar, q_bar_tan, q_bar_cfg, v_bar, vd_bar, nullptr, wext_bar), s)

@@ -1119,11 +1119,21 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, const Rollout& r,
   T* taud = vs + (size_t)9 * nv * B;
   T* qsi[4] = {qs, qs, qs, qs};
   T* vsi[4] = {vs, vs, vs, vs};
+  // the controller's stage torques and, in computed-torque mode, v̇_des (the inverse dynamics' input): one block for every stage,
+  // or with `stages` and a controller one block per stage behind the stage rows (pd_stage_rows), kept for the adjoint
+  T* taui[4] = {taud, taud, taud, taud};
+  T* vdes[4] = {vd[0], vd[1], vd[2], vd[3]};
   if (stages)
     for (int i = 0; i < 4; ++i) {
       qsi[i] = stages + (size_t)i * nq * B; vsi[i] = stages + (4 * nq + (size_t)i * nv) * B;
       phid[i] = stages + (4 * nq + (4 + (size_t)i) * nv) * B; vd[i] = stages + (4 * nq + (8 + (size_t)i) * nv) * B;
       if (ns) sd[i] = stages + ((size_t)stage_rows(nq, nv) + i * ns) * B;
+      vdes[i] = vd[i];
+      if (pd) {
+        T* pr = stages + ((size_t)stage_rows(nq, nv) + 4 * ns) * B;
+        taui[i] = pr + (size_t)i * nv * B;
+        if (computed_torque) vdes[i] = pr + (4 + (size_t)i) * nv * B;
+      }
     }
   T* qout = traj_q ? traj_q : (T*)q;       // the finishing kernels' target (block s + 1 of a trajectory)
   T* vout = traj_v ? traj_v : (T*)v;
@@ -1136,7 +1146,9 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, const Rollout& r,
   // the controller's saturation bounds on the device, behind the workspace rows (copied from pageable memory: staged before return)
   const T* pd_lo = nullptr;
   const T* pd_hi = nullptr;
-  if (pd && pd->effort_lo) {
+  if (pd && pd->effort_lo && r.pd_bounds) {
+    pd_lo = (const T*)r.pd_bounds; pd_hi = pd_lo + nv;
+  } else if (pd && pd->effort_lo) {
     std::vector<T> bounds(2 * nv);
     for (size_t k = 0; k < nv; ++k) { bounds[k] = (T)pd->effort_lo[k]; bounds[nv + k] = (T)pd->effort_hi[k]; }
     T* dev = (T*)work.p + rows * (size_t)B;
@@ -1183,14 +1195,15 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, const Rollout& r,
         }
       }
       StageArgs<T> sa{q0, v0, i ? phid[i - 1] : nullptr, i ? vd[i - 1] : nullptr, phid[i], qsi[i], vsi[i], (T)(dt * a[i]), B, vec_stage};
+      if (pd) tau_dense = taui[i];
       if (pd) {     // the references of step s start at s * q_ref_step_stride (q_ref) / s * v_ref_step_stride (v_ref, v̇_ref)
         const T* qref = (const T*)pd->q_ref + (size_t)s * pd->q_ref_step_stride;
         const size_t o = (size_t)s * pd->v_ref_step_stride;
         const T* vref = pd->v_ref ? (const T*)pd->v_ref + o : nullptr;
         const T *kp = (const T*)pd->kp, *kd = (const T*)pd->kd;
         sa.pd = computed_torque ? PdStage<T>{qref, vref, pd->vd_ref ? (const T*)pd->vd_ref + o : nullptr, kp, kd, pd->gain_ld, nullptr,
-                                             nullptr, vd[i], ld}
-                                : PdStage<T>{qref, vref, tau_at(s, i), kp, kd, pd->gain_ld, pd_lo, pd_hi, taud, ld};
+                                             nullptr, vdes[i], ld}
+                                : PdStage<T>{qref, vref, tau_at(s, i), kp, kd, pd->gain_ld, pd_lo, pd_hi, taui[i], ld};
       }
       if (vec_stage) {     // revolute / prismatic rows, VEC samples per thread
         integrate_stage_linear_kernel<T><<<dim3(grid_lin, hm.nb), 256, 0, stream>>>(M, sa);
@@ -1201,8 +1214,8 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, const Rollout& r,
         if (int rc = api_launched()) return rc;
       }
       if (computed_torque) {     // tau = clamp(ID(q_s, v_s, v̇_des) + τ_ff), without contact wrenches
-        if (int rc = inverse_dynamics_t<T>(model, B, B, qsi[i], vsi[i], vd[i], nullptr, taud, stream)) return rc;
-        const PdFinishArgs<T> pf{taud, tau_at(s, i), ld, pd_lo, pd_hi, (int64_t)nv, B};
+        if (int rc = inverse_dynamics_t<T>(model, B, B, qsi[i], vsi[i], vdes[i], nullptr, taui[i], stream)) return rc;
+        const PdFinishArgs<T> pf{taui[i], tau_at(s, i), ld, pd_lo, pd_hi, (int64_t)nv, B};
         pd_finish_kernel<T><<<(int)std::min<int64_t>(((int64_t)nv * B + 255) / 256, (int64_t)p.sms * 8), 256, 0, stream>>>(pf);
         if (int rc = api_launched()) return rc;
       }

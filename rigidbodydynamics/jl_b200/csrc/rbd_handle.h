@@ -167,10 +167,15 @@ struct Rollout {
   const rbd_contact_desc* contact = nullptr;   // the contact rollout, or the loop rollout's contact pass
   const rbd_loop_desc* loops = nullptr;        // every stage's dynamics is the KKT solve (loop_stage_launch)
   const rbd_pd_desc* pd = nullptr;             // feedback evaluated at every stage
+  const void* pd_bounds = nullptr;             // pd's effort bounds already on the device ([2 nv]: lo, then hi), or NULL: integrate
+                                               // copies them from the host arrays of pd (rbd_integrate_pd_vjp's recompute passes its copy)
 };
 // The recompute of one step (nsteps = 1, ld = B) keeps its four stages in stage_rows(nq, nv) x B rows of `stages` (4 ns more with
-// contact, for the ṡ_i) and skips the finishing step.
+// contact, for the ṡ_i) and skips the finishing step.  With a controller (pd) pd_stage_rows(nv, computed_torque) x B more follow:
+// the four stages' applied torques τ_i (nv rows each), then in computed-torque mode the four v̇_des,i (nv rows each), the
+// inverse dynamics' input; rbd_integrate_pd_vjp's adjoint reads both.
 inline int64_t stage_rows(int64_t nq, int64_t nv) { return 4 * nq + 12 * nv; }
+inline int64_t pd_stage_rows(int64_t nv, bool computed_torque) { return (computed_torque ? 8 : 4) * nv; }
 // Runs the rollout (fp32 / fp64, arguments checked by the caller).  RBD_OK at once when B == 0, or when nsteps == 0 and nothing is
 // recorded.  The loop rollout takes its contact pass only when there are contact pairs.
 int integrate(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const Rollout& r, cudaStream_t stream);
@@ -195,5 +200,10 @@ int api_check_loops(const rbd_model* model, const rbd_loop_desc* loops);
 // rbd_adjoint.cu's forward-dynamics VJP on dense [rows x B] arrays (no external wrenches); outputs may be NULL
 int dynamics_vjp_dense(const rbd_model* model, int32_t dtype, int64_t B, const void* q, const void* v, const void* vd, const void* vd_bar,
                        void* q_bar_cfg, void* v_bar, void* tau_bar, cudaStream_t stream);
+// ... and the inverse-dynamics VJP on dense arrays (no external wrenches): q̄_cfg, v̄, v̇̄ of τ = ID(q, v, v̇) from τ̄; outputs may be NULL
+int inverse_dynamics_vjp_dense(const rbd_model* model, int32_t dtype, int64_t B, const void* q, const void* v, const void* vd,
+                               const void* tau_bar, void* q_bar_cfg, void* v_bar, void* vd_bar, cudaStream_t stream);
+// The model limits of rbd_dynamics_vjp / rbd_inverse_dynamics_vjp (those of rbd_dynamics_derivatives): RBD_OK or RBD_EUNSUPPORTED
+int check_vjp_limits(const HostModel& hm, const char* who);
 
 }  // namespace rbd

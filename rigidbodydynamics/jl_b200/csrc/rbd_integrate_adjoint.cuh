@@ -23,6 +23,7 @@
 #include "rbd_adjoint.cuh"
 #include "rbd_dual.cuh"
 #include "rbd_integrate.cuh"
+#include "rbd_pd.cuh"
 
 namespace rbd {
 
@@ -190,8 +191,85 @@ template <class T> RBD_HD void adj_lin(const AdjStepArgs<T>& a, const LinIn<T>& 
   }
 }
 
-// any joint at sample column b
-template <class T> RBD_HD void adj_joint(const BodyDev<T>& bd, const AdjStepArgs<T>& a, int64_t b) {
+// ---- the closed-loop controller's adjoint (rbd_integrate_pd_vjp, DESIGN 4.19) ---------------------------------------------------
+// Stage l applies τ_l = clamp(u_l, lo, hi) with u_l = τ_ff - Kp e - Kd (v_s - v_ref) (PD) or u_l = ID(q_s, v_s, v̇_des) + τ_ff,
+// v̇_des = v̇_ref - Kp e - Kd (v_s - v_ref) (computed torque), e = joint_error(q_ref, q_s) (rbd_pd.cuh).  From τ̄_l (the stage's
+// forward-dynamics or contact VJP):
+//   m = τ̄_l where lo < τ_l < hi, 0 where the APPLIED torque equals a bound (no bounds: m = τ̄_l);  τ̄_ff += m
+//   PD: w = m.  Computed torque: the inverse-dynamics VJP at (q_s, v_s, v̇_des) seeded with m gives q̄_cfg, v̄ (added to q̄s, v̄s) and
+//   v̇̄_des; v̇̄_ref += v̇̄_des, w = v̇̄_des.
+//   per velocity row: K̄p -= w e,  K̄d -= w (v_s - v_ref),  v̄s -= Kd w,  v̄_ref += Kd w,  ē = -Kp w
+//   q̄s += (∂e/∂q_s)^T ē,  q̄_ref += (∂e/∂q_ref)^T ē   (configuration coordinates; closed forms where e = q_s - q_ref, else Dual1
+//   through joint_error, one direction per configuration coordinate, on the branch the forward took)
+// q̄_ref is the derivative with respect to the nq coordinates of q_ref as given (the law does not normalise q_ref).
+template <class T> struct PdAdjArgs {
+  const T* qref; const T* vref;            // at the step, leading dimension ld (vref NULL = 0)
+  const T* kp; const T* kd; int64_t g_ld;  // [nv] (g_ld = 0) or [nv x ld]
+  const T* tau;                            // applied torque of stage g [nv x ld]; NULL = no mask in this phase (no bounds, or
+  const T* lo; const T* hi;                //   computed-torque mode, whose mask kernel ran before the inverse-dynamics VJP)
+  const T* idq; const T* idv; const T* idvd;   // computed-torque mode: the inverse-dynamics VJP of stage g, else NULL
+  T* kpb; T* kdb;                          // [nv x ld] each, added to; NULL = not wanted
+  T* qrefb; T* vrefb; T* vdrefb;           // at the step, added to; NULL = not wanted
+};
+
+// the seed m of one velocity row: τ̄ where the applied torque is strictly inside the bounds
+template <class T> RBD_HD T pd_mask(T taub, T tau, T lo, T hi) { return (lo < tau && tau < hi) ? taub : T(0); }
+
+// The law's adjoint for one joint of one stage (sample column b, mid phase g < 4): cq [nq] / cv [nv] receive the additions to q̄s /
+// v̄s, m [nv] the torque seed (τ̄_ff); the gain and reference adjoints are accumulated in place (this thread owns the rows).
+template <class T> RBD_HD void pd_adj_joint(const BodyDev<T>& bd, const AdjStepArgs<T>& a, const PdAdjArgs<T>& c, int64_t b, T* cq, T* cv,
+                                            T* m) {
+  const int kind = bd.kind, qr = bd.qrow, vr = bd.vrow, nq = kind_nq_dev(kind), nv = kind_nv_dev(kind);
+  auto Q = [&](int k) { return (int64_t)(qr + k) * a.ld + b; };
+  auto V = [&](int k) { return (int64_t)(vr + k) * a.ld + b; };
+  T q[7], qref[7], e[6], eb[6];
+  for (int k = 0; k < nq; ++k) { q[k] = a.qs[a.g][Q(k)]; qref[k] = c.qref[Q(k)]; cq[k] = T(0); }
+  joint_error(kind, qref, q, e);
+  for (int k = 0; k < nv; ++k) {
+    const int64_t r = V(k), gi = c.g_ld ? r : vr + k;
+    m[k] = c.tau ? pd_mask(a.taub[r], c.tau[r], c.lo[vr + k], c.hi[vr + k]) : a.taub[r];
+    T w = m[k];
+    cv[k] = T(0);
+    if (c.idvd) {
+      w = c.idvd[r];
+      cv[k] = c.idv[r];
+      if (c.vdrefb) c.vdrefb[r] += w;
+    }
+    const T kd = c.kd[gi], dv = a.vs[a.g][r] - (c.vref ? c.vref[r] : T(0));
+    if (c.kpb) c.kpb[r] -= w * e[k];
+    if (c.kdb) c.kdb[r] -= w * dv;
+    if (c.vrefb) c.vrefb[r] += kd * w;
+    cv[k] -= kd * w;
+    eb[k] = -c.kp[gi] * w;
+  }
+  if (c.idq)
+    for (int k = 0; k < nq; ++k) cq[k] = c.idq[Q(k)];
+  if (kind == K_REV || kind == K_PRIS || kind == K_PLANAR || kind == K_SPQFLOAT) {     // e = q_s - q_ref
+    for (int k = 0; k < nq; ++k) {
+      cq[k] += eb[k];
+      if (c.qrefb) c.qrefb[Q(k)] -= eb[k];
+    }
+    return;
+  }
+  using D = Dual1<T>;
+  for (int dir = 0; dir < 2 * nq; ++dir) {
+    if (dir >= nq && !c.qrefb) break;
+    D dq[7], dr[7], de[6];
+    for (int k = 0; k < nq; ++k) {
+      dq[k] = D(q[k], dir == k ? T(1) : T(0));
+      dr[k] = D(qref[k], dir == nq + k ? T(1) : T(0));
+    }
+    joint_error<D>(kind, dr, dq, de);
+    T s = T(0);
+    for (int k = 0; k < nv; ++k) s += eb[k] * de[k].d;
+    if (dir < nq) cq[dir] += s;
+    else c.qrefb[Q(dir - nq)] += s;
+  }
+}
+
+// any joint at sample column b; PD: with the controller's adjoint of stage g (c) in the mid phases
+template <class T, bool PD = false>
+RBD_HD void adj_joint(const BodyDev<T>& bd, const AdjStepArgs<T>& a, int64_t b, const PdAdjArgs<T>* c = nullptr) {
   const int kind = bd.kind, qr = bd.qrow, vr = bd.vrow, nq = kind_nq_dev(kind), nv = kind_nv_dev(kind);
   if (nv == 0) return;
   auto Q = [&](int k) { return (int64_t)(qr + k) * a.ld + b; };
@@ -204,6 +282,11 @@ template <class T> RBD_HD void adj_joint(const BodyDev<T>& bd, const AdjStepArgs
       x.qcb = a.qcb[Q(0)]; x.vvb = a.vvb[V(0)]; x.vsb = a.vsb[V(0)]; x.qb0 = a.qb0[Q(0)]; x.vb0 = a.vb0[V(0)];
       x.taub = a.tau_bar ? a.taub[V(0)] : T(0);
       x.qtb = a.qtb ? a.qtb[Q(0)] : T(0); x.vtb = a.vtb ? a.vtb[V(0)] : T(0);
+      if constexpr (PD) {
+        T cq[7], cv[6], m[6];
+        pd_adj_joint(bd, a, *c, b, cq, cv, m);
+        x.qcb += cq[0]; x.vvb += cv[0]; x.taub = m[0];
+      }
     }
     adj_lin(a, x, o);
     a.qb0[Q(0)] = o.qb0; a.vb0[V(0)] = o.vb0;
@@ -229,13 +312,24 @@ template <class T> RBD_HD void adj_joint(const BodyDev<T>& bd, const AdjStepArgs
   } else {
     const int g = a.g;
     T phi[6], qsb[7], vsb[6], phib[6];
-    for (int k = 0; k < nq; ++k) { qsb[k] = a.qsb[Q(k)] + a.qcb[Q(k)]; q0b[k] = a.qb0[Q(k)]; }
+    T cq[7], cv[6], m[6];
+    if constexpr (PD) pd_adj_joint(bd, a, *c, b, cq, cv, m);
+    for (int k = 0; k < nq; ++k) {
+      qsb[k] = a.qsb[Q(k)] + a.qcb[Q(k)];
+      if constexpr (PD) qsb[k] += cq[k];
+      q0b[k] = a.qb0[Q(k)];
+    }
     for (int k = 0; k < nv; ++k) {
       const int64_t e = V(k);
       phi[k] = g ? a.wa[g] * a.pd[g - 1][e] : T(0);
       vsb[k] = a.vsb[e] + a.vvb[e];
+      if constexpr (PD) vsb[k] += cv[k];
       a.vb0[e] += vsb[k];
-      if (a.tau_bar) a.tau_bar[e] += a.taub[e];
+      if constexpr (PD) {
+        if (a.tau_bar) a.tau_bar[e] += m[k];
+      } else if (a.tau_bar) {
+        a.tau_bar[e] += a.taub[e];
+      }
     }
     g_adjoint(kind, q0, phi, qsb, q0b, g ? phib : (T*)nullptr);
     for (int k = 0; k < nv && g; ++k) { pn[k] = a.wa[g] * phib[k]; vn[k] = a.wa[g] * vsb[k]; }

@@ -16,6 +16,7 @@
 #include <memory>
 #include <optional>
 #include <string>
+#include <vector>
 
 #include "../../../include/rbd_b200.h"
 #define sincos_slow sincos_slow_integrate_vjp_tu
@@ -90,6 +91,113 @@ __global__ void __launch_bounds__(256) integrate_adjoint_linear_kernel(const __g
   }
 }
 
+// rbd_integrate_pd_vjp: the two phase kernels above with the controller's adjoint of stage g in the mid phases
+// (rbd_integrate_adjoint.cuh's pd_adj_joint); the open-loop instantiations above stay as they are.
+template <class T>
+__global__ void __launch_bounds__(128) integrate_adjoint_pd_kernel(const __grid_constant__ ModelDev<T> M, const AdjStepArgs<T> a,
+                                                                   const PdAdjArgs<T> c, const bool skip_linear) {
+  const BodyDev<T>& bd = M.body[blockIdx.y];
+  if (bd.kind == K_FIXED) return;
+  if (skip_linear && (bd.kind == K_REV || bd.kind == K_PRIS)) return;
+  for (int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; b < a.ld; b += (int64_t)gridDim.x * blockDim.x)
+    adj_joint<T, true>(bd, a, b, &c);
+}
+
+// revolute / prismatic rows, VEC samples per thread: per lane the arithmetic of adj_joint<T, true>'s revolute / prismatic branch
+template <class T>
+__global__ void __launch_bounds__(256) integrate_adjoint_pd_linear_kernel(const __grid_constant__ ModelDev<T> M, const AdjStepArgs<T> a,
+                                                                          const PdAdjArgs<T> c) {
+  using V = typename VecOf<T>::type;
+  constexpr int N = VecOf<T>::N;
+  const BodyDev<T>& bd = M.body[blockIdx.y];
+  if (bd.kind != K_REV && bd.kind != K_PRIS) return;
+  const int64_t qo = (int64_t)bd.qrow * a.ld, vo = (int64_t)bd.vrow * a.ld, nvec = a.ld / N;
+  auto ld = [&](const T* p, int64_t off, int64_t i, T* x) {
+    const V w = reinterpret_cast<const V*>(p + off)[i];
+    memcpy(x, &w, sizeof(V));
+  };
+  auto st = [&](T* p, int64_t off, int64_t i, const T* x) {
+    V w;
+    memcpy(&w, x, sizeof(V));
+    reinterpret_cast<V*>(p + off)[i] = w;
+  };
+  auto add = [&](T* p, int64_t off, int64_t i, const T* x, T sign) {     // p += sign x (sign = ±1: exact)
+    T y[N];
+    ld(p, off, i, y);
+#pragma unroll
+    for (int k = 0; k < N; ++k) y[k] += sign * x[k];
+    st(p, off, i, y);
+  };
+  const int64_t go = (int64_t)bd.vrow * c.g_ld;
+  const T lo = c.tau ? c.lo[bd.vrow] : T(0), hi = c.tau ? c.hi[bd.vrow] : T(0);
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < nvec; i += (int64_t)gridDim.x * blockDim.x) {
+    T qb[N], vb[N], phib[N], qcb[N], vvb[N], vsb[N], taub[N], qtb[N], vtb[N], qb0[N], vb0[N];
+    ld(a.qb, qo, i, qb); ld(a.vb, vo, i, vb); ld(a.phib, vo, i, phib);
+    const bool mid = a.g < 4;
+    T kpw[N], kdw[N], vrw[N], eb[N];      // the law's adjoint: w e (-> K̄p), w (v_s - v_ref) (-> K̄d), Kd w (-> v̄_ref), ē
+    if (mid) {
+      ld(a.qcb, qo, i, qcb); ld(a.vvb, vo, i, vvb); ld(a.vsb, vo, i, vsb); ld(a.qb0, qo, i, qb0); ld(a.vb0, vo, i, vb0);
+      ld(a.taub, vo, i, taub);
+      if (a.qtb) ld(a.qtb, qo, i, qtb);
+      if (a.vtb) ld(a.vtb, vo, i, vtb);
+      T qs[N], vs[N], qr[N], vr[N], kp[N], kd[N], tau[N], w[N], idq[N], idv[N];
+      ld(a.qs[a.g], qo, i, qs); ld(a.vs[a.g], vo, i, vs); ld(c.qref, qo, i, qr);
+      if (c.vref) ld(c.vref, vo, i, vr);
+      if (c.g_ld) { ld(c.kp, go, i, kp); ld(c.kd, go, i, kd); }
+      if (c.tau) ld(c.tau, vo, i, tau);
+      if (c.idvd) { ld(c.idvd, vo, i, w); ld(c.idq, qo, i, idq); ld(c.idv, vo, i, idv); }
+#pragma unroll
+      for (int k = 0; k < N; ++k) {
+        if (c.tau) taub[k] = pd_mask(taub[k], tau[k], lo, hi);
+        if (!c.idvd) w[k] = taub[k];
+        const T kpk = c.g_ld ? kp[k] : c.kp[bd.vrow], kdk = c.g_ld ? kd[k] : c.kd[bd.vrow];
+        const T e = qs[k] - qr[k], dv = vs[k] - (c.vref ? vr[k] : T(0));
+        kpw[k] = w[k] * e; kdw[k] = w[k] * dv; vrw[k] = kdk * w[k];
+        eb[k] = -kpk * w[k];
+        T cq = c.idvd ? idq[k] : T(0), cv = c.idvd ? idv[k] : T(0);      // pd_adj_joint's order of operations
+        cv -= vrw[k];
+        cq += eb[k];
+        qcb[k] += cq; vvb[k] += cv;
+      }
+      if (c.kpb) add(c.kpb, vo, i, kpw, T(-1));
+      if (c.kdb) add(c.kdb, vo, i, kdw, T(-1));
+      if (c.vrefb) add(c.vrefb, vo, i, vrw, T(1));
+      if (c.vdrefb) add(c.vdrefb, vo, i, w, T(1));
+      if (c.qrefb) add(c.qrefb, qo, i, eb, T(-1));
+    }
+    T o_qb[N], o_vb[N], o_qb0[N], o_vb0[N], o_phib[N], o_vdb[N], o_vsb[N], o_tau[N];
+#pragma unroll
+    for (int c_ = 0; c_ < N; ++c_) {
+      LinIn<T> x;
+      LinOut<T> o;
+      x.qb = qb[c_]; x.vb = vb[c_]; x.phib = phib[c_];
+      if (mid) {
+        x.qcb = qcb[c_]; x.vvb = vvb[c_]; x.vsb = vsb[c_]; x.qb0 = qb0[c_]; x.vb0 = vb0[c_];
+        x.taub = taub[c_]; x.qtb = a.qtb ? qtb[c_] : T(0); x.vtb = a.vtb ? vtb[c_] : T(0);
+      }
+      adj_lin(a, x, o);
+      o_qb[c_] = o.qb; o_vb[c_] = o.vb; o_qb0[c_] = o.qb0; o_vb0[c_] = o.vb0; o_phib[c_] = o.phib; o_vdb[c_] = o.vdb; o_vsb[c_] = o.vsb;
+      o_tau[c_] = o.tau;
+    }
+    st(a.qb0, qo, i, o_qb0); st(a.vb0, vo, i, o_vb0);
+    if (!mid) st(a.phib, vo, i, o_phib);
+    if (mid && a.tau_bar) add(a.tau_bar, vo, i, o_tau, T(1));
+    if (a.g == 0) { st(a.qb, qo, i, o_qb); st(a.vb, vo, i, o_vb); }
+    if (a.l >= 0) { st(a.vsb, vo, i, o_vsb); st(a.vdb, vo, i, o_vdb); }
+  }
+}
+
+// computed-torque mode with effort bounds: τ̄ of a stage -> the seed m = τ̄ 1[lo < τ < hi] of its inverse-dynamics VJP, in place
+template <class T> struct PdMaskArgs { T* taub; const T* tau; const T* lo; const T* hi; int64_t nv, B; };
+template <class T>
+__global__ void __launch_bounds__(256) pd_mask_kernel(const PdMaskArgs<T> a) {
+  const int64_t total = a.nv * a.B;
+  for (int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t k = e / a.B;
+    a.taub[e] = pd_mask(a.taub[e], a.tau[e], a.lo[k], a.hi[k]);
+  }
+}
+
 // q̄ (configuration coordinates) -> tangent and minimal-norm configuration forms: between steps (in place) and for the outputs
 template <class T> struct OutArgs { const T* q; const T* qb; T* qt; T* qc; int64_t B; };
 template <class T>
@@ -148,26 +256,56 @@ template <class T> struct ContactVjp {
   T* s0b;
 };
 
+// the controller of rbd_integrate_pd_vjp and the adjoints of its arrays (each NULL = not wanted)
+struct PdVjp {
+  const rbd_pd_desc* pd;
+  rbd_pd_bar bar;
+};
+
 template <class T>
 int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q_traj, const T* v_traj, const T* tau, int64_t step_stride,
                     int64_t stage_stride, double dt, int nsteps, const T* qtb, const T* vtb, T* q0t, T* q0c, T* v0b, T* taub,
-                    cudaStream_t stream, const ContactVjp<T>* contact = nullptr) {
+                    cudaStream_t stream, const ContactVjp<T>* contact = nullptr, const PdVjp* ctl = nullptr) {
   const HostModel& hm = model->hm;
   const ModelDev<T>& M = dev_model<T>(hm);
   const int64_t nq = hm.nq, nv = hm.nv, ns = contact ? contact->ns : 0;
+  const rbd_pd_desc* pd = ctl ? ctl->pd : nullptr;
+  const bool ct = pd && pd->mode == RBD_PD_COMPUTED_TORQUE, bounds = pd && pd->effort_lo;
   DeviceProps p;
   RBD_CUDA_TRY(device_props(p));
-  // workspace: the four stages (with contact: and their ṡ_i), then q̄_cfg / q̄ / q̄0 / q̄s (nq rows each), v̄ / τ̄ / v̄ / v̄0 / v̄s / v̇̄ / Φ̄
-  // (nv rows each), then with contact s̄1 / s̄0 / the carried dt a_i s̄_i (ns rows each)
-  const int64_t srows = stage_rows(nq, nv) + 4 * ns, rows = srows + 4 * nq + 7 * nv + 3 * ns;
+  // workspace: the four stages (with contact: and their ṡ_i; with a controller: their applied torques and, in computed-torque mode,
+  // v̇_des), then q̄_cfg / q̄ / q̄0 / q̄s (nq rows each), v̄ / τ̄ / v̄ / v̄0 / v̄s / v̇̄ / Φ̄ (nv rows each), then with contact s̄1 / s̄0 / the
+  // carried dt a_i s̄_i (ns rows each), then in computed-torque mode the inverse-dynamics VJP's q̄_cfg (nq) / v̄ / v̇̄_des (nv), then
+  // the effort bounds (2 nv values)
+  const int64_t prow = stage_rows(nq, nv) + 4 * ns;
+  const int64_t srows = prow + (pd ? pd_stage_rows(nv, ct) : 0);
+  const int64_t rows = srows + 4 * nq + 7 * nv + 3 * ns + (ct ? nq + 2 * nv : 0);
   StreamAlloc work;
-  RBD_CUDA_TRY(work.alloc((size_t)rows * B * sizeof(T), stream));
+  RBD_CUDA_TRY(work.alloc(((size_t)rows * B + (bounds ? 2 * nv : 0)) * sizeof(T), stream));
   T* stages = (T*)work.p;
   T* next = stages + srows * B;
   auto take = [&](int64_t r) { T* o = next; next += r * B; return o; };
   T *qcb = take(nq), *qb = take(nq), *qb0 = take(nq), *qsb = take(nq);
   T *vvb = take(nv), *tb = take(nv), *vb = take(nv), *vb0 = take(nv), *vsb = take(nv), *vdb = take(nv), *phib = take(nv);
   T *sb1 = take(ns), *sacc = take(ns), *sdc = take(ns);
+  T *idq = take(ct ? nq : 0), *idv = take(ct ? nv : 0), *idvd = take(ct ? nv : 0);
+  // the controller: device bounds (copied from pageable memory, as integrate_t does), the recompute's per-stage rows
+  const T* lo = nullptr;
+  const T* hi = nullptr;
+  if (bounds) {
+    std::vector<T> h(2 * nv);
+    for (int64_t k = 0; k < nv; ++k) { h[k] = (T)pd->effort_lo[k]; h[nv + k] = (T)pd->effort_hi[k]; }
+    T* dev = (T*)work.p + (size_t)rows * B;
+    RBD_CUDA_TRY(cudaMemcpyAsync(dev, h.data(), 2 * nv * sizeof(T), cudaMemcpyHostToDevice, stream));
+    lo = dev; hi = dev + nv;
+  }
+  const T* tau_applied[4] = {nullptr, nullptr, nullptr, nullptr};
+  const T* vd_des[4] = {nullptr, nullptr, nullptr, nullptr};
+  for (int i = 0; i < 4 && pd; ++i) {
+    tau_applied[i] = stages + (prow + (size_t)i * nv) * B;
+    if (ct) vd_des[i] = stages + (prow + (4 + (size_t)i) * nv) * B;
+  }
+  const bool want_tb = taub || pd;      // the controller's adjoint reads τ̄ of every stage
   const size_t qbytes = (size_t)nq * B * sizeof(T), vbytes = (size_t)nv * B * sizeof(T);
   if (qtb) RBD_CUDA_TRY(cudaMemcpyAsync(qb, qtb + (size_t)nsteps * nq * B, qbytes, cudaMemcpyDeviceToDevice, stream));
   else RBD_CUDA_TRY(cudaMemsetAsync(qb, 0, qbytes, stream));
@@ -190,7 +328,7 @@ int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q
     cva.work = (T*)cplan->work.p;
     cva.zero = cva.work + row_bytes / sizeof(T) * cplan->grid * 32;
     RBD_CUDA_TRY(cudaMemsetAsync(const_cast<T*>(cva.zero), 0, sizeof(T), stream));
-    cva.vdb = vdb; cva.qc = qcb; cva.vb = vvb; cva.taub = taub ? tb : nullptr;
+    cva.vdb = vdb; cva.qc = qcb; cva.vb = vvb; cva.taub = (taub || ctl) ? tb : nullptr;
     cva.sb1 = sb1; cva.sacc = sacc; cva.sdc = sdc; cva.B = B;
   }
   bool has_other = false;
@@ -198,8 +336,15 @@ int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q
   constexpr int N = VecOf<T>::N;
   const size_t va = sizeof(typename VecOf<T>::type);
   auto aligned = [&](const T* x, int64_t stride) { return !x || ((uintptr_t)x % va == 0 && stride % N == 0); };
-  const bool vec_ok = B % N == 0 && B >= 1024 && aligned(taub, step_stride) && aligned(taub, stage_stride) && aligned(qtb, 0) &&
-                      aligned(vtb, 0) && aligned(q_traj, 0);
+  bool vec_ok = B % N == 0 && B >= 1024 && aligned(taub, step_stride) && aligned(taub, stage_stride) && aligned(qtb, 0) &&
+                aligned(vtb, 0) && aligned(q_traj, 0);
+  if (pd) {     // ... and every controller array and controller adjoint (kp_bar / kd_bar are [nv x B] whatever gain_ld is)
+    const rbd_pd_bar& cb = ctl->bar;
+    vec_ok = vec_ok && aligned((const T*)pd->q_ref, pd->q_ref_step_stride) && aligned((const T*)pd->v_ref, pd->v_ref_step_stride) &&
+             (pd->gain_ld == 0 || (aligned((const T*)pd->kp, 0) && aligned((const T*)pd->kd, 0))) && aligned((const T*)cb.kp, 0) &&
+             aligned((const T*)cb.kd, 0) && aligned((const T*)cb.q_ref, pd->q_ref_step_stride) &&
+             aligned((const T*)cb.v_ref, pd->v_ref_step_stride) && aligned((const T*)cb.vd_ref, pd->v_ref_step_stride);
+  }
   const int grid = (int)std::min<int64_t>((B + 127) / 128, (int64_t)p.sms * 8);
   const int grid_lin = (int)std::min<int64_t>((B / N + 255) / 256, (int64_t)p.sms * 4);
   const double ca[4] = {0.0, 0.5, 0.5, 1.0}, cb[4] = {1.0 / 6, 1.0 / 3, 1.0 / 3, 1.0 / 6};   // runge_kutta_4, as integrate_t
@@ -222,19 +367,46 @@ int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q
               stage_stride, dt, 1};
     r.stages = stages;
     r.contact = contact ? contact->cd : nullptr;
+    rbd_pd_desc pds{};      // the recompute is a one-step rollout: the controller's references start at step s
+    if (pd) {
+      pds = *pd;
+      const size_t vo = (size_t)s * pd->v_ref_step_stride;
+      pds.q_ref = (const T*)pd->q_ref + (size_t)s * pd->q_ref_step_stride;
+      pds.v_ref = pd->v_ref ? (const T*)pd->v_ref + vo : nullptr;
+      pds.vd_ref = pd->vd_ref ? (const T*)pd->vd_ref + vo : nullptr;
+      r.pd = &pds;
+      r.pd_bounds = lo;      // the bounds copied above: one host copy per call
+    }
     if (int rc = integrate(model, dtype, B, B, r, stream)) return rc;
     a.q0 = q0;
     a.qtb = qtb ? qtb + (size_t)s * nq * B : nullptr;
     a.vtb = vtb ? vtb + (size_t)s * nv * B : nullptr;
+    PdAdjArgs<T> c{};
+    if (pd) {     // the references and their adjoints of step s, as integrate_t reads the references
+      const size_t qo = (size_t)s * pd->q_ref_step_stride, vo = (size_t)s * pd->v_ref_step_stride;
+      const rbd_pd_bar& cb = ctl->bar;
+      c.qref = (const T*)pd->q_ref + qo;
+      c.vref = pd->v_ref ? (const T*)pd->v_ref + vo : nullptr;
+      c.kp = (const T*)pd->kp; c.kd = (const T*)pd->kd; c.g_ld = pd->gain_ld;
+      c.lo = lo; c.hi = hi;
+      if (ct) { c.idq = idq; c.idv = idv; c.idvd = idvd; }
+      c.kpb = (T*)cb.kp; c.kdb = (T*)cb.kd;
+      c.qrefb = cb.q_ref ? (T*)cb.q_ref + qo : nullptr;
+      c.vrefb = cb.v_ref ? (T*)cb.v_ref + vo : nullptr;
+      c.vdrefb = cb.vd_ref ? (T*)cb.vd_ref + vo : nullptr;
+    }
     for (int g = 4; g >= 0; --g) {
       a.g = g; a.l = g == 4 ? 3 : g - 1;
       a.tau_bar = (taub && g < 4) ? taub + s * step_stride + g * stage_stride : nullptr;
+      c.tau = (bounds && !ct && g < 4) ? tau_applied[g] : nullptr;     // computed-torque mode: masked before its VJP
       if (vec_ok) {
-        integrate_adjoint_linear_kernel<T><<<dim3(grid_lin, hm.nb), 256, 0, stream>>>(M, a);
+        if (pd) integrate_adjoint_pd_linear_kernel<T><<<dim3(grid_lin, hm.nb), 256, 0, stream>>>(M, a, c);
+        else integrate_adjoint_linear_kernel<T><<<dim3(grid_lin, hm.nb), 256, 0, stream>>>(M, a);
         if (int rc = api_launched()) return rc;
       }
       if (!vec_ok || has_other) {
-        integrate_adjoint_kernel<T><<<dim3(grid, hm.nb), 128, 0, stream>>>(M, a, vec_ok);
+        if (pd) integrate_adjoint_pd_kernel<T><<<dim3(grid, hm.nb), 128, 0, stream>>>(M, a, c, vec_ok);
+        else integrate_adjoint_kernel<T><<<dim3(grid, hm.nb), 128, 0, stream>>>(M, a, vec_ok);
         if (int rc = api_launched()) return rc;
       }
       if (a.l < 0) {
@@ -253,8 +425,17 @@ int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q
         cva.wa = a.wa[l]; cva.wdb = (T)dt * a.wb[l]; cva.l = l;
         contact_vjp_kernel<T><<<cplan->grid, cplan->block, cplan->smem, stream>>>(Mz, *contact->C, cva);
         if (int rc = api_launched(&*cplan)) return rc;
-      } else if (int rc = dynamics_vjp_dense(model, dtype, B, a.qs[a.l], a.vs[a.l], vd[a.l], vdb, qcb, vvb, taub ? tb : nullptr, stream)) {
+      } else if (int rc = dynamics_vjp_dense(model, dtype, B, a.qs[a.l], a.vs[a.l], vd[a.l], vdb, qcb, vvb, want_tb ? tb : nullptr, stream)) {
         return rc;
+      }
+      if (ct) {     // m = τ̄ masked by the applied torque, then the inverse-dynamics VJP at (q_s, v_s, v̇_des) seeded with m
+        const int l = a.l;
+        if (bounds) {
+          const PdMaskArgs<T> ma{tb, tau_applied[l], lo, hi, nv, B};
+          pd_mask_kernel<T><<<(int)std::min<int64_t>((nv * B + 255) / 256, (int64_t)p.sms * 8), 256, 0, stream>>>(ma);
+          if (int rc = api_launched()) return rc;
+        }
+        if (int rc = inverse_dynamics_vjp_dense(model, dtype, B, a.qs[l], a.vs[l], vd_des[l], tb, idq, idv, idvd, stream)) return rc;
       }
     }
   }
@@ -265,6 +446,24 @@ int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q
   if (v0b) RBD_CUDA_TRY(cudaMemcpyAsync(v0b, vb, vbytes, cudaMemcpyDeviceToDevice, stream));
   if (ns && contact->s0b) RBD_CUDA_TRY(cudaMemcpyAsync(contact->s0b, sb1, sbytes, cudaMemcpyDeviceToDevice, stream));
   return RBD_OK;
+}
+
+template <class T>
+int integrate_pd_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const void* q_traj, const void* v_traj, const void* s_traj,
+                       const void* tau, int64_t step_stride, int64_t stage_stride, const rbd_pd_desc& pd, const rbd_contact_desc* cd,
+                       double dt, int nsteps, const void* qtb, const void* vtb, const void* stb, void* q0t, void* q0c, void* v0b,
+                       void* s0b, void* taub, const rbd_pd_bar* bar, cudaStream_t stream) {
+  const HostModel& hm = model->hm;
+  const PdVjp ctl{&pd, bar ? *bar : rbd_pd_bar{}};
+  std::unique_ptr<ContactDev<T>> C;
+  std::optional<ContactVjp<T>> cv;
+  if (cd) {
+    C.reset(new ContactDev<T>());
+    build_contact_dev<T>(hm.nb, hm.pos.data(), hm.alignT.data(), *cd, *C);
+    cv.emplace(ContactVjp<T>{cd, C.get(), (int64_t)3 * cd->npoints * cd->nhalfspaces, (const T*)s_traj, (const T*)stb, (T*)s0b});
+  }
+  return integrate_vjp_t<T>(model, dtype, B, (const T*)q_traj, (const T*)v_traj, (const T*)tau, step_stride, stage_stride, dt, nsteps,
+                            (const T*)qtb, (const T*)vtb, (T*)q0t, (T*)q0c, (T*)v0b, (T*)taub, stream, cv ? &*cv : nullptr, &ctl);
 }
 
 template <class T>
@@ -326,4 +525,50 @@ extern "C" int32_t rbd_integrate_contact_vjp(const rbd_model* model, int32_t dty
                                               nsteps, q_traj_bar, v_traj_bar, s_traj_bar, q0_bar_tan, q0_bar_cfg, v0_bar, s0_bar, tau_bar, s)
              : integrate_contact_vjp_t<double>(model, dtype, B, q_traj, v_traj, s_traj, tau, tau_step_stride, tau_stage_stride, *contact, dt,
                                                nsteps, q_traj_bar, v_traj_bar, s_traj_bar, q0_bar_tan, q0_bar_cfg, v0_bar, s0_bar, tau_bar, s);
+}
+
+extern "C" int32_t rbd_integrate_pd_vjp(const rbd_model* model, int32_t dtype, int64_t B, const void* q_traj, const void* v_traj,
+                                        const void* s_traj, const void* tau, int64_t tau_step_stride, int64_t tau_stage_stride,
+                                        const rbd_pd_desc* pd, const rbd_contact_desc* contact, double dt, int32_t nsteps,
+                                        const void* q_traj_bar, const void* v_traj_bar, const void* s_traj_bar, void* q0_bar_tan,
+                                        void* q0_bar_cfg, void* v0_bar, void* s0_bar, void* tau_bar, const rbd_pd_bar* pd_bar,
+                                        void* stream) {
+  const char* fn = "rbd_integrate_pd_vjp";
+  auto fail = [&](int status, const char* what) { return api_fail(status, std::string(fn) + ": " + what); };
+  if (int rc = api_check(model, dtype, B, B)) return rc;
+  const ApiCall call;
+  if (dtype != RBD_F32 && dtype != RBD_F64) return fail(RBD_EUNSUPPORTED, "fp32 and fp64 only");
+  if (nsteps < 0 || !(dt > 0)) return fail(RBD_EINVAL, "need dt > 0 and nsteps >= 0");
+  if (tau_step_stride < 0 || tau_stage_stride < 0) return fail(RBD_EINVAL, "torque strides must be >= 0");
+  if (!tau && tau_bar) return fail(RBD_EINVAL, "tau_bar needs tau");
+  if (contact)
+    if (int rc = api_check_contact(model, contact, fn)) return rc;
+  // the controller: rbd_integrate_pd's checks, with leading dimension B
+  if (!pd) return fail(RBD_EINVAL, "pd must not be NULL");
+  if (!pd->kp || !pd->kd || !pd->q_ref) return fail(RBD_EINVAL, "kp, kd and q_ref must not be NULL");
+  if (pd->mode != RBD_PD_TORQUE && pd->mode != RBD_PD_COMPUTED_TORQUE) return fail(RBD_EINVAL, "unknown mode");
+  if (pd->q_ref_step_stride < 0 || pd->v_ref_step_stride < 0) return fail(RBD_EINVAL, "reference strides must be >= 0");
+  if (pd->gain_ld != 0 && pd->gain_ld != B) return fail(RBD_EINVAL, "gain_ld must be 0 or B");
+  if (pd->mode == RBD_PD_TORQUE && pd->vd_ref) return fail(RBD_EINVAL, "vd_ref is for computed-torque mode only");
+  if (!pd->effort_lo != !pd->effort_hi) return fail(RBD_EINVAL, "effort_lo and effort_hi must be both NULL or both set");
+  if (pd->effort_lo)
+    for (int k = 0; k < model->hm.nv; ++k)
+      if (!(pd->effort_lo[k] <= pd->effort_hi[k])) return fail(RBD_EINVAL, "effort bounds need lo <= hi");
+  // the adjoint of an array exists only where the array does
+  if (pd_bar && ((pd_bar->v_ref && !pd->v_ref) || (pd_bar->vd_ref && !pd->vd_ref)))
+    return fail(RBD_EINVAL, "pd_bar->v_ref / vd_ref need pd->v_ref / vd_ref");
+  if (pd->mode == RBD_PD_COMPUTED_TORQUE)
+    if (int rc = check_vjp_limits(model->hm, fn)) return rc;
+  const int64_t ns = contact ? (int64_t)3 * contact->npoints * contact->nhalfspaces : 0;
+  if (B == 0 || model->hm.nv == 0) return RBD_OK;
+  if (!q_traj || !v_traj) return fail(RBD_EINVAL, "q_traj and v_traj must not be NULL");
+  if (ns > 0 && !s_traj) return fail(RBD_EINVAL, "s_traj must not be NULL when there are contact pairs");
+  cudaStream_t s = (cudaStream_t)stream;
+  return dtype == RBD_F32
+             ? integrate_pd_vjp_t<float>(model, dtype, B, q_traj, v_traj, s_traj, tau, tau_step_stride, tau_stage_stride, *pd, contact, dt,
+                                         nsteps, q_traj_bar, v_traj_bar, s_traj_bar, q0_bar_tan, q0_bar_cfg, v0_bar, s0_bar, tau_bar,
+                                         pd_bar, s)
+             : integrate_pd_vjp_t<double>(model, dtype, B, q_traj, v_traj, s_traj, tau, tau_step_stride, tau_stage_stride, *pd, contact,
+                                          dt, nsteps, q_traj_bar, v_traj_bar, s_traj_bar, q0_bar_tan, q0_bar_cfg, v0_bar, s0_bar, tau_bar,
+                                          pd_bar, s);
 }

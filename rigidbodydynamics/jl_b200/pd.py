@@ -29,13 +29,21 @@ class _RbdPdDesc(ctypes.Structure):
                 ("effort_lo", ctypes.POINTER(ctypes.c_double)), ("effort_hi", ctypes.POINTER(ctypes.c_double))]
 
 
+class _RbdPdBar(ctypes.Structure):
+    _fields_ = [("kp", ctypes.c_void_p), ("kd", ctypes.c_void_p), ("q_ref", ctypes.c_void_p), ("v_ref", ctypes.c_void_p),
+                ("vd_ref", ctypes.c_void_p)]
+
+
 class JointPD:
     """Joint-space feedback for a closed-loop rollout.
 
     ``kp``, ``kd``: gains per velocity DoF, [nv] (shared by the batch) or [nv, B] (per sample).  ``q_ref`` [nq, B] (held over the
     call) or [nsteps, nq, B] (per step); its quaternions must be unit quaternions (they are not normalised).  ``v_ref``, and
     ``vd_ref`` (computed-torque mode only), [nv, B] or [nsteps, nv, B]; None = 0.  ``effort_bounds``: ``(lo, hi)`` arrays [nv] in
-    velocity order, e.g. ``effort_bounds(mechanism)``; None = unbounded.  All tensors: the dtype and device of the state."""
+    velocity order, e.g. ``effort_bounds(mechanism)``; None = unbounded.  All tensors: the dtype and device of the state.
+
+    ``autodiff.simulate`` / ``autodiff.simulate_contact`` take one as ``controller=`` too: gradients then also flow to those of
+    ``kp``, ``kd``, ``q_ref``, ``v_ref`` and ``vd_ref`` that require grad (DESIGN 4.19); the effort bounds receive none."""
 
     def __init__(self, kp, kd, q_ref, v_ref=None, *, vd_ref=None, computed_torque: bool = False, effort_bounds=None):
         self.kp, self.kd, self.q_ref, self.v_ref, self.vd_ref = kp, kd, q_ref, v_ref, vd_ref
@@ -93,3 +101,9 @@ class JointPD:
                        ptr(vd_ref), qs, vs or vds, None if lo is None else lo.ctypes.data_as(dp),
                        None if hi is None else hi.ctypes.data_as(dp))
         return d, keep
+
+    def _steps_from(self, first: int) -> "JointPD":
+        """The controller of a rollout that starts at step ``first`` of this one (per-step references sliced)."""
+        cut = lambda t: t if t is None or t.dim() == 2 else t[first:]      # noqa: E731
+        return JointPD(self.kp, self.kd, cut(self.q_ref), cut(self.v_ref), vd_ref=cut(self.vd_ref), computed_torque=self.computed_torque,
+                       effort_bounds=self.effort_bounds)
