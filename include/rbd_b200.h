@@ -622,6 +622,23 @@ typedef struct rbd_task_out {
 int32_t rbd_task_kinematics(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                             const void* vd, const rbd_task_desc* tasks, const rbd_task_out* out, void* stream);
 
+/* Reverse mode of rbd_task_kinematics (DESIGN 4.20): for the same (q, v, vd, tasks), the product  Σ_outputs ȳ . ∂y/∂(q, v, v̇)  over
+ * any subset of the eight outputs.  `out_bar` reuses rbd_task_out: each member is NULL (zero cotangent) or the cotangent ȳ with
+ * exactly that output's layout and leading dimension ld.  Cotangent rows of Jacobian columns off a task's path are not read (those
+ * columns are structurally zero).  Outputs, each [rows x B] with leading dimension ld or NULL (not wanted), are WRITTEN, not
+ * accumulated, with the conventions of rbd_dynamics_vjp:
+ *   q_bar_tan [nv]  derivative along velocity_to_configuration_derivative(e_j)
+ *   q_bar_cfg [nq]  q_bar_tan mapped like configuration_derivative_to_velocity_adjoint! (no radial quaternion component)
+ *   v_bar [nv], vd_bar [nv]  (zero when no velocity / acceleration cotangent is given)
+ * Every forward quantity is recomputed from q, v and vd; the forward outputs are not needed.  Errors, all decided on the host before
+ * any CUDA call: those of rbd_task_kinematics with out_bar in place of out (the descriptor checks with the same codes; a cotangent
+ * on twist / point_velocity / acceleration / point_acceleration with v == NULL: RBD_EINVAL).  B == 0: RBD_OK, nothing written;
+ * ntasks == 0: RBD_OK, the requested gradients set to zero.  Otherwise one kernel launch per call, with a stream-ordered workspace
+ * of 42 rows per body plus 42 per distinct body the tasks name, per resident thread (at most 512 MB). */
+int32_t rbd_task_kinematics_vjp(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
+                                const void* vd, const rbd_task_desc* tasks, const rbd_task_out* out_bar, void* q_bar_tan,
+                                void* q_bar_cfg, void* v_bar, void* vd_bar, void* stream);
+
 /* Host-pointer variants: same semantics, host buffers in, host buffers out, copies inside the call. */
 int32_t rbd_dynamics_host(rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                           const void* tau, const void* wext, void* vd_out, void* qd_out);

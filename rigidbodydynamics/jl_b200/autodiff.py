@@ -5,12 +5,15 @@
     integrate_vjp_         gradient of a recorded rollout       rbd_integrate_vjp         (csrc/rbd_integrate_adjoint.cuh)
     integrate_contact_vjp_ gradient of a recorded contact rollout  rbd_integrate_contact_vjp  (csrc/rbd_contact_adjoint.cuh)
     integrate_pd_vjp_      gradient of a recorded closed-loop rollout  rbd_integrate_pd_vjp  (csrc/rbd_integrate_adjoint.cuh)
+    task_kinematics_vjp_   Σ ȳᵀ ∂y/∂(q, v, v̇) of task-space outputs  rbd_task_kinematics_vjp  (csrc/rbd_task_adjoint.cuh)
     dynamics(mechanism, q, v, tau=None, externalwrenches=None)         differentiable v̇ = dynamics!(...)
     inverse_dynamics(mechanism, q, v, vd, externalwrenches=None)       differentiable τ = inverse_dynamics!(...)
     simulate(mechanism, q0, v0, torques=None, *, dt, nsteps, ...)     differentiable RK4 rollout (simulate)
     simulate_contact(mechanism, q0, v0, s0, torques=None, *, contact, dt, nsteps, ...)
                                                                        differentiable RK4 rollout with soft contact
     both with controller=JointPD(...): closed loop, gradients also to the controller's gains and references
+    task_kinematics(mechanism, q, v=None, vd=None, *, tasks, outputs=("point",))
+                                                                       differentiable task-space kinematics (TaskFrame tasks)
 
 One product costs one Articulated-Body solve (forward dynamics only) plus one outward and one inward sweep: O(n) per sample, no
 nv x nv Jacobian is formed (``dynamics_derivatives_`` builds both full Jacobians instead).  Every tensor is ``[rows, B]``, contiguous,
@@ -25,18 +28,21 @@ depends on how the formula extends off the unit sphere, and a gradient should no
 """
 from __future__ import annotations
 
-from typing import Optional
+import ctypes
+from types import SimpleNamespace
+from typing import Dict, Optional, Sequence
 
 import torch
 from torch.autograd.function import once_differentiable
 
 from . import _cabi
 from .algorithms import DimensionMismatch, _check, _ptr, _require_tree
+from .kinematics import _TASK_NEEDS_V, _TASK_ROWS, TaskFrame, task_desc
 from .mechanism import Mechanism
 from .state import _DT, MechanismState, _model_handle
 
 __all__ = ["dynamics_vjp_", "inverse_dynamics_vjp_", "integrate_vjp_", "integrate_contact_vjp_", "integrate_pd_vjp_", "dynamics",
-           "inverse_dynamics", "simulate", "simulate_contact"]
+           "inverse_dynamics", "simulate", "simulate_contact", "task_kinematics_vjp_", "task_kinematics"]
 
 
 def _stream(t: torch.Tensor):
@@ -194,6 +200,100 @@ def inverse_dynamics(mechanism: Mechanism, q: torch.Tensor, v: torch.Tensor, vd:
     """Differentiable ``τ = inverse_dynamics!(τ, state, v̇, externalwrenches)``; backward runs ``rbd_inverse_dynamics_vjp``.  Not
     twice differentiable."""
     return _InverseDynamics.apply(mechanism, q, v, vd, externalwrenches)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# task-space kinematics: rbd_task_kinematics / rbd_task_kinematics_vjp
+# ----------------------------------------------------------------------------------------------------------------------
+def _task_out(tensors: Dict[str, Optional[torch.Tensor]], K: int, nv: int, like: torch.Tensor, what: str) -> _cabi.RbdTaskOut:
+    """rbd_task_out for {output: [rows * K, B] tensor or None}, checked against the dtype, device and batch of ``like``."""
+    to = _cabi.RbdTaskOut()
+    for name, t in tensors.items():
+        if name not in _TASK_ROWS:
+            raise TypeError(f"{what}: unknown task kinematics output {name!r}")
+        if t is None:
+            continue
+        rows = _TASK_ROWS[name](SimpleNamespace(nv=nv))
+        if t.dtype != like.dtype or t.device != like.device:
+            raise TypeError(f"{what}: {name} must have the dtype and device of q")
+        if t.dim() != 2 or tuple(t.shape) != (rows * K, like.shape[1]):
+            raise DimensionMismatch(f"{what}: {name} has wrong size: expected ({rows * K}, {like.shape[1]}), got {tuple(t.shape)}")
+        if not t.is_contiguous():
+            raise ValueError(f"{what}: {name} must be [rows, B] contiguous (batch index fastest)")
+        setattr(to, name, t.data_ptr())
+    return to
+
+
+def task_kinematics_vjp_(state: MechanismState, tasks: Sequence[TaskFrame], vd: Optional[torch.Tensor] = None, *, bars: dict,
+                         q_bar_tan: Optional[torch.Tensor] = None, q_bar_cfg: Optional[torch.Tensor] = None,
+                         v_bar: Optional[torch.Tensor] = None, vd_bar: Optional[torch.Tensor] = None):
+    """The product ``Σ ȳᵀ ∂y/∂(q, v, v̇)`` of ``task_kinematics_(state, tasks, vd, ...)`` for every sample.
+
+    ``bars``: {output name: ȳ} with each ȳ in that output's layout ([rows * len(tasks), B]); missing outputs have zero cotangent.
+    Everything is recomputed from the state and ``vd`` (None = zero).  Outputs (each optional, overwritten): ``q_bar_tan`` [nv, B],
+    ``q_bar_cfg`` [nq, B], ``v_bar`` [nv, B], ``vd_bar`` [nv, B] (see the module docstring for the two configuration covectors)."""
+    state.check_modcount()
+    lib = _cabi.load_library()
+    to = _task_out(bars, len(tasks), state.nv, state.q, "task_kinematics_vjp_")
+    for t, rows, name in ((vd, state.nv, "vd"), (q_bar_tan, state.nv, "q_bar_tan"), (q_bar_cfg, state.nq, "q_bar_cfg"),
+                          (v_bar, state.nv, "v_bar"), (vd_bar, state.nv, "vd_bar")):
+        _check(t, rows, state, name)
+    d, keep = task_desc(state.mechanism, tasks)
+    _cabi.check(lib.rbd_task_kinematics_vjp(state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q),
+                                            _ptr(state.v), _ptr(vd), ctypes.byref(d), ctypes.byref(to), _ptr(q_bar_tan),
+                                            _ptr(q_bar_cfg), _ptr(v_bar), _ptr(vd_bar), _stream(state.q)))
+
+
+class _TaskKinematics(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, mechanism, tasks, outputs, q, v, vd):
+        h, B = _inputs(mechanism, "autodiff.task_kinematics", q=q, v=v, vd=vd)
+        if v is None and any(k in _TASK_NEEDS_V for k in outputs):
+            raise ValueError(f"autodiff.task_kinematics: {', '.join(k for k in outputs if k in _TASK_NEEDS_V)} need v")
+        K, nv = len(tasks), h.info.nv
+        outs = {k: torch.empty((_TASK_ROWS[k](SimpleNamespace(nv=nv)) * K, B), dtype=q.dtype, device=q.device) for k in outputs}
+        to = _task_out(outs, K, nv, q, "autodiff.task_kinematics")
+        d, keep = task_desc(mechanism, tasks)
+        if B and K:
+            _cabi.check(_cabi.load_library().rbd_task_kinematics(h.ptr, _DT[q.dtype], B, B, _ptr(q), _ptr(v), _ptr(vd), ctypes.byref(d),
+                                                                 ctypes.byref(to), _stream(q)))
+        ctx.handle, ctx.mechanism, ctx.tasks, ctx.outputs = h, mechanism, tasks, outputs
+        ctx.save_for_backward(q, v, vd)
+        return tuple(outs[k] for k in outputs)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, *grads):
+        q, v, vd = ctx.saved_tensors
+        h = ctx.handle
+        need = ctx.needs_input_grad
+        qb = _out(need[3], q, q.shape[0])
+        vb = _out(need[4] and v is not None, q, h.info.nv)
+        ab = _out(need[5] and vd is not None, q, h.info.nv)
+        bars = {k: g.contiguous() for k, g in zip(ctx.outputs, grads) if g is not None}
+        B = q.shape[1]
+        if B and any(t is not None for t in (qb, vb, ab)):
+            to = _task_out(bars, len(ctx.tasks), h.info.nv, q, "autodiff.task_kinematics")
+            d, keep = task_desc(ctx.mechanism, ctx.tasks)
+            _cabi.check(_cabi.load_library().rbd_task_kinematics_vjp(h.ptr, _DT[q.dtype], B, B, _ptr(q), _ptr(v), _ptr(vd),
+                                                                     ctypes.byref(d), ctypes.byref(to), None, _ptr(qb), _ptr(vb),
+                                                                     _ptr(ab), _stream(q)))
+        return None, None, None, qb, vb, ab
+
+
+def task_kinematics(mechanism: Mechanism, q: torch.Tensor, v: Optional[torch.Tensor] = None, vd: Optional[torch.Tensor] = None, *,
+                    tasks: Sequence[TaskFrame], outputs: Sequence[str] = ("point",)) -> Dict[str, torch.Tensor]:
+    """Differentiable task-space kinematics: {name: [rows * len(tasks), B]} for the requested ``outputs`` (names and layout of
+    ``task_kinematics_``) of q [nq, B], v [nv, B] (needed by twist / point_velocity / acceleration / point_acceleration) and vd
+    [nv, B] or None (zero).  Forward is one ``rbd_task_kinematics`` call for all outputs; backward one ``rbd_task_kinematics_vjp``
+    with the incoming gradients.  The gradient of ``q`` is ``q_bar_cfg`` (see the module docstring).  Not twice differentiable."""
+    tasks, outputs = tuple(tasks), tuple(outputs)
+    for k in outputs:
+        if k not in _TASK_ROWS:
+            raise TypeError(f"autodiff.task_kinematics: unknown task kinematics output {k!r}")
+    if len(set(outputs)) != len(outputs):
+        raise ValueError("autodiff.task_kinematics: outputs must be distinct")
+    return dict(zip(outputs, _TaskKinematics.apply(mechanism, tasks, outputs, q, v, vd)))
 
 
 # ----------------------------------------------------------------------------------------------------------------------
