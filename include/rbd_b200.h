@@ -639,6 +639,56 @@ int32_t rbd_task_kinematics_vjp(const rbd_model* model, int32_t dtype, int64_t B
                                 const void* vd, const rbd_task_desc* tasks, const rbd_task_out* out_bar, void* q_bar_tan,
                                 void* q_bar_cfg, void* v_bar, void* vd_bar, void* stream);
 
+/* Task-space feedback (DESIGN 4.21): the closed-loop rollouts of rbd_integrate_pd with a controller built from up to RBD_MAX_TASKS
+ * tasks of an rbd_task_desc, evaluated at EVERY RK4 stage on the stage state.  Each task yields f_t in its task frame and the
+ * controller adds u_task = Σ_t J_t^T f_t, with the reference's pd(gains, e, ė) = -k e - d ė (src/pdcontrol.jl:35), gains diagonal:
+ *   RBD_TASK_POINT (3 rows)  x = transform(state, point, base) in base coordinates, F = frame[t]:  e = R_F<-base (x - x_ref),
+ *                            ė = point_velocity in F - R_F<-base ẋ_ref,  f = -Kp e - Kd ė,  J_t = point_jacobian in F
+ *   RBD_TASK_POSE  (6 rows)  the frame C with origin at point[t] and the body's axes (frame[t] must equal body[t]); x = C -> base,
+ *                            T = twist of C w.r.t. base in C; e = inv(x_ref) x, ψ = rotation vector of R_e, p_e its translation:
+ *                            ang = -Kω ψ - Dω (ω - ω_ref),  lin = -Kv R_e^T p_e - Dv (v - v_ref)  (SE3PDGains, SE3PDMethod{:DoubleGeodesic},
+ *                            src/pdcontrol.jl:83-107), f = [ang; lin],  J_t = geometric Jacobian of C in C
+ * with R = Σ_t (3 | 6) gain / velocity rows and X = Σ_t (3 | 12) target rows in task order.  x_ref of a pose task is 12 rows in the
+ * layout of rbd_task_kinematics' transform (rotation row-major, translation); its rotation must be orthonormal (it is not
+ * re-orthonormalised).  Modes, with the optional joint-space term J = rbd_integrate_pd's law of `joint` (same mode):
+ *   RBD_PD_TORQUE            τ = τ_ff + J + u_task
+ *   RBD_PD_COMPUTED_TORQUE   v̇_des = J (with its v̇_ref) + u_task,  τ = inverse_dynamics!(q_s, v_s, v̇_des) + τ_ff
+ * then the effort bounds clamp the sum once.  kp / kd: device [R] (gain_ld 0) or [R x B] (gain_ld = ld); x_ref [X x B] and xd_ref
+ * [R x B] (NULL = 0) with leading dimension ld, the block of step s at s * step stride (0 = held over the call).  Everything else is
+ * rbd_integrate_pd's, with `ctrl` in place of `pd`.  Argument errors (before any CUDA call): JointPD's checks on `joint` and the
+ * descriptor checks of rbd_task_kinematics, with their codes; ctrl NULL, an unknown mode or kind, kind / kp / kd / x_ref NULL with
+ * tasks, a pose task with frame != body, negative strides, gain_ld other than 0 / ld, a joint term whose mode differs or that has its
+ * own effort bounds, only one of effort_lo / effort_hi, or lo > hi: RBD_EINVAL; RBD_PD_COMPUTED_TORQUE with loops: RBD_ELOOP.  When
+ * the per-sample working set does not fit a block (as rbd_task_kinematics): RBD_EUNSUPPORTED, before any kernel.  Kernels per
+ * stage: rbd_integrate_pd's with this controller's joint term (the open-loop rollout's without one), plus one task kernel. */
+#define RBD_TASK_POINT 0
+#define RBD_TASK_POSE 1
+typedef struct rbd_task_pd_desc {
+  int32_t mode;                          /* RBD_PD_TORQUE or RBD_PD_COMPUTED_TORQUE */
+  rbd_task_desc tasks;                   /* host arrays; frame[t] == body[t] for pose tasks */
+  const int32_t* kind;                   /* host [ntasks]: RBD_TASK_POINT / RBD_TASK_POSE */
+  const void* kp; const void* kd;        /* device [R] (gain_ld 0) or [R x B] (gain_ld = ld) */
+  int64_t gain_ld;
+  const void* x_ref;                     /* device [X x B] block per step */
+  int64_t x_ref_step_stride;             /* elements between the x_ref blocks of consecutive steps; 0 = held */
+  const void* xd_ref;                    /* device [R x B] block per step, NULL = 0 */
+  int64_t xd_ref_step_stride;
+  const rbd_pd_desc* joint;              /* NULL = no joint-space term; same mode; its effort bounds NULL */
+  const double* effort_lo;               /* host [nv], NULL = unbounded; clamp the sum */
+  const double* effort_hi;
+} rbd_task_pd_desc;
+int32_t rbd_integrate_task_pd(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau,
+                              int64_t tau_step_stride, int64_t tau_stage_stride, const rbd_task_pd_desc* ctrl,
+                              const rbd_loop_desc* loops /* NULL = tree or contact rollout */,
+                              const rbd_contact_desc* contact /* NULL = no contact */, double dt, int32_t nsteps, void* q_traj,
+                              void* v_traj, void* s_traj, void* stream);
+/* The law of rbd_integrate_task_pd at one state (q, v) with the references of step `step`: tau_out [nv x B] = the torques the
+ * rollout applies at a stage with that state (τ_ff = tau_ff, NULL = 0), every array with leading dimension ld.  The argument errors
+ * of rbd_integrate_task_pd (step < 0: RBD_EINVAL); B == 0: nothing to do.  Kernels: one in RBD_PD_TORQUE mode; in computed-torque
+ * mode the task kernel, the inverse dynamics and one elementwise kernel. */
+int32_t rbd_task_pd_torques(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
+                            const void* tau_ff, const rbd_task_pd_desc* ctrl, int32_t step, void* tau_out, void* stream);
+
 /* Host-pointer variants: same semantics, host buffers in, host buffers out, copies inside the call. */
 int32_t rbd_dynamics_host(rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                           const void* tau, const void* wext, void* vd_out, void* qd_out);

@@ -435,6 +435,68 @@ function task_kinematics!(state::BatchedState{T}, tasks; vd = nothing, outs...) 
     outs
 end
 
+"Mirror of `rbd_task_pd_desc` (include/rbd_b200.h)."
+struct rbd_task_pd_desc
+    mode::Int32
+    tasks::rbd_task_desc
+    kind::Ptr{Int32}
+    kp::Ptr{Cvoid}
+    kd::Ptr{Cvoid}
+    gain_ld::Int64
+    x_ref::Ptr{Cvoid}
+    x_ref_step_stride::Int64
+    xd_ref::Ptr{Cvoid}
+    xd_ref_step_stride::Int64
+    joint::Ptr{rbd_pd_desc}
+    effort_lo::Ptr{Float64}
+    effort_hi::Ptr{Float64}
+end
+
+"""
+    simulate_task_pd(state, final_time, tasks, kinds, kp, kd, x_ref; xd_ref = nothing, computed_torque = false,
+                     effort_bounds = nothing, torques = nothing, Δt = 1e-4)
+
+`simulate` with task-space feedback at every RK4 stage (rbd_integrate_task_pd, DESIGN 4.21): `tasks` as in `task_kinematics!`
+(for a pose task `frame` must be `nothing` or the body), `kinds` a vector of `:point` / `:pose`.  Each task adds J_t' f_t with
+f_t = -kp e - kd ė in its task frame: a point task's position relative to `base` (FramePDGains in `frame`), or the reference's
+double-geodesic `pd(SE3PDGains, x, x_ref, T, T_ref)` on the frame at the task's point with the body's axes (pdcontrol.jl:83-107).
+`kp`, `kd`: a vector of R = Σ (3 | 6) gains or a B × R matrix; `x_ref`: B × X (X = Σ (3 | 12), pose targets as `transform` of
+`task_kinematics!`), `xd_ref`: B × R or `nothing`, held over the call.  No joint-space term here.  Tree mechanisms without contact
+points.  (Not run here: no Julia installation is available to the project's tests; the Python binding exercises the same entry
+point.)
+"""
+function simulate_task_pd(state::BatchedState{T}, final_time, tasks, kinds, kp, kd, x_ref; xd_ref = nothing,
+                          computed_torque::Bool = false, effort_bounds = nothing, torques = nothing, Δt = 1e-4) where {T <: Union{Float32, Float64}}
+    checkstate(state)
+    B = size(state.q, 1)
+    model = state.model
+    nsteps = 0; t = 0.0
+    while t < final_time; t += Δt; nsteps += 1; end            # the reference's `while t < final_time` (ode_integrators.jl:311)
+    body = Int32[body_index(model, t[1]) for t in tasks]
+    base = Int32[body_index(model, t[2]) for t in tasks]
+    frame = Int32[k == :pose ? body[i] : (t[4] === nothing ? Int32(-1) : body_index(model, t[4]))
+                  for (i, (t, k)) in enumerate(zip(tasks, kinds))]
+    point = zeros(Float64, 3, length(tasks))
+    for (k, t) in enumerate(tasks)
+        t[3] === nothing || (point[:, k] .= t[3])
+    end
+    kind = Int32[k == :pose ? 1 : 0 for k in kinds]
+    lo, hi = effort_bounds === nothing ? (nothing, nothing) : (Vector{Float64}(effort_bounds[1]), Vector{Float64}(effort_bounds[2]))
+    ptr(x) = x === nothing ? C_NULL : devptr(x)
+    GC.@preserve state kp kd x_ref xd_ref torques lo hi body base frame point kind begin
+        td = rbd_task_desc(Int32(length(tasks)), pointer(body), pointer(base), pointer(frame), pointer(point))
+        desc = rbd_task_pd_desc(Int32(computed_torque ? 1 : 0), td, pointer(kind), devptr(kp), devptr(kd),
+                                ndims(kp) == 2 ? Int64(B) : Int64(0), devptr(x_ref), 0, ptr(xd_ref), 0, Ptr{rbd_pd_desc}(C_NULL),
+                                lo === nothing ? Ptr{Float64}(C_NULL) : pointer(lo), hi === nothing ? Ptr{Float64}(C_NULL) : pointer(hi))
+        check(ccall((:rbd_integrate_task_pd, librbd), Int32,
+                    (Ptr{Cvoid}, Int32, Int64, Int64, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Int64, Int64, Ref{rbd_task_pd_desc},
+                     Ptr{Cvoid}, Ptr{Cvoid}, Float64, Int32, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
+                    model.handle, dtype_code(T), B, B, devptr(state.q), devptr(state.v), C_NULL, ptr(torques), 0, 0, desc,
+                    C_NULL, C_NULL, Float64(Δt), Int32(nsteps), C_NULL, C_NULL, C_NULL, stream_ptr()))
+    end
+    nsteps
+end
+
 # ---- SURVEY 8(f) rank 3: Jacobians of forward dynamics ----------------------------------------------------------------------
 
 """

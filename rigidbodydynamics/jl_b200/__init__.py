@@ -33,7 +33,7 @@ from .loops import (LoopDesc, PDGains, SE3PDGains, constraint_wrench_subspace, d
                     dynamics_loops_, loop_desc, num_constraints, simulate_loops_, simulate_loops_trajectory_)
 from .mechanism import maximal_coordinates  # noqa: F401
 from .mechanism import Bounds, effort_bounds  # noqa: F401
-from .pd import JointPD  # noqa: F401
+from .pd import JointPD, TaskPD, task_pd_torques  # noqa: F401
 from . import autodiff  # noqa: F401  (rbd.autodiff.dynamics / inverse_dynamics: differentiable, kept out of this namespace)
 from .autodiff import dynamics_vjp_, integrate_contact_vjp_, integrate_pd_vjp_, integrate_vjp_, inverse_dynamics_vjp_  # noqa: F401
 from ._cabi import RbdError, launch_info, load_library  # noqa: F401

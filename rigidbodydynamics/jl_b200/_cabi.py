@@ -142,6 +142,8 @@ SYMBOLS = {
     "rbd_integrate_contact": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _vp, c_double, _i32, _vp, _vp, _vp, _vp]),
     "rbd_integrate_loops": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, c_double, _i32, _vp, _vp, _vp, _vp]),
     "rbd_integrate_pd": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, c_double, _i32, _vp, _vp, _vp, _vp]),
+    "rbd_integrate_task_pd": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, c_double, _i32, _vp, _vp, _vp, _vp]),
+    "rbd_task_pd_torques": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _i32, _vp, _vp]),
     "rbd_integrate_contact_vjp":(c_int32, [_vp, _i32, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _vp, c_double, _i32] + [_vp] * 9),
     "rbd_integrate_pd_vjp":   (c_int32, [_vp, _i32, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, c_double, _i32] + [_vp] * 10),
     "rbd_kinematics": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, POINTER(RbdKinematicsOut), _vp]),

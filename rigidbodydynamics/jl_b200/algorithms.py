@@ -17,7 +17,7 @@ from typing import Optional
 import torch
 
 from . import _cabi
-from .pd import JointPD
+from .pd import JointPD, TaskPD
 from .state import DynamicsResult, MechanismState, _DT
 
 __all__ = ["dynamics_", "dynamics_dual_", "dynamics_derivatives_", "dynamics_ode_", "simulate_", "simulate_trajectory_", "inverse_dynamics_", "inverse_dynamics", "mass_matrix_", "mass_matrix",
@@ -208,7 +208,11 @@ def _rollout(state: MechanismState, nsteps: int, torques: Optional[torch.Tensor]
     head = (state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q), _ptr(state.v))
     steps = (float(dt), nsteps)
     out = tuple(_ptr(t) for t in traj)
-    if controller is not None:
+    if isinstance(controller, TaskPD):
+        tpd, keep_tpd = controller._c_struct(state, nsteps, what)
+        _call(lib.rbd_integrate_task_pd(*head, _ptr(contact_state), _ptr(torques), step, stage, ctypes.byref(tpd), ref(lst), ref(cst),
+                                        *steps, *out, _stream()))
+    elif controller is not None:
         if not isinstance(controller, JointPD):
             raise TypeError(f"{what}: controller must be a JointPD")
         pd, keep_pd = controller._c_struct(state, nsteps, what)

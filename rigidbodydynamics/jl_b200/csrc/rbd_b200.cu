@@ -33,6 +33,7 @@
 #include "rbd_dual.cuh"
 #include "rbd_integrate.cuh"
 #include "rbd_pd.cuh"
+#include "rbd_task_pd.cuh"
 #include "rbd_model.h"
 
 using namespace rbd;
@@ -533,6 +534,61 @@ task_kernel(const __grid_constant__ ModelDev<T> M, const __grid_constant__ TaskD
     io.tr = out(a.tr); io.pt = out(a.pt); io.tw = out(a.tw); io.pv = out(a.pv);
     io.J = out(a.J); io.Jp = out(a.Jp); io.acc = out(a.acc); io.pacc = out(a.pacc);
     task_sample<T>(M, D, io, st);
+  }
+}
+
+// Task-space feedback (task_pd_sample, rbd_task_pd.cuh): one thread per sample, stash = pending slots + named-body slots + one
+// wrench per task.  Row k of `out` receives  base_k + Σ_t J_t^T f_t, clamped to [lo_k, hi_k] when lo is set, where base_k is
+//   the row itself            add (the rollout's stage kernels have already written the joint-space term there),
+//   rbd_pd.cuh's joint law    jkp set (rbd_task_pd_torques with a joint term: pd_joint on the same state, unclamped),
+//   ff_k                      otherwise (τ_ff in torque mode, NULL = 0).
+// Only the nv rows of `out` go to HBM; no Jacobian is stored.
+template <class T> struct TaskPdArgs {
+  const T *q, *v; int64_t sld;                       // state, leading dimension sld
+  const T *xref, *xdref, *kp, *kd; int64_t gain_ld;  // the task references of this step and the gains (caller arrays, ld)
+  const T* ff;                                       // base rows (caller array, ld) or NULL
+  const T *jqref, *jvref, *jff, *jkp, *jkd; int64_t jgain_ld;   // the joint term evaluated here (jkp NULL: none)
+  const T *lo, *hi;                                  // device [nv] or NULL
+  T* out; int64_t old;                               // out, leading dimension old
+  bool add;
+  int64_t ld, B;
+};
+static_assert(sizeof(ModelDev<double>) + sizeof(TaskPdDev<double>) + sizeof(TaskPdArgs<double>) <= 32764,
+              "task_pd_kernel's parameters exceed the kernel-parameter limit");
+template <class T, int NT>
+__global__ void __launch_bounds__(NT, sizeof(T) == 4 ? 16 : 8)
+task_pd_kernel(const __grid_constant__ ModelDev<T> M, const __grid_constant__ TaskPdDev<T> D, const TaskPdArgs<T> a) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const Stash<T, NT> st{reinterpret_cast<T*>(smem_raw) + threadIdx.x};
+  const int64_t ngroups = (a.B + NT - 1) / NT;
+  const bool readback = a.add || a.jkp;
+  for (int64_t g = blockIdx.x; g < ngroups; g += gridDim.x) {
+    const int64_t gn = g + gridDim.x;
+    if (gn < ngroups) {
+      const int64_t bn = gn * NT + (threadIdx.x & ~31);
+      prefetch_rows(a.q, M.nq, a.sld, bn);
+      prefetch_rows(a.v, M.nv, a.sld, bn);
+    }
+    const int64_t b = g * NT + threadIdx.x;
+    const bool active = b < a.B;
+    const int64_t bl = active ? b : a.B - 1;
+    const Col<T> q{a.q + bl, a.sld}, v{a.v + bl, a.sld};
+    const int64_t gc = a.gain_ld ? bl : 0;
+    const TaskPdSample<T> s{a.xref ? a.xref + bl : nullptr, a.xdref ? a.xdref + bl : nullptr, a.ld,
+                            a.kp ? a.kp + gc : nullptr, a.kd ? a.kd + gc : nullptr, a.gain_ld ? a.gain_ld : 1};
+    const ColOut<T> out{a.out + bl, a.old, active};
+    if (a.jkp) {
+      const int64_t jc = a.jgain_ld ? bl : 0;
+      const PdSample<T> js{a.q + bl, a.v + bl, a.sld, a.jqref + bl, a.jvref ? a.jvref + bl : nullptr, a.jff ? a.jff + bl : nullptr,
+                           a.ld, a.jkp + jc, a.jkd + jc, a.jgain_ld ? a.jgain_ld : 1, nullptr, nullptr};
+      for (int i = 0; i < M.nb; ++i) pd_joint(M.body[i], js, out);
+    }
+    task_pd_sample<T>(M, D, q, v, s, st, [&](int row, T u) {
+      T x = readback ? a.out[bl + (int64_t)row * a.old] : (a.ff ? a.ff[bl + (int64_t)row * a.ld] : T(0));
+      x += u;
+      if (a.lo) x = clamp_t(x, a.lo[row], a.hi[row]);
+      out.st(row, x);
+    });
   }
 }
 
@@ -1074,6 +1130,9 @@ int contact_stage_launch(const HostModel& hm, const ModelDev<T>& M, const Contac
 // taud rows, which the stage's dynamics (any of the three) reads in place of tau; τ_ff (tau and its strides) is read by the law.  In
 // computed-torque mode they write v̇_des into vd[i] instead (the dynamics overwrites it), and inverse_dynamics_t plus
 // pd_finish_kernel turn it into the torques.  Gains and references are caller arrays with leading dimension ld.
+// task (rbd_integrate_task_pd): its joint term, if any, runs as pd above but unclamped; then task_pd_kernel adds Σ_t J_t^T f_t to
+// the same rows (writes τ_ff + it, or it alone, without a joint term) and clamps them in torque mode; computed-torque mode then
+// continues as pd.
 template <class T>
 int integrate_t(const rbd_model* model, int64_t B, int64_t ld, const Rollout& r, cudaStream_t stream) {
   const HostModel& hm = model->hm;
@@ -1087,8 +1146,21 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, const Rollout& r,
   const double dt = r.dt;
   const int nsteps = r.nsteps;
   T *traj_q = (T*)r.q_traj, *traj_v = (T*)r.v_traj, *traj_s = (T*)r.s_traj, *stages = (T*)r.stages;
-  const rbd_pd_desc* pd = r.pd;
-  const bool computed_torque = pd && pd->mode == RBD_PD_COMPUTED_TORQUE;
+  const rbd_task_pd_desc* task = r.task;
+  const rbd_pd_desc* pd = task ? task->joint : r.pd;
+  const bool closed = pd || task;
+  const bool computed_torque = task ? task->mode == RBD_PD_COMPUTED_TORQUE : pd && pd->mode == RBD_PD_COMPUTED_TORQUE;
+  const double* effort_lo = task ? task->effort_lo : (pd ? pd->effort_lo : nullptr);
+  const double* effort_hi = task ? task->effort_hi : (pd ? pd->effort_hi : nullptr);
+  // the task kernel's descriptor and plan, decided before anything is enqueued (RBD_EUNSUPPORTED when its stash does not fit)
+  std::unique_ptr<TaskPdDev<T>> TD;
+  LaunchPlan task_plan;
+  if (task) {
+    TD.reset(new TaskPdDev<T>());
+    const int trows = std::max(1, build_task_pd_dev<T>(hm, *task, *TD));
+    if (int rc = plan_persistent((const void*)task_pd_kernel<T, kNT>, kNT, (size_t)trows * kNT * sizeof(T), (B + kNT - 1) / kNT, stream,
+                                 task_plan)) return rc;
+  }
   const rbd_contact_desc* cd = r.contact;
   const size_t ns = cd ? (size_t)3 * cd->npoints * cd->nhalfspaces : 0;
   // the contact rollout's descriptor in device form, passed by value to every stage's launch (the loop rollout's stage kernel
@@ -1098,9 +1170,9 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, const Rollout& r,
     C.reset(new ContactDev<T>());
     build_contact_dev<T>(hm.nb, hm.pos.data(), hm.alignT.data(), *cd, *C);
   }
-  const size_t rows = 2 * nq + 10 * nv + (pd || (tau && ld != B) ? nv : 0);
+  const size_t rows = 2 * nq + 10 * nv + (closed || (tau && ld != B) ? nv : 0);
   StreamAlloc work, swork;
-  RBD_CUDA_TRY(work.alloc((rows * (size_t)B + (pd ? 2 * nv : 0)) * sizeof(T), stream));
+  RBD_CUDA_TRY(work.alloc((rows * (size_t)B + (closed ? 2 * nv : 0)) * sizeof(T), stream));
   // contact state: s0 (the state at the start of the step, refreshed like q0 / v0) and the four stages' ṡ_i, [ns x B] each
   T* s0 = nullptr;
   T* sd[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -1129,7 +1201,7 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, const Rollout& r,
       phid[i] = stages + (4 * nq + (4 + (size_t)i) * nv) * B; vd[i] = stages + (4 * nq + (8 + (size_t)i) * nv) * B;
       if (ns) sd[i] = stages + ((size_t)stage_rows(nq, nv) + i * ns) * B;
       vdes[i] = vd[i];
-      if (pd) {
+      if (closed) {
         T* pr = stages + ((size_t)stage_rows(nq, nv) + 4 * ns) * B;
         taui[i] = pr + (size_t)i * nv * B;
         if (computed_torque) vdes[i] = pr + (4 + (size_t)i) * nv * B;
@@ -1146,16 +1218,16 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, const Rollout& r,
   // the controller's saturation bounds on the device, behind the workspace rows (copied from pageable memory: staged before return)
   const T* pd_lo = nullptr;
   const T* pd_hi = nullptr;
-  if (pd && pd->effort_lo && r.pd_bounds) {
+  if (effort_lo && r.pd_bounds) {
     pd_lo = (const T*)r.pd_bounds; pd_hi = pd_lo + nv;
-  } else if (pd && pd->effort_lo) {
+  } else if (effort_lo) {
     std::vector<T> bounds(2 * nv);
-    for (size_t k = 0; k < nv; ++k) { bounds[k] = (T)pd->effort_lo[k]; bounds[nv + k] = (T)pd->effort_hi[k]; }
+    for (size_t k = 0; k < nv; ++k) { bounds[k] = (T)effort_lo[k]; bounds[nv + k] = (T)effort_hi[k]; }
     T* dev = (T*)work.p + rows * (size_t)B;
     RBD_CUDA_TRY(cudaMemcpyAsync(dev, bounds.data(), 2 * nv * sizeof(T), cudaMemcpyHostToDevice, stream));
     pd_lo = dev; pd_hi = dev + nv;
   }
-  if (pd) tau_dense = taud;
+  if (closed) tau_dense = taud;
   else if (tau && ld != B && !varying) {
     RBD_CUDA_TRY(cudaMemcpy2DAsync(taud, B * sizeof(T), tau, ld * sizeof(T), B * sizeof(T), nv, cudaMemcpyDeviceToDevice, stream));
     tau_dense = taud;
@@ -1187,7 +1259,7 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, const Rollout& r,
   }
   for (int s = 0; s < nsteps; ++s) {
     for (int i = 0; i < 4; ++i) {
-      if (varying && !pd) {
+      if (varying && !closed) {
         tau_dense = tau_at(s, i);
         if (tau && ld != B) {
           RBD_CUDA_TRY(cudaMemcpy2DAsync(taud, B * sizeof(T), tau_dense, ld * sizeof(T), B * sizeof(T), nv, cudaMemcpyDeviceToDevice, stream));
@@ -1195,7 +1267,7 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, const Rollout& r,
         }
       }
       StageArgs<T> sa{q0, v0, i ? phid[i - 1] : nullptr, i ? vd[i - 1] : nullptr, phid[i], qsi[i], vsi[i], (T)(dt * a[i]), B, vec_stage};
-      if (pd) tau_dense = taui[i];
+      if (closed) tau_dense = taui[i];
       if (pd) {     // the references of step s start at s * q_ref_step_stride (q_ref) / s * v_ref_step_stride (v_ref, v̇_ref)
         const T* qref = (const T*)pd->q_ref + (size_t)s * pd->q_ref_step_stride;
         const size_t o = (size_t)s * pd->v_ref_step_stride;
@@ -1203,7 +1275,8 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, const Rollout& r,
         const T *kp = (const T*)pd->kp, *kd = (const T*)pd->kd;
         sa.pd = computed_torque ? PdStage<T>{qref, vref, pd->vd_ref ? (const T*)pd->vd_ref + o : nullptr, kp, kd, pd->gain_ld, nullptr,
                                              nullptr, vdes[i], ld}
-                                : PdStage<T>{qref, vref, tau_at(s, i), kp, kd, pd->gain_ld, pd_lo, pd_hi, taui[i], ld};
+                                : PdStage<T>{qref, vref, tau_at(s, i), kp, kd, pd->gain_ld, task ? nullptr : pd_lo,
+                                             task ? nullptr : pd_hi, taui[i], ld};
       }
       if (vec_stage) {     // revolute / prismatic rows, VEC samples per thread
         integrate_stage_linear_kernel<T><<<dim3(grid_lin, hm.nb), 256, 0, stream>>>(M, sa);
@@ -1211,6 +1284,18 @@ int integrate_t(const rbd_model* model, int64_t B, int64_t ld, const Rollout& r,
       }
       if (!vec_stage || has_other) {
         integrate_stage_kernel<T><<<dim3(grid, hm.nb), 128, 0, stream>>>(M, sa);
+        if (int rc = api_launched()) return rc;
+      }
+      if (task) {     // the task references of step s start at s * x_ref_step_stride / s * xd_ref_step_stride
+        const TaskPdArgs<T> ta{qsi[i], vsi[i], B,
+                               task->x_ref ? (const T*)task->x_ref + (size_t)s * task->x_ref_step_stride : nullptr,
+                               task->xd_ref ? (const T*)task->xd_ref + (size_t)s * task->xd_ref_step_stride : nullptr,
+                               (const T*)task->kp, (const T*)task->kd, task->gain_ld,
+                               pd || computed_torque ? nullptr : tau_at(s, i),
+                               nullptr, nullptr, nullptr, nullptr, nullptr, 0,
+                               computed_torque ? nullptr : pd_lo, computed_torque ? nullptr : pd_hi,
+                               computed_torque ? vdes[i] : taui[i], B, pd != nullptr, ld, B};
+        task_pd_kernel<T, kNT><<<task_plan.grid, task_plan.block, task_plan.smem, stream>>>(M, *TD, ta);
         if (int rc = api_launched()) return rc;
       }
       if (computed_torque) {     // tau = clamp(ID(q_s, v_s, v̇_des) + τ_ff), without contact wrenches
@@ -1412,7 +1497,7 @@ int check_common(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, b
 // controller) report every dtype but fp32 / fp64 as unsupported, and check q, v and s even when they take no step.
 int check_rollout(const char* fn, const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const Rollout& r) {
   const std::string f = fn;
-  const bool described = r.contact || r.loops || r.pd;
+  const bool described = r.contact || r.loops || r.pd || r.task;
   if (!model) return fail(RBD_EINVAL, "model handle is NULL");
   if (described && dtype != RBD_F32 && dtype != RBD_F64) return fail(RBD_EUNSUPPORTED, f + ": fp32 / fp64 only");
   if (int rc = check_common(model, dtype, B, ld)) return rc;
@@ -1429,6 +1514,94 @@ int check_rollout(const char* fn, const rbd_model* model, int32_t dtype, int64_t
   if (B == 0 || (r.nsteps == 0 && !rec && !described)) return RBD_OK;
   if (!r.q || !r.v) return fail(RBD_EINVAL, f + ": q and v must not be NULL");
   if (ns > 0 && !r.s) return fail(RBD_EINVAL, f + ": s must not be NULL when there are contact pairs");
+  return RBD_OK;
+}
+
+// The controller checks of rbd_integrate_pd (fn: the entry point named in the messages), pd not NULL.
+int check_pd(const char* fn, const rbd_model* model, int64_t ld, const rbd_pd_desc* pd) {
+  const std::string f = fn;
+  if (!pd->kp || !pd->kd || !pd->q_ref) return fail(RBD_EINVAL, f + ": kp, kd and q_ref must not be NULL");
+  if (pd->mode != RBD_PD_TORQUE && pd->mode != RBD_PD_COMPUTED_TORQUE) return fail(RBD_EINVAL, f + ": unknown mode");
+  if (pd->q_ref_step_stride < 0 || pd->v_ref_step_stride < 0) return fail(RBD_EINVAL, f + ": reference strides must be >= 0");
+  if (pd->gain_ld != 0 && pd->gain_ld != ld) return fail(RBD_EINVAL, f + ": gain_ld must be 0 or ld");
+  if (pd->mode == RBD_PD_TORQUE && pd->vd_ref) return fail(RBD_EINVAL, f + ": vd_ref is for computed-torque mode only");
+  if (!pd->effort_lo != !pd->effort_hi) return fail(RBD_EINVAL, f + ": effort_lo and effort_hi must be both NULL or both set");
+  if (pd->effort_lo)
+    for (int k = 0; k < model->hm.nv; ++k)
+      if (!(pd->effort_lo[k] <= pd->effort_hi[k])) return fail(RBD_EINVAL, f + ": effort bounds need lo <= hi");
+  return RBD_OK;
+}
+
+// The checks of a task-space controller: its joint term's JointPD checks, then check_task_pd (rbd_task_pd.cuh).
+int check_task_ctrl(const char* fn, const rbd_model* model, int64_t ld, const rbd_task_pd_desc* ctrl) {
+  const std::string f = fn;
+  if (ctrl && ctrl->joint)
+    if (int rc = check_pd((f + " (joint term)").c_str(), model, ld, ctrl->joint)) return rc;
+  std::string err;
+  if (int rc = check_task_pd(model->hm.nb, model->hm.nv, ld, ctrl, err)) return fail(rc, f + ": " + err);
+  return RBD_OK;
+}
+
+// rbd_task_pd_torques: the law at (q, v) with the references of `step`.  Torque mode: one task_pd_kernel straight into tau_out.
+// Computed-torque mode: v̇_des (task kernel) -> inverse dynamics -> pd_finish_kernel (τ_ff, clamp) on dense rows, copied out.
+template <class T>
+int task_pd_torques_t(const rbd_model* model, int64_t B, int64_t ld, const void* q, const void* v, const void* tau_ff,
+                      const rbd_task_pd_desc& c, int step, void* tau_out, cudaStream_t stream) {
+  const HostModel& hm = model->hm;
+  const ModelDev<T>& M = dev_model<T>(hm);
+  const size_t nq = hm.nq, nv = hm.nv;
+  const bool ct = c.mode == RBD_PD_COMPUTED_TORQUE;
+  std::unique_ptr<TaskPdDev<T>> D(new TaskPdDev<T>());
+  const int trows = std::max(1, build_task_pd_dev<T>(hm, c, *D));
+  LaunchPlan pl;
+  if (int rc = plan_persistent((const void*)task_pd_kernel<T, kNT>, kNT, (size_t)trows * kNT * sizeof(T), (B + kNT - 1) / kNT, stream, pl))
+    return rc;
+  DeviceProps p;
+  RBD_CUDA_TRY(device_props(p));
+  // workspace: effort bounds [2 nv]; computed-torque mode also dense q, v, v̇_des and τ [rows x B]
+  const size_t dense = ct ? (nq + 3 * nv) * (size_t)B : 0;
+  StreamAlloc work;
+  RBD_CUDA_TRY(work.alloc((dense + 2 * nv) * sizeof(T) + 16, stream));
+  T* lo = nullptr;
+  T* hi = nullptr;
+  if (c.effort_lo) {
+    std::vector<T> bounds(2 * nv);
+    for (size_t k = 0; k < nv; ++k) { bounds[k] = (T)c.effort_lo[k]; bounds[nv + k] = (T)c.effort_hi[k]; }
+    lo = (T*)work.p + dense; hi = lo + nv;
+    RBD_CUDA_TRY(cudaMemcpyAsync(lo, bounds.data(), 2 * nv * sizeof(T), cudaMemcpyHostToDevice, stream));
+  }
+  const T* qs = (const T*)q;
+  const T* vs = (const T*)v;
+  int64_t sld = ld;
+  T* vdes = nullptr;
+  T* tau_d = nullptr;
+  if (ct) {
+    T* qd = (T*)work.p; T* vd = qd + nq * B;
+    vdes = vd + nv * B; tau_d = vdes + nv * B;
+    RBD_CUDA_TRY(cudaMemcpy2DAsync(qd, B * sizeof(T), q, ld * sizeof(T), B * sizeof(T), nq, cudaMemcpyDeviceToDevice, stream));
+    RBD_CUDA_TRY(cudaMemcpy2DAsync(vd, B * sizeof(T), v, ld * sizeof(T), B * sizeof(T), nv, cudaMemcpyDeviceToDevice, stream));
+    qs = qd; vs = vd; sld = B;
+  }
+  const rbd_pd_desc* j = c.joint;
+  const size_t xo = (size_t)step * c.x_ref_step_stride, xdo = (size_t)step * c.xd_ref_step_stride;
+  const size_t jqo = j ? (size_t)step * j->q_ref_step_stride : 0, jvo = j ? (size_t)step * j->v_ref_step_stride : 0;
+  const T* jff = j ? (ct ? (j->vd_ref ? (const T*)j->vd_ref + jvo : nullptr) : (const T*)tau_ff) : nullptr;
+  // the caller arrays (references, gains, τ_ff) keep leading dimension ld; in computed-torque mode the state is the dense copy,
+  // so the joint term reads its columns through sld and the references through ld
+  const TaskPdArgs<T> a{qs, vs, sld, c.x_ref ? (const T*)c.x_ref + xo : nullptr, c.xd_ref ? (const T*)c.xd_ref + xdo : nullptr,
+                        (const T*)c.kp, (const T*)c.kd, c.gain_ld, ct ? nullptr : (const T*)tau_ff,
+                        j ? (const T*)j->q_ref + jqo : nullptr, j && j->v_ref ? (const T*)j->v_ref + jvo : nullptr, jff,
+                        j ? (const T*)j->kp : nullptr, j ? (const T*)j->kd : nullptr, j ? j->gain_ld : 0,
+                        ct ? nullptr : lo, ct ? nullptr : hi, ct ? vdes : (T*)tau_out, ct ? B : ld, false, ld, B};
+  task_pd_kernel<T, kNT><<<pl.grid, pl.block, pl.smem, stream>>>(M, *D, a);
+  if (int rc = api_launched(&pl)) return rc;
+  if (!ct) return RBD_OK;
+  const KeepLaunchRecord keep;
+  if (int rc = inverse_dynamics_t<T>(model, B, B, qs, vs, vdes, nullptr, tau_d, stream)) return rc;
+  const PdFinishArgs<T> pf{tau_d, (const T*)tau_ff, ld, lo, hi, (int64_t)nv, B};
+  pd_finish_kernel<T><<<(int)std::min<int64_t>(((int64_t)nv * B + 255) / 256, (int64_t)p.sms * 8), 256, 0, stream>>>(pf);
+  if (int rc = api_launched()) return rc;
+  RBD_CUDA_TRY(cudaMemcpy2DAsync(tau_out, ld * sizeof(T), tau_d, B * sizeof(T), B * sizeof(T), nv, cudaMemcpyDeviceToDevice, stream));
   return RBD_OK;
 }
 
@@ -1793,19 +1966,40 @@ int32_t rbd_integrate_pd(const rbd_model* model, int32_t dtype, int64_t B, int64
   const Rollout r{q, v, s, tau, tau_step_stride, tau_stage_stride, dt, nsteps, q_traj, v_traj, s_traj, nullptr, contact, loops, pd};
   if (int rc = check_rollout("rbd_integrate_pd", model, dtype, B, ld, r)) return rc;
   if (!pd) return fail(RBD_EINVAL, "rbd_integrate_pd: pd must not be NULL");
-  if (!pd->kp || !pd->kd || !pd->q_ref) return fail(RBD_EINVAL, "rbd_integrate_pd: kp, kd and q_ref must not be NULL");
-  if (pd->mode != RBD_PD_TORQUE && pd->mode != RBD_PD_COMPUTED_TORQUE) return fail(RBD_EINVAL, "rbd_integrate_pd: unknown mode");
-  if (pd->q_ref_step_stride < 0 || pd->v_ref_step_stride < 0) return fail(RBD_EINVAL, "rbd_integrate_pd: reference strides must be >= 0");
-  if (pd->gain_ld != 0 && pd->gain_ld != ld) return fail(RBD_EINVAL, "rbd_integrate_pd: gain_ld must be 0 or ld");
-  if (pd->mode == RBD_PD_TORQUE && pd->vd_ref) return fail(RBD_EINVAL, "rbd_integrate_pd: vd_ref is for computed-torque mode only");
-  if (!pd->effort_lo != !pd->effort_hi) return fail(RBD_EINVAL, "rbd_integrate_pd: effort_lo and effort_hi must be both NULL or both set");
-  if (pd->effort_lo)
-    for (int k = 0; k < model->hm.nv; ++k)
-      if (!(pd->effort_lo[k] <= pd->effort_hi[k])) return fail(RBD_EINVAL, "rbd_integrate_pd: effort bounds need lo <= hi");
+  if (int rc = check_pd("rbd_integrate_pd", model, ld, pd)) return rc;
   if (pd->mode == RBD_PD_COMPUTED_TORQUE && loops && loops->nloops > 0)
     return fail(RBD_ELOOP, "rbd_integrate_pd: computed-torque mode needs inverse_dynamics!, which has no kinematic loops");
   const ApiCall call;
   return rbd::integrate(model, dtype, B, ld, r, (cudaStream_t)stream);
+}
+
+int32_t rbd_integrate_task_pd(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, void* q, void* v, void* s, const void* tau,
+                              int64_t tau_step_stride, int64_t tau_stage_stride, const rbd_task_pd_desc* ctrl,
+                              const rbd_loop_desc* loops, const rbd_contact_desc* contact, double dt, int32_t nsteps, void* q_traj,
+                              void* v_traj, void* s_traj, void* stream) {
+  Rollout r{q, v, s, tau, tau_step_stride, tau_stage_stride, dt, nsteps, q_traj, v_traj, s_traj, nullptr, contact, loops};
+  r.task = ctrl;
+  if (int rc = check_rollout("rbd_integrate_task_pd", model, dtype, B, ld, r)) return rc;
+  if (int rc = check_task_ctrl("rbd_integrate_task_pd", model, ld, ctrl)) return rc;
+  if (ctrl->mode == RBD_PD_COMPUTED_TORQUE && loops && loops->nloops > 0)
+    return fail(RBD_ELOOP, "rbd_integrate_task_pd: computed-torque mode needs inverse_dynamics!, which has no kinematic loops");
+  const ApiCall call;
+  return rbd::integrate(model, dtype, B, ld, r, (cudaStream_t)stream);
+}
+
+int32_t rbd_task_pd_torques(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
+                            const void* tau_ff, const rbd_task_pd_desc* ctrl, int32_t step, void* tau_out, void* stream) {
+  const ApiCall call;
+  if (!model) return fail(RBD_EINVAL, "rbd_task_pd_torques: model handle is NULL");
+  if (dtype != RBD_F32 && dtype != RBD_F64) return fail(RBD_EUNSUPPORTED, "rbd_task_pd_torques: fp32 and fp64 only");
+  if (B < 0 || ld < B) return fail(RBD_EDIM, "rbd_task_pd_torques: batch size / leading dimension mismatch (need ld >= B >= 0)");
+  if (int rc = check_task_ctrl("rbd_task_pd_torques", model, ld, ctrl)) return rc;
+  if (step < 0) return fail(RBD_EINVAL, "rbd_task_pd_torques: step must be >= 0");
+  if (B == 0) return RBD_OK;
+  if (!q || !v || !tau_out) return fail(RBD_EINVAL, "rbd_task_pd_torques: q, v and tau_out must not be NULL");
+  cudaStream_t s = (cudaStream_t)stream;
+  return dtype == RBD_F32 ? task_pd_torques_t<float>(model, B, ld, q, v, tau_ff, *ctrl, step, tau_out, s)
+                          : task_pd_torques_t<double>(model, B, ld, q, v, tau_ff, *ctrl, step, tau_out, s);
 }
 
 int32_t rbd_dynamics_result(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,

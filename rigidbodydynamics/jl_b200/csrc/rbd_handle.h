@@ -169,6 +169,8 @@ struct Rollout {
   const rbd_pd_desc* pd = nullptr;             // feedback evaluated at every stage
   const void* pd_bounds = nullptr;             // pd's effort bounds already on the device ([2 nv]: lo, then hi), or NULL: integrate
                                                // copies them from the host arrays of pd (rbd_integrate_pd_vjp's recompute passes its copy)
+  const rbd_task_pd_desc* task = nullptr;      // task-space feedback at every stage (pd NULL; its joint term takes pd's place);
+                                               // never set together with `stages`
 };
 // The recompute of one step (nsteps = 1, ld = B) keeps its four stages in stage_rows(nq, nv) x B rows of `stages` (4 ns more with
 // contact, for the ṡ_i) and skips the finishing step.  With a controller (pd) pd_stage_rows(nv, computed_torque) x B more follow:

@@ -88,6 +88,52 @@ template <class T> RBD_HD void task_to_frame(const T* RF, const T* pF, const Mot
   matT_vec(RF, l, o.l);
 }
 
+// Sweep A: the root-frame pose w of every body in preorder; the named bodies' poses are parked in their slots, and body_fn(bd, w)
+// runs for every body (rbd_task_pd.cuh's J^T pass walks the joints with it).
+template <class T, class ST, class F>
+RBD_HD void task_pose_sweep(const ModelDev<T>& M, const TaskDev<T>& D, const Col<T>& q, const ST& st, F&& body_fn) {
+  Pose<T> cur;
+  pose_identity(cur);
+  for (int i = 0; i < M.nb; ++i) {
+    const BodyDev<T>& bd = M.body[i];
+    Pose<T> pp;
+    if (bd.flags & F_ROOT_CHILD) pose_identity(pp);
+    else if (bd.flags & F_FIRST_CHILD) pp = cur;
+    else {
+      const int row = bd.pslot * kSlotRowsKin;
+#pragma unroll
+      for (int k = 0; k < 9; ++k) pp.R[k] = st.ld(row + k);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) pp.p[k] = st.ld(row + 9 + k);
+    }
+    T R[9], r[3], t[3];
+    frame_any(bd, q, R, r);
+    Pose<T> w;
+    mat_mul3(pp.R, R, w.R);
+    mat_vec(pp.R, r, t);
+    w.p[0] = pp.p[0] + t[0]; w.p[1] = pp.p[1] + t[1]; w.p[2] = pp.p[2] + t[2];
+    const int s = D.named[i];
+    if (s >= 0) {
+      T Rc[9];
+      mat_mul3(w.R, D.At[s], Rc);
+      const int row = D.named_base + s * D.slot_rows;
+#pragma unroll
+      for (int k = 0; k < 9; ++k) st.st(row + k, Rc[k]);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) st.st(row + 9 + k, w.p[k]);
+    }
+    body_fn(i, bd, w);
+    if (bd.flags & F_HAS_PENDING) {
+      const int row = bd.oslot * kSlotRowsKin;
+#pragma unroll
+      for (int k = 0; k < 9; ++k) st.st(row + k, w.R[k]);
+#pragma unroll
+      for (int k = 0; k < 3; ++k) st.st(row + 9 + k, w.p[k]);
+    }
+    cur = w;
+  }
+}
+
 template <class T, class ST>
 RBD_HD void task_sample(const ModelDev<T>& M, const TaskDev<T>& D, const TaskIO<T>& io, const ST& st) {
   const int nb = M.nb, nv = M.nv, K = D.ntasks;
@@ -97,47 +143,7 @@ RBD_HD void task_sample(const ModelDev<T>& M, const TaskDev<T>& D, const TaskIO<
   const int vel_off = 12, acc_off = 18;
 
   // ---- sweep A: poses of the named bodies ----
-  {
-    Pose<T> cur;
-    pose_identity(cur);
-    for (int i = 0; i < nb; ++i) {
-      const BodyDev<T>& bd = M.body[i];
-      Pose<T> pp;
-      if (bd.flags & F_ROOT_CHILD) pose_identity(pp);
-      else if (bd.flags & F_FIRST_CHILD) pp = cur;
-      else {
-        const int row = bd.pslot * kSlotRowsKin;
-#pragma unroll
-        for (int k = 0; k < 9; ++k) pp.R[k] = st.ld(row + k);
-#pragma unroll
-        for (int k = 0; k < 3; ++k) pp.p[k] = st.ld(row + 9 + k);
-      }
-      T R[9], r[3], t[3];
-      frame_any(bd, io.q, R, r);
-      Pose<T> w;
-      mat_mul3(pp.R, R, w.R);
-      mat_vec(pp.R, r, t);
-      w.p[0] = pp.p[0] + t[0]; w.p[1] = pp.p[1] + t[1]; w.p[2] = pp.p[2] + t[2];
-      const int s = D.named[i];
-      if (s >= 0) {
-        T Rc[9];
-        mat_mul3(w.R, D.At[s], Rc);
-        const int row = D.named_base + s * D.slot_rows;
-#pragma unroll
-        for (int k = 0; k < 9; ++k) st.st(row + k, Rc[k]);
-#pragma unroll
-        for (int k = 0; k < 3; ++k) st.st(row + 9 + k, w.p[k]);
-      }
-      if (bd.flags & F_HAS_PENDING) {
-        const int row = bd.oslot * kSlotRowsKin;
-#pragma unroll
-        for (int k = 0; k < 9; ++k) st.st(row + k, w.R[k]);
-#pragma unroll
-        for (int k = 0; k < 3; ++k) st.st(row + 9 + k, w.p[k]);
-      }
-      cur = w;
-    }
-  }
+  task_pose_sweep(M, D, io.q, st, [](int, const BodyDev<T>&, const Pose<T>&) {});
 
   // ---- sweep B: twists, accelerations, Jacobian columns ----
   if (jac || want_vel) {
