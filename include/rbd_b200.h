@@ -689,6 +689,43 @@ int32_t rbd_integrate_task_pd(const rbd_model* model, int32_t dtype, int64_t B, 
 int32_t rbd_task_pd_torques(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                             const void* tau_ff, const rbd_task_pd_desc* ctrl, int32_t step, void* tau_out, void* stream);
 
+/* Reverse mode through a task-space closed-loop rollout (DESIGN 4.22): rbd_integrate_pd_vjp for the trajectory
+ * rbd_integrate_task_pd recorded with the controller `ctrl` (tree or contact rollout, leading dimension B, gain_ld 0 or B).  Gradients
+ * reach the initial state and τ_ff as there, and the controller's device arrays through `ctrl_bar` (each ADDED TO, NULL = not wanted;
+ * ctrl_bar NULL: none):
+ *   kp, kd          [R x B]: per-sample contributions, also for shared gains (the caller sums over the batch)
+ *   x_ref, xd_ref   the shapes of ctrl->x_ref / ctrl->xd_ref; a pose target's 12 entries as given (the law does not re-orthonormalise)
+ *   joint           the joint term's adjoints, as rbd_integrate_pd_vjp's pd_bar (needs ctrl->joint)
+ * The saturation's derivative is rbd_integrate_pd_vjp's.  Nothing reaches the task points, the effort bounds, dt or the contact
+ * parameters.  Argument errors (before any CUDA call): rbd_integrate_task_pd's controller checks, those of rbd_integrate_pd_vjp, a bar
+ * without its array (xd_ref, joint, and the joint term's v_ref / vd_ref): RBD_EINVAL; in computed-torque mode the model limits of
+ * rbd_inverse_dynamics_vjp: RBD_EUNSUPPORTED.  There is no loop rollout here.  Kernels per step: the recompute of
+ * rbd_integrate_task_pd's step without its finishing kernels, then as rbd_integrate_pd_vjp with this controller's joint term
+ * (rbd_integrate_vjp / rbd_integrate_contact_vjp without one), plus per stage one task-law adjoint kernel and, in torque mode with
+ * effort bounds, one elementwise mask kernel. */
+typedef struct rbd_task_pd_bar {
+  void* kp; void* kd;                    /* [R x B] */
+  void* x_ref; void* xd_ref;             /* the shapes of ctrl->x_ref / ctrl->xd_ref */
+  const rbd_pd_bar* joint;               /* the joint term's, NULL = not wanted */
+} rbd_task_pd_bar;
+int32_t rbd_integrate_task_pd_vjp(const rbd_model* model, int32_t dtype, int64_t B, const void* q_traj, const void* v_traj,
+                                  const void* s_traj, const void* tau, int64_t tau_step_stride, int64_t tau_stage_stride,
+                                  const rbd_task_pd_desc* ctrl, const rbd_contact_desc* contact /* NULL = tree rollout */, double dt,
+                                  int32_t nsteps, const void* q_traj_bar, const void* v_traj_bar, const void* s_traj_bar,
+                                  void* q0_bar_tan, void* q0_bar_cfg, void* v0_bar, void* s0_bar, void* tau_bar,
+                                  const rbd_task_pd_bar* ctrl_bar, void* stream);
+/* The adjoint of rbd_task_pd_torques at one state, every array [rows x B] (gain_ld 0 or B): for the cotangent tau_out_bar of the
+ * torques, q_bar_tan [nv x B], q_bar_cfg [nq x B] (rbd_dynamics_vjp's conventions), v_bar [nv x B] and tau_ff_bar [nv x B] are
+ * WRITTEN (each may be NULL), the controller's bars ADDED TO as in rbd_integrate_task_pd_vjp.  The saturation's derivative is
+ * rbd_integrate_pd_vjp's.  Argument errors: those of rbd_task_pd_torques (leading dimension B), tau_ff_bar without tau_ff, a bar
+ * without its array: RBD_EINVAL; in computed-torque mode the model limits of rbd_inverse_dynamics_vjp: RBD_EUNSUPPORTED; all before
+ * any CUDA call.  Kernels: with effort bounds or in computed-torque mode the forward law first (rbd_task_pd_torques' kernels) and,
+ * with bounds, one mask kernel; in computed-torque mode one inverse-dynamics VJP; then one task-adjoint kernel (the joint term's
+ * adjoint in the same pass) and, when q_bar_tan or q_bar_cfg is wanted, one elementwise kernel. */
+int32_t rbd_task_pd_torques_vjp(const rbd_model* model, int32_t dtype, int64_t B, const void* q, const void* v, const void* tau_ff,
+                                const rbd_task_pd_desc* ctrl, int32_t step, const void* tau_out_bar, void* q_bar_tan, void* q_bar_cfg,
+                                void* v_bar, void* tau_ff_bar, const rbd_task_pd_bar* ctrl_bar, void* stream);
+
 /* Host-pointer variants: same semantics, host buffers in, host buffers out, copies inside the call. */
 int32_t rbd_dynamics_host(rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                           const void* tau, const void* wext, void* vd_out, void* qd_out);

@@ -146,6 +146,8 @@ SYMBOLS = {
     "rbd_task_pd_torques": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _i32, _vp, _vp]),
     "rbd_integrate_contact_vjp":(c_int32, [_vp, _i32, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _vp, c_double, _i32] + [_vp] * 9),
     "rbd_integrate_pd_vjp":   (c_int32, [_vp, _i32, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, c_double, _i32] + [_vp] * 10),
+    "rbd_integrate_task_pd_vjp": (c_int32, [_vp, _i32, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, c_double, _i32] + [_vp] * 10),
+    "rbd_task_pd_torques_vjp": (c_int32, [_vp, _i32, _i64, _vp, _vp, _vp, _vp, _i32] + [_vp] * 7),
     "rbd_kinematics": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, POINTER(RbdKinematicsOut), _vp]),
     "rbd_task_kinematics": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, POINTER(RbdTaskDesc), POINTER(RbdTaskOut), _vp]),
     "rbd_task_kinematics_vjp": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, POINTER(RbdTaskDesc), POINTER(RbdTaskOut)] + [_vp] * 5),

@@ -5,15 +5,18 @@
     integrate_vjp_         gradient of a recorded rollout       rbd_integrate_vjp         (csrc/rbd_integrate_adjoint.cuh)
     integrate_contact_vjp_ gradient of a recorded contact rollout  rbd_integrate_contact_vjp  (csrc/rbd_contact_adjoint.cuh)
     integrate_pd_vjp_      gradient of a recorded closed-loop rollout  rbd_integrate_pd_vjp  (csrc/rbd_integrate_adjoint.cuh)
+    integrate_task_pd_vjp_ gradient of a recorded task-space closed-loop rollout  rbd_integrate_task_pd_vjp  (csrc/rbd_task_pd_adjoint.cuh)
+    task_pd_torques_vjp_   τ̄ᵀ ∂τ/∂(q, v, τ_ff, controller) of a TaskPD's torques at one state  rbd_task_pd_torques_vjp
     task_kinematics_vjp_   Σ ȳᵀ ∂y/∂(q, v, v̇) of task-space outputs  rbd_task_kinematics_vjp  (csrc/rbd_task_adjoint.cuh)
     dynamics(mechanism, q, v, tau=None, externalwrenches=None)         differentiable v̇ = dynamics!(...)
     inverse_dynamics(mechanism, q, v, vd, externalwrenches=None)       differentiable τ = inverse_dynamics!(...)
     simulate(mechanism, q0, v0, torques=None, *, dt, nsteps, ...)     differentiable RK4 rollout (simulate)
     simulate_contact(mechanism, q0, v0, s0, torques=None, *, contact, dt, nsteps, ...)
                                                                        differentiable RK4 rollout with soft contact
-    both with controller=JointPD(...): closed loop, gradients also to the controller's gains and references
+    both with controller=JointPD(...) or TaskPD(...): closed loop, gradients also to the controller's gains and references
     task_kinematics(mechanism, q, v=None, vd=None, *, tasks, outputs=("point",))
                                                                        differentiable task-space kinematics (TaskFrame tasks)
+    task_pd_torques(state, controller, torques=None, step=0)          differentiable torques of a TaskPD at one state
 
 One product costs one Articulated-Body solve (forward dynamics only) plus one outward and one inward sweep: O(n) per sample, no
 nv x nv Jacobian is formed (``dynamics_derivatives_`` builds both full Jacobians instead).  Every tensor is ``[rows, B]``, contiguous,
@@ -41,7 +44,8 @@ from .kinematics import _TASK_NEEDS_V, _TASK_ROWS, TaskFrame, task_desc
 from .mechanism import Mechanism
 from .state import _DT, MechanismState, _model_handle
 
-__all__ = ["dynamics_vjp_", "inverse_dynamics_vjp_", "integrate_vjp_", "integrate_contact_vjp_", "integrate_pd_vjp_", "dynamics",
+__all__ = ["dynamics_vjp_", "inverse_dynamics_vjp_", "integrate_vjp_", "integrate_contact_vjp_", "integrate_pd_vjp_", "integrate_task_pd_vjp_",
+           "task_pd_torques_vjp_", "task_pd_torques", "dynamics",
            "inverse_dynamics", "simulate", "simulate_contact", "task_kinematics_vjp_", "task_kinematics"]
 
 
@@ -433,7 +437,12 @@ def simulate(mechanism: Mechanism, q0: torch.Tensor, v0: torch.Tensor, torques: 
 
     ``controller``: a ``JointPD`` evaluated at every stage (``torques`` is then τ_ff), as ``simulate_(..., controller=)``.  Gradients
     then also flow to those of its ``kp``, ``kd``, ``q_ref``, ``v_ref`` and ``vd_ref`` that require grad (shared gains: summed over
-    the batch); backward runs ``rbd_integrate_pd_vjp``."""
+    the batch); backward runs ``rbd_integrate_pd_vjp``.  Or a ``TaskPD``: gradients to its ``kp``, ``kd``, ``x_ref``, ``xd_ref`` and
+    its joint term's arrays; backward runs ``rbd_integrate_task_pd_vjp``."""
+    from .pd import TaskPD
+    if isinstance(controller, TaskPD):
+        return _simulate_task_pd(mechanism, q0, v0, None, torques, controller, None, dt, nsteps, trajectory, checkpoint_every,
+                                 "autodiff.simulate")
     if controller is not None:
         return _simulate_pd(mechanism, q0, v0, None, torques, controller, None, dt, nsteps, trajectory, checkpoint_every,
                             "autodiff.simulate")
@@ -578,6 +587,10 @@ def simulate_contact(mechanism: Mechanism, q0: torch.Tensor, v0: torch.Tensor, s
     if mechanism.has_loops():
         raise _cabi.RbdError(_cabi.RBD_ELOOP, "autodiff.simulate_contact: This method can currently only handle tree Mechanisms.")
     cd = contact if contact is not None else contact_desc(mechanism)
+    from .pd import TaskPD
+    if isinstance(controller, TaskPD):
+        return _simulate_task_pd(mechanism, q0, v0, s0, torques, controller, cd, dt, nsteps, trajectory, checkpoint_every,
+                                 "autodiff.simulate_contact")
     if controller is not None:
         return _simulate_pd(mechanism, q0, v0, s0, torques, controller, cd, dt, nsteps, trajectory, checkpoint_every,
                             "autodiff.simulate_contact")
@@ -588,10 +601,11 @@ def simulate_contact(mechanism: Mechanism, q0: torch.Tensor, v0: torch.Tensor, s
 # closed-loop rollouts: rbd_integrate_pd (recording) / rbd_integrate_pd_vjp
 # ----------------------------------------------------------------------------------------------------------------------
 class _Batch:
-    """What JointPD._c_struct reads from a state: sizes, dtype and device of a rollout's initial q0."""
+    """What JointPD._c_struct / TaskPD._c_struct read from a state: sizes, dtype and device of a rollout's initial q0, the mechanism."""
 
-    def __init__(self, h, q0: torch.Tensor):
+    def __init__(self, h, q0: torch.Tensor, mechanism: Optional[Mechanism] = None):
         self.nq, self.nv, self.batch, self.dtype, self.q = h.info.nq, h.info.nv, q0.shape[1], q0.dtype, q0
+        self.mechanism = mechanism
 
 
 def _pd_struct(controller, h, q0, nsteps, what):
@@ -773,7 +787,319 @@ class _SimulatePD(torch.autograd.Function):
 def _simulate_pd(mechanism, q0, v0, s0, torques, controller, contact, dt, nsteps, trajectory, every, what):
     from .pd import JointPD
     if not isinstance(controller, JointPD):
-        raise TypeError(f"{what}: controller must be a JointPD")
+        raise TypeError(f"{what}: controller must be a JointPD or a TaskPD")
     c = controller
     return _SimulatePD.apply(mechanism, q0, v0, s0, torques, c.kp, c.kd, c.q_ref, c.v_ref, c.vd_ref, (c.computed_torque, c.effort_bounds),
                              contact, float(dt), int(nsteps), bool(trajectory), every)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# task-space closed-loop rollouts: rbd_integrate_task_pd (recording) / rbd_integrate_task_pd_vjp
+# ----------------------------------------------------------------------------------------------------------------------
+def _task_struct(controller, mechanism, h, q0, nsteps, what):
+    from .pd import TaskPD
+    if not isinstance(controller, TaskPD):
+        raise TypeError(f"{what}: controller must be a TaskPD")
+    return controller._c_struct(_Batch(h, q0, mechanism), nsteps, what)
+
+
+def integrate_task_pd_vjp_(mechanism: Mechanism, q_traj: torch.Tensor, v_traj: torch.Tensor, torques: Optional[torch.Tensor] = None, *,
+                           controller, dt: float, contact=None, s_traj: Optional[torch.Tensor] = None,
+                           q_traj_bar: Optional[torch.Tensor] = None, v_traj_bar: Optional[torch.Tensor] = None,
+                           s_traj_bar: Optional[torch.Tensor] = None, q0_bar_tan: Optional[torch.Tensor] = None,
+                           q0_bar_cfg: Optional[torch.Tensor] = None, v0_bar: Optional[torch.Tensor] = None,
+                           s0_bar: Optional[torch.Tensor] = None, tau_bar: Optional[torch.Tensor] = None,
+                           kp_bar: Optional[torch.Tensor] = None, kd_bar: Optional[torch.Tensor] = None,
+                           x_ref_bar: Optional[torch.Tensor] = None, xd_ref_bar: Optional[torch.Tensor] = None,
+                           joint_bars: Optional[Sequence[Optional[torch.Tensor]]] = None):
+    """``integrate_pd_vjp_`` for a trajectory recorded with ``controller`` (a ``TaskPD``) by ``simulate_trajectory_`` or, with
+    ``contact`` and ``s_traj``, by ``simulate_contact_trajectory_``.  Controller outputs, each optional and ADDED TO: ``kp_bar`` /
+    ``kd_bar`` [R, B] (per sample, also for shared gains), ``x_ref_bar`` / ``xd_ref_bar`` with the shapes of ``x_ref`` / ``xd_ref``,
+    and ``joint_bars`` = (kp, kd, q_ref, v_ref, vd_ref) bars of the joint term as in ``integrate_pd_vjp_``.  Mechanisms with loops
+    are refused (RBD_ELOOP)."""
+    what = "integrate_task_pd_vjp_"
+    nsteps = q_traj.shape[0] - 1
+    h, B, step, stage = _rollout_inputs(mechanism, what, q_traj[0], v_traj[0], torques, nsteps)
+    nq, nv = h.info.nq, h.info.nv
+    ns = 0 if contact is None else contact.nstates
+    ctl, keep = _task_struct(controller, mechanism, h, q_traj[0], nsteps, what)
+    R, _ = controller.rows()
+    shape = lambda t: None if t is None else tuple(t.shape)      # noqa: E731
+    if xd_ref_bar is not None and controller.xd_ref is None:
+        raise ValueError(f"{what}: xd_ref_bar needs the controller's xd_ref")
+    j = controller.joint
+    jb = tuple(joint_bars) if joint_bars is not None else (None,) * 5
+    if any(t is not None for t in jb) and j is None:
+        raise ValueError(f"{what}: joint_bars need the controller's joint term")
+    if contact is None and (s_traj is not None or s_traj_bar is not None or s0_bar is not None):
+        raise ValueError(f"{what}: s_traj, s_traj_bar and s0_bar need contact")
+    items = [(q_traj, (nsteps + 1, nq, B), "q_traj"), (v_traj, (nsteps + 1, nv, B), "v_traj"),
+             (s_traj, (nsteps + 1, ns, B), "s_traj"), (q_traj_bar, (nsteps + 1, nq, B), "q_traj_bar"),
+             (v_traj_bar, (nsteps + 1, nv, B), "v_traj_bar"), (s_traj_bar, (nsteps + 1, ns, B), "s_traj_bar"),
+             (q0_bar_tan, (nv, B), "q0_bar_tan"), (q0_bar_cfg, (nq, B), "q0_bar_cfg"), (v0_bar, (nv, B), "v0_bar"), (s0_bar, (ns, B), "s0_bar"),
+             (tau_bar, shape(torques), "tau_bar"), (kp_bar, (R, B), "kp_bar"), (kd_bar, (R, B), "kd_bar"),
+             (x_ref_bar, shape(controller.x_ref), "x_ref_bar"), (xd_ref_bar, shape(controller.xd_ref), "xd_ref_bar")]
+    if j is not None:
+        for bar, ref, name in ((jb[3], j.v_ref, "v_ref"), (jb[4], j.vd_ref, "vd_ref")):
+            if bar is not None and ref is None:
+                raise ValueError(f"{what}: the joint term's {name} bar needs its {name}")
+        items += [(jb[0], (nv, B), "joint kp_bar"), (jb[1], (nv, B), "joint kd_bar"), (jb[2], shape(j.q_ref), "joint q_ref_bar"),
+                  (jb[3], shape(j.v_ref), "joint v_ref_bar"), (jb[4], shape(j.vd_ref), "joint vd_ref_bar")]
+    _check_blocks(what, q_traj, items)
+    if contact is not None and ns > 0 and s_traj is None:
+        raise ValueError(f"{what}: s_traj is needed with contact pairs")
+    _task_vjp_call(h, q_traj, v_traj, s_traj, torques, step, stage, ctl, contact, dt, nsteps, q_traj_bar, v_traj_bar, s_traj_bar,
+                   q0_bar_tan, q0_bar_cfg, v0_bar, s0_bar, tau_bar, (kp_bar, kd_bar, x_ref_bar, xd_ref_bar), jb)
+    del keep
+
+
+def _task_vjp_call(h, qt, vt, st, tau, step, stage, ctl, contact, dt, n, qtb, vtb, stb, q0t, qc, vb, sb, tb, bars, joint_bars):
+    from .pd import _RbdPdBar, _RbdTaskPdBar
+    B = qt.shape[2]
+    c, keep = contact.c_struct() if contact is not None else (None, None)
+    jb = _RbdPdBar(*[_ptr(t) for t in joint_bars])
+    tb_ = _RbdTaskPdBar(*[_ptr(t) for t in bars], ctypes.pointer(jb) if any(t is not None for t in joint_bars) else None)
+    _cabi.check(_cabi.load_library().rbd_integrate_task_pd_vjp(
+        h.ptr, _DT[qt.dtype], B, _ptr(qt), _ptr(vt), _ptr(st), _ptr(tau), step, stage, ctypes.byref(ctl),
+        None if c is None else ctypes.byref(c), float(dt), n, _ptr(qtb), _ptr(vtb), _ptr(stb), _ptr(q0t), _ptr(qc), _ptr(vb), _ptr(sb),
+        _ptr(tb), ctypes.byref(tb_), _stream(qt)))
+    del keep
+
+
+def _task_trajectory(h, mechanism, q0, v0, s0, tau, first, m, step, stage, ctl, contact, dt, what):
+    """rbd_integrate_task_pd recording steps first .. first + m from (q0, v0[, s0]) (not modified): [m + 1, rows, B] blocks."""
+    B = q0.shape[1]
+    q, v = q0.clone(), v0.clone()
+    s = None if s0 is None else s0.clone()
+    new = lambda x: torch.empty((m + 1,) + tuple(x.shape), dtype=x.dtype, device=x.device)   # noqa: E731
+    qt, vt = new(q0), new(v0)
+    st = None if s0 is None else new(s0)
+    t = None if tau is None else (tau if tau.dim() == 2 else tau[first:])
+    d, keep = _task_struct(ctl._steps_from(first), mechanism, h, q0, m, what)
+    c, keep2 = contact.c_struct() if contact is not None else (None, None)
+    _cabi.check(_cabi.load_library().rbd_integrate_task_pd(
+        h.ptr, _DT[q0.dtype], B, B, _ptr(q), _ptr(v), _ptr(s), _ptr(t), step, stage, ctypes.byref(d), None,
+        None if c is None else ctypes.byref(c), float(dt), m, _ptr(qt), _ptr(vt), _ptr(st), _stream(q0)))
+    del keep, keep2
+    return qt, vt, st
+
+
+class _SimulateTaskPD(torch.autograd.Function):
+    """The task-space closed-loop rollout; the controller's tensors are inputs (kp, kd, x_ref, xd_ref, then the joint term's kp, kd,
+    q_ref, v_ref, vd_ref), `ctl` the TaskPD they were taken from.  s0 / contact are None for the tree rollout."""
+
+    @staticmethod
+    def forward(ctx, mechanism, q0, v0, s0, tau, kp, kd, x_ref, xd_ref, jkp, jkd, jq_ref, jv_ref, jvd_ref, ctl, contact, dt, nsteps,
+                trajectory, every):
+        what = "autodiff.simulate" if contact is None else "autodiff.simulate_contact"
+        h, B, step, stage = _rollout_inputs(mechanism, what, q0, v0, tau, nsteps)
+        _task_struct(ctl, mechanism, h, q0, nsteps, what)          # the controller's checks, before any call
+        if contact is not None:
+            ns = contact.nstates
+            if s0.dtype != q0.dtype or s0.device != q0.device or not s0.is_contiguous() or tuple(s0.shape) != (ns, B):
+                raise DimensionMismatch(f"{what}: s0 must be a contiguous [{ns}, {B}] tensor with the dtype and device of q0")
+        ctx.handle, ctx.mechanism, ctx.ctl, ctx.contact, ctx.dt, ctx.nsteps, ctx.trajectory = h, mechanism, ctl, contact, dt, nsteps, trajectory
+        ctx.step, ctx.stage, ctx.what = step, stage, what
+        if trajectory or B == 0:
+            every = nsteps
+        else:       # checkpoints every `every` steps; backward re-records each segment before its VJP
+            every = max(1, min(every or nsteps, nsteps)) if nsteps else 1
+        ctx.every = every
+        q, v, s = q0, v0, s0
+        qs, vs, ss = [q0], [v0], [s0]
+        for first in range(0, max(nsteps, 1), every):
+            m = min(every, nsteps - first)
+            qt, vt, st = _task_trajectory(h, mechanism, q, v, s, tau, first, m, step, stage, ctl, contact, dt, what)
+            if trajectory or B == 0:
+                break
+            q, v, s = qt[-1].clone(), vt[-1].clone(), None if st is None else st[-1].clone()
+            qs.append(q); vs.append(v); ss.append(s)
+        ctl_tensors = (kp, kd, x_ref, xd_ref, jkp, jkd, jq_ref, jv_ref, jvd_ref)
+        if trajectory or B == 0:
+            ctx.save_for_backward(tau, qt, vt, st, *ctl_tensors)
+            out = (qt, vt) if contact is None else (qt, vt, st)
+            return out if trajectory else tuple(x[-1].clone() for x in out)
+        ctx.save_for_backward(tau, torch.stack(qs[:-1]), torch.stack(vs[:-1]), None if s0 is None else torch.stack(ss[:-1]), *ctl_tensors)
+        return (q, v) if contact is None else (q, v, s)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, *grads):
+        tau, qck, vck, sck = ctx.saved_tensors[:4]      # the controller's tensors are saved to catch in-place changes; ctl holds them
+        h, dt, n, cd, ctl, mech = ctx.handle, ctx.dt, ctx.nsteps, ctx.contact, ctx.ctl, ctx.mechanism
+        need = ctx.needs_input_grad
+        gq, gv = grads[0].contiguous(), grads[1].contiguous()
+        gs = grads[2].contiguous() if cd is not None else None
+        q0, v0 = qck[0], vck[0]
+        s0 = None if sck is None else sck[0]
+        B = q0.shape[1]
+        R, _ = ctl.rows()
+        j = ctl.joint
+        zero = lambda want, like: torch.zeros_like(like) if (want and like is not None) else None       # noqa: E731
+        per_sample = lambda want, rows: q0.new_zeros((rows, B)) if want else None                         # noqa: E731
+        tb = zero(need[4], tau)
+        bars = [per_sample(need[5], R), per_sample(need[6], R), zero(need[7], ctl.x_ref), zero(need[8], ctl.xd_ref)]
+        jbars = [None] * 5
+        if j is not None:
+            jbars = [per_sample(need[9], v0.shape[0]), per_sample(need[10], v0.shape[0]), zero(need[11], j.q_ref),
+                     zero(need[12], j.v_ref), zero(need[13], j.vd_ref)]
+        qa, va = torch.zeros_like(q0), torch.zeros_like(v0)
+        sa = None if s0 is None else torch.zeros_like(s0)
+        if B and any(need[1:14]):
+            seg_of = lambda t, first: t if t is None or t.dim() == 2 else t[first:]      # noqa: E731
+            if ctx.trajectory:
+                d, keep = _task_struct(ctl, mech, h, q0, n, ctx.what)
+                _task_vjp_call(h, qck, vck, sck, tau, ctx.step, ctx.stage, d, cd, dt, n, gq, gv, gs, None, qa, va, sa, tb, bars, jbars)
+                del keep
+            else:
+                # segments last to first; the adjoint of a segment's end state is its successor's q0_bar_cfg / v0_bar (/ s0_bar)
+                k = ctx.every
+                starts = list(range(0, n, k)) if n else [0]
+                qa, va, sa = gq, gv, gs
+                for jx in reversed(range(len(starts))):
+                    first = starts[jx]
+                    m = min(k, n - first)
+                    qt, vt, st = _task_trajectory(h, mech, qck[jx], vck[jx], None if sck is None else sck[jx], tau, first, m, ctx.step,
+                                                  ctx.stage, ctl, cd, dt, ctx.what)
+                    qtb, vtb = torch.zeros_like(qt), torch.zeros_like(vt)
+                    qtb[-1] = qa; vtb[-1] = va
+                    stb = None
+                    if st is not None:
+                        stb = torch.zeros_like(st)
+                        stb[-1] = sa
+                    d, keep = _task_struct(ctl._steps_from(first), mech, h, q0, m, ctx.what)
+                    qa, va = torch.empty_like(q0), torch.empty_like(v0)
+                    sa = None if s0 is None else torch.empty_like(s0)
+                    _task_vjp_call(h, qt, vt, st, seg_of(tau, first), ctx.step, ctx.stage, d, cd, dt, m, qtb, vtb, stb, None, qa, va, sa,
+                                   seg_of(tb, first), [bars[0], bars[1], seg_of(bars[2], first), seg_of(bars[3], first)],
+                                   [jbars[0], jbars[1], seg_of(jbars[2], first), seg_of(jbars[3], first), seg_of(jbars[4], first)])
+                    del keep
+        # shared gains: the per-sample bars summed over the batch
+        for i, g in ((0, ctl.kp), (1, ctl.kd)):
+            if bars[i] is not None and g.dim() == 1:
+                bars[i] = bars[i].sum(1)
+        for i, g in ((0, None if j is None else j.kp), (1, None if j is None else j.kd)):
+            if jbars[i] is not None and g.dim() == 1:
+                jbars[i] = jbars[i].sum(1)
+        return ((None, qa if need[1] else None, va if need[2] else None, sa if (need[3] and sa is not None) else None, tb) + tuple(bars)
+                + tuple(jbars) + (None,) * 6)
+
+
+def _simulate_task_pd(mechanism, q0, v0, s0, torques, controller, contact, dt, nsteps, trajectory, every, what):
+    if mechanism.has_loops():
+        raise _cabi.RbdError(_cabi.RBD_ELOOP, f"{what}: This method can currently only handle tree Mechanisms.")
+    c = controller
+    j = c.joint
+    jt = (None,) * 5 if j is None else (j.kp, j.kd, j.q_ref, j.v_ref, j.vd_ref)
+    return _SimulateTaskPD.apply(mechanism, q0, v0, s0, torques, c.kp, c.kd, c.x_ref, c.xd_ref, *jt, c, contact, float(dt), int(nsteps),
+                                 bool(trajectory), every)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# the task-space law at one state: rbd_task_pd_torques / rbd_task_pd_torques_vjp
+# ----------------------------------------------------------------------------------------------------------------------
+def task_pd_torques_vjp_(state: MechanismState, controller, tau_out_bar: torch.Tensor, torques: Optional[torch.Tensor] = None,
+                         step: int = 0, *, q_bar_tan: Optional[torch.Tensor] = None, q_bar_cfg: Optional[torch.Tensor] = None,
+                         v_bar: Optional[torch.Tensor] = None, tau_bar: Optional[torch.Tensor] = None,
+                         kp_bar: Optional[torch.Tensor] = None, kd_bar: Optional[torch.Tensor] = None,
+                         x_ref_bar: Optional[torch.Tensor] = None, xd_ref_bar: Optional[torch.Tensor] = None,
+                         joint_bars: Optional[Sequence[Optional[torch.Tensor]]] = None):
+    """τ̄ᵀ ∂τ/∂(...) of ``task_pd_torques(state, controller, torques, step)`` for ``tau_out_bar`` [nv, B]: ``q_bar_tan`` [nv, B],
+    ``q_bar_cfg`` [nq, B], ``v_bar`` [nv, B] and ``tau_bar`` (τ_ff, [nv, B]) are written; ``kp_bar`` / ``kd_bar`` [R, B] (per sample,
+    also for shared gains), ``x_ref_bar`` / ``xd_ref_bar`` (shapes of x_ref / xd_ref) and ``joint_bars`` = (kp, kd, q_ref, v_ref,
+    vd_ref) bars of the joint term ([nv, B] for the gains) are ADDED TO.  Each output is optional."""
+    from .pd import TaskPD
+    what = "task_pd_torques_vjp_"
+    if not isinstance(controller, TaskPD):
+        raise TypeError(f"{what}: controller must be a TaskPD")
+    _require_tree(state, what)
+    state.check_modcount()
+    _check(torques, state.nv, state, "torques")
+    _check(tau_out_bar, state.nv, state, "tau_out_bar")
+    if step < 0:
+        raise ValueError(f"{what}: step must be >= 0")
+    if tau_bar is not None and torques is None:
+        raise ValueError(f"{what}: tau_bar needs torques")
+    if xd_ref_bar is not None and controller.xd_ref is None:
+        raise ValueError(f"{what}: xd_ref_bar needs the controller's xd_ref")
+    j = controller.joint
+    jb = tuple(joint_bars) if joint_bars is not None else (None,) * 5
+    if any(t is not None for t in jb) and j is None:
+        raise ValueError(f"{what}: joint_bars need the controller's joint term")
+    B, nq, nv = state.batch, state.nq, state.nv
+    R, _ = controller.rows()
+    shape = lambda t: None if t is None else tuple(t.shape)      # noqa: E731
+    items = [(q_bar_tan, (nv, B), "q_bar_tan"), (q_bar_cfg, (nq, B), "q_bar_cfg"), (v_bar, (nv, B), "v_bar"), (tau_bar, (nv, B), "tau_bar"),
+             (kp_bar, (R, B), "kp_bar"), (kd_bar, (R, B), "kd_bar"), (x_ref_bar, shape(controller.x_ref), "x_ref_bar"),
+             (xd_ref_bar, shape(controller.xd_ref), "xd_ref_bar")]
+    if j is not None:
+        for bar, ref, name in ((jb[3], j.v_ref, "v_ref"), (jb[4], j.vd_ref, "vd_ref")):
+            if bar is not None and ref is None:
+                raise ValueError(f"{what}: the joint term's {name} bar needs its {name}")
+        items += [(jb[0], (nv, B), "joint kp_bar"), (jb[1], (nv, B), "joint kd_bar"), (jb[2], shape(j.q_ref), "joint q_ref_bar"),
+                  (jb[3], shape(j.v_ref), "joint v_ref_bar"), (jb[4], shape(j.vd_ref), "joint vd_ref_bar")]
+    _check_blocks(what, state.q, items)
+    d, keep = controller._c_struct(state, step + 1, what)
+    _torques_vjp_call(state, d, torques, int(step), tau_out_bar.contiguous(), q_bar_tan, q_bar_cfg, v_bar, tau_bar,
+                      (kp_bar, kd_bar, x_ref_bar, xd_ref_bar), jb)
+    del keep
+
+
+def _torques_vjp_call(state, d, torques, step, taub, qt, qc, vb, tb, bars, joint_bars):
+    from .pd import _RbdPdBar, _RbdTaskPdBar
+    jb = _RbdPdBar(*[_ptr(t) for t in joint_bars])
+    tb_ = _RbdTaskPdBar(*[_ptr(t) for t in bars], ctypes.pointer(jb) if any(t is not None for t in joint_bars) else None)
+    _cabi.check(_cabi.load_library().rbd_task_pd_torques_vjp(
+        state.handle.ptr, _DT[state.dtype], state.batch, _ptr(state.q), _ptr(state.v), _ptr(torques), ctypes.byref(d), step, _ptr(taub),
+        _ptr(qt), _ptr(qc), _ptr(vb), _ptr(tb), ctypes.byref(tb_), _stream(state.q)))
+
+
+class _TaskPdTorques(torch.autograd.Function):
+    """τ = task_pd_torques(state, ctl, torques, step) with q, v, τ_ff and the controller's tensors as inputs."""
+
+    @staticmethod
+    def forward(ctx, state, ctl, step, q, v, tau, kp, kd, x_ref, xd_ref, jkp, jkd, jq_ref, jv_ref, jvd_ref):
+        from .pd import task_pd_torques
+        ctx.state, ctx.ctl, ctx.step = state, ctl, step
+        ctx.save_for_backward(q, v, tau, kp, kd, x_ref, xd_ref, jkp, jkd, jq_ref, jv_ref, jvd_ref)
+        return task_pd_torques(state, ctl, tau, step)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, g):
+        q, v, tau, kp, kd, x_ref, xd_ref, jkp, jkd, jq_ref, jv_ref, jvd_ref = ctx.saved_tensors
+        state, ctl, step = ctx.state, ctx.ctl, ctx.step
+        need = ctx.needs_input_grad
+        B, nv = state.batch, state.nv
+        R, _ = ctl.rows()
+        z = lambda want, like: torch.zeros_like(like) if (want and like is not None) else None       # noqa: E731
+        per_sample = lambda want, rows: q.new_zeros((rows, B)) if want else None                        # noqa: E731
+        qc = torch.empty_like(q) if need[3] else None
+        vb = torch.empty_like(v) if need[4] else None
+        tb = torch.empty_like(v) if (need[5] and tau is not None) else None
+        bars = [per_sample(need[6], R), per_sample(need[7], R), z(need[8], x_ref), z(need[9], xd_ref)]
+        jbars = [per_sample(need[10], nv), per_sample(need[11], nv), z(need[12], jq_ref), z(need[13], jv_ref), z(need[14], jvd_ref)]
+        if B and any(need[3:15]):
+            d, keep = ctl._c_struct(state, step + 1, "autodiff.task_pd_torques")
+            _torques_vjp_call(state, d, tau, step, g.contiguous(), None, qc, vb, tb, bars, jbars)
+            del keep
+        for i, t in ((0, kp), (1, kd)):
+            if bars[i] is not None and t.dim() == 1:
+                bars[i] = bars[i].sum(1)
+        for i, t in ((0, jkp), (1, jkd)):
+            if jbars[i] is not None and t.dim() == 1:
+                jbars[i] = jbars[i].sum(1)
+        return (None, None, None, qc, vb, tb) + tuple(bars) + tuple(jbars)
+
+
+def task_pd_torques(state: MechanismState, controller, torques: Optional[torch.Tensor] = None, step: int = 0) -> torch.Tensor:
+    """Differentiable ``task_pd_torques``: the torques ``controller`` (a ``TaskPD``) applies at ``state`` with the references of
+    ``step`` and feedforward ``torques``.  Gradients flow to ``state.q`` (as ``q_bar_cfg``), ``state.v``, ``torques`` and the TaskPD's
+    kp, kd, x_ref, xd_ref and its joint term's arrays, whichever require grad (shared gains: summed over the batch); backward runs
+    ``rbd_task_pd_torques_vjp``.  Not twice differentiable."""
+    from .pd import TaskPD
+    if not isinstance(controller, TaskPD):
+        raise TypeError("autodiff.task_pd_torques: controller must be a TaskPD")
+    c, j = controller, controller.joint
+    jt = (None,) * 5 if j is None else (j.kp, j.kd, j.q_ref, j.v_ref, j.vd_ref)
+    return _TaskPdTorques.apply(state, c, int(step), state.q, state.v, torques, c.kp, c.kd, c.x_ref, c.xd_ref, *jt)

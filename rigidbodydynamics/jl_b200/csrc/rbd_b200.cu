@@ -1546,7 +1546,7 @@ int check_task_ctrl(const char* fn, const rbd_model* model, int64_t ld, const rb
 // Computed-torque mode: v̇_des (task kernel) -> inverse dynamics -> pd_finish_kernel (τ_ff, clamp) on dense rows, copied out.
 template <class T>
 int task_pd_torques_t(const rbd_model* model, int64_t B, int64_t ld, const void* q, const void* v, const void* tau_ff,
-                      const rbd_task_pd_desc& c, int step, void* tau_out, cudaStream_t stream) {
+                      const rbd_task_pd_desc& c, int step, void* tau_out, cudaStream_t stream, void* vdes_out = nullptr) {
   const HostModel& hm = model->hm;
   const ModelDev<T>& M = dev_model<T>(hm);
   const size_t nq = hm.nq, nv = hm.nv;
@@ -1602,6 +1602,7 @@ int task_pd_torques_t(const rbd_model* model, int64_t B, int64_t ld, const void*
   pd_finish_kernel<T><<<(int)std::min<int64_t>(((int64_t)nv * B + 255) / 256, (int64_t)p.sms * 8), 256, 0, stream>>>(pf);
   if (int rc = api_launched()) return rc;
   RBD_CUDA_TRY(cudaMemcpy2DAsync(tau_out, ld * sizeof(T), tau_d, B * sizeof(T), B * sizeof(T), nv, cudaMemcpyDeviceToDevice, stream));
+  if (vdes_out) RBD_CUDA_TRY(cudaMemcpyAsync(vdes_out, vdes, nv * B * sizeof(T), cudaMemcpyDeviceToDevice, stream));
   return RBD_OK;
 }
 
@@ -1611,6 +1612,14 @@ int task_pd_torques_t(const rbd_model* model, int64_t B, int64_t ld, const void*
 namespace rbd {
 int api_check(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld) { return check_common(model, dtype, B, ld); }
 int api_check_contact(const rbd_model* model, const rbd_contact_desc* contact, const char* fn) { return check_contact(model, contact, fn); }
+int api_check_task_ctrl(const char* fn, const rbd_model* model, int64_t ld, const rbd_task_pd_desc* ctrl) {
+  return check_task_ctrl(fn, model, ld, ctrl);
+}
+int task_pd_law(const rbd_model* model, int32_t dtype, int64_t B, const void* q, const void* v, const void* tau_ff, const rbd_task_pd_desc& c,
+                int step, void* tau_out, void* vdes_out, cudaStream_t stream) {
+  return dtype == RBD_F32 ? task_pd_torques_t<float>(model, B, B, q, v, tau_ff, c, step, tau_out, stream, vdes_out)
+                          : task_pd_torques_t<double>(model, B, B, q, v, tau_ff, c, step, tau_out, stream, vdes_out);
+}
 int integrate(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const Rollout& r, cudaStream_t stream) {
   if (B == 0 || (r.nsteps == 0 && !r.q_traj)) return RBD_OK;
   Rollout n = r;

@@ -207,5 +207,11 @@ int inverse_dynamics_vjp_dense(const rbd_model* model, int32_t dtype, int64_t B,
                                const void* tau_bar, void* q_bar_cfg, void* v_bar, void* vd_bar, cudaStream_t stream);
 // The model limits of rbd_dynamics_vjp / rbd_inverse_dynamics_vjp (those of rbd_dynamics_derivatives): RBD_OK or RBD_EUNSUPPORTED
 int check_vjp_limits(const HostModel& hm, const char* who);
+// rbd_b200.cu's controller checks of rbd_integrate_task_pd (the joint term's JointPD checks, then check_task_pd), leading dimension ld
+int api_check_task_ctrl(const char* fn, const rbd_model* model, int64_t ld, const rbd_task_pd_desc* ctrl);
+// rbd_task_pd_torques on dense [rows x B] arrays (arguments checked by the caller): tau_out the applied torques; in computed-torque
+// mode also v̇_des, the inverse dynamics' input, into vdes_out [nv x B] when it is not NULL
+int task_pd_law(const rbd_model* model, int32_t dtype, int64_t B, const void* q, const void* v, const void* tau_ff, const rbd_task_pd_desc& c,
+                int step, void* tau_out, void* vdes_out, cudaStream_t stream);
 
 }  // namespace rbd

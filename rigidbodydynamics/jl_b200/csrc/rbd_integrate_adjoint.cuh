@@ -31,6 +31,7 @@ template <class F> struct ScalarOf<Dual1<F>> { using type = F; };
 
 template <class F> RBD_HD bool operator<(const Dual1<F>& a, const Dual1<F>& b) { return a.v < b.v; }
 template <class F> RBD_HD bool operator>(const Dual1<F>& a, const Dual1<F>& b) { return a.v > b.v; }
+template <class F> RBD_HD bool operator>=(const Dual1<F>& a, const Dual1<F>& b) { return a.v >= b.v; }
 template <class F> RBD_HD Dual1<F> sqrt_t(const Dual1<F>& x) {
   const F r = sqrt_t(x.v);
   return {r, r > F(0) ? x.d * F(0.5) / r : F(0)};      // sqrt(0): only the Taylor branches read it, with a zero derivative

@@ -122,6 +122,11 @@ class _RbdTaskPdDesc(ctypes.Structure):
                 ("effort_lo", ctypes.POINTER(ctypes.c_double)), ("effort_hi", ctypes.POINTER(ctypes.c_double))]
 
 
+class _RbdTaskPdBar(ctypes.Structure):
+    _fields_ = [("kp", ctypes.c_void_p), ("kd", ctypes.c_void_p), ("x_ref", ctypes.c_void_p), ("xd_ref", ctypes.c_void_p),
+                ("joint", ctypes.POINTER(_RbdPdBar))]
+
+
 _KINDS = {"point": 0, "pose": 1}
 
 
@@ -137,7 +142,11 @@ class TaskPD:
     [nsteps, R, B], None = 0 -- the target point velocity in ``base`` coordinates, or the target twist of the pose frame in that frame.
     ``joint``: a ``JointPD`` added in the same mode (its own ``effort_bounds`` must be None), e.g. posture or damping.
     ``computed_torque``: v̇_des = joint term + Σ J^T f, τ = inverse_dynamics!(q, v, v̇_des) + τ_ff; otherwise τ = τ_ff + joint term +
-    Σ J^T f.  ``effort_bounds`` clamp the sum.  Not differentiable: ``autodiff.simulate`` refuses it."""
+    Σ J^T f.  ``effort_bounds`` clamp the sum.
+
+    ``autodiff.simulate`` / ``autodiff.simulate_contact`` take one as ``controller=`` too: gradients then also flow to those of
+    ``kp``, ``kd``, ``x_ref``, ``xd_ref`` and of the joint term's arrays that require grad (DESIGN 4.22); the task points and the
+    effort bounds receive none."""
 
     def __init__(self, tasks, kinds, kp, kd, x_ref, xd_ref=None, *, joint=None, computed_torque: bool = False, effort_bounds=None):
         self.tasks, self.kinds = list(tasks), list(kinds)
