@@ -566,6 +566,27 @@ typedef struct rbd_kinematics_out {
 int32_t rbd_kinematics(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                        const int8_t* path_sign, const rbd_kinematics_out* out, void* stream);
 
+/* Reverse mode of rbd_kinematics (DESIGN 4.23): for the same (q, v, path_sign), the product  Σ_outputs ȳ . ∂y/∂(q, v)  over any
+ * subset of the eight outputs.  `out_bar` reuses rbd_kinematics_out: each member is NULL (zero cotangent) or the cotangent ȳ with
+ * exactly that output's layout and leading dimension ld.  Cotangent rows of geometric-Jacobian columns off the path (sign 0) are not
+ * read.  Outputs, each [rows x B] with leading dimension ld or NULL (not wanted), are WRITTEN, not accumulated, with the conventions
+ * of rbd_dynamics_vjp: q_bar_tan [nv], q_bar_cfg [nq] (no radial quaternion component), v_bar [nv] (zero when no kinetic_energy,
+ * momentum or momentum_rate_bias cotangent is given).  Every forward quantity is recomputed from q and v.  Derivation
+ * (csrc/rbd_kin_adjoint.cuh): each output is pulled back onto a pose, a twist and an acceleration covector per body -- the transform
+ * term of rbd_task_kinematics_vjp for transforms_to_root, (mc_i x c, m_i c) for the centre of mass and the potential energy, I_i
+ * times the cotangent plus the rigid motion of I_i for the energy and momenta -- and Jacobian-like columns add S_k x* φ_k at their
+ * body (φ_k = s_k J̄_k for the geometric Jacobian, Ic Ā_k for the momentum matrix, whose I_i S_k products also give every body a pose
+ * covector accumulated along its path).  One inward sweep maps them to the coordinates.  Errors, all decided on the host before any
+ * CUDA call: those of rbd_kinematics with out_bar in place of out (a kinetic_energy / momentum / momentum_rate_bias cotangent with
+ * v == NULL, path_sign given without a geometric_jacobian cotangent or missing with one, a sign outside {-1, 0, +1}, a
+ * center_of_mass cotangent on a massless mechanism: RBD_EINVAL; dtype other than fp32 / fp64: RBD_EUNSUPPORTED; ld < B: RBD_EDIM).
+ * B == 0: RBD_OK, nothing written; every cotangent NULL: RBD_OK, the requested gradients set to zero, no kernel launched.  Otherwise
+ * one kernel launch per call, with a stream-ordered workspace of 42 rows per body per resident thread, and with a momentum_matrix
+ * cotangent 10 more per body plus 21 for the current body and 21 per pending slot (at most 512 MB in all). */
+int32_t rbd_kinematics_vjp(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
+                           const int8_t* path_sign, const rbd_kinematics_out* out_bar, void* q_bar_tan, void* q_bar_cfg,
+                           void* v_bar, void* stream);
+
 /* Task-space kinematics (DESIGN 4.17): point Jacobians, relative transforms, twists and accelerations of chosen bodies, in any
  * body frame, for up to RBD_MAX_TASKS tasks from ONE launch.  A task is a body of interest, a base body, a point fixed in the body
  * and a frame to express results in.  The descriptor holds plain HOST arrays, read at call time like rbd_contact_desc:

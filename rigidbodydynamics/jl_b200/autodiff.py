@@ -8,6 +8,7 @@
     integrate_task_pd_vjp_ gradient of a recorded task-space closed-loop rollout  rbd_integrate_task_pd_vjp  (csrc/rbd_task_pd_adjoint.cuh)
     task_pd_torques_vjp_   τ̄ᵀ ∂τ/∂(q, v, τ_ff, controller) of a TaskPD's torques at one state  rbd_task_pd_torques_vjp
     task_kinematics_vjp_   Σ ȳᵀ ∂y/∂(q, v, v̇) of task-space outputs  rbd_task_kinematics_vjp  (csrc/rbd_task_adjoint.cuh)
+    kinematics_vjp_        Σ ȳᵀ ∂y/∂(q, v) of whole-body kinematics outputs  rbd_kinematics_vjp  (csrc/rbd_kin_adjoint.cuh)
     dynamics(mechanism, q, v, tau=None, externalwrenches=None)         differentiable v̇ = dynamics!(...)
     inverse_dynamics(mechanism, q, v, vd, externalwrenches=None)       differentiable τ = inverse_dynamics!(...)
     simulate(mechanism, q0, v0, torques=None, *, dt, nsteps, ...)     differentiable RK4 rollout (simulate)
@@ -17,6 +18,9 @@
     task_kinematics(mechanism, q, v=None, vd=None, *, tasks, outputs=("point",))
                                                                        differentiable task-space kinematics (TaskFrame tasks)
     task_pd_torques(state, controller, torques=None, step=0)          differentiable torques of a TaskPD at one state
+    kinematics(mechanism, q, v=None, *, outputs=("center_of_mass",), path=None)
+                                                                       differentiable whole-body kinematics (centre of mass,
+                                                                       energies, momentum, momentum matrix, ...)
 
 One product costs one Articulated-Body solve (forward dynamics only) plus one outward and one inward sweep: O(n) per sample, no
 nv x nv Jacobian is formed (``dynamics_derivatives_`` builds both full Jacobians instead).  Every tensor is ``[rows, B]``, contiguous,
@@ -35,18 +39,19 @@ import ctypes
 from types import SimpleNamespace
 from typing import Dict, Optional, Sequence
 
+import numpy as np
 import torch
 from torch.autograd.function import once_differentiable
 
 from . import _cabi
 from .algorithms import DimensionMismatch, _check, _ptr, _require_tree
-from .kinematics import _TASK_NEEDS_V, _TASK_ROWS, TaskFrame, task_desc
+from .kinematics import _NEEDS_V, _ROWS, _TASK_NEEDS_V, _TASK_ROWS, TaskFrame, TreePath, task_desc
 from .mechanism import Mechanism
 from .state import _DT, MechanismState, _model_handle
 
 __all__ = ["dynamics_vjp_", "inverse_dynamics_vjp_", "integrate_vjp_", "integrate_contact_vjp_", "integrate_pd_vjp_", "integrate_task_pd_vjp_",
            "task_pd_torques_vjp_", "task_pd_torques", "dynamics",
-           "inverse_dynamics", "simulate", "simulate_contact", "task_kinematics_vjp_", "task_kinematics"]
+           "inverse_dynamics", "simulate", "simulate_contact", "task_kinematics_vjp_", "task_kinematics", "kinematics_vjp_", "kinematics"]
 
 
 def _stream(t: torch.Tensor):
@@ -298,6 +303,117 @@ def task_kinematics(mechanism: Mechanism, q: torch.Tensor, v: Optional[torch.Ten
     if len(set(outputs)) != len(outputs):
         raise ValueError("autodiff.task_kinematics: outputs must be distinct")
     return dict(zip(outputs, _TaskKinematics.apply(mechanism, tasks, outputs, q, v, vd)))
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# whole-body kinematics: rbd_kinematics / rbd_kinematics_vjp
+# ----------------------------------------------------------------------------------------------------------------------
+def _kin_out(tensors: Dict[str, Optional[torch.Tensor]], nb: int, nv: int, like: torch.Tensor, what: str) -> _cabi.RbdKinematicsOut:
+    """rbd_kinematics_out for {output: [rows, B] tensor or None}, checked against the dtype, device and batch of ``like``."""
+    ko = _cabi.RbdKinematicsOut()
+    dims = SimpleNamespace(nv=nv, mechanism=SimpleNamespace(joints=range(nb)))
+    for name, t in tensors.items():
+        if name not in _ROWS:
+            raise TypeError(f"{what}: unknown kinematics output {name!r}")
+        if t is None:
+            continue
+        rows = _ROWS[name](dims)
+        if t.dtype != like.dtype or t.device != like.device:
+            raise TypeError(f"{what}: {name} must have the dtype and device of q")
+        if t.dim() != 2 or tuple(t.shape) != (rows, like.shape[1]):
+            raise DimensionMismatch(f"{what}: {name} has wrong size: expected ({rows}, {like.shape[1]}), got {tuple(t.shape)}")
+        if not t.is_contiguous():
+            raise ValueError(f"{what}: {name} must be [rows, B] contiguous (batch index fastest)")
+        setattr(ko, name, t.data_ptr())
+    return ko
+
+
+def _path_sign(path_: Optional[TreePath], want_jac: bool, nb: int):
+    """The host int8 array of ``path_``'s signs, or None without a geometric Jacobian (the messages of ``kinematics_``)."""
+    if not want_jac:
+        return None
+    if path_ is None:
+        raise ValueError("geometric_jacobian needs a path")
+    sign = np.ascontiguousarray(path_.sign, np.int8)
+    if sign.shape != (nb,):
+        raise DimensionMismatch("path does not belong to this mechanism")
+    return sign
+
+
+def _sign_ptr(sign):
+    return None if sign is None else sign.ctypes.data_as(ctypes.c_void_p)
+
+
+def kinematics_vjp_(state: MechanismState, path_: Optional[TreePath] = None, *, bars: dict, q_bar_tan: Optional[torch.Tensor] = None,
+                    q_bar_cfg: Optional[torch.Tensor] = None, v_bar: Optional[torch.Tensor] = None):
+    """The product ``Σ ȳᵀ ∂y/∂(q, v)`` of ``kinematics_(state, path_, ...)`` for every sample.
+
+    ``bars``: {output name: ȳ} with the names and layouts of ``kinematics_``; missing outputs have zero cotangent, and a
+    ``geometric_jacobian`` cotangent needs ``path_``.  Everything is recomputed from the state.  Outputs (each optional, overwritten):
+    ``q_bar_tan`` [nv, B], ``q_bar_cfg`` [nq, B], ``v_bar`` [nv, B] (see the module docstring for the two configuration covectors)."""
+    state.check_modcount()
+    lib = _cabi.load_library()
+    nb = len(state.mechanism.joints)
+    ko = _kin_out(bars, nb, state.nv, state.q, "kinematics_vjp_")
+    for t, rows, name in ((q_bar_tan, state.nv, "q_bar_tan"), (q_bar_cfg, state.nq, "q_bar_cfg"), (v_bar, state.nv, "v_bar")):
+        _check(t, rows, state, name)
+    sign = _path_sign(path_, bars.get("geometric_jacobian") is not None, nb)
+    _cabi.check(lib.rbd_kinematics_vjp(state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q), _ptr(state.v),
+                                       _sign_ptr(sign), ctypes.byref(ko), _ptr(q_bar_tan), _ptr(q_bar_cfg), _ptr(v_bar),
+                                       _stream(state.q)))
+
+
+class _Kinematics(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, mechanism, outputs, sign, q, v):
+        h, B = _inputs(mechanism, "autodiff.kinematics", q=q, v=v)
+        if v is None and any(k in _NEEDS_V for k in outputs):
+            raise ValueError(f"autodiff.kinematics: {', '.join(k for k in outputs if k in _NEEDS_V)} need v")
+        nb, nv = h.info.nb, h.info.nv
+        dims = SimpleNamespace(nv=nv, mechanism=SimpleNamespace(joints=range(nb)))
+        outs = {k: torch.empty((_ROWS[k](dims), B), dtype=q.dtype, device=q.device) for k in outputs}
+        ko = _kin_out(outs, nb, nv, q, "autodiff.kinematics")
+        if B and outputs:
+            _cabi.check(_cabi.load_library().rbd_kinematics(h.ptr, _DT[q.dtype], B, B, _ptr(q), _ptr(v), _sign_ptr(sign),
+                                                            ctypes.byref(ko), _stream(q)))
+        ctx.handle, ctx.outputs, ctx.sign = h, outputs, sign
+        ctx.save_for_backward(q, v)
+        return tuple(outs[k] for k in outputs)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, *grads):
+        q, v = ctx.saved_tensors
+        h = ctx.handle
+        need = ctx.needs_input_grad
+        qb = _out(need[3], q, q.shape[0])
+        vb = _out(need[4] and v is not None, q, h.info.nv)
+        bars = {k: g.contiguous() for k, g in zip(ctx.outputs, grads) if g is not None}
+        B = q.shape[1]
+        if B and any(t is not None for t in (qb, vb)):
+            ko = _kin_out(bars, h.info.nb, h.info.nv, q, "autodiff.kinematics")
+            sign = ctx.sign if "geometric_jacobian" in bars else None
+            _cabi.check(_cabi.load_library().rbd_kinematics_vjp(h.ptr, _DT[q.dtype], B, B, _ptr(q), _ptr(v), _sign_ptr(sign),
+                                                                ctypes.byref(ko), None, _ptr(qb), _ptr(vb), _stream(q)))
+        return None, None, None, qb, vb
+
+
+def kinematics(mechanism: Mechanism, q: torch.Tensor, v: Optional[torch.Tensor] = None, *,
+               outputs: Sequence[str] = ("center_of_mass",), path: Optional[TreePath] = None) -> Dict[str, torch.Tensor]:
+    """Differentiable whole-body kinematics: {name: [rows, B]} for the requested ``outputs`` (names and layout of ``kinematics_``:
+    transforms_to_root, center_of_mass, kinetic_energy, gravitational_potential_energy, momentum, momentum_rate_bias,
+    momentum_matrix, geometric_jacobian) of q [nq, B] and v [nv, B] (needed by kinetic_energy / momentum / momentum_rate_bias);
+    ``path`` is the geometric Jacobian's ``TreePath``.  Forward is one ``rbd_kinematics`` call for all outputs; backward one
+    ``rbd_kinematics_vjp`` with the incoming gradients.  The gradient of ``q`` is ``q_bar_cfg`` (see the module docstring).  Not
+    twice differentiable."""
+    outputs = tuple(outputs)
+    for k in outputs:
+        if k not in _ROWS:
+            raise TypeError(f"autodiff.kinematics: unknown kinematics output {k!r}")
+    if len(set(outputs)) != len(outputs):
+        raise ValueError("autodiff.kinematics: outputs must be distinct")
+    sign = _path_sign(path, "geometric_jacobian" in outputs, len(mechanism.joints))
+    return dict(zip(outputs, _Kinematics.apply(mechanism, outputs, sign, q, v)))
 
 
 # ----------------------------------------------------------------------------------------------------------------------

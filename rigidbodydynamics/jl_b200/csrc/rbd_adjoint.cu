@@ -1,5 +1,6 @@
 // rbd_dynamics_vjp / rbd_inverse_dynamics_vjp: reverse-mode products of dynamics! and inverse_dynamics! (csrc/rbd_adjoint.cuh has
-// the mathematics); rbd_task_kinematics_vjp: the reverse mode of rbd_task_kinematics (csrc/rbd_task_adjoint.cuh).
+// the mathematics); rbd_task_kinematics_vjp: the reverse mode of rbd_task_kinematics (csrc/rbd_task_adjoint.cuh);
+// rbd_kinematics_vjp: the reverse mode of rbd_kinematics (csrc/rbd_kin_adjoint.cuh).
 //
 // One generic persistent kernel per entry point, one thread per sample, one launch per call: blocks of one warp looping over groups
 // of 32 samples, launched through plan_persistent (rbd_handle.h).  The per-sample working set -- 54 rows per body plus μ -- lives
@@ -20,6 +21,7 @@
 #define sincos_slow sincos_slow_adjoint_tu
 #include "rbd_adjoint.cuh"
 #include "rbd_handle.h"
+#include "rbd_kin_adjoint.cuh"
 #include "rbd_task_adjoint.cuh"
 
 using namespace rbd;
@@ -176,6 +178,64 @@ int task_vjp_t(const rbd_model* model, int64_t B, int64_t ld, const void* q, con
   return api_launched(&pl);
 }
 
+// ---- whole-body kinematics VJP ----
+template <class T> struct KinVjpArgs {
+  const T *q, *v;
+  const T *tr, *com, *ke, *pe, *mom, *mrb, *A, *J;    // cotangents, NULL = zero
+  T *qt, *qc, *vb;                                    // outputs, NULL = not wanted
+  T* work;                                            // [rows][grid * NT]
+  int64_t ld, B;
+};
+static_assert(sizeof(ModelDev<double>) + sizeof(KinDev<double>) + sizeof(KinVjpArgs<double>) <= 32764,
+              "kin_vjp_kernel's parameters exceed the kernel-parameter limit");
+
+template <class T>
+__global__ void __launch_bounds__(kNT, 1)
+kin_vjp_kernel(const __grid_constant__ ModelDev<T> M, const __grid_constant__ KinDev<T> K, const KinVjpArgs<T> a) {
+  const int64_t tid = (int64_t)blockIdx.x * kNT + threadIdx.x;
+  const int64_t ngroups = (a.B + kNT - 1) / kNT;
+  for (int64_t g = blockIdx.x; g < ngroups; g += gridDim.x) {
+    const int64_t b = g * kNT + threadIdx.x;
+    const bool active = b < a.B;
+    const int64_t bl = active ? b : a.B - 1;      // inactive lanes recompute the last sample, stores are masked
+    KinBarIO<T> io;
+    auto in = [&](const T* p) { return Col<T>{p ? p + bl : nullptr, a.ld}; };
+    auto out = [&](T* p) { return ColOut<T>{p ? p + bl : nullptr, a.ld, active}; };
+    io.q = in(a.q); io.v = in(a.v);
+    io.tr = in(a.tr); io.com = in(a.com); io.ke = in(a.ke); io.pe = in(a.pe);
+    io.mom = in(a.mom); io.mrb = in(a.mrb); io.A = in(a.A); io.J = in(a.J);
+    io.qt = out(a.qt); io.qc = out(a.qc); io.vb = out(a.vb);
+    io.s = {a.work + tid, (int64_t)gridDim.x * kNT};
+    kin_vjp_sample<T>(M, K, io);
+  }
+}
+
+template <class T>
+int kin_vjp_t(const rbd_model* model, int64_t B, int64_t ld, const void* q, const void* v, const int8_t* path_sign,
+              const rbd_kinematics_out& o, void* qt, void* qc, void* vb, cudaStream_t stream) {
+  const HostModel& hm = model->hm;
+  const void* const bars[8] = {o.transforms_to_root, o.center_of_mass, o.kinetic_energy, o.gravitational_potential_energy,
+                               o.momentum, o.momentum_rate_bias, o.momentum_matrix, o.geometric_jacobian};
+  if (std::all_of(bars, bars + 8, [](const void* p) { return p == nullptr; })) {    // zero cotangent: zero gradients
+    for (auto [p, rows] : {std::pair<void*, int>{qt, hm.nv}, {qc, hm.nq}, {vb, hm.nv}})
+      if (int rc = zero_rows<T>((T*)p, rows, B, ld, stream)) return rc;
+    return RBD_OK;
+  }
+  const ModelDev<T>& M = dev_model<T>(hm);
+  std::unique_ptr<KinDev<T>> K(new KinDev<T>());
+  build_kin_dev<T>(hm, path_sign, *K);
+  KinVjpArgs<T> a{(const T*)q, (const T*)v, (const T*)o.transforms_to_root, (const T*)o.center_of_mass, (const T*)o.kinetic_energy,
+                  (const T*)o.gravitational_potential_energy, (const T*)o.momentum, (const T*)o.momentum_rate_bias,
+                  (const T*)o.momentum_matrix, (const T*)o.geometric_jacobian, (T*)qt, (T*)qc, (T*)vb, nullptr, ld, B};
+  const size_t row_bytes = (size_t)kin_adjoint_rows(hm.nb, M.nslots, o.momentum_matrix != nullptr) * sizeof(T);
+  LaunchPlan pl;
+  if (int rc = plan_persistent((const void*)kin_vjp_kernel<T>, kNT, 0, (B + kNT - 1) / kNT, stream, pl, row_bytes, 0, kWorkspaceCap))
+    return rc;
+  a.work = (T*)pl.work.p;
+  kin_vjp_kernel<T><<<pl.grid, pl.block, pl.smem, stream>>>(M, *K, a);
+  return api_launched(&pl);
+}
+
 }  // namespace
 
 // Same model limits as rbd_dynamics_derivatives
@@ -247,4 +307,27 @@ extern "C" int32_t rbd_task_kinematics_vjp(const rbd_model* model, int32_t dtype
   cudaStream_t s = (cudaStream_t)stream;
   return dtype == RBD_F32 ? task_vjp_t<float>(model, B, ld, q, v, vd, *tasks, *out_bar, q_bar_tan, q_bar_cfg, v_bar, vd_bar, s)
                           : task_vjp_t<double>(model, B, ld, q, v, vd, *tasks, *out_bar, q_bar_tan, q_bar_cfg, v_bar, vd_bar, s);
+}
+
+extern "C" int32_t rbd_kinematics_vjp(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
+                                      const int8_t* path_sign, const rbd_kinematics_out* out_bar, void* q_bar_tan, void* q_bar_cfg,
+                                      void* v_bar, void* stream) {
+  if (int rc = api_check(model, dtype, B, ld)) return rc;
+  const ApiCall call;
+  if (dtype != RBD_F32 && dtype != RBD_F64) return api_fail(RBD_EUNSUPPORTED, "rbd_kinematics_vjp: fp32 and fp64 only");
+  if (!out_bar) return api_fail(RBD_EINVAL, "rbd_kinematics_vjp: out_bar must not be NULL");
+  if (B == 0) return RBD_OK;      // empty batch: nothing to read or write, pointers may be NULL
+  if (!q) return api_fail(RBD_EINVAL, "rbd_kinematics_vjp: q must not be NULL");
+  if (!v && (out_bar->kinetic_energy || out_bar->momentum || out_bar->momentum_rate_bias))
+    return api_fail(RBD_EINVAL, "rbd_kinematics_vjp: kinetic_energy / momentum / momentum_rate_bias cotangents need v");
+  if ((out_bar->geometric_jacobian != nullptr) != (path_sign != nullptr))
+    return api_fail(RBD_EINVAL, "rbd_kinematics_vjp: path_sign must be given iff the geometric_jacobian cotangent is");
+  if (path_sign)
+    for (int i = 0; i < model->hm.nb; ++i)
+      if (path_sign[i] < -1 || path_sign[i] > 1)
+        return api_fail(RBD_EINVAL, "rbd_kinematics_vjp: path_sign entries must be -1, 0 or +1");
+  if (model->hm.total_mass <= 0 && out_bar->center_of_mass) return api_fail(RBD_EINVAL, "rbd_kinematics_vjp: mechanism has no mass");
+  cudaStream_t s = (cudaStream_t)stream;
+  return dtype == RBD_F32 ? kin_vjp_t<float>(model, B, ld, q, v, path_sign, *out_bar, q_bar_tan, q_bar_cfg, v_bar, s)
+                          : kin_vjp_t<double>(model, B, ld, q, v, path_sign, *out_bar, q_bar_tan, q_bar_cfg, v_bar, s);
 }

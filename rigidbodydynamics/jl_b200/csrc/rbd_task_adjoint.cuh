@@ -88,6 +88,65 @@ template <class T> RBD_HD void task_fcross_add(const Mot<T>& m, const T* n, cons
   for (int k = 0; k < 3; ++k) { on[k] += sg * a[k]; of[k] += sg * b[k]; }
 }
 
+// The inward sweep's step at one body: the adjoints of its joint's coordinates from the body's completed subtree sums A, T, W
+// (v̇̄_j, v̄_j and q̄_j of the derivation above; q̄_cfg through cfg_adjoint).  `row` is the body's first workspace row (kTaskAdjRows
+// layout: pose, and with want_vel the twist and acceleration of the body and of its parent); vi is the body's twist.  Any output may
+// be invalid.  Shared by task_vjp_sample and kin_vjp_sample (rbd_kin_adjoint.cuh).
+template <class T>
+RBD_HD void task_joint_adjoint(const BodyDev<T>& bd, const Scr<T>& s, int row, const T* A, const T* Tt, const T* W, const Mot<T>& vi,
+                               bool want_vel, bool want_acc, bool want_q, const Col<T>& q, const ColOut<T>& qt, const ColOut<T>& qc,
+                               const ColOut<T>& vb, const ColOut<T>& vdb) {
+  const int nvj = kind_nv_dev(bd.kind);
+  if (nvj == 0) return;
+  Pose<T> X;
+#pragma unroll
+  for (int k = 0; k < 9; ++k) X.R[k] = s.get(row + k);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) X.p[k] = s.get(row + 9 + k);
+  Mot<T> vp, ap;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) vp.w[k] = vp.l[k] = ap.w[k] = ap.l[k] = T(0);
+  if (want_vel && !(bd.flags & F_ROOT_CHILD)) {
+    const int prow = kTaskAdjRows * bd.parent;
+    ld_mot(s, prow + kTaV, vp);
+    ld_mot(s, prow + kTaA, ap);
+  }
+  T ft[6] = {T(0), T(0), T(0), T(0), T(0), T(0)};
+  for (int k = 0; k < nvj; ++k) {
+    Mot<T> S;
+    world_subspace(X, sub_comp(bd.kind, k), S);
+    if (vdb.valid()) vdb.st(bd.vrow + k, want_acc ? dot_mf(S, A, A + 3) : T(0));
+    if (vb.valid()) {
+      T x = T(0);
+      if (want_vel) {
+        Mot<T> vs, sdp;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) { vs.w[c] = vi.w[c] + vp.w[c]; vs.l[c] = vi.l[c] + vp.l[c]; }
+        motion_cross(vs, S, sdp);
+        x = dot_mf(S, Tt, Tt + 3) + dot_mf(sdp, A, A + 3);
+      }
+      vb.st(bd.vrow + k, x);
+    }
+    if (want_q) {
+      T x = dot_mf(S, W, W + 3);
+      if (want_vel) {
+        Mot<T> pd, pdd, t1, t2;
+        motion_cross(vp, S, pd);
+        motion_cross(ap, S, t1);
+        motion_cross(vp, pd, t2);
+#pragma unroll
+        for (int c = 0; c < 3; ++c) { pdd.w[c] = t1.w[c] + t2.w[c]; pdd.l[c] = t1.l[c] + t2.l[c]; }
+        x += dot_mf(pd, Tt, Tt + 3) + dot_mf(pdd, A, A + 3);
+      }
+      if (qt.valid()) qt.st(bd.vrow + k, x);
+      // ft[k] = x with a warp-uniform k: a select chain keeps ft in registers
+#pragma unroll
+      for (int c = 0; c < 6; ++c) if (c == k) ft[c] = x;
+    }
+  }
+  if (qc.valid()) cfg_adjoint(bd, q, ft, qc);
+}
+
 template <class T>
 RBD_HD void task_vjp_sample(const ModelDev<T>& M, const TaskDev<T>& D, const TaskBarIO<T>& io) {
   const int nb = M.nb, nv = M.nv, K = D.ntasks;
@@ -404,56 +463,7 @@ RBD_HD void task_vjp_sample(const ModelDev<T>& M, const TaskDev<T>& D, const Tas
         task_fcross_add(ai, al, al + 3, T(1), W, W + 3);
       }
     }
-    const int nvj = kind_nv_dev(bd.kind);
-    if (nvj > 0) {
-      Pose<T> X;
-#pragma unroll
-      for (int k = 0; k < 9; ++k) X.R[k] = w.ld(row + k);
-#pragma unroll
-      for (int k = 0; k < 3; ++k) X.p[k] = w.ld(row + 9 + k);
-      Mot<T> vp, ap;
-#pragma unroll
-      for (int k = 0; k < 3; ++k) vp.w[k] = vp.l[k] = ap.w[k] = ap.l[k] = T(0);
-      if (want_vel && !(bd.flags & F_ROOT_CHILD)) {
-        const int prow = kTaskAdjRows * bd.parent;
-        ld_mot(io.s, prow + kTaV, vp);
-        ld_mot(io.s, prow + kTaA, ap);
-      }
-      T ft[6] = {T(0), T(0), T(0), T(0), T(0), T(0)};
-      for (int k = 0; k < nvj; ++k) {
-        Mot<T> S;
-        world_subspace(X, sub_comp(bd.kind, k), S);
-        if (io.vdb.valid()) io.vdb.st(bd.vrow + k, want_acc ? dot_mf(S, A, A + 3) : T(0));
-        if (io.vb.valid()) {
-          T x = T(0);
-          if (want_vel) {
-            Mot<T> vs, sdp;
-#pragma unroll
-            for (int c = 0; c < 3; ++c) { vs.w[c] = vi.w[c] + vp.w[c]; vs.l[c] = vi.l[c] + vp.l[c]; }
-            motion_cross(vs, S, sdp);
-            x = dot_mf(S, Tt, Tt + 3) + dot_mf(sdp, A, A + 3);
-          }
-          io.vb.st(bd.vrow + k, x);
-        }
-        if (want_q) {
-          T x = dot_mf(S, W, W + 3);
-          if (want_vel) {
-            Mot<T> pd, pdd, t1, t2;
-            motion_cross(vp, S, pd);
-            motion_cross(ap, S, t1);
-            motion_cross(vp, pd, t2);
-#pragma unroll
-            for (int c = 0; c < 3; ++c) { pdd.w[c] = t1.w[c] + t2.w[c]; pdd.l[c] = t1.l[c] + t2.l[c]; }
-            x += dot_mf(pd, Tt, Tt + 3) + dot_mf(pdd, A, A + 3);
-          }
-          if (io.qt.valid()) io.qt.st(bd.vrow + k, x);
-          // ft[k] = x with a warp-uniform k: a select chain keeps ft in registers
-#pragma unroll
-          for (int c = 0; c < 6; ++c) if (c == k) ft[c] = x;
-        }
-      }
-      if (io.qc.valid()) cfg_adjoint(bd, io.q, ft, io.qc);
-    }
+    task_joint_adjoint(bd, io.s, row, A, Tt, W, vi, want_vel, want_acc, want_q, io.q, io.qt, io.qc, io.vb, io.vdb);
     if (bd.flags & F_ROOT_CHILD) continue;
     const int prow = kTaskAdjRows * bd.parent;
 #pragma unroll
