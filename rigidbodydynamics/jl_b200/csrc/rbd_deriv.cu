@@ -233,6 +233,8 @@ int derivatives_t(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, 
   if (const char* e = std::getenv("RBD_DERIV_SCRATCH_MB")) budget_mb = std::max<int64_t>(1, std::atoll(e));
   const int64_t per_sample = (int64_t)D.rows * (int64_t)sizeof(T);
   int64_t C = std::min<int64_t>(B, std::max<int64_t>(kNT, (budget_mb << 20) / per_sample / kNT * kNT));
+  // deriv_pairs_kernel puts the sample groups of a chunk in grid.y (bodies fastest, see there), which holds at most 65535 blocks
+  C = std::min<int64_t>(C, (int64_t)65535 * kNT);
   const int64_t sld = (C + 31) / 32 * 32;
   StreamAlloc scratch_;
   if (cudaError_t e = scratch_.alloc((size_t)per_sample * sld, stream))

@@ -15,7 +15,10 @@ from tests import hostsim
 from tests.util import axis_aligned_tree, double_pendulum, oracle_dynamics_derivatives, rand_inputs, randmech, rel_err
 
 TOL64 = 1e-8          # parity with the oracle's DualN run in fp64
-TOL32 = 5e-3          # fp32: a 36 x 36 factorisation in single precision
+# fp32: a 36 x 36 factorisation in single precision.  Worst rel_err of the fp32 kernels against the fp64 run of the same code at the
+# fp32-rounded inputs, 512 columns, measured on an H100 80GB HBM3 (700 W): 7.3e-4 on Atlas at B = 2^17; up to 1.2e-3 on Atlas with
+# fixed tool bodies attached (tests/test_deriv_paths.py)
+TOL32 = 2e-3
 
 
 def _models():
@@ -72,12 +75,14 @@ def test_derivatives_hostsim_fp32():
 
 def test_specialised_solve_kernel_compiles_without_a_gpu(tmp_path, monkeypatch):
     """The generator of the model-specialised solve kernel (csrc/rbd_deriv_jit.cpp) on mechanisms of different shapes -- 51
-    coordinates with every joint type (one fp64 column per thread), Valkyrie, a serial chain -- through NVRTC (no GPU needed); the
-    cubins land in the cache directory."""
+    coordinates with every joint type (one fp64 column per thread), Valkyrie, a serial chain, 66 coordinates (the high word of the
+    relation masks) -- through NVRTC (no GPU needed); the cubins land in the cache directory."""
     from rigidbodydynamics.jl_b200 import _cabi
+    from tests.test_deriv_paths import legs_model
     monkeypatch.setenv("RBD_JIT_CACHE", str(tmp_path))
     rng = np.random.default_rng(0)
-    for mech in (randmech(6, shuffle=True), rbd.load_model("valkyrie", floating=True), rbd.rand_chain_mechanism(rng, [rbd.Revolute] * 30)):
+    for mech in (randmech(6, shuffle=True), rbd.load_model("valkyrie", floating=True), rbd.rand_chain_mechanism(rng, [rbd.Revolute] * 30),
+                 legs_model()):
         h = _cabi.ModelHandle(mech.flatten())
         for code in (_cabi.RBD_F64, _cabi.RBD_F32):
             try:
@@ -87,7 +92,7 @@ def test_specialised_solve_kernel_compiles_without_a_gpu(tmp_path, monkeypatch):
                     pytest.skip("NVRTC not available")
                 raise
         h.close()
-    assert len([f for f in os.listdir(tmp_path) if "deriv" in f]) == 6
+    assert len([f for f in os.listdir(tmp_path) if "deriv" in f]) == 8
     # a 40-joint serial chain has 820 stored mass-matrix entries: in fp64 that does not fit into shared memory next to nothing
     # else -> RBD_EUNSUPPORTED, and rbd_dynamics_derivatives serves the model with the table-driven kernels
     h = _cabi.ModelHandle(rbd.rand_chain_mechanism(rng, [rbd.Revolute] * 40).flatten())
