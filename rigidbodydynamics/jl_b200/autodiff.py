@@ -450,17 +450,8 @@ def integrate_vjp_(mechanism: Mechanism, q_traj: torch.Tensor, v_traj: torch.Ten
     [nv, B] and ``tau_bar`` (shape of ``torques``), to which the torque gradient is ADDED."""
     nsteps = q_traj.shape[0] - 1
     h, B, step, stage = _rollout_inputs(mechanism, "integrate_vjp_", q_traj[0], v_traj[0], torques, nsteps)
-    nq, nv = h.info.nq, h.info.nv
-    for t, shape, name in ((q_traj, (nsteps + 1, nq, B), "q_traj"), (v_traj, (nsteps + 1, nv, B), "v_traj"),
-                           (q_traj_bar, (nsteps + 1, nq, B), "q_traj_bar"), (v_traj_bar, (nsteps + 1, nv, B), "v_traj_bar"),
-                           (q0_bar_tan, (nv, B), "q0_bar_tan"), (q0_bar_cfg, (nq, B), "q0_bar_cfg"), (v0_bar, (nv, B), "v0_bar"),
-                           (tau_bar, None if torques is None else tuple(torques.shape), "tau_bar")):
-        if t is None:
-            continue
-        if t.dtype != q_traj.dtype or t.device != q_traj.device or not t.is_contiguous():
-            raise TypeError(f"integrate_vjp_: {name} must be contiguous, with the dtype and device of q_traj")
-        if shape is None or tuple(t.shape) != shape:
-            raise DimensionMismatch(f"integrate_vjp_: {name} has wrong size: expected {shape}, got {tuple(t.shape)}")
+    _check_blocks("integrate_vjp_", q_traj, _rollout_vjp_rows("integrate_vjp_", h, B, torques, None, q_traj, v_traj, None, q_traj_bar,
+                                                              v_traj_bar, None, q0_bar_tan, q0_bar_cfg, v0_bar, None, tau_bar))
     _cabi.check(_cabi.load_library().rbd_integrate_vjp(h.ptr, _DT[q_traj.dtype], B, _ptr(q_traj), _ptr(v_traj), _ptr(torques), step,
                                                        stage, float(dt), nsteps, _ptr(q_traj_bar), _ptr(v_traj_bar), _ptr(q0_bar_tan),
                                                        _ptr(q0_bar_cfg), _ptr(v0_bar), _ptr(tau_bar), _stream(q_traj)))
@@ -578,6 +569,24 @@ def _check_blocks(what: str, like: torch.Tensor, items):
             raise DimensionMismatch(f"{what}: {name} has wrong size: expected {shape}, got {tuple(t.shape)}")
 
 
+def _rollout_vjp_rows(what, h, B, torques, contact, q_traj, v_traj, s_traj, q_traj_bar, v_traj_bar, s_traj_bar, q0_bar_tan, q0_bar_cfg,
+                      v0_bar, s0_bar, tau_bar):
+    """The (tensor, shape, name) rows of ``_check_blocks`` that every rollout VJP shares: the trajectories, their adjoints and the
+    state and torque outputs.  The contact state's arrays need ``contact``, and ``s_traj`` is needed with contact pairs."""
+    nsteps = q_traj.shape[0] - 1
+    nq, nv = h.info.nq, h.info.nv
+    ns = 0 if contact is None else contact.nstates
+    if contact is None and (s_traj is not None or s_traj_bar is not None or s0_bar is not None):
+        raise ValueError(f"{what}: s_traj, s_traj_bar and s0_bar need contact")
+    if ns > 0 and s_traj is None:
+        raise ValueError(f"{what}: s_traj is needed with contact pairs")
+    return [(q_traj, (nsteps + 1, nq, B), "q_traj"), (v_traj, (nsteps + 1, nv, B), "v_traj"), (s_traj, (nsteps + 1, ns, B), "s_traj"),
+            (q_traj_bar, (nsteps + 1, nq, B), "q_traj_bar"), (v_traj_bar, (nsteps + 1, nv, B), "v_traj_bar"),
+            (s_traj_bar, (nsteps + 1, ns, B), "s_traj_bar"), (q0_bar_tan, (nv, B), "q0_bar_tan"), (q0_bar_cfg, (nq, B), "q0_bar_cfg"),
+            (v0_bar, (nv, B), "v0_bar"), (s0_bar, (ns, B), "s0_bar"),
+            (tau_bar, None if torques is None else tuple(torques.shape), "tau_bar")]
+
+
 def integrate_contact_vjp_(mechanism: Mechanism, q_traj: torch.Tensor, v_traj: torch.Tensor, s_traj: torch.Tensor,
                            torques: Optional[torch.Tensor] = None, *, contact, dt: float, q_traj_bar: Optional[torch.Tensor] = None,
                            v_traj_bar: Optional[torch.Tensor] = None, s_traj_bar: Optional[torch.Tensor] = None,
@@ -590,13 +599,9 @@ def integrate_contact_vjp_(mechanism: Mechanism, q_traj: torch.Tensor, v_traj: t
     B]; ``tau_bar`` (shape of ``torques``) is ADDED TO."""
     nsteps = q_traj.shape[0] - 1
     h, B, step, stage = _rollout_inputs(mechanism, "integrate_contact_vjp_", q_traj[0], v_traj[0], torques, nsteps)
-    nq, nv, ns = h.info.nq, h.info.nv, contact.nstates
-    _check_blocks("integrate_contact_vjp_", q_traj, (
-        (q_traj, (nsteps + 1, nq, B), "q_traj"), (v_traj, (nsteps + 1, nv, B), "v_traj"), (s_traj, (nsteps + 1, ns, B), "s_traj"),
-        (q_traj_bar, (nsteps + 1, nq, B), "q_traj_bar"), (v_traj_bar, (nsteps + 1, nv, B), "v_traj_bar"),
-        (s_traj_bar, (nsteps + 1, ns, B), "s_traj_bar"), (q0_bar_tan, (nv, B), "q0_bar_tan"), (q0_bar_cfg, (nq, B), "q0_bar_cfg"),
-        (v0_bar, (nv, B), "v0_bar"), (s0_bar, (ns, B), "s0_bar"),
-        (tau_bar, None if torques is None else tuple(torques.shape), "tau_bar")))
+    _check_blocks("integrate_contact_vjp_", q_traj, _rollout_vjp_rows(
+        "integrate_contact_vjp_", h, B, torques, contact, q_traj, v_traj, s_traj, q_traj_bar, v_traj_bar, s_traj_bar, q0_bar_tan,
+        q0_bar_cfg, v0_bar, s0_bar, tau_bar))
     _contact_vjp_call(h, q_traj, v_traj, s_traj, torques, step, stage, contact, dt, nsteps, q_traj_bar, v_traj_bar, s_traj_bar,
                       q0_bar_tan, q0_bar_cfg, v0_bar, s0_bar, tau_bar)
 
@@ -749,25 +754,17 @@ def integrate_pd_vjp_(mechanism: Mechanism, q_traj: torch.Tensor, v_traj: torch.
     what = "integrate_pd_vjp_"
     nsteps = q_traj.shape[0] - 1
     h, B, step, stage = _rollout_inputs(mechanism, what, q_traj[0], v_traj[0], torques, nsteps)
-    nq, nv = h.info.nq, h.info.nv
-    ns = 0 if contact is None else contact.nstates
+    nv = h.info.nv
     pd, keep = _pd_struct(controller, h, q_traj[0], nsteps, what)
     shape = lambda t: None if t is None else tuple(t.shape)      # noqa: E731
     for bar, ref, name in ((v_ref_bar, controller.v_ref, "v_ref"), (vd_ref_bar, controller.vd_ref, "vd_ref")):
         if bar is not None and ref is None:
             raise ValueError(f"{what}: {name}_bar needs the controller's {name}")
-    if contact is None and (s_traj is not None or s_traj_bar is not None or s0_bar is not None):
-        raise ValueError(f"{what}: s_traj, s_traj_bar and s0_bar need contact")
-    _check_blocks(what, q_traj, (
-        (q_traj, (nsteps + 1, nq, B), "q_traj"), (v_traj, (nsteps + 1, nv, B), "v_traj"),
-        (s_traj, (nsteps + 1, ns, B), "s_traj"), (q_traj_bar, (nsteps + 1, nq, B), "q_traj_bar"),
-        (v_traj_bar, (nsteps + 1, nv, B), "v_traj_bar"), (s_traj_bar, (nsteps + 1, ns, B), "s_traj_bar"),
-        (q0_bar_tan, (nv, B), "q0_bar_tan"), (q0_bar_cfg, (nq, B), "q0_bar_cfg"), (v0_bar, (nv, B), "v0_bar"), (s0_bar, (ns, B), "s0_bar"),
-        (tau_bar, shape(torques), "tau_bar"), (kp_bar, (nv, B), "kp_bar"), (kd_bar, (nv, B), "kd_bar"),
-        (q_ref_bar, shape(controller.q_ref), "q_ref_bar"), (v_ref_bar, shape(controller.v_ref), "v_ref_bar"),
-        (vd_ref_bar, shape(controller.vd_ref), "vd_ref_bar")))
-    if contact is not None and ns > 0 and s_traj is None:
-        raise ValueError(f"{what}: s_traj is needed with contact pairs")
+    items = _rollout_vjp_rows(what, h, B, torques, contact, q_traj, v_traj, s_traj, q_traj_bar, v_traj_bar, s_traj_bar, q0_bar_tan,
+                              q0_bar_cfg, v0_bar, s0_bar, tau_bar)
+    _check_blocks(what, q_traj, items + [
+        (kp_bar, (nv, B), "kp_bar"), (kd_bar, (nv, B), "kd_bar"), (q_ref_bar, shape(controller.q_ref), "q_ref_bar"),
+        (v_ref_bar, shape(controller.v_ref), "v_ref_bar"), (vd_ref_bar, shape(controller.vd_ref), "vd_ref_bar")])
     _pd_vjp_call(h, q_traj, v_traj, s_traj, torques, step, stage, pd, contact, dt, nsteps, q_traj_bar, v_traj_bar, s_traj_bar,
                  q0_bar_tan, q0_bar_cfg, v0_bar, s0_bar, tau_bar, (kp_bar, kd_bar, q_ref_bar, v_ref_bar, vd_ref_bar))
     del keep
@@ -936,8 +933,7 @@ def integrate_task_pd_vjp_(mechanism: Mechanism, q_traj: torch.Tensor, v_traj: t
     what = "integrate_task_pd_vjp_"
     nsteps = q_traj.shape[0] - 1
     h, B, step, stage = _rollout_inputs(mechanism, what, q_traj[0], v_traj[0], torques, nsteps)
-    nq, nv = h.info.nq, h.info.nv
-    ns = 0 if contact is None else contact.nstates
+    nv = h.info.nv
     ctl, keep = _task_struct(controller, mechanism, h, q_traj[0], nsteps, what)
     R, _ = controller.rows()
     shape = lambda t: None if t is None else tuple(t.shape)      # noqa: E731
@@ -947,14 +943,10 @@ def integrate_task_pd_vjp_(mechanism: Mechanism, q_traj: torch.Tensor, v_traj: t
     jb = tuple(joint_bars) if joint_bars is not None else (None,) * 5
     if any(t is not None for t in jb) and j is None:
         raise ValueError(f"{what}: joint_bars need the controller's joint term")
-    if contact is None and (s_traj is not None or s_traj_bar is not None or s0_bar is not None):
-        raise ValueError(f"{what}: s_traj, s_traj_bar and s0_bar need contact")
-    items = [(q_traj, (nsteps + 1, nq, B), "q_traj"), (v_traj, (nsteps + 1, nv, B), "v_traj"),
-             (s_traj, (nsteps + 1, ns, B), "s_traj"), (q_traj_bar, (nsteps + 1, nq, B), "q_traj_bar"),
-             (v_traj_bar, (nsteps + 1, nv, B), "v_traj_bar"), (s_traj_bar, (nsteps + 1, ns, B), "s_traj_bar"),
-             (q0_bar_tan, (nv, B), "q0_bar_tan"), (q0_bar_cfg, (nq, B), "q0_bar_cfg"), (v0_bar, (nv, B), "v0_bar"), (s0_bar, (ns, B), "s0_bar"),
-             (tau_bar, shape(torques), "tau_bar"), (kp_bar, (R, B), "kp_bar"), (kd_bar, (R, B), "kd_bar"),
-             (x_ref_bar, shape(controller.x_ref), "x_ref_bar"), (xd_ref_bar, shape(controller.xd_ref), "xd_ref_bar")]
+    items = _rollout_vjp_rows(what, h, B, torques, contact, q_traj, v_traj, s_traj, q_traj_bar, v_traj_bar, s_traj_bar, q0_bar_tan,
+                              q0_bar_cfg, v0_bar, s0_bar, tau_bar)
+    items += [(kp_bar, (R, B), "kp_bar"), (kd_bar, (R, B), "kd_bar"), (x_ref_bar, shape(controller.x_ref), "x_ref_bar"),
+              (xd_ref_bar, shape(controller.xd_ref), "xd_ref_bar")]
     if j is not None:
         for bar, ref, name in ((jb[3], j.v_ref, "v_ref"), (jb[4], j.vd_ref, "vd_ref")):
             if bar is not None and ref is None:
@@ -962,8 +954,6 @@ def integrate_task_pd_vjp_(mechanism: Mechanism, q_traj: torch.Tensor, v_traj: t
         items += [(jb[0], (nv, B), "joint kp_bar"), (jb[1], (nv, B), "joint kd_bar"), (jb[2], shape(j.q_ref), "joint q_ref_bar"),
                   (jb[3], shape(j.v_ref), "joint v_ref_bar"), (jb[4], shape(j.vd_ref), "joint vd_ref_bar")]
     _check_blocks(what, q_traj, items)
-    if contact is not None and ns > 0 and s_traj is None:
-        raise ValueError(f"{what}: s_traj is needed with contact pairs")
     _task_vjp_call(h, q_traj, v_traj, s_traj, torques, step, stage, ctl, contact, dt, nsteps, q_traj_bar, v_traj_bar, s_traj_bar,
                    q0_bar_tan, q0_bar_cfg, v0_bar, s0_bar, tau_bar, (kp_bar, kd_bar, x_ref_bar, xd_ref_bar), jb)
     del keep

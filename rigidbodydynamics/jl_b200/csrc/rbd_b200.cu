@@ -1612,6 +1612,7 @@ int task_pd_torques_t(const rbd_model* model, int64_t B, int64_t ld, const void*
 namespace rbd {
 int api_check(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld) { return check_common(model, dtype, B, ld); }
 int api_check_contact(const rbd_model* model, const rbd_contact_desc* contact, const char* fn) { return check_contact(model, contact, fn); }
+int api_check_pd(const char* fn, const rbd_model* model, int64_t ld, const rbd_pd_desc* pd) { return check_pd(fn, model, ld, pd); }
 int api_check_task_ctrl(const char* fn, const rbd_model* model, int64_t ld, const rbd_task_pd_desc* ctrl) {
   return check_task_ctrl(fn, model, ld, ctrl);
 }

@@ -169,8 +169,7 @@ struct Rollout {
   const rbd_pd_desc* pd = nullptr;             // feedback evaluated at every stage
   const void* pd_bounds = nullptr;             // pd's effort bounds already on the device ([2 nv]: lo, then hi), or NULL: integrate
                                                // copies them from the host arrays of pd (rbd_integrate_pd_vjp's recompute passes its copy)
-  const rbd_task_pd_desc* task = nullptr;      // task-space feedback at every stage (pd NULL; its joint term takes pd's place);
-                                               // never set together with `stages`
+  const rbd_task_pd_desc* task = nullptr;      // task-space feedback at every stage (pd NULL; its joint term takes pd's place)
 };
 // The recompute of one step (nsteps = 1, ld = B) keeps its four stages in stage_rows(nq, nv) x B rows of `stages` (4 ns more with
 // contact, for the ṡ_i) and skips the finishing step.  With a controller (pd) pd_stage_rows(nv, computed_torque) x B more follow:
@@ -207,6 +206,8 @@ int inverse_dynamics_vjp_dense(const rbd_model* model, int32_t dtype, int64_t B,
                                const void* tau_bar, void* q_bar_cfg, void* v_bar, void* vd_bar, cudaStream_t stream);
 // The model limits of rbd_dynamics_vjp / rbd_inverse_dynamics_vjp (those of rbd_dynamics_derivatives): RBD_OK or RBD_EUNSUPPORTED
 int check_vjp_limits(const HostModel& hm, const char* who);
+// rbd_b200.cu's controller checks of rbd_integrate_pd (pd not NULL), leading dimension ld
+int api_check_pd(const char* fn, const rbd_model* model, int64_t ld, const rbd_pd_desc* pd);
 // rbd_b200.cu's controller checks of rbd_integrate_task_pd (the joint term's JointPD checks, then check_task_pd), leading dimension ld
 int api_check_task_ctrl(const char* fn, const rbd_model* model, int64_t ld, const rbd_task_pd_desc* ctrl);
 // rbd_task_pd_torques on dense [rows x B] arrays (arguments checked by the caller): tau_out the applied torques; in computed-torque

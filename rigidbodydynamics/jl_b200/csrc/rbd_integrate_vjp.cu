@@ -16,6 +16,7 @@
 #include <memory>
 #include <optional>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../../include/rbd_b200.h"
@@ -281,38 +282,92 @@ template <class T> struct TaskPdVjpPlan {
   }
 };
 
-// the contact part of a rollout adjoint: the descriptor in device form, the recorded contact states and their adjoints
-template <class T> struct ContactVjp {
-  const rbd_contact_desc* cd;
-  const ContactDev<T>* C;
-  int64_t ns;
-  const T* s_traj; const T* stb;
-  T* s0b;
+// One request to the rollout adjoint, in the form the C entry points receive it (include/rbd_b200.h): the recorded trajectories
+// [(nsteps + 1) x rows x B] and their adjoints (NULL: zero), the torques as Rollout has them, the outputs (each NULL: not wanted),
+// and the optional contact descriptor and controller, with the adjoints of the controller's arrays (NULL: none wanted).
+struct RolloutVjp {
+  const void *q_traj, *v_traj, *s_traj;
+  const void* tau;
+  int64_t tau_step_stride, tau_stage_stride;
+  double dt;
+  int nsteps;
+  const void *q_traj_bar, *v_traj_bar, *s_traj_bar;
+  void *q0_bar_tan, *q0_bar_cfg, *v0_bar, *s0_bar, *tau_bar;
+  const rbd_contact_desc* contact = nullptr;
+  const rbd_pd_desc* pd = nullptr;
+  const rbd_pd_bar* pd_bar = nullptr;
+  const rbd_task_pd_desc* task = nullptr;      // pd NULL: the joint term, if any, is task->joint
+  const rbd_task_pd_bar* task_bar = nullptr;
 };
 
-// the controller of rbd_integrate_pd_vjp and the adjoints of its arrays (each NULL = not wanted)
-struct PdVjp {
-  const rbd_pd_desc* pd;
-  rbd_pd_bar bar;
-};
-// the controller of rbd_integrate_task_pd_vjp and the adjoints of its arrays (each NULL = not wanted)
-struct TaskPdVjp {
-  const rbd_task_pd_desc* ctrl;
-  rbd_task_pd_bar bar;
-};
+// the effort bounds [2 nv] (lo, then hi) in T, copied from the host arrays (pageable memory, as integrate_t copies them) to dev
+template <class T>
+int upload_bounds(T* dev, const double* lo, const double* hi, int64_t nv, cudaStream_t stream) {
+  std::vector<T> h(2 * nv);
+  for (int64_t k = 0; k < nv; ++k) { h[k] = (T)lo[k]; h[nv + k] = (T)hi[k]; }
+  RBD_CUDA_TRY(cudaMemcpyAsync(dev, h.data(), 2 * nv * sizeof(T), cudaMemcpyHostToDevice, stream));
+  return RBD_OK;
+}
 
 template <class T>
-int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q_traj, const T* v_traj, const T* tau, int64_t step_stride,
-                    int64_t stage_stride, double dt, int nsteps, const T* qtb, const T* vtb, T* q0t, T* q0c, T* v0b, T* taub,
-                    cudaStream_t stream, const ContactVjp<T>* contact = nullptr, const PdVjp* ctl = nullptr,
-                    const TaskPdVjp* tctl = nullptr) {
+int launch_pd_mask(const PdMaskArgs<T>& ma, int sms, cudaStream_t stream) {
+  pd_mask_kernel<T><<<(int)std::min<int64_t>((ma.nv * ma.B + 255) / 256, (int64_t)sms * 8), 256, 0, stream>>>(ma);
+  return api_launched();
+}
+
+// The JointPD law's adjoint at step s: the references and their adjoints of step s, as integrate_t reads the references.  The
+// caller adds the mask and, in computed-torque mode, the inverse-dynamics VJP's rows.
+template <class T>
+PdAdjArgs<T> pd_adj_step(const rbd_pd_desc& pd, const rbd_pd_bar* bar, int64_t s) {
+  const size_t qo = (size_t)s * pd.q_ref_step_stride, vo = (size_t)s * pd.v_ref_step_stride;
+  const rbd_pd_bar cb = bar ? *bar : rbd_pd_bar{};
+  PdAdjArgs<T> c{};
+  c.qref = (const T*)pd.q_ref + qo;
+  c.vref = pd.v_ref ? (const T*)pd.v_ref + vo : nullptr;
+  c.kp = (const T*)pd.kp; c.kd = (const T*)pd.kd; c.g_ld = pd.gain_ld;
+  c.kpb = (T*)cb.kp; c.kdb = (T*)cb.kd;
+  c.qrefb = cb.q_ref ? (T*)cb.q_ref + qo : nullptr;
+  c.vrefb = cb.v_ref ? (T*)cb.v_ref + vo : nullptr;
+  c.vdrefb = cb.vd_ref ? (T*)cb.vd_ref + vo : nullptr;
+  return c;
+}
+
+// ... and the task law's: the task references, gains and their adjoints of step s.  The caller adds the state, the seed, where
+// q̄ / v̄ go, and the joint term.
+template <class T>
+TaskPdVjpArgs<T> task_vjp_step(const rbd_task_pd_desc& c, const rbd_task_pd_bar* bar, int64_t s) {
+  const size_t xo = (size_t)s * c.x_ref_step_stride, xdo = (size_t)s * c.xd_ref_step_stride;
+  const rbd_task_pd_bar cb = bar ? *bar : rbd_task_pd_bar{};
+  TaskPdVjpArgs<T> ta{};
+  ta.xref = (const T*)c.x_ref + xo; ta.xdref = c.xd_ref ? (const T*)c.xd_ref + xdo : nullptr;
+  ta.kp = (const T*)c.kp; ta.kd = (const T*)c.kd; ta.gain_ld = c.gain_ld;
+  ta.kpb = (T*)cb.kp; ta.kdb = (T*)cb.kd;
+  ta.xrefb = cb.x_ref ? (T*)cb.x_ref + xo : nullptr; ta.xdrefb = cb.xd_ref ? (T*)cb.xd_ref + xdo : nullptr;
+  return ta;
+}
+
+template <class T>
+int integrate_vjp_t(const rbd_model* model, int64_t B, const RolloutVjp& r, cudaStream_t stream) {
+  const int32_t dtype = std::is_same<T, float>::value ? RBD_F32 : RBD_F64;
   const HostModel& hm = model->hm;
   const ModelDev<T>& M = dev_model<T>(hm);
-  const int64_t nq = hm.nq, nv = hm.nv, ns = contact ? contact->ns : 0;
+  const T *q_traj = (const T*)r.q_traj, *v_traj = (const T*)r.v_traj, *s_traj = (const T*)r.s_traj, *tau = (const T*)r.tau;
+  const T *qtb = (const T*)r.q_traj_bar, *vtb = (const T*)r.v_traj_bar, *stb = (const T*)r.s_traj_bar;
+  T *q0t = (T*)r.q0_bar_tan, *q0c = (T*)r.q0_bar_cfg, *v0b = (T*)r.v0_bar, *s0b = (T*)r.s0_bar, *taub = (T*)r.tau_bar;
+  const int64_t step_stride = r.tau_step_stride, stage_stride = r.tau_stage_stride;
+  const double dt = r.dt;
+  const int nsteps = r.nsteps;
+  const rbd_contact_desc* cd = r.contact;
+  std::unique_ptr<ContactDev<T>> C;
+  if (cd) {
+    C.reset(new ContactDev<T>());
+    build_contact_dev<T>(hm.nb, hm.pos.data(), hm.alignT.data(), *cd, *C);
+  }
+  const int64_t nq = hm.nq, nv = hm.nv, ns = cd ? (int64_t)3 * cd->npoints * cd->nhalfspaces : 0;
   // task-space control: its joint term, if any, takes the JointPD controller's place in the phase kernels
-  const rbd_task_pd_desc* task = tctl ? tctl->ctrl : nullptr;
-  const rbd_pd_desc* pd = task ? task->joint : (ctl ? ctl->pd : nullptr);
-  const rbd_pd_bar* pd_bar = task ? task->joint ? tctl->bar.joint : nullptr : (ctl ? &ctl->bar : nullptr);
+  const rbd_task_pd_desc* task = r.task;
+  const rbd_pd_desc* pd = task ? task->joint : r.pd;
+  const rbd_pd_bar* pd_bar = task ? (task->joint && r.task_bar ? r.task_bar->joint : nullptr) : r.pd_bar;
   const bool closed = pd || task;
   const bool ct = task ? task->mode == RBD_PD_COMPUTED_TORQUE : pd && pd->mode == RBD_PD_COMPUTED_TORQUE;
   const double* effort_lo = task ? task->effort_lo : (pd ? pd->effort_lo : nullptr);
@@ -343,10 +398,8 @@ int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q
   const T* lo = nullptr;
   const T* hi = nullptr;
   if (bounds) {
-    std::vector<T> h(2 * nv);
-    for (int64_t k = 0; k < nv; ++k) { h[k] = (T)effort_lo[k]; h[nv + k] = (T)effort_hi[k]; }
     T* dev = (T*)work.p + (size_t)rows * B;
-    RBD_CUDA_TRY(cudaMemcpyAsync(dev, h.data(), 2 * nv * sizeof(T), cudaMemcpyHostToDevice, stream));
+    if (int rc = upload_bounds(dev, effort_lo, effort_hi, nv, stream)) return rc;
     lo = dev; hi = dev + nv;
   }
   const T* tau_applied[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -362,13 +415,13 @@ int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q
   if (vtb) RBD_CUDA_TRY(cudaMemcpyAsync(vb, vtb + (size_t)nsteps * nv * B, vbytes, cudaMemcpyDeviceToDevice, stream));
   else RBD_CUDA_TRY(cudaMemsetAsync(vb, 0, vbytes, stream));
   const size_t sbytes = (size_t)ns * B * sizeof(T);
-  if (ns && contact->stb) RBD_CUDA_TRY(cudaMemcpyAsync(sb1, contact->stb + (size_t)nsteps * ns * B, sbytes, cudaMemcpyDeviceToDevice, stream));
+  if (ns && stb) RBD_CUDA_TRY(cudaMemcpyAsync(sb1, stb + (size_t)nsteps * ns * B, sbytes, cudaMemcpyDeviceToDevice, stream));
   else if (ns) RBD_CUDA_TRY(cudaMemsetAsync(sb1, 0, sbytes, stream));
   // the contact stage adjoint: one plan (grid, workspace and the solve's zero) for the whole call
   ContactVjpArgs<T> cva{};
   std::optional<LaunchPlan> cplan;
   ModelDev<T> Mz;
-  if (contact && nsteps > 0) {
+  if (cd && nsteps > 0) {
     Mz = M;
     for (int k = 0; k < 3; ++k) { cva.g[k] = M.g[k]; Mz.g[k] = T(0); }
     const size_t row_bytes = (size_t)contact_vjp_rows(hm.nb, hm.nv) * sizeof(T);
@@ -412,11 +465,11 @@ int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q
   for (int s = nsteps - 1; s >= 0; --s) {
     const T* q0 = q_traj + (size_t)s * nq * B;
     const T* v0 = v_traj + (size_t)s * nv * B;
-    const T* s0 = contact ? contact->s_traj + (size_t)s * ns * B : nullptr;
-    Rollout r{const_cast<T*>(q0), const_cast<T*>(v0), const_cast<T*>(s0), tau ? tau + s * step_stride : nullptr, step_stride,
-              stage_stride, dt, 1};
-    r.stages = stages;
-    r.contact = contact ? contact->cd : nullptr;
+    const T* s0 = cd ? s_traj + (size_t)s * ns * B : nullptr;
+    Rollout rec{const_cast<T*>(q0), const_cast<T*>(v0), const_cast<T*>(s0), tau ? tau + s * step_stride : nullptr, step_stride,
+                stage_stride, dt, 1};
+    rec.stages = stages;
+    rec.contact = cd;
     rbd_pd_desc pds{};      // the recompute is a one-step rollout: the controller's references start at step s
     rbd_task_pd_desc tds{};
     if (pd) {
@@ -425,35 +478,27 @@ int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q
       pds.q_ref = (const T*)pd->q_ref + (size_t)s * pd->q_ref_step_stride;
       pds.v_ref = pd->v_ref ? (const T*)pd->v_ref + vo : nullptr;
       pds.vd_ref = pd->vd_ref ? (const T*)pd->vd_ref + vo : nullptr;
-      r.pd = &pds;
-      r.pd_bounds = lo;      // the bounds copied above: one host copy per call
+      rec.pd = &pds;
+      rec.pd_bounds = lo;      // the bounds copied above: one host copy per call
     }
     if (task) {
       tds = *task;
       tds.x_ref = (const T*)task->x_ref + (size_t)s * task->x_ref_step_stride;
       tds.xd_ref = task->xd_ref ? (const T*)task->xd_ref + (size_t)s * task->xd_ref_step_stride : nullptr;
       tds.joint = pd ? &pds : nullptr;
-      r.task = &tds;
-      r.pd = nullptr;
-      r.pd_bounds = lo;
+      rec.task = &tds;
+      rec.pd = nullptr;
+      rec.pd_bounds = lo;
     }
-    if (int rc = integrate(model, dtype, B, B, r, stream)) return rc;
+    if (int rc = integrate(model, dtype, B, B, rec, stream)) return rc;
     a.q0 = q0;
     a.qtb = qtb ? qtb + (size_t)s * nq * B : nullptr;
     a.vtb = vtb ? vtb + (size_t)s * nv * B : nullptr;
     PdAdjArgs<T> c{};
-    if (pd) {     // the references and their adjoints of step s, as integrate_t reads the references
-      const size_t qo = (size_t)s * pd->q_ref_step_stride, vo = (size_t)s * pd->v_ref_step_stride;
-      const rbd_pd_bar cb = pd_bar ? *pd_bar : rbd_pd_bar{};
-      c.qref = (const T*)pd->q_ref + qo;
-      c.vref = pd->v_ref ? (const T*)pd->v_ref + vo : nullptr;
-      c.kp = (const T*)pd->kp; c.kd = (const T*)pd->kd; c.g_ld = pd->gain_ld;
+    if (pd) {
+      c = pd_adj_step<T>(*pd, pd_bar, s);
       c.lo = lo; c.hi = hi;
       if (ct) { c.idq = idq; c.idv = idv; c.idvd = idvd; }
-      c.kpb = (T*)cb.kp; c.kdb = (T*)cb.kd;
-      c.qrefb = cb.q_ref ? (T*)cb.q_ref + qo : nullptr;
-      c.vrefb = cb.v_ref ? (T*)cb.v_ref + vo : nullptr;
-      c.vdrefb = cb.vd_ref ? (T*)cb.vd_ref + vo : nullptr;
     }
     for (int g = 4; g >= 0; --g) {
       a.g = g; a.l = g == 4 ? 3 : g - 1;
@@ -477,42 +522,26 @@ int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q
         }
         continue;
       }
-      if (contact) {
-        const int l = a.l;
+      const int l = a.l;
+      if (cd) {
         const T* sd = stages + (size_t)stage_rows(nq, nv) * B;
         cva.q = a.qs[l]; cva.v = a.vs[l]; cva.vd = vd[l];
         cva.s0 = s0; cva.sdp = l ? sd + (size_t)(l - 1) * ns * B : nullptr;
-        cva.stb = (l == 0 && contact->stb) ? contact->stb + (size_t)s * ns * B : nullptr;
+        cva.stb = (l == 0 && stb) ? stb + (size_t)s * ns * B : nullptr;
         cva.wa = a.wa[l]; cva.wdb = (T)dt * a.wb[l]; cva.l = l;
-        contact_vjp_kernel<T><<<cplan->grid, cplan->block, cplan->smem, stream>>>(Mz, *contact->C, cva);
+        contact_vjp_kernel<T><<<cplan->grid, cplan->block, cplan->smem, stream>>>(Mz, *C, cva);
         if (int rc = api_launched(&*cplan)) return rc;
-      } else if (int rc = dynamics_vjp_dense(model, dtype, B, a.qs[a.l], a.vs[a.l], vd[a.l], vdb, qcb, vvb, want_tb ? tb : nullptr, stream)) {
+      } else if (int rc = dynamics_vjp_dense(model, dtype, B, a.qs[l], a.vs[l], vd[l], vdb, qcb, vvb, want_tb ? tb : nullptr, stream)) {
         return rc;
       }
-      if (ct) {     // m = τ̄ masked by the applied torque, then the inverse-dynamics VJP at (q_s, v_s, v̇_des) seeded with m
-        const int l = a.l;
-        if (bounds) {
-          const PdMaskArgs<T> ma{tb, tau_applied[l], lo, hi, nv, B};
-          pd_mask_kernel<T><<<(int)std::min<int64_t>((nv * B + 255) / 256, (int64_t)p.sms * 8), 256, 0, stream>>>(ma);
-          if (int rc = api_launched()) return rc;
-        }
+      // computed-torque mode and task-space control: m = τ̄ masked by the applied torque, the seed of the VJPs below
+      if (bounds && (ct || task))
+        if (int rc = launch_pd_mask(PdMaskArgs<T>{tb, tau_applied[l], lo, hi, nv, B}, p.sms, stream)) return rc;
+      if (ct)     // the inverse-dynamics VJP at (q_s, v_s, v̇_des) seeded with m
         if (int rc = inverse_dynamics_vjp_dense(model, dtype, B, a.qs[l], a.vs[l], vd_des[l], tb, idq, idv, idvd, stream)) return rc;
-      }
       if (task) {     // the task law's adjoint at (q_s, v_s) with the references of step s, seeded with m (torque) or v̇̄_des
-        const int l = a.l;
-        if (bounds && !ct) {
-          const PdMaskArgs<T> ma{tb, tau_applied[l], lo, hi, nv, B};
-          pd_mask_kernel<T><<<(int)std::min<int64_t>((nv * B + 255) / 256, (int64_t)p.sms * 8), 256, 0, stream>>>(ma);
-          if (int rc = api_launched()) return rc;
-        }
-        const rbd_task_pd_bar& tb_ = tctl->bar;
-        const size_t xo = (size_t)s * task->x_ref_step_stride, xdo = (size_t)s * task->xd_ref_step_stride;
-        TaskPdVjpArgs<T> ta{};
+        TaskPdVjpArgs<T> ta = task_vjp_step<T>(*task, r.task_bar, s);
         ta.q = a.qs[l]; ta.v = a.vs[l]; ta.w = ct ? idvd : tb;
-        ta.xref = (const T*)task->x_ref + xo; ta.xdref = task->xd_ref ? (const T*)task->xd_ref + xdo : nullptr;
-        ta.kp = (const T*)task->kp; ta.kd = (const T*)task->kd; ta.gain_ld = task->gain_ld;
-        ta.kpb = (T*)tb_.kp; ta.kdb = (T*)tb_.kd;
-        ta.xrefb = tb_.x_ref ? (T*)tb_.x_ref + xo : nullptr; ta.xdrefb = tb_.xd_ref ? (T*)tb_.xd_ref + xdo : nullptr;
         // where the next phase kernel reads q̄ / v̄: the PD phase kernels add the inverse-dynamics VJP's rows themselves, the
         // open-loop ones do not, so without a joint term those are folded into the dynamics VJP's rows here
         ta.qacc = ct && pd ? idq : qcb; ta.vacc = ct && pd ? idv : vvb;
@@ -527,57 +556,8 @@ int integrate_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const T* q
     if (int rc = api_launched()) return rc;
   }
   if (v0b) RBD_CUDA_TRY(cudaMemcpyAsync(v0b, vb, vbytes, cudaMemcpyDeviceToDevice, stream));
-  if (ns && contact->s0b) RBD_CUDA_TRY(cudaMemcpyAsync(contact->s0b, sb1, sbytes, cudaMemcpyDeviceToDevice, stream));
+  if (ns && s0b) RBD_CUDA_TRY(cudaMemcpyAsync(s0b, sb1, sbytes, cudaMemcpyDeviceToDevice, stream));
   return RBD_OK;
-}
-
-template <class T>
-int integrate_pd_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const void* q_traj, const void* v_traj, const void* s_traj,
-                       const void* tau, int64_t step_stride, int64_t stage_stride, const rbd_pd_desc& pd, const rbd_contact_desc* cd,
-                       double dt, int nsteps, const void* qtb, const void* vtb, const void* stb, void* q0t, void* q0c, void* v0b,
-                       void* s0b, void* taub, const rbd_pd_bar* bar, cudaStream_t stream) {
-  const HostModel& hm = model->hm;
-  const PdVjp ctl{&pd, bar ? *bar : rbd_pd_bar{}};
-  std::unique_ptr<ContactDev<T>> C;
-  std::optional<ContactVjp<T>> cv;
-  if (cd) {
-    C.reset(new ContactDev<T>());
-    build_contact_dev<T>(hm.nb, hm.pos.data(), hm.alignT.data(), *cd, *C);
-    cv.emplace(ContactVjp<T>{cd, C.get(), (int64_t)3 * cd->npoints * cd->nhalfspaces, (const T*)s_traj, (const T*)stb, (T*)s0b});
-  }
-  return integrate_vjp_t<T>(model, dtype, B, (const T*)q_traj, (const T*)v_traj, (const T*)tau, step_stride, stage_stride, dt, nsteps,
-                            (const T*)qtb, (const T*)vtb, (T*)q0t, (T*)q0c, (T*)v0b, (T*)taub, stream, cv ? &*cv : nullptr, &ctl);
-}
-
-template <class T>
-int integrate_contact_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const void* q_traj, const void* v_traj, const void* s_traj,
-                            const void* tau, int64_t step_stride, int64_t stage_stride, const rbd_contact_desc& cd, double dt, int nsteps,
-                            const void* qtb, const void* vtb, const void* stb, void* q0t, void* q0c, void* v0b, void* s0b, void* taub,
-                            cudaStream_t stream) {
-  const HostModel& hm = model->hm;
-  std::unique_ptr<ContactDev<T>> C(new ContactDev<T>());
-  build_contact_dev<T>(hm.nb, hm.pos.data(), hm.alignT.data(), cd, *C);
-  const ContactVjp<T> cv{&cd, C.get(), (int64_t)3 * cd.npoints * cd.nhalfspaces, (const T*)s_traj, (const T*)stb, (T*)s0b};
-  return integrate_vjp_t<T>(model, dtype, B, (const T*)q_traj, (const T*)v_traj, (const T*)tau, step_stride, stage_stride, dt, nsteps,
-                            (const T*)qtb, (const T*)vtb, (T*)q0t, (T*)q0c, (T*)v0b, (T*)taub, stream, &cv);
-}
-
-template <class T>
-int integrate_task_pd_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, const void* q_traj, const void* v_traj, const void* s_traj,
-                            const void* tau, int64_t step_stride, int64_t stage_stride, const rbd_task_pd_desc& ctrl,
-                            const rbd_contact_desc* cd, double dt, int nsteps, const void* qtb, const void* vtb, const void* stb, void* q0t,
-                            void* q0c, void* v0b, void* s0b, void* taub, const rbd_task_pd_bar* bar, cudaStream_t stream) {
-  const HostModel& hm = model->hm;
-  const TaskPdVjp ctl{&ctrl, bar ? *bar : rbd_task_pd_bar{}};
-  std::unique_ptr<ContactDev<T>> C;
-  std::optional<ContactVjp<T>> cv;
-  if (cd) {
-    C.reset(new ContactDev<T>());
-    build_contact_dev<T>(hm.nb, hm.pos.data(), hm.alignT.data(), *cd, *C);
-    cv.emplace(ContactVjp<T>{cd, C.get(), (int64_t)3 * cd->npoints * cd->nhalfspaces, (const T*)s_traj, (const T*)stb, (T*)s0b});
-  }
-  return integrate_vjp_t<T>(model, dtype, B, (const T*)q_traj, (const T*)v_traj, (const T*)tau, step_stride, stage_stride, dt, nsteps,
-                            (const T*)qtb, (const T*)vtb, (T*)q0t, (T*)q0c, (T*)v0b, (T*)taub, stream, cv ? &*cv : nullptr, nullptr, &ctl);
 }
 
 // rbd_task_pd_torques_vjp: the law at (q, v) recomputed (task_pd_law), τ̄ masked by the applied torque, in computed-torque mode the
@@ -603,47 +583,27 @@ int task_pd_torques_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, cons
   T *m = tau + nv * B, *vdes = m + nv * B, *idv = vdes + nv * B, *idvd = idv + nv * B, *vacc = idvd + nv * B;
   T *qacc = vacc + nv * B, *idq = qacc + nq * B;
   T* lohi = idq + nq * B;
-  if (bounds) {
-    std::vector<T> h(2 * nv);
-    for (int64_t k = 0; k < nv; ++k) { h[k] = (T)c.effort_lo[k]; h[nv + k] = (T)c.effort_hi[k]; }
-    RBD_CUDA_TRY(cudaMemcpyAsync(lohi, h.data(), 2 * nv * sizeof(T), cudaMemcpyHostToDevice, stream));
-  }
+  if (bounds)
+    if (int rc = upload_bounds(lohi, c.effort_lo, c.effort_hi, nv, stream)) return rc;
   const size_t vbytes = (size_t)nv * B * sizeof(T), qbytes = (size_t)nq * B * sizeof(T);
   RBD_CUDA_TRY(cudaMemcpyAsync(m, taub_out, vbytes, cudaMemcpyDeviceToDevice, stream));
   RBD_CUDA_TRY(cudaMemsetAsync(qacc, 0, qbytes, stream));
   RBD_CUDA_TRY(cudaMemsetAsync(vacc, 0, vbytes, stream));
   if (bounds || ct)
     if (int rc = task_pd_law(model, dtype, B, q, v, tau_ff, c, step, tau, ct ? vdes : nullptr, stream)) return rc;
-  if (bounds) {
-    const PdMaskArgs<T> ma{m, tau, lohi, lohi + nv, nv, B};
-    pd_mask_kernel<T><<<(int)std::min<int64_t>((nv * B + 255) / 256, (int64_t)p.sms * 8), 256, 0, stream>>>(ma);
-    if (int rc = api_launched()) return rc;
-  }
+  if (bounds)
+    if (int rc = launch_pd_mask(PdMaskArgs<T>{m, tau, lohi, lohi + nv, nv, B}, p.sms, stream)) return rc;
   if (tffb) RBD_CUDA_TRY(cudaMemcpyAsync(tffb, m, vbytes, cudaMemcpyDeviceToDevice, stream));
   if (ct)
     if (int rc = inverse_dynamics_vjp_dense(model, dtype, B, q, v, vdes, m, idq, idv, idvd, stream)) return rc;
-  const rbd_task_pd_bar cb = bar ? *bar : rbd_task_pd_bar{};
-  const size_t xo = (size_t)step * c.x_ref_step_stride, xdo = (size_t)step * c.xd_ref_step_stride;
-  TaskPdVjpArgs<T> ta{};
+  TaskPdVjpArgs<T> ta = task_vjp_step<T>(c, bar, step);
   ta.q = q; ta.v = v; ta.w = ct ? idvd : m;
-  ta.xref = (const T*)c.x_ref + xo; ta.xdref = c.xd_ref ? (const T*)c.xd_ref + xdo : nullptr;
-  ta.kp = (const T*)c.kp; ta.kd = (const T*)c.kd; ta.gain_ld = c.gain_ld;
-  ta.kpb = (T*)cb.kp; ta.kdb = (T*)cb.kd;
-  ta.xrefb = cb.x_ref ? (T*)cb.x_ref + xo : nullptr; ta.xdrefb = cb.xd_ref ? (T*)cb.xd_ref + xdo : nullptr;
   ta.qacc = qacc; ta.vacc = vacc;
   ta.qfold = ct && !j ? idq : nullptr; ta.vfold = ct && !j ? idv : nullptr;
   if (j) {     // the joint term at the references of `step`; in computed-torque mode it also adds the inverse-dynamics VJP's q̄ / v̄
-    const rbd_pd_bar jb = cb.joint ? *cb.joint : rbd_pd_bar{};
-    const size_t qo = (size_t)step * j->q_ref_step_stride, vo = (size_t)step * j->v_ref_step_stride;
-    PdAdjArgs<T>& pa = ta.joint;
     ta.has_joint = true;
-    pa.qref = (const T*)j->q_ref + qo; pa.vref = j->v_ref ? (const T*)j->v_ref + vo : nullptr;
-    pa.kp = (const T*)j->kp; pa.kd = (const T*)j->kd; pa.g_ld = j->gain_ld;
-    if (ct) { pa.idq = idq; pa.idv = idv; pa.idvd = idvd; }
-    pa.kpb = (T*)jb.kp; pa.kdb = (T*)jb.kd;
-    pa.qrefb = jb.q_ref ? (T*)jb.q_ref + qo : nullptr;
-    pa.vrefb = jb.v_ref ? (T*)jb.v_ref + vo : nullptr;
-    pa.vdrefb = jb.vd_ref ? (T*)jb.vd_ref + vo : nullptr;
+    ta.joint = pd_adj_step<T>(*j, bar ? bar->joint : nullptr, step);
+    if (ct) { ta.joint.idq = idq; ta.joint.idv = idv; ta.joint.idvd = idvd; }
   }
   ta.B = B;
   if (int rc = tplan.launch(M, ta, stream)) return rc;
@@ -656,19 +616,52 @@ int task_pd_torques_vjp_t(const rbd_model* model, int32_t dtype, int64_t B, cons
   return RBD_OK;
 }
 
-// rbd_integrate_pd's JointPD checks with leading dimension B (fn: the entry point named in the messages), pd not NULL
-int check_pd_vjp(const std::string& fn, const rbd_model* model, int64_t B, const rbd_pd_desc* pd) {
-  auto fail = [&](int status, const char* what) { return api_fail(status, fn + ": " + what); };
-  if (!pd->kp || !pd->kd || !pd->q_ref) return fail(RBD_EINVAL, "kp, kd and q_ref must not be NULL");
-  if (pd->mode != RBD_PD_TORQUE && pd->mode != RBD_PD_COMPUTED_TORQUE) return fail(RBD_EINVAL, "unknown mode");
-  if (pd->q_ref_step_stride < 0 || pd->v_ref_step_stride < 0) return fail(RBD_EINVAL, "reference strides must be >= 0");
-  if (pd->gain_ld != 0 && pd->gain_ld != B) return fail(RBD_EINVAL, "gain_ld must be 0 or B");
-  if (pd->mode == RBD_PD_TORQUE && pd->vd_ref) return fail(RBD_EINVAL, "vd_ref is for computed-torque mode only");
-  if (!pd->effort_lo != !pd->effort_hi) return fail(RBD_EINVAL, "effort_lo and effort_hi must be both NULL or both set");
-  if (pd->effort_lo)
-    for (int k = 0; k < model->hm.nv; ++k)
-      if (!(pd->effort_lo[k] <= pd->effort_hi[k])) return fail(RBD_EINVAL, "effort bounds need lo <= hi");
+// the adjoint of an array of a task-space controller exists only where the array does (fn: the entry point named in the messages)
+int check_task_pd_bar(const std::string& fn, const rbd_task_pd_desc& c, const rbd_task_pd_bar* bar) {
+  auto fail = [&](const char* what) { return api_fail(RBD_EINVAL, fn + ": " + what); };
+  if (!bar) return RBD_OK;
+  if (bar->xd_ref && !c.xd_ref) return fail("ctrl_bar->xd_ref needs ctrl->xd_ref");
+  if (bar->joint && !c.joint) return fail("ctrl_bar->joint needs ctrl->joint");
+  if (bar->joint && ((bar->joint->v_ref && !c.joint->v_ref) || (bar->joint->vd_ref && !c.joint->vd_ref)))
+    return fail("ctrl_bar->joint->v_ref / vd_ref need the joint term's v_ref / vd_ref");
   return RBD_OK;
+}
+
+// The argument checks of the rollout VJP entry points, after api_check (fn: the entry point named in the messages); each entry
+// point adds the check of the argument that names it.  The controller's are rbd_integrate_pd's / rbd_integrate_task_pd's with
+// leading dimension B.  RBD_OK also when there is nothing to compute.
+int check_rollout_vjp(const std::string& fn, const rbd_model* model, int32_t dtype, int64_t B, const RolloutVjp& r) {
+  auto fail = [&](int status, const char* what) { return api_fail(status, fn + ": " + what); };
+  if (dtype != RBD_F32 && dtype != RBD_F64) return fail(RBD_EUNSUPPORTED, "fp32 and fp64 only");
+  if (r.nsteps < 0 || !(r.dt > 0)) return fail(RBD_EINVAL, "need dt > 0 and nsteps >= 0");
+  if (r.tau_step_stride < 0 || r.tau_stage_stride < 0) return fail(RBD_EINVAL, "torque strides must be >= 0");
+  if (!r.tau && r.tau_bar) return fail(RBD_EINVAL, "tau_bar needs tau");
+  if (r.contact)
+    if (int rc = api_check_contact(model, r.contact, fn.c_str())) return rc;
+  if (r.pd) {
+    if (int rc = api_check_pd(fn.c_str(), model, B, r.pd)) return rc;
+    // the adjoint of an array exists only where the array does
+    if (r.pd_bar && ((r.pd_bar->v_ref && !r.pd->v_ref) || (r.pd_bar->vd_ref && !r.pd->vd_ref)))
+      return fail(RBD_EINVAL, "pd_bar->v_ref / vd_ref need pd->v_ref / vd_ref");
+  }
+  if (r.task) {
+    if (int rc = api_check_task_ctrl(fn.c_str(), model, B, r.task)) return rc;
+    if (int rc = check_task_pd_bar(fn, *r.task, r.task_bar)) return rc;
+  }
+  if ((r.pd && r.pd->mode == RBD_PD_COMPUTED_TORQUE) || (r.task && r.task->mode == RBD_PD_COMPUTED_TORQUE))
+    if (int rc = check_vjp_limits(model->hm, fn.c_str())) return rc;
+  if (B == 0 || model->hm.nv == 0) return RBD_OK;
+  if (!r.q_traj || !r.v_traj) return fail(RBD_EINVAL, "q_traj and v_traj must not be NULL");
+  if (r.contact && r.contact->npoints * r.contact->nhalfspaces > 0 && !r.s_traj)
+    return fail(RBD_EINVAL, "s_traj must not be NULL when there are contact pairs");
+  return RBD_OK;
+}
+
+// runs a checked request
+int integrate_vjp(const rbd_model* model, int32_t dtype, int64_t B, const RolloutVjp& r, void* stream) {
+  if (B == 0 || model->hm.nv == 0) return RBD_OK;
+  cudaStream_t s = (cudaStream_t)stream;
+  return dtype == RBD_F32 ? integrate_vjp_t<float>(model, B, r, s) : integrate_vjp_t<double>(model, B, r, s);
 }
 
 }  // namespace
@@ -679,20 +672,10 @@ extern "C" int32_t rbd_integrate_vjp(const rbd_model* model, int32_t dtype, int6
                                      void* tau_bar, void* stream) {
   if (int rc = api_check(model, dtype, B, B)) return rc;
   const ApiCall call;
-  if (dtype != RBD_F32 && dtype != RBD_F64) return api_fail(RBD_EUNSUPPORTED, "rbd_integrate_vjp: fp32 and fp64 only");
-  if (nsteps < 0 || !(dt > 0)) return api_fail(RBD_EINVAL, "rbd_integrate_vjp: need dt > 0 and nsteps >= 0");
-  if (tau_step_stride < 0 || tau_stage_stride < 0) return api_fail(RBD_EINVAL, "rbd_integrate_vjp: torque strides must be >= 0");
-  if (!tau && tau_bar) return api_fail(RBD_EINVAL, "rbd_integrate_vjp: tau_bar needs tau");
-  if (B == 0 || model->hm.nv == 0) return RBD_OK;
-  if (!q_traj || !v_traj) return api_fail(RBD_EINVAL, "rbd_integrate_vjp: q_traj and v_traj must not be NULL");
-  cudaStream_t s = (cudaStream_t)stream;
-  return dtype == RBD_F32
-             ? integrate_vjp_t<float>(model, dtype, B, (const float*)q_traj, (const float*)v_traj, (const float*)tau, tau_step_stride,
-                                      tau_stage_stride, dt, nsteps, (const float*)q_traj_bar, (const float*)v_traj_bar, (float*)q0_bar_tan,
-                                      (float*)q0_bar_cfg, (float*)v0_bar, (float*)tau_bar, s)
-             : integrate_vjp_t<double>(model, dtype, B, (const double*)q_traj, (const double*)v_traj, (const double*)tau, tau_step_stride,
-                                       tau_stage_stride, dt, nsteps, (const double*)q_traj_bar, (const double*)v_traj_bar,
-                                       (double*)q0_bar_tan, (double*)q0_bar_cfg, (double*)v0_bar, (double*)tau_bar, s);
+  const RolloutVjp r{q_traj, v_traj, nullptr, tau, tau_step_stride, tau_stage_stride, dt, nsteps, q_traj_bar, v_traj_bar, nullptr,
+                     q0_bar_tan, q0_bar_cfg, v0_bar, nullptr, tau_bar};
+  if (int rc = check_rollout_vjp("rbd_integrate_vjp", model, dtype, B, r)) return rc;
+  return integrate_vjp(model, dtype, B, r, stream);
 }
 
 extern "C" int32_t rbd_integrate_contact_vjp(const rbd_model* model, int32_t dtype, int64_t B, const void* q_traj, const void* v_traj,
@@ -702,21 +685,12 @@ extern "C" int32_t rbd_integrate_contact_vjp(const rbd_model* model, int32_t dty
                                              void* v0_bar, void* s0_bar, void* tau_bar, void* stream) {
   if (int rc = api_check(model, dtype, B, B)) return rc;
   const ApiCall call;
-  if (dtype != RBD_F32 && dtype != RBD_F64) return api_fail(RBD_EUNSUPPORTED, "rbd_integrate_contact_vjp: fp32 and fp64 only");
-  if (nsteps < 0 || !(dt > 0)) return api_fail(RBD_EINVAL, "rbd_integrate_contact_vjp: need dt > 0 and nsteps >= 0");
-  if (tau_step_stride < 0 || tau_stage_stride < 0) return api_fail(RBD_EINVAL, "rbd_integrate_contact_vjp: torque strides must be >= 0");
-  if (!tau && tau_bar) return api_fail(RBD_EINVAL, "rbd_integrate_contact_vjp: tau_bar needs tau");
-  if (int rc = api_check_contact(model, contact, "rbd_integrate_contact_vjp")) return rc;
-  const int64_t ns = (int64_t)3 * contact->npoints * contact->nhalfspaces;
-  if (B == 0 || model->hm.nv == 0) return RBD_OK;
-  if (!q_traj || !v_traj) return api_fail(RBD_EINVAL, "rbd_integrate_contact_vjp: q_traj and v_traj must not be NULL");
-  if (ns > 0 && !s_traj) return api_fail(RBD_EINVAL, "rbd_integrate_contact_vjp: s_traj must not be NULL when there are contact pairs");
-  cudaStream_t s = (cudaStream_t)stream;
-  return dtype == RBD_F32
-             ? integrate_contact_vjp_t<float>(model, dtype, B, q_traj, v_traj, s_traj, tau, tau_step_stride, tau_stage_stride, *contact, dt,
-                                              nsteps, q_traj_bar, v_traj_bar, s_traj_bar, q0_bar_tan, q0_bar_cfg, v0_bar, s0_bar, tau_bar, s)
-             : integrate_contact_vjp_t<double>(model, dtype, B, q_traj, v_traj, s_traj, tau, tau_step_stride, tau_stage_stride, *contact, dt,
-                                               nsteps, q_traj_bar, v_traj_bar, s_traj_bar, q0_bar_tan, q0_bar_cfg, v0_bar, s0_bar, tau_bar, s);
+  RolloutVjp r{q_traj, v_traj, s_traj, tau, tau_step_stride, tau_stage_stride, dt, nsteps, q_traj_bar, v_traj_bar, s_traj_bar,
+               q0_bar_tan, q0_bar_cfg, v0_bar, s0_bar, tau_bar};
+  r.contact = contact;
+  if (int rc = check_rollout_vjp("rbd_integrate_contact_vjp", model, dtype, B, r)) return rc;
+  if (!contact) return api_fail(RBD_EINVAL, "rbd_integrate_contact_vjp: contact must not be NULL");
+  return integrate_vjp(model, dtype, B, r, stream);
 }
 
 extern "C" int32_t rbd_integrate_pd_vjp(const rbd_model* model, int32_t dtype, int64_t B, const void* q_traj, const void* v_traj,
@@ -725,36 +699,14 @@ extern "C" int32_t rbd_integrate_pd_vjp(const rbd_model* model, int32_t dtype, i
                                         const void* q_traj_bar, const void* v_traj_bar, const void* s_traj_bar, void* q0_bar_tan,
                                         void* q0_bar_cfg, void* v0_bar, void* s0_bar, void* tau_bar, const rbd_pd_bar* pd_bar,
                                         void* stream) {
-  const char* fn = "rbd_integrate_pd_vjp";
-  auto fail = [&](int status, const char* what) { return api_fail(status, std::string(fn) + ": " + what); };
   if (int rc = api_check(model, dtype, B, B)) return rc;
   const ApiCall call;
-  if (dtype != RBD_F32 && dtype != RBD_F64) return fail(RBD_EUNSUPPORTED, "fp32 and fp64 only");
-  if (nsteps < 0 || !(dt > 0)) return fail(RBD_EINVAL, "need dt > 0 and nsteps >= 0");
-  if (tau_step_stride < 0 || tau_stage_stride < 0) return fail(RBD_EINVAL, "torque strides must be >= 0");
-  if (!tau && tau_bar) return fail(RBD_EINVAL, "tau_bar needs tau");
-  if (contact)
-    if (int rc = api_check_contact(model, contact, fn)) return rc;
-  // the controller: rbd_integrate_pd's checks, with leading dimension B
-  if (!pd) return fail(RBD_EINVAL, "pd must not be NULL");
-  if (int rc = check_pd_vjp(fn, model, B, pd)) return rc;
-  // the adjoint of an array exists only where the array does
-  if (pd_bar && ((pd_bar->v_ref && !pd->v_ref) || (pd_bar->vd_ref && !pd->vd_ref)))
-    return fail(RBD_EINVAL, "pd_bar->v_ref / vd_ref need pd->v_ref / vd_ref");
-  if (pd->mode == RBD_PD_COMPUTED_TORQUE)
-    if (int rc = check_vjp_limits(model->hm, fn)) return rc;
-  const int64_t ns = contact ? (int64_t)3 * contact->npoints * contact->nhalfspaces : 0;
-  if (B == 0 || model->hm.nv == 0) return RBD_OK;
-  if (!q_traj || !v_traj) return fail(RBD_EINVAL, "q_traj and v_traj must not be NULL");
-  if (ns > 0 && !s_traj) return fail(RBD_EINVAL, "s_traj must not be NULL when there are contact pairs");
-  cudaStream_t s = (cudaStream_t)stream;
-  return dtype == RBD_F32
-             ? integrate_pd_vjp_t<float>(model, dtype, B, q_traj, v_traj, s_traj, tau, tau_step_stride, tau_stage_stride, *pd, contact, dt,
-                                         nsteps, q_traj_bar, v_traj_bar, s_traj_bar, q0_bar_tan, q0_bar_cfg, v0_bar, s0_bar, tau_bar,
-                                         pd_bar, s)
-             : integrate_pd_vjp_t<double>(model, dtype, B, q_traj, v_traj, s_traj, tau, tau_step_stride, tau_stage_stride, *pd, contact,
-                                          dt, nsteps, q_traj_bar, v_traj_bar, s_traj_bar, q0_bar_tan, q0_bar_cfg, v0_bar, s0_bar, tau_bar,
-                                          pd_bar, s);
+  RolloutVjp r{q_traj, v_traj, s_traj, tau, tau_step_stride, tau_stage_stride, dt, nsteps, q_traj_bar, v_traj_bar, s_traj_bar,
+               q0_bar_tan, q0_bar_cfg, v0_bar, s0_bar, tau_bar};
+  r.contact = contact; r.pd = pd; r.pd_bar = pd_bar;
+  if (int rc = check_rollout_vjp("rbd_integrate_pd_vjp", model, dtype, B, r)) return rc;
+  if (!pd) return api_fail(RBD_EINVAL, "rbd_integrate_pd_vjp: pd must not be NULL");
+  return integrate_vjp(model, dtype, B, r, stream);
 }
 
 extern "C" int32_t rbd_integrate_task_pd_vjp(const rbd_model* model, int32_t dtype, int64_t B, const void* q_traj, const void* v_traj,
@@ -763,40 +715,14 @@ extern "C" int32_t rbd_integrate_task_pd_vjp(const rbd_model* model, int32_t dty
                                              const void* q_traj_bar, const void* v_traj_bar, const void* s_traj_bar, void* q0_bar_tan,
                                              void* q0_bar_cfg, void* v0_bar, void* s0_bar, void* tau_bar, const rbd_task_pd_bar* ctrl_bar,
                                              void* stream) {
-  const std::string fn = "rbd_integrate_task_pd_vjp";
-  auto fail = [&](int status, const std::string& what) { return api_fail(status, fn + ": " + what); };
   if (int rc = api_check(model, dtype, B, B)) return rc;
   const ApiCall call;
-  if (dtype != RBD_F32 && dtype != RBD_F64) return fail(RBD_EUNSUPPORTED, "fp32 and fp64 only");
-  if (nsteps < 0 || !(dt > 0)) return fail(RBD_EINVAL, "need dt > 0 and nsteps >= 0");
-  if (tau_step_stride < 0 || tau_stage_stride < 0) return fail(RBD_EINVAL, "torque strides must be >= 0");
-  if (!tau && tau_bar) return fail(RBD_EINVAL, "tau_bar needs tau");
-  if (contact)
-    if (int rc = api_check_contact(model, contact, fn.c_str())) return rc;
-  // the controller: rbd_integrate_task_pd's checks (the joint term's JointPD checks, then check_task_pd), with leading dimension B
-  if (ctrl && ctrl->joint)
-    if (int rc = check_pd_vjp(fn + " (joint term)", model, B, ctrl->joint)) return rc;
-  std::string err;
-  if (int rc = check_task_pd(model->hm.nb, model->hm.nv, B, ctrl, err)) return fail(rc, err);
-  // the adjoint of an array exists only where the array does
-  if (ctrl_bar && ctrl_bar->xd_ref && !ctrl->xd_ref) return fail(RBD_EINVAL, "ctrl_bar->xd_ref needs ctrl->xd_ref");
-  if (ctrl_bar && ctrl_bar->joint && !ctrl->joint) return fail(RBD_EINVAL, "ctrl_bar->joint needs ctrl->joint");
-  if (ctrl_bar && ctrl_bar->joint && ((ctrl_bar->joint->v_ref && !ctrl->joint->v_ref) || (ctrl_bar->joint->vd_ref && !ctrl->joint->vd_ref)))
-    return fail(RBD_EINVAL, "ctrl_bar->joint->v_ref / vd_ref need the joint term's v_ref / vd_ref");
-  if (ctrl->mode == RBD_PD_COMPUTED_TORQUE)
-    if (int rc = check_vjp_limits(model->hm, fn.c_str())) return rc;
-  const int64_t ns = contact ? (int64_t)3 * contact->npoints * contact->nhalfspaces : 0;
-  if (B == 0 || model->hm.nv == 0) return RBD_OK;
-  if (!q_traj || !v_traj) return fail(RBD_EINVAL, "q_traj and v_traj must not be NULL");
-  if (ns > 0 && !s_traj) return fail(RBD_EINVAL, "s_traj must not be NULL when there are contact pairs");
-  cudaStream_t s = (cudaStream_t)stream;
-  return dtype == RBD_F32
-             ? integrate_task_pd_vjp_t<float>(model, dtype, B, q_traj, v_traj, s_traj, tau, tau_step_stride, tau_stage_stride, *ctrl,
-                                              contact, dt, nsteps, q_traj_bar, v_traj_bar, s_traj_bar, q0_bar_tan, q0_bar_cfg, v0_bar,
-                                              s0_bar, tau_bar, ctrl_bar, s)
-             : integrate_task_pd_vjp_t<double>(model, dtype, B, q_traj, v_traj, s_traj, tau, tau_step_stride, tau_stage_stride, *ctrl,
-                                               contact, dt, nsteps, q_traj_bar, v_traj_bar, s_traj_bar, q0_bar_tan, q0_bar_cfg, v0_bar,
-                                               s0_bar, tau_bar, ctrl_bar, s);
+  RolloutVjp r{q_traj, v_traj, s_traj, tau, tau_step_stride, tau_stage_stride, dt, nsteps, q_traj_bar, v_traj_bar, s_traj_bar,
+               q0_bar_tan, q0_bar_cfg, v0_bar, s0_bar, tau_bar};
+  r.contact = contact; r.task = ctrl; r.task_bar = ctrl_bar;
+  if (int rc = check_rollout_vjp("rbd_integrate_task_pd_vjp", model, dtype, B, r)) return rc;
+  if (!ctrl) return api_fail(RBD_EINVAL, "rbd_integrate_task_pd_vjp: ctrl must not be NULL");
+  return integrate_vjp(model, dtype, B, r, stream);
 }
 
 extern "C" int32_t rbd_task_pd_torques_vjp(const rbd_model* model, int32_t dtype, int64_t B, const void* q, const void* v,
@@ -811,10 +737,7 @@ extern "C" int32_t rbd_task_pd_torques_vjp(const rbd_model* model, int32_t dtype
   if (int rc = api_check_task_ctrl(fn.c_str(), model, B, ctrl)) return rc;
   if (step < 0) return fail(RBD_EINVAL, "step must be >= 0");
   if (!tau_ff && tau_ff_bar) return fail(RBD_EINVAL, "tau_ff_bar needs tau_ff");
-  if (ctrl_bar && ctrl_bar->xd_ref && !ctrl->xd_ref) return fail(RBD_EINVAL, "ctrl_bar->xd_ref needs ctrl->xd_ref");
-  if (ctrl_bar && ctrl_bar->joint && !ctrl->joint) return fail(RBD_EINVAL, "ctrl_bar->joint needs ctrl->joint");
-  if (ctrl_bar && ctrl_bar->joint && ((ctrl_bar->joint->v_ref && !ctrl->joint->v_ref) || (ctrl_bar->joint->vd_ref && !ctrl->joint->vd_ref)))
-    return fail(RBD_EINVAL, "ctrl_bar->joint->v_ref / vd_ref need the joint term's v_ref / vd_ref");
+  if (int rc = check_task_pd_bar(fn, *ctrl, ctrl_bar)) return rc;
   if (ctrl->mode == RBD_PD_COMPUTED_TORQUE)
     if (int rc = check_vjp_limits(model->hm, fn.c_str())) return rc;
   if (B == 0 || model->hm.nv == 0) return RBD_OK;
