@@ -288,10 +288,36 @@ int32_t rbd_dynamics_result(const rbd_model* model, int32_t dtype, int64_t B, in
  *                            the tangent space, which is what the Munthe-Kaas integrator's local coordinates need and which does
  *                            not depend on how the rotation is extended to non-unit quaternions.
  *   dvd_dv_out  [nv*nv x B]  d v̇_i / d v_j, same layout.
- * d v̇ / d tau is M^-1: mass_matrix! gives M.  tau may be NULL (zero torques).  fp32 / fp64; no external wrenches (RBD_EUNSUPPORTED
- * is never returned for them: the argument does not exist -- use the reference's Dual path, rbd_dynamics with RBD_DUAL64X6). */
+ * tau may be NULL (zero torques).  fp32 / fp64 (RBD_DUAL64X6 -> RBD_EUNSUPPORTED).  More than 128 velocity coordinates or 4096
+ * stored mass-matrix entries -> RBD_EUNSUPPORTED before any launch.  External wrenches and d v̇ / d tau: rbd_dynamics_derivatives_ext,
+ * of which this is the call with wext = dvd_dtau_out = NULL. */
 int32_t rbd_dynamics_derivatives(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                                  const void* tau, void* vd_out, void* dvd_dq_out, void* dvd_dv_out, void* stream);
+
+/* rbd_dynamics_derivatives with external wrenches and d v̇ / d tau, the complete continuous-time linearisation of dynamics!:
+ *   wext          [6*nb x B] or NULL: root-frame wrenches, rows as in rbd_dynamics.  v̇ = rbd_dynamics(q, v, tau, wext) is the
+ *                 linearisation point; the wrenches are held fixed in the root frame while q moves.
+ *   dvd_dtau_out  [nv*nv x B] or NULL: d v̇ / d tau = M^-1, entry (i, j) at row i + j*nv (solved from the factor the call already
+ *                 builds, with the constant right-hand sides e_j).
+ * Other arguments, layouts and errors as rbd_dynamics_derivatives. */
+int32_t rbd_dynamics_derivatives_ext(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
+                                     const void* tau, const void* wext, void* vd_out, void* dvd_dq_out, void* dvd_dv_out,
+                                     void* dvd_dtau_out, void* stream);
+
+/* Jacobians of inverse_dynamics! (mechanism_algorithms.jl:542-553) at the caller's v̇, without forward dynamics or a factorisation --
+ * what inverse-dynamics trajectory optimisation, torque residuals and system identification linearise:
+ *   q [nq x B], v [nv x B], vd [nv x B] = v̇, wext [6*nb x B] or NULL (root-frame wrenches as in rbd_dynamics)
+ *   dtau_dq_out [nv*nv x B]  entry (i, j) at row i + j*nv: d tau_i / d q_j along velocity_to_configuration_derivative(e_j) (tangent
+ *                            space, as dvd_dq_out of rbd_dynamics_derivatives)
+ *   dtau_dv_out [nv*nv x B]  d tau_i / d v_j, same layout
+ *   tau_out     [nv x B] or NULL: tau = inverse_dynamics!(q, v, v̇, wext) (equal to rbd_inverse_dynamics up to rounding)
+ *   M_out       [nv*nv x B] or NULL: d tau / d v̇ = M, both triangles (layout of rbd_mass_matrix)
+ * Every entry of the Jacobians is written, zeros included.  q, v, vd, dtau_dq_out and dtau_dv_out must not be NULL (RBD_EINVAL);
+ * fp32 / fp64 (RBD_DUAL64X6 -> RBD_EUNSUPPORTED); the model limits of rbd_dynamics_derivatives apply; B == 0 or nv == 0: nothing
+ * to do. */
+int32_t rbd_inverse_dynamics_derivatives(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q,
+                                         const void* v, const void* vd, const void* wext, void* tau_out, void* dtau_dq_out,
+                                         void* dtau_dv_out, void* M_out, void* stream);
 
 /* Reverse mode (SURVEY 8(f) rank 3, second half): vector-Jacobian products of dynamics! / inverse_dynamics! -- what a reference user
  * gets from reverse-mode AD over those functions (ChainRules / ReverseDiff) -- in O(n) per sample, without forming any nv x nv
@@ -334,6 +360,9 @@ int32_t rbd_inverse_dynamics_vjp(const rbd_model* model, int32_t dtype, int64_t 
  * its cubin is cached or the batch is at least RBD_JIT_MIN_BATCH (default 4096 for this entry point); RBD_DERIV_JIT=0 / RBD_JIT=0
  * keep the generic table-driven kernel.  This call compiles it ahead of time (no GPU needed). */
 int32_t rbd_model_precompile_derivatives(rbd_model* model, int32_t dtype);
+/* The same for rbd_dynamics_derivatives_ext: with_dtau != 0 compiles the variant that also solves d v̇ / d tau (its own kernel and
+ * cubin); with_dtau == 0 is rbd_model_precompile_derivatives. */
+int32_t rbd_model_precompile_derivatives_ext(rbd_model* model, int32_t dtype, int32_t with_dtau);
 
 /* dynamics_bias!(result, state) / dynamics_bias!(torques, biasaccelerations, wrenches, state, externalwrenches)
  *                                                             src/mechanism_algorithms.jl:484-498

@@ -500,25 +500,60 @@ end
 # ---- SURVEY 8(f) rank 3: Jacobians of forward dynamics ----------------------------------------------------------------------
 
 """
-    dynamics_derivatives!(dvd_dq, dvd_dv, result, state, torques = nothing)
+    dynamics_derivatives!(dvd_dq, dvd_dv, result, state, torques = nothing; externalwrenches = nothing, dvd_dtau = nothing)
 
 Analytic `∂v̇/∂q` (tangent space) and `∂v̇/∂v` of `dynamics!` for every sample in one call -- what
 `ForwardDiff.jacobian(x -> dynamics!(...), ...)` over the reference's generic path produces with 2 nv / 6 Dual sweeps per sample
 (examples/5. Derivatives and gradients using ForwardDiff, test/test_mechanism_algorithms.jl:600-675).  `dvd_dq`, `dvd_dv` are
 B x (nv*nv) device matrices, entry (i, j) of sample b at `[b, i + (j - 1) * nv]` (column-major like `M.data`);
 `dvd_dq[:, :, j]` is the derivative along `velocity_to_configuration_derivative(e_j)`, i.e. `(∂v̇/∂q) * velocity_to_configuration_derivative_jacobian(state)`.
-`result.v̇` receives v̇.  External wrenches: use the Dual path (`dynamics!` on `Dual` inputs).
+`result.v̇` receives v̇.  `externalwrenches`: B x 6nb root-frame wrenches as in `dynamics!`, held fixed while q moves; `dvd_dtau`:
+a B x (nv*nv) matrix that receives `∂v̇/∂τ = M⁻¹` (rbd_dynamics_derivatives_ext).  (Not run here: no Julia installation is
+available to the project's tests; the Python binding exercises the same entry points.)
 """
-function dynamics_derivatives!(dvd_dq, dvd_dv, result::BatchedResult{T}, state::BatchedState{T}, torques = nothing) where {T <: Union{Float32, Float64}}
+function dynamics_derivatives!(dvd_dq, dvd_dv, result::BatchedResult{T}, state::BatchedState{T}, torques = nothing;
+                               externalwrenches = nothing, dvd_dtau = nothing) where {T <: Union{Float32, Float64}}
     checkstate(state)
     B = size(state.q, 1)
-    GC.@preserve state result torques dvd_dq dvd_dv begin
-        check(ccall((:rbd_dynamics_derivatives, librbd), Int32,
-                    (Ptr{Cvoid}, Int32, Int64, Int64, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
-                    state.model.handle, dtype_code(T), B, B, devptr(state.q), devptr(state.v),
-                    torques === nothing ? C_NULL : devptr(torques), devptr(result.v̇), devptr(dvd_dq), devptr(dvd_dv), stream_ptr()))
+    GC.@preserve state result torques dvd_dq dvd_dv externalwrenches dvd_dtau begin
+        if externalwrenches === nothing && dvd_dtau === nothing
+            check(ccall((:rbd_dynamics_derivatives, librbd), Int32,
+                        (Ptr{Cvoid}, Int32, Int64, Int64, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
+                        state.model.handle, dtype_code(T), B, B, devptr(state.q), devptr(state.v),
+                        torques === nothing ? C_NULL : devptr(torques), devptr(result.v̇), devptr(dvd_dq), devptr(dvd_dv), stream_ptr()))
+        else
+            check(ccall((:rbd_dynamics_derivatives_ext, librbd), Int32,
+                        (Ptr{Cvoid}, Int32, Int64, Int64, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid},
+                         Ptr{Cvoid}, Ptr{Cvoid}),
+                        state.model.handle, dtype_code(T), B, B, devptr(state.q), devptr(state.v),
+                        torques === nothing ? C_NULL : devptr(torques), externalwrenches === nothing ? C_NULL : devptr(externalwrenches),
+                        devptr(result.v̇), devptr(dvd_dq), devptr(dvd_dv), dvd_dtau === nothing ? C_NULL : devptr(dvd_dtau), stream_ptr()))
+        end
     end
     dvd_dq, dvd_dv
+end
+
+"""
+    inverse_dynamics_derivatives!(dtau_dq, dtau_dv, state, v̇, externalwrenches = nothing; torques = nothing, massmatrix = nothing)
+
+Analytic `∂τ/∂q` (tangent space, as in `dynamics_derivatives!`) and `∂τ/∂v` of `inverse_dynamics!` at the given v̇ for every sample
+in one call (rbd_inverse_dynamics_derivatives), B x (nv*nv) each in the layout of `dynamics_derivatives!`.  `torques` (B x nv)
+receives τ itself and `massmatrix` (B x (nv*nv)) receives `∂τ/∂v̇ = M`, both triangles.  (Not run here: no Julia installation is
+available to the project's tests; the Python binding exercises the same entry point.)
+"""
+function inverse_dynamics_derivatives!(dtau_dq, dtau_dv, state::BatchedState{T}, v̇::AbstractMatrix{T}, externalwrenches = nothing;
+                                       torques = nothing, massmatrix = nothing) where {T <: Union{Float32, Float64}}
+    checkstate(state)
+    B = size(state.q, 1)
+    GC.@preserve state v̇ externalwrenches dtau_dq dtau_dv torques massmatrix begin
+        check(ccall((:rbd_inverse_dynamics_derivatives, librbd), Int32,
+                    (Ptr{Cvoid}, Int32, Int64, Int64, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid},
+                     Ptr{Cvoid}, Ptr{Cvoid}),
+                    state.model.handle, dtype_code(T), B, B, devptr(state.q), devptr(state.v), devptr(v̇),
+                    externalwrenches === nothing ? C_NULL : devptr(externalwrenches), torques === nothing ? C_NULL : devptr(torques),
+                    devptr(dtau_dq), devptr(dtau_dv), massmatrix === nothing ? C_NULL : devptr(massmatrix), stream_ptr()))
+    end
+    dtau_dq, dtau_dv
 end
 
 "Compile the model-specialised solve kernel of `dynamics_derivatives!` ahead of time (cubin cache; no GPU needed)."

@@ -18,7 +18,8 @@ from .urdf import (default_urdf_joint_types, load_description, load_model, mecha
 from .state import (DynamicsResult, MechanismState, rand_, rand_configuration_, rand_velocity_, zero_,  # noqa: F401
                     zero_configuration_, zero_velocity_)
 from .algorithms import (DimensionMismatch, dynamics_, dynamics_derivatives_, dynamics_dual_, dynamics_bias, dynamics_bias_, dynamics_ode_,  # noqa: F401
-                         inverse_dynamics, inverse_dynamics_, mass_matrix, mass_matrix_, simulate_,
+                         inverse_dynamics, inverse_dynamics_, inverse_dynamics_derivatives, inverse_dynamics_derivatives_,
+                         mass_matrix, mass_matrix_, simulate_,
                          simulate_trajectory_)
 from .kinematics import (TreePath, center_of_mass, geometric_jacobian, geometric_jacobian_,  # noqa: F401
                          gravitational_potential_energy, kinematics_, kinetic_energy, momentum, momentum_matrix,

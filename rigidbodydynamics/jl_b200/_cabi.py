@@ -130,6 +130,9 @@ SYMBOLS = {
     "rbd_dynamics_result": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rbd_dynamics_derivatives": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "rbd_model_precompile_derivatives": (c_int32, [_vp, _i32]),
+    "rbd_dynamics_derivatives_ext": (c_int32, [_vp, _i32, _i64, _i64] + [_vp] * 9),
+    "rbd_inverse_dynamics_derivatives": (c_int32, [_vp, _i32, _i64, _i64] + [_vp] * 9),
+    "rbd_model_precompile_derivatives_ext": (c_int32, [_vp, _i32, _i32]),
     "rbd_dynamics_vjp": (c_int32, [_vp, _i32, _i64, _i64] + [_vp] * 12),
     "rbd_inverse_dynamics_vjp": (c_int32, [_vp, _i32, _i64, _i64] + [_vp] * 11),
     "rbd_dynamics_bias": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _vp]),
@@ -208,9 +211,13 @@ class ModelHandle:
         unless ``load``)."""
         check(self._lib.rbd_model_precompile(self._h, int(dtype), int(what), 1 if load else 0))
 
-    def precompile_derivatives(self, dtype: int = RBD_F64):
-        """rbd_model_precompile_derivatives: the model-specialised solve kernel of rbd_dynamics_derivatives into the cubin cache."""
-        check(self._lib.rbd_model_precompile_derivatives(self._h, int(dtype)))
+    def precompile_derivatives(self, dtype: int = RBD_F64, with_dtau: bool = False):
+        """rbd_model_precompile_derivatives: the model-specialised solve kernel of rbd_dynamics_derivatives into the cubin cache.
+        ``with_dtau``: the variant that also solves d v̇ / d tau (rbd_model_precompile_derivatives_ext)."""
+        if with_dtau:
+            check(self._lib.rbd_model_precompile_derivatives_ext(self._h, int(dtype), 1))
+        else:
+            check(self._lib.rbd_model_precompile_derivatives(self._h, int(dtype)))
 
     def close(self):
         if getattr(self, "_h", None):

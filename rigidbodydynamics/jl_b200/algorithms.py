@@ -20,7 +20,7 @@ from . import _cabi
 from .pd import JointPD, TaskPD
 from .state import DynamicsResult, MechanismState, _DT
 
-__all__ = ["dynamics_", "dynamics_dual_", "dynamics_derivatives_", "dynamics_ode_", "simulate_", "simulate_trajectory_", "inverse_dynamics_", "inverse_dynamics", "mass_matrix_", "mass_matrix",
+__all__ = ["dynamics_", "dynamics_dual_", "dynamics_derivatives_", "inverse_dynamics_derivatives_", "inverse_dynamics_derivatives", "dynamics_ode_", "simulate_", "simulate_trajectory_", "inverse_dynamics_", "inverse_dynamics", "mass_matrix_", "mass_matrix",
            "dynamics_bias_", "dynamics_bias", "DimensionMismatch"]
 
 
@@ -125,26 +125,68 @@ def dynamics_dual_(vd_out: torch.Tensor, state: MechanismState, q: torch.Tensor,
 
 
 def dynamics_derivatives_(dvd_dq: torch.Tensor, dvd_dv: torch.Tensor, result: DynamicsResult, state: MechanismState,
-                          torques: Optional[torch.Tensor] = None):
+                          torques: Optional[torch.Tensor] = None, externalwrenches: Optional[torch.Tensor] = None,
+                          dvd_dtau: Optional[torch.Tensor] = None):
     """Jacobians of ``dynamics!`` with respect to the configuration (tangent space) and the velocity for every sample, in one call:
     the batched, analytic counterpart of ``ForwardDiff.jacobian`` over the reference's generic ``dynamics!`` (examples/5,
     test/test_mechanism_algorithms.jl:600-675).  ``dvd_dq`` / ``dvd_dv`` are [nv*nv, B], entry (i, j) at row i + j*nv (column-major
     like ``M.data``); ``dvd_dq[:, j]`` is the derivative along ``velocity_to_configuration_derivative(e_j)``, i.e.
-    ``(d v̇/d q) * velocity_to_configuration_derivative_jacobian(state)``.  ``result.vd`` receives v̇."""
+    ``(d v̇/d q) * velocity_to_configuration_derivative_jacobian(state)``.  ``result.vd`` receives v̇.
+    ``externalwrenches`` [6*nb, B] (root frame, as in ``dynamics_``, held fixed while q moves) or None; ``dvd_dtau`` [nv*nv, B] or
+    None receives d v̇ / d tau = M^-1 in the same layout."""
     _require_tree(state, "dynamics_derivatives_")
     state.check_modcount()
     lib = _cabi.load_library()
     _check(torques, state.nv, state, "torques")
+    _check(externalwrenches, 6 * len(state.mechanism.joints), state, "externalwrenches")
     _check(result.vd, state.nv, state, "result.vd")
     _check(dvd_dq, state.nv * state.nv, state, "dvd_dq")
     _check(dvd_dv, state.nv * state.nv, state, "dvd_dv")
+    _check(dvd_dtau, state.nv * state.nv, state, "dvd_dtau")
     if dvd_dq is None or dvd_dv is None:
         raise ValueError("dvd_dq and dvd_dv must be given")
+    head = (state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q), _ptr(state.v), _ptr(torques))
     with torch.cuda.device(state.q.device):
-        _call(lib.rbd_dynamics_derivatives(state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q), _ptr(state.v),
-                                           _ptr(torques), _ptr(result.vd), _ptr(dvd_dq), _ptr(dvd_dv),
-                                           torch.cuda.current_stream(state.q.device).cuda_stream))
+        stream = torch.cuda.current_stream(state.q.device).cuda_stream
+        if externalwrenches is None and dvd_dtau is None:
+            _call(lib.rbd_dynamics_derivatives(*head, _ptr(result.vd), _ptr(dvd_dq), _ptr(dvd_dv), stream))
+        else:
+            _call(lib.rbd_dynamics_derivatives_ext(*head, _ptr(externalwrenches), _ptr(result.vd), _ptr(dvd_dq), _ptr(dvd_dv),
+                                                   _ptr(dvd_dtau), stream))
     return dvd_dq, dvd_dv
+
+
+def inverse_dynamics_derivatives_(dtau_dq: torch.Tensor, dtau_dv: torch.Tensor, state: MechanismState, vd: torch.Tensor,
+                                  externalwrenches: Optional[torch.Tensor] = None, torques: Optional[torch.Tensor] = None,
+                                  massmatrix: Optional[torch.Tensor] = None):
+    """Jacobians of ``inverse_dynamics!`` at the given v̇ for every sample, in one call (no forward dynamics, no factorisation):
+    ``dtau_dq`` / ``dtau_dv`` [nv*nv, B], entry (i, j) at row i + j*nv, d tau / d q along ``velocity_to_configuration_derivative(e_j)``
+    as in ``dynamics_derivatives_``.  ``vd`` [nv, B]; ``externalwrenches`` [6*nb, B] or None (root frame, held fixed while q moves).
+    ``torques`` [nv, B] or None receives tau = inverse_dynamics!(state, v̇, externalwrenches); ``massmatrix`` [nv*nv, B] or None
+    receives d tau / d v̇ = M, both triangles."""
+    _require_tree(state, "inverse_dynamics_derivatives_")
+    state.check_modcount()
+    lib = _cabi.load_library()
+    nv2 = state.nv * state.nv
+    _check(vd, state.nv, state, "v̇")
+    _check(externalwrenches, 6 * len(state.mechanism.joints), state, "externalwrenches")
+    _check(dtau_dq, nv2, state, "dtau_dq")
+    _check(dtau_dv, nv2, state, "dtau_dv")
+    _check(torques, state.nv, state, "torques")
+    _check(massmatrix, nv2, state, "massmatrix")
+    if dtau_dq is None or dtau_dv is None or vd is None:
+        raise ValueError("dtau_dq, dtau_dv and vd must be given")
+    with torch.cuda.device(state.q.device):
+        _call(lib.rbd_inverse_dynamics_derivatives(state.handle.ptr, _DT[state.dtype], state.batch, state.batch, _ptr(state.q),
+                                                   _ptr(state.v), _ptr(vd), _ptr(externalwrenches), _ptr(torques), _ptr(dtau_dq),
+                                                   _ptr(dtau_dv), _ptr(massmatrix), torch.cuda.current_stream(state.q.device).cuda_stream))
+    return dtau_dq, dtau_dv
+
+
+def inverse_dynamics_derivatives(state: MechanismState, vd: torch.Tensor, externalwrenches: Optional[torch.Tensor] = None):
+    """Allocating form of ``inverse_dynamics_derivatives_``: returns ``(dtau_dq, dtau_dv)``."""
+    new = lambda: torch.empty((state.nv * state.nv, state.batch), dtype=state.dtype, device=state.q.device)   # noqa: E731
+    return inverse_dynamics_derivatives_(new(), new(), state, vd, externalwrenches)
 
 
 def dynamics_ode_(xdot: torch.Tensor, result: DynamicsResult, state: MechanismState, x: torch.Tensor,

@@ -20,8 +20,15 @@
 // q̇ = velocity_to_configuration_derivative(e_j) (mechanism_state.jl:905-910): for 1-DoF joints that is d/dq itself; for
 // quaternion joints it is the tangent-space derivative [dv̇/dq_raw] * velocity_to_configuration_derivative_jacobian.
 //
+// External wrenches W_i (root frame, fixed while the subtree moves) enter ID as f_i = I a + v x* I v - W_i.  Only the inertial part
+// moves with a subtree, so with W_K = sum W_i over K's subtree the closed form gains one term, for K a descendant-or-self of J:
+//   d tau_k / d q_j += S_k . (S_j x* W_K)          (from d S_k = S_j x S_k acting on -W_K)
+// while the strict-ancestor rows keep S_j x* F_K with the INERTIAL F_K, and d tau / d v does not change.  tau itself is
+// S_k . (F_K - W_K).
+//
 // M is then factored per sample as L^T D L with the tree's own sparsity (entry (k, i) only for i an ancestor of k in the
-// chain of velocity coordinates) and every column of both right-hand sides is solved in place.
+// chain of velocity coordinates) and every column of the right-hand sides is solved in place: d ID / dq, d ID / dv and, for
+// d v̇ / d tau = M^-1, the constant columns -e_j.  The inverse-dynamics Jacobians are the pair entries themselves (no solve).
 //
 // Work split (rbd_deriv.cu): world pass = one thread per sample; subtree sums = one thread per (sample, component);
 // pair entries = one thread per (sample, body); factor = one thread per sample; solves = one thread per (sample, column).
@@ -39,6 +46,7 @@ constexpr int kBodyRows = 52;    // Ic (m, h, J: 10), G (36, row-major), F (6)
 struct DerivDev {
   int32_t nb, nv, nnz;           // nnz: stored entries of M / its factor (row p holds depth[p] + 1 of them)
   int32_t dof_base, body_base, h_base, rows;   // scratch rows
+  int32_t w_base;                // rows of W (6 per body, behind M's entries) when the call has external wrenches, else 0
   int16_t pdof0[kMaxBodies + 1]; // preorder body -> its first velocity coordinate in PREORDER numbering
   int16_t vrow[kMaxDofs];        // preorder coordinate -> row of v (reference order)
   int16_t pdof[kMaxDofs];        // row of v -> preorder coordinate
@@ -92,6 +100,11 @@ template <class T> inline bool build_deriv_dev(const ModelDev<T>& M, DerivDev& D
   return true;
 }
 
+// External wrenches: 6 more scratch rows per body (W_i, then the subtree sums W_K).  Without them the layout is unchanged.
+inline void deriv_dev_add_wrenches(DerivDev& D) {
+  D.w_base = D.rows;
+  D.rows += 6 * D.nb;
+}
 // v x* f for a force vector (n, f)
 template <class T> RBD_HD void force_cross(const Mot<T>& v, const T* n, const T* f, T* on, T* of) {
   T a[3], b[3];
@@ -124,12 +137,14 @@ template <class T> RBD_HD void store_mot(T* s, int64_t ld, int row, const Mot<T>
 // ------------------------------------------------------------------------------------------------------------------
 template <class T> struct DerivIO {
   Col<T> q, v, vd;
+  Col<T> wext{nullptr, 0};       // root-frame external wrenches (rows 6 refidx + c, as rbd_dynamics), read when EXT
   T* s;
   int64_t sld;
   bool active;
 };
 
-template <class T, class ST>
+// EXT: also store each body's external wrench W_i in rows D.w_base + 6 i (deriv_dev_add_wrenches)
+template <class T, class ST, bool EXT = false>
 RBD_HD void deriv_world_sample(const ModelDev<T>& M, const DerivDev& D, const DerivIO<T>& io, const ST& st) {
   const int nb = M.nb;
   Pose<T> cur;
@@ -221,6 +236,10 @@ RBD_HD void deriv_world_sample(const ModelDev<T>& M, const DerivDev& D, const De
         io.s[(int64_t)(row + 46 + k) * io.sld] = fn[k] + bn[k];
         io.s[(int64_t)(row + 49 + k) * io.sld] = ff[k] + bf[k];
       }
+      if (EXT) {
+#pragma unroll
+        for (int k = 0; k < 6; ++k) io.s[(int64_t)(D.w_base + 6 * i + k) * io.sld] = io.wext(6 * bd.refidx + k);
+      }
       // G e_c = I (e_c x v) + e_c x* (I v) + v x* (I e_c)
 #pragma unroll
       for (int c = 0; c < 6; ++c) {
@@ -256,7 +275,7 @@ RBD_HD void deriv_world_sample(const ModelDev<T>& M, const DerivDev& D, const De
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// 2. subtree sums of (Ic, G, F): one thread per (sample, component c of the 52)
+// 2. subtree sums of (Ic, G, F): one thread per (sample, component c of the 52); of W: one per (sample, component c of the 6)
 // ------------------------------------------------------------------------------------------------------------------
 template <class T> RBD_HD void deriv_accumulate(const ModelDev<T>& M, const DerivDev& D, T* s, int64_t sld, int c) {
   for (int i = M.nb - 1; i > 0; --i) {
@@ -265,10 +284,18 @@ template <class T> RBD_HD void deriv_accumulate(const ModelDev<T>& M, const Deri
     s[(int64_t)(D.body_base + kBodyRows * par + c) * sld] += s[(int64_t)(D.body_base + kBodyRows * i + c) * sld];
   }
 }
+template <class T> RBD_HD void deriv_accumulate_wrench(const ModelDev<T>& M, const DerivDev& D, T* s, int64_t sld, int c) {
+  for (int i = M.nb - 1; i > 0; --i) {
+    const int par = M.body[i].parent;
+    if (par < 0) continue;
+    s[(int64_t)(D.w_base + 6 * par + c) * sld] += s[(int64_t)(D.w_base + 6 * i + c) * sld];
+  }
+}
 
 // ------------------------------------------------------------------------------------------------------------------
 // 3. pair entries: one thread per (sample, body K).  Writes d tau / dq and d tau / dv into dq / dv (column-major nv x nv like
-//    M.data, rows x batch) and the related entries of M into the scratch.
+//    M.data, rows x batch) and the related entries of M into the scratch.  EXT: with the wrench term (W_K from the scratch).
+//    TAU: also K's rows of tau = ID(q, v, v̇, W).
 // ------------------------------------------------------------------------------------------------------------------
 template <class T> RBD_HD void apply_IG(const Rbi<T>& I, const T* G, const Mot<T>& xi, const Mot<T>& xg, T* y) {
   T n[3], f[3];
@@ -283,13 +310,14 @@ template <class T> RBD_HD void apply_IG(const Rbi<T>& I, const T* G, const Mot<T
   }
 }
 
-template <class T>
-RBD_HD void deriv_pairs(const DerivDev& D, const DerivAnc& A, T* s, int64_t sld, T* dq, T* dv, int64_t ld, int K, bool active) {
+template <class T, bool EXT = false, bool TAU = false>
+RBD_HD void deriv_pairs(const DerivDev& D, const DerivAnc& A, T* s, int64_t sld, T* dq, T* dv, int64_t ld, int K, bool active,
+                        T* tau = nullptr) {
   const int nv = D.nv;
   const int pk0 = D.pdof0[K], nk = D.pdof0[K + 1] - pk0;
   if (nk == 0) return;
   Rbi<T> Ic;
-  T G[36], Fn[3], Ff[3];
+  T G[36], Fn[3], Ff[3], Wn[3], Wf[3];
   {
     const T* p = s + (int64_t)(D.body_base + kBodyRows * K) * sld;
     Ic.m = *p; p += sld;
@@ -303,6 +331,21 @@ RBD_HD void deriv_pairs(const DerivDev& D, const DerivAnc& A, T* s, int64_t sld,
     for (int k = 0; k < 3; ++k) { Fn[k] = *p; p += sld; }
 #pragma unroll
     for (int k = 0; k < 3; ++k) { Ff[k] = *p; p += sld; }
+  }
+  if (EXT) {
+    const T* p = s + (int64_t)(D.w_base + 6 * K) * sld;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) { Wn[k] = p[k * sld]; Wf[k] = p[(3 + k) * sld]; }
+  }
+  if (TAU) {
+    T f[6];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) { f[k] = EXT ? Fn[k] - Wn[k] : Fn[k]; f[3 + k] = EXT ? Ff[k] - Wf[k] : Ff[k]; }
+    for (int kk = 0; kk < nk; ++kk) {
+      Mot<T> Sk;
+      load_mot(s, sld, D.dof_base + kDofRows * (pk0 + kk), Sk);
+      if (active) tau[(int64_t)D.vrow[pk0 + kk] * ld] = dot6(Sk, f);
+    }
   }
   // all coordinates at or above K, deepest first: the ancestor list of K's last coordinate
   const int plast = pk0 + nk - 1, rl = D.rowstart[plast];
@@ -321,17 +364,26 @@ RBD_HD void deriv_pairs(const DerivDev& D, const DerivAnc& A, T* s, int64_t sld,
         pdd.w[k] = t[12 + k]; pdd.l[k] = t[15 + k]; sdp.w[k] = t[18 + k]; sdp.l[k] = t[21 + k];
       }
     }
-    T yq[6], yv[6], ym[6];
+    T yq[6], yv[6], ym[6], yw[6];
     apply_IG(Ic, G, pdd, pd, yq);
     apply_IG(Ic, G, sdp, Sj, yv);
     rbi_mul(Ic, Sj, ym, ym + 3);
+    // K's own rows: yq + S_j x* W_K.  yq itself stays inertial for the strict-ancestor rows below.
+#pragma unroll
+    for (int c = 0; c < 6; ++c) yw[c] = yq[c];
+    if (EXT) {
+      T wn[3], wf[3];
+      force_cross(Sj, Wn, Wf, wn, wf);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) { yw[c] += wn[c]; yw[3 + c] += wf[c]; }
+    }
     const int64_t colj = (int64_t)nv * D.vrow[pj];
     for (int kk = 0; kk < nk; ++kk) {
       const int pk = pk0 + kk;
       Mot<T> Sk;
       load_mot(s, sld, D.dof_base + kDofRows * pk, Sk);
       if (active) {
-        dq[(colj + D.vrow[pk]) * ld] = dot6(Sk, yq);
+        dq[(colj + D.vrow[pk]) * ld] = dot6(Sk, yw);
         dv[(colj + D.vrow[pk]) * ld] = dot6(Sk, yv);
         if (pj <= pk) s[(int64_t)(D.h_base + D.rowstart[pk] + D.depth[pj]) * sld] = dot6(Sk, ym);
       }
@@ -374,17 +426,19 @@ template <class T> RBD_HD void deriv_factor(const DerivDev& D, const DerivAnc& A
 
 // ------------------------------------------------------------------------------------------------------------------
 // 5. one column of  X = -M^-1 R  in place.  x: per-thread vector of nv entries (shared memory, stride XS);
-//    H(row) reads the factor; col: this sample's column of the nv x nv array, rows x batch.
+//    H(row) reads the factor; col: this sample's column of the nv x nv array, rows x batch.  unit: R = -e_vj (a column of
+//    d v̇ / d tau = M^-1; nothing is read), whose only non-zero row is pj itself.
 // ------------------------------------------------------------------------------------------------------------------
 template <class T, class HF>
-RBD_HD void deriv_solve_column(const DerivDev& D, const DerivAnc& A, const HF& H, T* x, int xs, T* col, int64_t ld, int vj, bool active) {
+RBD_HD void deriv_solve_column(const DerivDev& D, const DerivAnc& A, const HF& H, T* x, int xs, T* col, int64_t ld, int vj, bool active,
+                               bool unit = false) {
   const int nv = D.nv;
   const int pj = D.pdof[vj];
-  const int lo = pj, hi = pj + D.dsub[pj];
+  const int lo = pj, hi = unit ? pj + 1 : pj + D.dsub[pj];
   // right-hand side: non-zero only on the subtree and the ancestors of pj
   for (int p = 0; p < nv; ++p) {
     const bool rel = (p >= lo && p < hi) || (pj >= p && pj < p + D.dsub[p]);
-    x[p * xs] = rel ? col[(int64_t)D.vrow[p] * ld] : T(0);
+    x[p * xs] = unit ? (p == pj ? T(-1) : T(0)) : rel ? col[(int64_t)D.vrow[p] * ld] : T(0);
   }
   // L^-T: coordinates push to their ancestors; only the subtree and the ancestor chain of pj carry anything.  The ancestors of
   // one coordinate are distinct, so four read-modify-writes go out together (the compiler cannot know they do not alias).
@@ -408,6 +462,29 @@ RBD_HD void deriv_solve_column(const DerivDev& D, const DerivAnc& A, const HF& H
     for (int d = D.depth[i] - 1; d >= 0; --d) acc -= H(ri + d) * x[A.anc[ri + d] * xs];
     x[i * xs] = acc;
     if (active) col[(int64_t)D.vrow[i] * ld] = -acc;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// 6. inverse-dynamics Jacobians: one thread per (sample, column vj).  Zeroes the rows of dq / dv that deriv_pairs leaves alone
+//    (pairs unrelated in the tree) and, when Mo != NULL, writes column vj of M, both triangles, from the scratch entries.
+// ------------------------------------------------------------------------------------------------------------------
+template <class T>
+RBD_HD void deriv_expand_column(const DerivDev& D, const T* H, int64_t sld, T* dq, T* dv, T* Mo, int64_t ld, int vj, bool active) {
+  const int nv = D.nv;
+  const int pj = D.pdof[vj];
+  for (int vi = 0; vi < nv; ++vi) {
+    const int p = D.pdof[vi];
+    const int64_t o = ((int64_t)vj * nv + vi) * ld;
+    const bool below = p >= pj && p < pj + D.dsub[pj], above = pj >= p && pj < p + D.dsub[p];
+    if (!active) continue;
+    if (!below && !above) {
+      dq[o] = T(0);
+      dv[o] = T(0);
+      if (Mo) Mo[o] = T(0);
+    } else if (Mo) {
+      Mo[o] = below ? H[(int64_t)(D.rowstart[p] + D.depth[pj]) * sld] : H[(int64_t)(D.rowstart[pj] + D.depth[p]) * sld];
+    }
   }
 }
 

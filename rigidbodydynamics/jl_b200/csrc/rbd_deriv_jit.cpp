@@ -6,6 +6,8 @@
 // live in REGISTERS (x<u>_<p> are scalars), each entry of the factor is read from shared memory once per `cg` columns, and the
 // two sweeps are straight-line fused multiply-adds.  The factorisation itself stays the table-driven cooperative loop (its
 // tables become __constant__ arrays of the module).  Same arithmetic, same operation order per column as deriv_solve_column.
+// With a third block (plan.blocks == 3) the columns 2 nv .. 3 nv - 1 solve the constant right-hand sides -e_j (d v̇ / d tau =
+// M^-1, into dtau); nothing is loaded for them.  With two blocks the text is exactly that of the two-block kernel alone.
 #include "rbd_deriv_jit.h"
 
 #include <algorithm>
@@ -14,14 +16,15 @@
 
 namespace rbd {
 
-bool deriv_jit_plan(const DerivDev& D, bool f64, DerivJitPlan& plan) {
+bool deriv_jit_plan(const DerivDev& D, bool f64, DerivJitPlan& plan, int blocks) {
   const int words = f64 ? 2 : 1;                     // 32-bit registers per scalar
   const int budget = f64 ? 150 : 110;                // registers for right-hand sides (measured: Atlas fp64 2 columns, fp32 3)
   int cg = budget / (D.nv * words);
   if (cg < 1) return false;
   if (cg > 4) cg = 4;
   if (const char* e = std::getenv("RBD_DERIV_CG")) cg = std::max(1, std::min(cg, std::atoi(e)));     // experiments
-  const int ncols = 2 * D.nv;
+  const int ncols = blocks * D.nv;
+  plan.blocks = blocks;
   plan.cg = cg;
   plan.ngroups = (ncols + cg - 1) / cg;
   const int wmax = 12;
@@ -60,8 +63,11 @@ void deriv_jit_source(const DerivDev& D, const DerivAnc& A, bool f64, const Deri
     s += b;
   }
   s += "};\n";
-  add("extern \"C\" __global__ void __launch_bounds__(32 * NW, 1) rbd_deriv_solve(const T* __restrict__ Hg0, long long sld, T* dq, T* dv,\n"
-      "                                                                     long long ld, long long C) {\n"
+  const bool tau = plan.blocks == 3;
+  add("extern \"C\" __global__ void __launch_bounds__(32 * NW, 1) rbd_deriv_solve(const T* __restrict__ Hg0, long long sld, T* dq, T* dv,\n");
+  add(tau ? "                                                                     long long ld, long long C, T* dtau) {\n"
+          : "                                                                     long long ld, long long C) {\n");
+  add(
       "  extern __shared__ __align__(16) unsigned char smem_raw[];\n"
       "  T* Hs = reinterpret_cast<T*>(smem_raw) + (threadIdx.x & 31);\n"
       "  const int w = threadIdx.x >> 5;\n"
@@ -91,6 +97,30 @@ void deriv_jit_source(const DerivDev& D, const DerivAnc& A, bool f64, const Deri
       "    const volatile T* Hv = Hs;\n"
       "    for (int cgi = w; cgi < NGRP; cgi += NW) {\n");
   for (int u = 0; u < cg; ++u) {
+    if (tau) {
+      // the unit columns: mask = {pj}, the right-hand side -1 there (bits of p and pj in the same word compare as the loads below)
+      snprintf(b, sizeof b,
+               "      const int c%d = cgi * CG + %d;\n"
+               "      const bool ok%d = active && c%d < 3 * NV;\n"
+               "      const int cc%d = c%d < 3 * NV ? c%d : 3 * NV - 1;\n"
+               "      const bool e%d = cc%d >= 2 * NV;\n"
+               "      const int vj%d = cc%d < NV ? cc%d : (e%d ? cc%d - 2 * NV : cc%d - NV);\n"
+               "      T* col%d = (cc%d < NV ? dq : e%d ? dtau : dv) + (long long)vj%d * NV * ld + bl;\n",
+               u, u, u, u, u, u, u, u, u, u, u, u, u, u, u, u, u, u, u);
+      add(b);
+      snprintf(b, sizeof b,
+               "      const int pj%d = kPdof[vj%d];\n"
+               "      const unsigned long long ml%d = e%d ? (pj%d < 64 ? 1ull << pj%d : 0ull) : kRel[pj%d][0],\n"
+               "                               mh%d = e%d ? (pj%d >= 64 ? 1ull << (pj%d - 64) : 0ull) : kRel[pj%d][1];\n",
+               u, u, u, u, u, u, u, u, u, u, u, u);
+      add(b);
+      for (int p = 0; p < nv; ++p) {
+        snprintf(b, sizeof b, "      T x%d_%d = ((%s%d >> %d) & 1ull) ? (e%d ? T(-1) : col%d[%dll * ld]) : T(0);\n", u, p, p < 64 ? "ml" : "mh", u,
+                 p & 63, u, u, (int)D.vrow[p]);
+        add(b);
+      }
+      continue;
+    }
     snprintf(b, sizeof b,
              "      const int c%d = cgi * CG + %d;\n"
              "      const bool ok%d = active && c%d < 2 * NV;\n"
