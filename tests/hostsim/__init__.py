@@ -1,31 +1,78 @@
-"""TEST INFRASTRUCTURE: runs the device algorithms of csrc/rbd_device.cuh on the CPU (see hostsim.cpp)."""
-import ctypes, os, subprocess
+"""TEST INFRASTRUCTURE: runs the device algorithms of csrc/rbd_device.cuh on the CPU (see hostsim.cpp).
+
+Every host library of the CPU tier (the shims tests/hostsim/<name>.cpp, the specialised programs of SpecProgram) is compiled
+into one per-user cache, <tempdir>/rbd_hostsim_<uid>/, under a key hashed from the compiler argv, the bytes of every compiled
+file and of every header it can include (csrc/*.h, csrc/*.cuh, include/rbd_b200.h), and the generated text."""
+import ctypes, functools, hashlib, os, subprocess, tempfile
 import numpy as np
 from rigidbodydynamics.jl_b200._cabi import RbdModelDesc, make_desc
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-_CSRC = os.path.join(_HERE, "..", "..", "rigidbodydynamics", "jl_b200", "csrc")
-_LIB = os.path.join(_HERE, "libhostsim.so")
+_ROOT = os.path.dirname(os.path.dirname(_HERE))
+_CSRC = os.path.join(_ROOT, "rigidbodydynamics", "jl_b200", "csrc")
+SHIM_FLAGS = ["-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas"]
+# the specialised programs are the bit-for-bit reference of the fp32 kernels: no contraction into FMAs the generator did not plan
+SPEC_FLAGS = ["-O1", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-ffp-contract=off", "-I", _CSRC]
 
 
-def build(force=False):
-    srcs = [os.path.join(_HERE, "hostsim.cpp")] + [os.path.join(_CSRC, f) for f in os.listdir(_CSRC)
-                                                   if f.endswith((".cuh", ".h", ".cpp"))]
-    if force or not os.path.exists(_LIB) or any(os.path.getmtime(s) > os.path.getmtime(_LIB) for s in srcs):
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-o", _LIB,
-                               os.path.join(_HERE, "hostsim.cpp"), os.path.join(_CSRC, "rbd_model.cpp"),
-                               os.path.join(_CSRC, "rbd_codegen.cpp")])
-    return _LIB
+def cache_dir():
+    return os.path.join(tempfile.gettempdir(), f"rbd_hostsim_{os.getuid()}")
 
 
-_lib = None
+def headers():
+    """Every header a host library can include."""
+    return sorted(os.path.join(_CSRC, f) for f in os.listdir(_CSRC) if f.endswith((".h", ".cuh"))) + [
+        os.path.join(_ROOT, "include", "rbd_b200.h")]
+
+
+def _read(path):
+    with open(path, "rb") as f:
+        return f.read()
+
+
+def compile_lib(flags, srcs=(), text=None):
+    """g++ ``flags`` over ``srcs`` plus, if given, the generated C++ ``text``, into the cache; returns the library's path."""
+    argv = ["g++", *flags, *srcs]
+    h = hashlib.sha1("\0".join(argv).encode())
+    for f in [*srcs, *headers()]:
+        data = _read(f)
+        h.update(b"%s\0%d\0" % (f.encode(), len(data)) + data)
+    if text is not None:
+        h.update(text.encode())
+    name = os.path.splitext(os.path.basename(srcs[0]))[0] if srcs else "spec"
+    stem = os.path.join(cache_dir(), f"{name}_{h.hexdigest()[:16]}")
+    if not os.path.exists(stem + ".so"):
+        os.makedirs(cache_dir(), exist_ok=True)
+        tmp = f"{stem}.{os.getpid()}"
+        if text is not None:
+            with open(tmp + ".cpp", "w") as f:
+                f.write(text)
+            argv.append(tmp + ".cpp")
+        subprocess.check_call(argv + ["-o", tmp + ".so"])
+        if text is not None:
+            os.replace(tmp + ".cpp", stem + ".cpp")
+        os.replace(tmp + ".so", stem + ".so")
+    return stem + ".so"
+
+
+_load = functools.cache(ctypes.CDLL)
+
+
+def build(name="hostsim"):
+    """tests/hostsim/<name>.cpp linked with csrc/rbd_model.cpp (and rbd_codegen.cpp for hostsim.cpp), compiled into the cache;
+    returns the library's path."""
+    extra = ["rbd_model.cpp"] + (["rbd_codegen.cpp"] if name == "hostsim" else [])
+    return compile_lib(SHIM_FLAGS, [os.path.join(_HERE, name + ".cpp")] + [os.path.join(_CSRC, f) for f in extra])
+
+
+@functools.cache
+def shim(name):
+    """The loaded library of tests/hostsim/<name>.cpp; its caller declares the argtypes of the functions it calls."""
+    return _load(build(name))
 
 
 def lib():
-    global _lib
-    if _lib is None:
-        _lib = ctypes.CDLL(build())
-    return _lib
+    return shim("hostsim")
 
 
 def _p(a):
@@ -162,18 +209,20 @@ def flags(desc):
     return list(out)
 
 
-SPEC_STATS = ("nodes_traced", "nodes_live", "add", "mul", "div", "neg", "sincos", "load", "store", "sld", "sst", "stash_rows")
+SPEC_STATS = ("nodes_traced", "nodes_live", "add", "mul", "div", "neg", "sincos", "load", "store", "sld", "sst", "stash_rows",
+              "fold_loops", "fold_bodies", "pairs")
 
 
-def spec_source(desc, algo="aba", dtype=np.float64, has_in2=True, has_out1=False, flavor=0):
-    """Source text + statistics of the model-specialised program csrc/rbd_codegen.cpp generates for this mechanism."""
+def spec_source(desc, algo="aba", dtype=np.float64, has_in2=True, has_out1=False, flavor=0, *, fold=True):
+    """Source text + statistics of the model-specialised program csrc/rbd_codegen.cpp generates for this mechanism.  ``fold`` =
+    False keeps mirror-image chains straight-line (flavours 0-2)."""
     d, keep = make_desc(desc)
     fn = lib().hostsim_spec_source
     fn.restype = ctypes.c_void_p
-    fn.argtypes = [ctypes.POINTER(RbdModelDesc)] + [ctypes.c_int] * 5 + [ctypes.c_void_p]
-    stats = (ctypes.c_int * 12)()
+    fn.argtypes = [ctypes.POINTER(RbdModelDesc)] + [ctypes.c_int] * 6 + [ctypes.c_void_p]
+    stats = (ctypes.c_int * len(SPEC_STATS))()
     p = fn(ctypes.byref(d), {"aba": 0, "rnea": 1, "crba": 2, "kin": 3}[algo], 0 if np.dtype(dtype) == np.float32 else 1, int(has_in2),
-           int(has_out1), flavor, stats)
+           int(has_out1), flavor, int(fold), stats)
     assert p, "specialisation failed"
     src = ctypes.string_at(p).decode()
     lib().hostsim_free.argtypes = [ctypes.c_void_p]
@@ -192,22 +241,10 @@ def spec_kin(mask, sign=None, nb=0):
 class SpecProgram:
     """The specialised program compiled for the CPU (g++) -- the same straight-line code the NVRTC kernels run."""
 
-    def __init__(self, desc, algo="aba", dtype=np.float64, has_in2=True, has_out1=False):
-        import hashlib, tempfile
+    def __init__(self, desc, algo="aba", dtype=np.float64, has_in2=True, has_out1=False, *, fold=True):
         self.desc, self.algo, self.dtype = desc, algo, np.dtype(dtype)
-        src, self.stats = spec_source(desc, algo, dtype, has_in2, has_out1, 0)
-        tag = hashlib.sha1(src.encode()).hexdigest()[:16]
-        d = os.path.join(tempfile.gettempdir(), "rbd_spec_cpu")
-        os.makedirs(d, exist_ok=True)
-        so = os.path.join(d, f"spec_{tag}.so")
-        if not os.path.exists(so):
-            cpp = os.path.join(d, f"spec_{tag}.cpp")
-            with open(cpp, "w") as f:
-                f.write(src)
-            subprocess.check_call(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-ffp-contract=off",
-                                   "-I", _CSRC, "-o", so + ".tmp", cpp])
-            os.replace(so + ".tmp", so)
-        self.fn = ctypes.CDLL(so).rbd_spec_cpu
+        self.src, self.stats = spec_source(desc, algo, dtype, has_in2, has_out1, 0, fold=fold)
+        self.fn = _load(compile_lib(SPEC_FLAGS, text=self.src)).rbd_spec_cpu
         self.fn.argtypes = [ctypes.c_void_p] * 5 + [ctypes.c_longlong, ctypes.c_void_p] + ([ctypes.c_void_p] if algo == "kin" else [])
         self.has_in2, self.has_out1 = has_in2, has_out1
 

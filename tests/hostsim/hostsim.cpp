@@ -179,8 +179,9 @@ void run_integrate(const HostModel& hm, int64_t B, T* q, T* v, const T* tau, dou
 
 extern "C" {
 // Model-specialised program (csrc/rbd_codegen.cpp) for the mechanism: flavor 0 = self-contained C++ (one sample per call),
-// 1 = the per-sample CUDA function body, 3 = the whole NVRTC translation unit.  Returns a malloc'ed string (free with
-// hostsim_free) or NULL; stats = {nodes_traced, nodes_live, add, mul, div, neg, sincos, load, store, sld, sst, stash_rows}.
+// 1 = the per-sample CUDA function body, 3 = the whole NVRTC translation unit; fold = 0 keeps mirror-image chains straight-line
+// (flavours 0-2).  Returns a malloc'ed string (free with hostsim_free) or NULL; stats = {nodes_traced, nodes_live, add, mul, div,
+// neg, sincos, load, store, sld, sst, stash_rows, fold_loops, fold_bodies, pairs}.
 // kin_mask / kin_sign (reference joint order, may be NULL): the rbd_kinematics variant (algo 3)
 static int g_kin_mask = 0;
 static int8_t g_kin_sign[rbd::kMaxBodies] = {0};
@@ -188,7 +189,8 @@ void hostsim_spec_kin(int mask, const int8_t* sign, int nb) {
   g_kin_mask = mask;
   for (int i = 0; i < rbd::kMaxBodies; ++i) g_kin_sign[i] = (sign && i < nb) ? sign[i] : 0;
 }
-char* hostsim_spec_source(const rbd_model_desc* d, int algo, int dtype, int has_in2, int has_out1, int flavor, int* stats) {
+char* hostsim_spec_source(const rbd_model_desc* d, int algo, int dtype, int has_in2, int has_out1, int flavor, int fold,
+                          int* stats) {
   HostModel hm; std::string err;
   if (build_host_model(d, hm, err) != RBD_OK) return nullptr;
   SpecKey key; key.algo = algo; key.f64 = dtype == 1; key.has_in2 = (has_in2 & 1) != 0; key.has_out1 = has_out1 != 0;
@@ -199,14 +201,14 @@ char* hostsim_spec_source(const rbd_model_desc* d, int algo, int dtype, int has_
   }
   SpecStats st; std::string out;
   bool ok;
-  if (flavor == 0) ok = spec_emit_cpu_tu(hm, key, "rbd_spec_cpu", out, &st, err);
+  if (flavor == 0) ok = spec_emit_cpu_tu(hm, key, "rbd_spec_cpu", out, &st, err, fold != 0);
   else if (flavor == 3) ok = spec_emit_cuda_tu(hm, key, out, &st, err);
-  else ok = spec_emit_function(hm, key, flavor, "rbd_spec_fn", out, &st, err);
+  else ok = spec_emit_function(hm, key, flavor, "rbd_spec_fn", out, &st, err, fold != 0);
   if (!ok) return nullptr;
   if (stats) {
-    const int v[12] = {st.nodes_traced, st.nodes_live, st.n_add, st.n_mul, st.n_div, st.n_neg, st.n_sincos, st.n_load, st.n_store,
-                       st.n_sld, st.n_sst, st.stash_rows};
-    for (int k = 0; k < 12; ++k) stats[k] = v[k];
+    const int v[15] = {st.nodes_traced, st.nodes_live, st.n_add, st.n_mul, st.n_div, st.n_neg, st.n_sincos, st.n_load, st.n_store,
+                       st.n_sld, st.n_sst, st.stash_rows, st.n_fold_loops, st.n_fold_bodies, (int)hm.pairs.size()};
+    for (int k = 0; k < 15; ++k) stats[k] = v[k];
   }
   char* r = (char*)malloc(out.size() + 1);
   std::memcpy(r, out.c_str(), out.size() + 1);

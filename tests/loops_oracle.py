@@ -13,10 +13,7 @@ tests/hostsim/hostsim_loops.cpp (the kernel's per-sample function compiled for t
 from __future__ import annotations
 
 import ctypes
-import hashlib
-import os
-import subprocess
-import tempfile
+import functools
 
 import numpy as np
 import scipy.linalg as sla
@@ -26,6 +23,7 @@ from oracle import Oracle
 from rigidbodydynamics.jl_b200._cabi import RbdModelDesc, make_desc
 from rigidbodydynamics.jl_b200.loops import _DEFAULT, constraint_wrench_subspace, loop_desc
 from rigidbodydynamics.jl_b200.spatial import SpatialInertia, Transform3D
+from tests import hostsim
 
 RCOND = 1e-10       # singular_value_zero_tolerance, mechanism_algorithms.jl:804
 
@@ -249,32 +247,13 @@ def body_accelerations(lo, q, v, vd):
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
-# loops_sample on the CPU (tests/hostsim/hostsim_loops.cpp), compiled on first use into a temporary directory
+# loops_sample on the CPU (tests/hostsim/hostsim_loops.cpp, compiled and loaded by hostsim.shim)
 # ------------------------------------------------------------------------------------------------------------------------------
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_CSRC = os.path.join(_HERE, "..", "rigidbodydynamics", "jl_b200", "csrc")
-_hl = None
-
-
+@functools.cache
 def _hostsim_loops():
-    global _hl
-    if _hl is not None:
-        return _hl
-    srcs = [os.path.join(_HERE, "hostsim", "hostsim_loops.cpp")] + sorted(
-        os.path.join(_CSRC, f) for f in os.listdir(_CSRC) if f.endswith((".cuh", ".h")) or f == "rbd_model.cpp")
-    srcs.append(os.path.join(_HERE, "..", "include", "rbd_b200.h"))
-    h = hashlib.sha1(b"".join(open(s, "rb").read() for s in srcs)).hexdigest()[:16]
-    d = os.path.join(tempfile.gettempdir(), f"rbd_hostsim_loops_{os.getuid()}")
-    os.makedirs(d, exist_ok=True)
-    so = os.path.join(d, f"hostsim_loops_{h}.so")
-    if not os.path.exists(so):
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-o", so + f".{os.getpid()}",
-                               srcs[0], os.path.join(_CSRC, "rbd_model.cpp")])
-        os.replace(so + f".{os.getpid()}", so)
-    lib = ctypes.CDLL(so)
+    lib = hostsim.shim("hostsim_loops")
     lib.hostsim_dynamics_loops.argtypes = [ctypes.POINTER(RbdModelDesc), ctypes.c_void_p, ctypes.c_int, ctypes.c_int64] + \
         [ctypes.c_void_p] * 9
-    _hl = lib
     return lib
 
 

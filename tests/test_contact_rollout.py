@@ -10,10 +10,7 @@ The kernel's per-stage device code (contact_stage_pass + aba_sample, compiled fo
 must agree with the oracle's contact_dynamics + dynamics at random stage states, and the GPU rollout with the oracle integrator.
 """
 import ctypes
-import hashlib
-import os
-import subprocess
-import tempfile
+import functools
 
 import numpy as np
 import pytest
@@ -22,13 +19,11 @@ import rigidbodydynamics.jl_b200 as rbd
 from oracle import Oracle
 from rigidbodydynamics.jl_b200 import _cabi
 from rigidbodydynamics.jl_b200._cabi import RbdModelDesc, make_desc
+from tests import hostsim
 from tests.contact_oracle import integrate_contact
 from tests.test_contact import _free_body, _with_contacts
 from tests.util import config_distance, rand_inputs, randmech, rel_err
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_CSRC = os.path.join(_HERE, "..", "rigidbodydynamics", "jl_b200", "csrc")
-_lib = None
 
 TOL64 = 1e-9          # GPU rollout against the fp64 oracle integrator, relative (rel_err)
 # fp32 rollout against the fp64 oracle, 5 steps at dt = 1e-3.  Measured on an H100: 9.7e-6 (q) / 9.4e-6 (v) on the random tree,
@@ -37,26 +32,13 @@ TOL64 = 1e-9          # GPU rollout against the fp64 oracle integrator, relative
 TOL32 = 2e-3
 
 
+@functools.cache
 def _shim():
-    """tests/hostsim/hostsim_contact_rollout.cpp, compiled on first use into a temporary directory."""
-    global _lib
-    if _lib is not None:
-        return _lib
-    srcs = [os.path.join(_HERE, "hostsim", "hostsim_contact_rollout.cpp")] + sorted(
-        os.path.join(_CSRC, f) for f in os.listdir(_CSRC) if f.endswith((".cuh", ".h")) or f == "rbd_model.cpp")
-    h = hashlib.sha1(b"".join(open(s, "rb").read() for s in srcs)).hexdigest()[:16]
-    d = os.path.join(tempfile.gettempdir(), f"rbd_hostsim_contact_rollout_{os.getuid()}")
-    os.makedirs(d, exist_ok=True)
-    so = os.path.join(d, f"hostsim_contact_rollout_{h}.so")
-    if not os.path.exists(so):
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-o", so + f".{os.getpid()}",
-                               srcs[0], os.path.join(_CSRC, "rbd_model.cpp")])
-        os.replace(so + f".{os.getpid()}", so)
-    lib = ctypes.CDLL(so)
+    """tests/hostsim/hostsim_contact_rollout.cpp, compiled and loaded by hostsim.shim."""
+    lib = hostsim.shim("hostsim_contact_rollout")
     vp = ctypes.c_void_p
     lib.hostsim_contact_stage.argtypes = [ctypes.POINTER(RbdModelDesc), ctypes.c_int, ctypes.c_int64, vp, vp, vp, vp, vp, vp,
                                           ctypes.c_double, vp, vp]
-    _lib = lib
     return lib
 
 

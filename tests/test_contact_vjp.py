@@ -6,10 +6,7 @@ CPU tier: the adjoint of the force law against central differences, branch by br
 (tests/hostsim/hostsim_contact_vjp.cpp) against central differences of the fp64 oracle integrator (tests/contact_oracle.py) along
 random directions of q (as q̇(u)), v, s and the torques.  GPU tier: the kernels against that CPU run and the torch.autograd function."""
 import ctypes
-import hashlib
-import os
-import subprocess
-import tempfile
+import functools
 
 import numpy as np
 import pytest
@@ -18,6 +15,7 @@ import rigidbodydynamics.jl_b200 as rbd
 from oracle import Oracle
 from rigidbodydynamics.jl_b200 import _cabi
 from rigidbodydynamics.jl_b200._cabi import RbdModelDesc, make_desc
+from tests import hostsim
 from tests.contact_oracle import integrate_contact
 from tests.test_contact import _free_body, _with_contacts
 from tests.test_contact_rollout import _atlas_on_floor, _atlas_states, _empty_desc
@@ -36,33 +34,16 @@ TOL64_STIFF = 1e-8
 TOL32 = 2e-2
 DT = 1e-3
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_CSRC = os.path.join(_HERE, "..", "rigidbodydynamics", "jl_b200", "csrc")
-_lib = None
 
-
+@functools.cache
 def _shim():
-    """tests/hostsim/hostsim_contact_vjp.cpp, compiled on first use into a temporary directory."""
-    global _lib
-    if _lib is not None:
-        return _lib
-    srcs = [os.path.join(_HERE, "hostsim", "hostsim_contact_vjp.cpp")] + sorted(
-        os.path.join(_CSRC, f) for f in os.listdir(_CSRC) if f.endswith((".cuh", ".h")) or f == "rbd_model.cpp")
-    h = hashlib.sha1(b"".join(open(s, "rb").read() for s in srcs)).hexdigest()[:16]
-    d = os.path.join(tempfile.gettempdir(), f"rbd_hostsim_contact_vjp_{os.getuid()}")
-    os.makedirs(d, exist_ok=True)
-    so = os.path.join(d, f"hostsim_contact_vjp_{h}.so")
-    if not os.path.exists(so):
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-o", so + f".{os.getpid()}",
-                               srcs[0], os.path.join(_CSRC, "rbd_model.cpp")])
-        os.replace(so + f".{os.getpid()}", so)
-    lib = ctypes.CDLL(so)
+    """tests/hostsim/hostsim_contact_vjp.cpp, compiled and loaded by hostsim.shim."""
+    lib = hostsim.shim("hostsim_contact_vjp")
     vp, i64, c_int, c_double = ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_double
     lib.hostsim_integrate_contact_vjp.argtypes = [ctypes.POINTER(RbdModelDesc), c_int, i64, vp, vp, vp, vp, i64, i64, vp, c_double,
                                                   c_int] + [vp] * 8
     lib.hostsim_contact_force.argtypes = [vp, vp, vp, c_double, vp, vp, vp, vp]
     lib.hostsim_contact_force_adjoint.argtypes = [vp, vp, vp, c_double] + [vp] * 7
-    _lib = lib
     return lib
 
 

@@ -7,10 +7,8 @@ whose products with any cotangent the Jacobians must reproduce.
 CPU tier: the per-sample device functions compiled for the host (tests/hostsim/hostsim_deriv_ext.cpp), the NVRTC generator and the
 argument checks.  GPU tier: the kernels through the C ABI on every path, fp32, and the Python wrappers."""
 import ctypes
-import hashlib
+import functools
 import os
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
@@ -35,30 +33,12 @@ TOL_CPU = 1e-10       # GPU against the CPU run of the same per-sample code, fp6
 TOL32_ID = 1e-5
 TOL32_TOOLS = 4e-3
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_CSRC = os.path.join(_HERE, "..", "rigidbodydynamics", "jl_b200", "csrc")
-_lib = None
 
-
+@functools.cache
 def _shim():
-    """tests/hostsim/hostsim_deriv_ext.cpp, compiled on first use into a temporary directory."""
-    global _lib
-    if _lib is not None:
-        return _lib
-    srcs = [os.path.join(_HERE, "hostsim", "hostsim_deriv_ext.cpp")] + sorted(
-        os.path.join(_CSRC, f) for f in os.listdir(_CSRC) if f.endswith((".cuh", ".h")) or f == "rbd_model.cpp")
-    srcs.append(os.path.join(_HERE, "..", "include", "rbd_b200.h"))
-    h = hashlib.sha1(b"".join(open(s, "rb").read() for s in srcs)).hexdigest()[:16]
-    d = os.path.join(tempfile.gettempdir(), f"rbd_hostsim_deriv_ext_{os.getuid()}")
-    os.makedirs(d, exist_ok=True)
-    so = os.path.join(d, f"hostsim_deriv_ext_{h}.so")
-    if not os.path.exists(so):
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-o", so + f".{os.getpid()}",
-                               srcs[0], os.path.join(_CSRC, "rbd_model.cpp")])
-        os.replace(so + f".{os.getpid()}", so)
-    lib = ctypes.CDLL(so)
+    """tests/hostsim/hostsim_deriv_ext.cpp, compiled and loaded by hostsim.shim."""
+    lib = hostsim.shim("hostsim_deriv_ext")
     lib.hostsim_deriv_ext.argtypes = [ctypes.POINTER(RbdModelDesc), ctypes.c_int, ctypes.c_int, ctypes.c_int64] + [ctypes.c_void_p] * 9
-    _lib = lib
     return lib
 
 

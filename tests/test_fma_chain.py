@@ -16,7 +16,7 @@ import torch
 import rigidbodydynamics.jl_b200 as rbd
 from oracle import Oracle
 from tests import hostsim
-from tests.test_fold import _check_bit_identical, _source, shim  # noqa: F401  (shim: the fold shim fixture)
+from tests.test_fold import _check_bit_identical
 from tests.test_reg_stash import _models
 from tests.util import axis_aligned_tree, rand_inputs, rel_err
 
@@ -76,17 +76,17 @@ def test_no_add_of_two_single_use_products_cpu(built, monkeypatch):
 
 @pytest.mark.parametrize("cap", ["0", "4"])
 @pytest.mark.parametrize("name", ["atlas", "valkyrie", "mirrored"])
-def test_folded_equals_straight_line_cpu(shim, monkeypatch, name, cap):  # noqa: F811
+def test_folded_equals_straight_line_cpu(built, monkeypatch, name, cap):
     monkeypatch.delenv("RBD_JIT_FMA_CHAIN", raising=False)
     monkeypatch.setenv("RBD_JIT_FMA_CAP", cap)
-    _check_bit_identical(shim, MODELS[name], np.float32, True)
+    _check_bit_identical(MODELS[name], np.float32, True)
 
 
 @pytest.mark.parametrize("cap", ["0", "4"])
-def test_atlas_still_folds_cpu(shim, monkeypatch, cap):  # noqa: F811
+def test_atlas_still_folds_cpu(built, monkeypatch, cap):
     monkeypatch.delenv("RBD_JIT_FMA_CHAIN", raising=False)
     monkeypatch.setenv("RBD_JIT_FMA_CAP", cap)
-    _, st = _source(shim, rbd.load_model("atlas", floating=True).flatten(), np.float32, True)
+    _, st = hostsim.spec_source(rbd.load_model("atlas", floating=True).flatten(), "aba", np.float32)
     assert st["fold_loops"] == 6 and st["fold_bodies"] == 39
 
 

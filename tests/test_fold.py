@@ -4,84 +4,26 @@ The left / right legs and arms of a humanoid run the same code with different mo
 pair's steps once per ABA pass, as a two-iteration loop.  CPU tier: the folded program's CPU flavour is bit-identical to the
 straight-line form of the same trace, the bundled humanoids actually fold, and a pair whose chains differ in a joint's fast
 class stays straight-line."""
-import ctypes
-import os
-import subprocess
-import tempfile
-
 import numpy as np
 import pytest
 
 import rigidbodydynamics.jl_b200 as rbd
-from rigidbodydynamics.jl_b200._cabi import RbdModelDesc, make_desc
+from tests import hostsim
 from tests.util import rand_inputs
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_CSRC = os.path.join(_HERE, "..", "rigidbodydynamics", "jl_b200", "csrc")
 
-
-@pytest.fixture(scope="module")
-def shim():
-    d = tempfile.mkdtemp(prefix="rbd_fold_")
-    so = os.path.join(d, "libfold.so")
-    subprocess.check_call(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-I", _CSRC, "-o", so,
-                           os.path.join(_HERE, "hostsim", "hostsim_fold.cpp"), os.path.join(_CSRC, "rbd_model.cpp"),
-                           os.path.join(_CSRC, "rbd_codegen.cpp")])
-    lib = ctypes.CDLL(so)
-    lib.fold_spec_source.restype = ctypes.c_void_p
-    lib.fold_spec_source.argtypes = [ctypes.POINTER(RbdModelDesc), ctypes.c_int, ctypes.c_int, ctypes.c_int, ctypes.c_int,
-                                     ctypes.c_void_p]
-    lib.fold_free.argtypes = [ctypes.c_void_p]
-    return lib, d
-
-
-def _source(shim, desc, dtype, fold, has_in2=True, has_out1=False):
-    lib, _ = shim
-    d, keep = make_desc(desc)
-    st = (ctypes.c_int * 4)()
-    p = lib.fold_spec_source(ctypes.byref(d), 0 if dtype == np.float32 else 1, int(has_in2), int(has_out1), int(fold), st)
-    assert p
-    src = ctypes.string_at(p).decode()
-    lib.fold_free(p)
-    return src, dict(zip(("nodes_live", "fold_loops", "fold_bodies", "pairs"), st))
-
-
-def _run(shim, src, desc, dtype, q, v, tau, has_out1=False):
-    _, d = shim
-    import hashlib
-    tag = hashlib.sha1(src.encode()).hexdigest()[:16]
-    so = os.path.join(d, f"spec_{tag}.so")
-    if not os.path.exists(so):
-        cpp = os.path.join(d, f"spec_{tag}.cpp")
-        with open(cpp, "w") as f:
-            f.write(src)
-        subprocess.check_call(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-ffp-contract=off",
-                               "-I", _CSRC, "-o", so, cpp])
-    fn = ctypes.CDLL(so).rbd_spec_cpu
-    fn.argtypes = [ctypes.c_void_p] * 5 + [ctypes.c_longlong, ctypes.c_void_p]
-    q = np.ascontiguousarray(q, dtype); v = np.ascontiguousarray(v, dtype); tau = np.ascontiguousarray(tau, dtype)
-    B = q.shape[1]
-    vd = np.full((desc.nv, B), np.nan, dtype)
-    qd = np.full((desc.nq, B), np.nan, dtype) if has_out1 else None
-    sh = np.zeros(4096, dtype)
-    es = np.dtype(dtype).itemsize
-    for b in range(B):
-        fn(q.ctypes.data + b * es, v.ctypes.data + b * es, tau.ctypes.data + b * es, vd.ctypes.data + b * es,
-           None if qd is None else qd.ctypes.data + b * es, B, sh.ctypes.data)
-    return vd, qd
-
-
-def _check_bit_identical(shim, mech, dtype, expect_fold):
+def _check_bit_identical(mech, dtype, expect_fold):
     desc = mech.flatten()
     q, v, tau, _, _ = rand_inputs(mech, 16, 3)
     for has_out1 in (False, True):
-        src0, st0 = _source(shim, desc, dtype, False, has_out1=has_out1)
-        src1, st1 = _source(shim, desc, dtype, True, has_out1=has_out1)
+        p0, p1 = (hostsim.SpecProgram(desc, "aba", dtype, True, has_out1, fold=fold) for fold in (False, True))
+        st0, src1, st1 = p0.stats, p1.src, p1.stats
         assert st0["fold_loops"] == 0
         if expect_fold:
             assert st1["fold_loops"] > 0 and st1["fold_bodies"] > 0 and "rbd_it" in src1
-        a, qa = _run(shim, src0, desc, dtype, q, v, tau, has_out1)
-        b, qb = _run(shim, src1, desc, dtype, q, v, tau, has_out1)
+        a, b = p0.run(q, v, tau), p1.run(q, v, tau)
+        if has_out1:
+            (a, qa), (b, qb) = a, b
         assert np.isfinite(a).all() and np.array_equal(a, b)
         if has_out1:
             assert np.array_equal(qa, qb)
@@ -90,8 +32,8 @@ def _check_bit_identical(shim, mech, dtype, expect_fold):
 
 @pytest.mark.parametrize("dtype", [np.float32, np.float64])
 @pytest.mark.parametrize("name", ["atlas", "valkyrie"])
-def test_humanoid_program_folds_bit_identical(shim, name, dtype):
-    st = _check_bit_identical(shim, rbd.load_model(name, floating=True), dtype, True)
+def test_humanoid_program_folds_bit_identical(name, dtype):
+    st = _check_bit_identical(rbd.load_model(name, floating=True), dtype, True)
     assert st["pairs"] == 2                       # legs and arms
     assert st["fold_loops"] >= 4 and st["fold_bodies"] >= 4 * 6
 
@@ -133,16 +75,16 @@ def _mirrored_tree(seed, spoil=False):
 
 
 @pytest.mark.parametrize("dtype", [np.float32, np.float64])
-def test_mirrored_random_chains_fold_bit_identical(shim, dtype):
+def test_mirrored_random_chains_fold_bit_identical(dtype):
     for seed in (1, 2):
-        st = _check_bit_identical(shim, _mirrored_tree(seed), dtype, True)
+        st = _check_bit_identical(_mirrored_tree(seed), dtype, True)
         assert st["pairs"] == 1 and st["fold_loops"] == 3 and st["fold_bodies"] == 3 * 4
 
 
-def test_mismatched_fast_class_stays_straight_line(shim):
+def test_mismatched_fast_class_stays_straight_line():
     mech = _mirrored_tree(1, spoil=True)
     desc = mech.flatten()
-    src0, st0 = _source(shim, desc, np.float32, False)
-    src1, st1 = _source(shim, desc, np.float32, True)
+    src0, st0 = hostsim.spec_source(desc, "aba", np.float32, fold=False)
+    src1, st1 = hostsim.spec_source(desc, "aba", np.float32, fold=True)
     assert st1["pairs"] == 0 and st1["fold_loops"] == 0
     assert src0 == src1 and "rbd_it" not in src1 and "rbd_par_tab" not in src1

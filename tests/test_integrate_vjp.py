@@ -7,10 +7,7 @@ CPU tier: the per-joint adjoints of the coordinate maps against central differen
 along q + eps q̇(e_k), v + eps e_k and tau + eps e_k.  GPU tier: the kernels against that CPU run, the trajectory against
 rbd_integrate, and the torch.autograd function."""
 import ctypes
-import hashlib
-import os
-import subprocess
-import tempfile
+import functools
 
 import numpy as np
 import pytest
@@ -18,6 +15,7 @@ import pytest
 import rigidbodydynamics.jl_b200 as rbd
 from oracle import Oracle
 from rigidbodydynamics.jl_b200._cabi import RbdModelDesc, make_desc
+from tests import hostsim
 from tests.test_vjp import _qdot_dirs
 from tests.util import double_pendulum, rand_inputs, randmech, rel_err
 
@@ -31,29 +29,14 @@ TOL64 = 1e-10        # GPU kernels against the CPU run of the same code, fp64
 TOL32 = 5e-3
 DT = 2e-3
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_CSRC = os.path.join(_HERE, "..", "rigidbodydynamics", "jl_b200", "csrc")
-_lib = None
 K_REV, K_PRIS, K_FIXED, K_PLANAR, K_QFLOAT, K_SPQFLOAT, K_QSPH, K_SINCOS = range(8)
 NQ, NV = (1, 1, 0, 3, 7, 6, 4, 2), (1, 1, 0, 3, 6, 6, 3, 1)
 
 
+@functools.cache
 def _shim():
-    """tests/hostsim/hostsim_integrate_vjp.cpp, compiled on first use into a temporary directory."""
-    global _lib
-    if _lib is not None:
-        return _lib
-    srcs = [os.path.join(_HERE, "hostsim", "hostsim_integrate_vjp.cpp")] + sorted(
-        os.path.join(_CSRC, f) for f in os.listdir(_CSRC) if f.endswith((".cuh", ".h")) or f == "rbd_model.cpp")
-    h = hashlib.sha1(b"".join(open(s, "rb").read() for s in srcs)).hexdigest()[:16]
-    d = os.path.join(tempfile.gettempdir(), f"rbd_hostsim_integrate_vjp_{os.getuid()}")
-    os.makedirs(d, exist_ok=True)
-    so = os.path.join(d, f"hostsim_integrate_vjp_{h}.so")
-    if not os.path.exists(so):
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-o", so + f".{os.getpid()}",
-                               srcs[0], os.path.join(_CSRC, "rbd_model.cpp")])
-        os.replace(so + f".{os.getpid()}", so)
-    lib = ctypes.CDLL(so)
+    """tests/hostsim/hostsim_integrate_vjp.cpp, compiled and loaded by hostsim.shim."""
+    lib = hostsim.shim("hostsim_integrate_vjp")
     vp, i64, c_int, c_double = ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_double
     lib.hostsim_integrate_traj.argtypes = [ctypes.POINTER(RbdModelDesc), c_int, i64, vp, vp, vp, i64, i64, c_double, c_int]
     lib.hostsim_integrate_vjp.argtypes = [ctypes.POINTER(RbdModelDesc), c_int, i64, vp, vp, vp, i64, i64, c_double, c_int] + [vp] * 6
@@ -61,7 +44,6 @@ def _shim():
     lib.hostsim_joint_rate.argtypes = [c_int] + [vp] * 4
     lib.hostsim_joint_g_adjoint.argtypes = [c_int] + [vp] * 5
     lib.hostsim_joint_l_adjoint.argtypes = [c_int] + [vp] * 7
-    _lib = lib
     return lib
 
 

@@ -14,10 +14,7 @@ GPU tier: the kernel against the CPU run of the same code, strides, ragged and m
 composition with autodiff.simulate, and Atlas fp32 at 2^20.
 """
 import ctypes
-import hashlib
-import os
-import subprocess
-import tempfile
+import functools
 
 import numpy as np
 import pytest
@@ -29,9 +26,6 @@ from rigidbodydynamics.jl_b200._cabi import RbdModelDesc, make_desc
 from tests import hostsim
 from tests.util import double_pendulum, rand_inputs, randmech, rel_err
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_CSRC = os.path.join(_HERE, "..", "rigidbodydynamics", "jl_b200", "csrc")
-_lib = None
 
 TOL_FD = 2e-6         # central finite differences, eps = 1e-6 (test_vjp.py)
 GRADS = ("qt", "qc", "vb")
@@ -47,26 +41,12 @@ def _rows(name, nb, nv):
             "momentum": 6, "momentum_rate_bias": 6, "momentum_matrix": 6 * nv, "geometric_jacobian": 6 * nv}[name]
 
 
+@functools.cache
 def _shim():
-    """tests/hostsim/hostsim_kin_vjp.cpp, compiled on first use into a temporary directory."""
-    global _lib
-    if _lib is not None:
-        return _lib
-    srcs = [os.path.join(_HERE, "hostsim", "hostsim_kin_vjp.cpp")] + sorted(
-        os.path.join(_CSRC, f) for f in os.listdir(_CSRC) if f.endswith((".cuh", ".h")) or f == "rbd_model.cpp")
-    srcs.append(os.path.join(_HERE, "..", "include", "rbd_b200.h"))
-    h = hashlib.sha1(b"".join(open(s, "rb").read() for s in srcs)).hexdigest()[:16]
-    d = os.path.join(tempfile.gettempdir(), f"rbd_hostsim_kin_vjp_{os.getuid()}")
-    os.makedirs(d, exist_ok=True)
-    so = os.path.join(d, f"hostsim_kin_vjp_{h}.so")
-    if not os.path.exists(so):
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-o", so + f".{os.getpid()}",
-                               srcs[0], os.path.join(_CSRC, "rbd_model.cpp")])
-        os.replace(so + f".{os.getpid()}", so)
-    lib = ctypes.CDLL(so)
+    """tests/hostsim/hostsim_kin_vjp.cpp, compiled and loaded by hostsim.shim."""
+    lib = hostsim.shim("hostsim_kin_vjp")
     lib.hostsim_kinematics_vjp.argtypes = [ctypes.POINTER(RbdModelDesc), ctypes.c_void_p, ctypes.c_int, ctypes.c_int64,
                                            ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
-    _lib = lib
     return lib
 
 

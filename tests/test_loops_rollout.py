@@ -9,10 +9,7 @@ The kernel's per-stage device code (loops_contact_sample compiled for the host: 
 with the host integrator's stage dynamics, and the GPU rollout with the host integrator.
 """
 import ctypes
-import hashlib
-import os
-import subprocess
-import tempfile
+import functools
 
 import numpy as np
 import pytest
@@ -22,15 +19,13 @@ from rigidbodydynamics.jl_b200 import _cabi
 from rigidbodydynamics.jl_b200._cabi import RbdModelDesc, make_desc
 from rigidbodydynamics.jl_b200.loops import _DEFAULT
 from rigidbodydynamics.jl_b200.spatial import Transform3D
+from tests import hostsim
 from tests.contact_oracle import RK4_A, RK4_B, global_coordinates, integrate_contact, local_rate
 from tests.loops_oracle import (FOUR_BAR_Q0, LoopOracle, _pose, atlas_double_support, closure_distance, energy, four_bar,
                                 maximal_coordinate_pair, mc_state_from_tree)
 from tests.test_contact import _with_contacts
 from tests.util import config_distance, rand_inputs, rel_err
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_CSRC = os.path.join(_HERE, "..", "rigidbodydynamics", "jl_b200", "csrc")
-_lib = None
 
 TOL64 = 1e-9          # GPU rollout against the fp64 host integrator, relative (the contact rollout's bound)
 # fp32 rollout against the fp64 host integrator, 5 steps at dt = 1e-3.  Measured on an H100: q 2.3e-7 / v 1.5e-7 (four-bar),
@@ -204,27 +199,13 @@ def test_host_integrator_four_bar_without_stabilization():
 # ------------------------------------------------------------------------------------------------------------------
 # CPU tier: the kernel's per-stage code compiled for the host
 # ------------------------------------------------------------------------------------------------------------------
+@functools.cache
 def _shim():
-    """tests/hostsim/hostsim_loops_rollout.cpp, compiled on first use into a temporary directory."""
-    global _lib
-    if _lib is not None:
-        return _lib
-    srcs = [os.path.join(_HERE, "hostsim", "hostsim_loops_rollout.cpp")] + sorted(
-        os.path.join(_CSRC, f) for f in os.listdir(_CSRC) if f.endswith((".cuh", ".h")) or f == "rbd_model.cpp")
-    srcs.append(os.path.join(_HERE, "..", "include", "rbd_b200.h"))
-    h = hashlib.sha1(b"".join(open(s, "rb").read() for s in srcs)).hexdigest()[:16]
-    d = os.path.join(tempfile.gettempdir(), f"rbd_hostsim_loops_rollout_{os.getuid()}")
-    os.makedirs(d, exist_ok=True)
-    so = os.path.join(d, f"hostsim_loops_rollout_{h}.so")
-    if not os.path.exists(so):
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-o", so + f".{os.getpid()}",
-                               srcs[0], os.path.join(_CSRC, "rbd_model.cpp")])
-        os.replace(so + f".{os.getpid()}", so)
-    lib = ctypes.CDLL(so)
+    """tests/hostsim/hostsim_loops_rollout.cpp, compiled and loaded by hostsim.shim."""
+    lib = hostsim.shim("hostsim_loops_rollout")
     vp = ctypes.c_void_p
     lib.hostsim_loops_contact_stage.argtypes = [ctypes.POINTER(RbdModelDesc), vp, vp, ctypes.c_int, ctypes.c_int64, vp, vp, vp, vp, vp,
                                                 ctypes.c_double, vp, vp]
-    _lib = lib
     return lib
 
 

@@ -10,11 +10,8 @@ then clamped to the effort bounds.  It is pinned on the CPU by Oracle.integrate 
 with the host integrator.
 """
 import ctypes
-import hashlib
+import functools
 import math
-import os
-import subprocess
-import tempfile
 import zlib
 
 import numpy as np
@@ -24,13 +21,11 @@ import rigidbodydynamics.jl_b200 as rbd
 from oracle import Oracle
 from rigidbodydynamics.jl_b200 import _cabi
 from rigidbodydynamics.jl_b200._cabi import RbdModelDesc, make_desc
+from tests import hostsim
 from tests.contact_oracle import (K_QFLOAT, K_QSPH, K_SINCOS, NQ, RK4_A, RK4_B, _conj, _mtv, _quat_mul,
                                   _quat_to_rotvec, _rot, _rotvec_to_quat, global_coordinates, integrate_contact, local_rate)
 from tests.util import config_distance, rand_inputs, randmech, ref_urdf, rel_err
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_CSRC = os.path.join(_HERE, "..", "rigidbodydynamics", "jl_b200", "csrc")
-_lib = None
 
 TOL64 = 1e-9          # GPU rollout against the fp64 host integrator, relative (the other rollouts' bound)
 # fp32 rollout against the fp64 host integrator, 5 steps at dt = 1e-3 from fp32-representable inputs, per mode.  Measured on an H100:
@@ -187,26 +182,12 @@ def test_effort_bounds_of_bundled_models():
 # ------------------------------------------------------------------------------------------------------------------
 # CPU tier: the device law compiled for the host
 # ------------------------------------------------------------------------------------------------------------------
+@functools.cache
 def _shim():
-    """tests/hostsim/hostsim_pd.cpp, compiled on first use into a temporary directory."""
-    global _lib
-    if _lib is not None:
-        return _lib
-    srcs = [os.path.join(_HERE, "hostsim", "hostsim_pd.cpp")] + sorted(
-        os.path.join(_CSRC, f) for f in os.listdir(_CSRC) if f.endswith((".cuh", ".h")) or f == "rbd_model.cpp")
-    srcs.append(os.path.join(_HERE, "..", "include", "rbd_b200.h"))
-    h = hashlib.sha1(b"".join(open(s, "rb").read() for s in srcs)).hexdigest()[:16]
-    d = os.path.join(tempfile.gettempdir(), f"rbd_hostsim_pd_{os.getuid()}")
-    os.makedirs(d, exist_ok=True)
-    so = os.path.join(d, f"hostsim_pd_{h}.so")
-    if not os.path.exists(so):
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-o", so + f".{os.getpid()}",
-                               srcs[0], os.path.join(_CSRC, "rbd_model.cpp")])
-        os.replace(so + f".{os.getpid()}", so)
-    lib = ctypes.CDLL(so)
+    """tests/hostsim/hostsim_pd.cpp, compiled and loaded by hostsim.shim."""
+    lib = hostsim.shim("hostsim_pd")
     vp = ctypes.c_void_p
     lib.hostsim_pd_law.argtypes = [ctypes.POINTER(RbdModelDesc), ctypes.c_int, ctypes.c_int64] + [vp] * 7 + [ctypes.c_int, vp, vp, vp]
-    _lib = lib
     return lib
 
 

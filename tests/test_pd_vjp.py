@@ -8,10 +8,7 @@ against its per-(sample, joint) fallback, autograd against the direct call and a
 gradient-descent use case.
 """
 import ctypes
-import hashlib
-import os
-import subprocess
-import tempfile
+import functools
 import zlib
 
 import numpy as np
@@ -19,6 +16,7 @@ import pytest
 
 import rigidbodydynamics.jl_b200 as rbd
 from rigidbodydynamics.jl_b200 import _cabi
+from tests import hostsim
 from tests.contact_oracle import K_PLANAR, K_PRIS, K_QFLOAT, K_QSPH, K_REV, K_SINCOS, K_SPQFLOAT, NQ, _quat_mul, _rotvec_to_quat
 from oracle import Oracle
 from rigidbodydynamics.jl_b200._cabi import RbdModelDesc, make_desc
@@ -26,9 +24,6 @@ from tests.test_integrate_vjp import EPS_FD, TOL64, TOL_FD, host_ivjp
 from tests.test_pd_rollout import Ctrl, _PdDesc, _controller, _model, _tau_at, integrate_pd
 from tests.util import rand_inputs, rel_err
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_CSRC = os.path.join(_HERE, "..", "rigidbodydynamics", "jl_b200", "csrc")
-_lib = None
 NV = {K_REV: 1, K_PRIS: 1, K_PLANAR: 3, K_QFLOAT: 6, K_SPQFLOAT: 6, K_QSPH: 3, K_SINCOS: 1}
 
 
@@ -40,22 +35,10 @@ class _PdBar(ctypes.Structure):
 # ------------------------------------------------------------------------------------------------------------------
 # CPU tier: the law's adjoint compiled for the host
 # ------------------------------------------------------------------------------------------------------------------
+@functools.cache
 def _shim():
-    """tests/hostsim/hostsim_pd_vjp.cpp, compiled on first use into a temporary directory."""
-    global _lib
-    if _lib is not None:
-        return _lib
-    srcs = [os.path.join(_HERE, "hostsim", "hostsim_pd_vjp.cpp")] + sorted(
-        os.path.join(_CSRC, f) for f in os.listdir(_CSRC) if f.endswith((".cuh", ".h")) or f == "rbd_model.cpp")
-    h = hashlib.sha1(b"".join(open(s, "rb").read() for s in srcs)).hexdigest()[:16]
-    d = os.path.join(tempfile.gettempdir(), f"rbd_hostsim_pd_vjp_{os.getuid()}")
-    os.makedirs(d, exist_ok=True)
-    so = os.path.join(d, f"hostsim_pd_vjp_{h}.so")
-    if not os.path.exists(so):
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-o", so + f".{os.getpid()}",
-                               srcs[0], os.path.join(_CSRC, "rbd_model.cpp")])
-        os.replace(so + f".{os.getpid()}", so)
-    lib = ctypes.CDLL(so)
+    """tests/hostsim/hostsim_pd_vjp.cpp, compiled and loaded by hostsim.shim."""
+    lib = hostsim.shim("hostsim_pd_vjp")
     vp = ctypes.c_void_p
     lib.hostsim_joint_error.argtypes = [ctypes.c_int, vp, vp, vp]
     lib.hostsim_pd_adj_joint.argtypes = [ctypes.c_int] + [vp] * 19
@@ -63,7 +46,6 @@ def _shim():
     ctl = [ci, vp, vp, i64, vp, vp, vp, i64, i64, vp, vp, vp, i64, i64, ctypes.c_double, ci]
     lib.hostsim_pd_traj.argtypes = [ctypes.POINTER(RbdModelDesc), ci, i64, vp, vp] + ctl
     lib.hostsim_pd_vjp.argtypes = [ctypes.POINTER(RbdModelDesc), ci, i64, vp, vp] + ctl + [vp] * 7
-    _lib = lib
     return lib
 
 

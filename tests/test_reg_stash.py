@@ -14,7 +14,7 @@ import torch
 
 import rigidbodydynamics.jl_b200 as rbd
 from tests import hostsim
-from tests.test_fold import _mirrored_tree, _run, _source, shim  # noqa: F401  (shim: the fold shim fixture)
+from tests.test_fold import _mirrored_tree
 from tests.util import rand_inputs, randmech
 
 ATLAS_ROWS = 213                       # 31 bodies x 6 rows + the 27-row pending slot
@@ -28,15 +28,15 @@ def _models():
 
 @pytest.mark.parametrize("fold", [True, False])
 @pytest.mark.parametrize("name", ["atlas", "valkyrie", "iiwa14", "randmech1", "randmech2", "mirrored"])
-def test_register_rows_bit_identical_cpu(shim, monkeypatch, name, fold):  # noqa: F811
+def test_register_rows_bit_identical_cpu(built, monkeypatch, name, fold):
     mech = dict(_models())[name]
     desc = mech.flatten()
     q, v, tau, _, _ = rand_inputs(mech, 8, 5)
     outs, srcs = {}, {}
     for budget in ("0", "27", "-1"):
         monkeypatch.setenv("RBD_JIT_REG_ROWS", budget)
-        srcs[budget], _ = _source(shim, desc, np.float32, fold, has_out1=True)
-        outs[budget] = _run(shim, srcs[budget], desc, np.float32, q, v, tau, has_out1=True)
+        prog = hostsim.SpecProgram(desc, "aba", np.float32, True, True, fold=fold)
+        srcs[budget], outs[budget] = prog.src, prog.run(q, v, tau)
     assert "rbd_r" not in srcs["0"]
     assert "rbd_r" in srcs["-1"]
     a, qa = outs["0"]

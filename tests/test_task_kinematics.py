@@ -15,10 +15,7 @@ CPU tier
 GPU tier: the kernel against the oracle, bit identity across output subsets, strides, alignment and tiles, the Python conveniences.
 """
 import ctypes
-import hashlib
-import os
-import subprocess
-import tempfile
+import functools
 
 import numpy as np
 import pytest
@@ -27,38 +24,22 @@ import rigidbodydynamics.jl_b200 as rbd
 from rigidbodydynamics.jl_b200 import _cabi
 from rigidbodydynamics.jl_b200._cabi import RbdModelDesc, RbdTaskDesc, make_desc
 from rigidbodydynamics.jl_b200.kinematics import TaskFrame, task_desc
+from tests import hostsim
 from tests.task_oracle import OUTPUTS, TaskOracle, cross
 from tests.util import double_pendulum, rand_inputs, randmech
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_CSRC = os.path.join(_HERE, "..", "rigidbodydynamics", "jl_b200", "csrc")
-_lib = None
 
 TOL = {np.float64: 1e-11, np.float32: 2e-5}        # relative to max(1, |ref|), the scales of test_kinematics.py
 MODELS = [("atlas", True), ("valkyrie", False), ("iiwa14", False), ("double_pendulum", False)]
 VEL_OUTPUTS = ("twist", "point_velocity", "acceleration", "point_acceleration")
 
 
+@functools.cache
 def _shim():
-    """tests/hostsim/hostsim_task.cpp, compiled on first use into a temporary directory."""
-    global _lib
-    if _lib is not None:
-        return _lib
-    srcs = [os.path.join(_HERE, "hostsim", "hostsim_task.cpp")] + sorted(
-        os.path.join(_CSRC, f) for f in os.listdir(_CSRC) if f.endswith((".cuh", ".h")) or f == "rbd_model.cpp")
-    srcs.append(os.path.join(_HERE, "..", "include", "rbd_b200.h"))
-    h = hashlib.sha1(b"".join(open(s, "rb").read() for s in srcs)).hexdigest()[:16]
-    d = os.path.join(tempfile.gettempdir(), f"rbd_hostsim_task_{os.getuid()}")
-    os.makedirs(d, exist_ok=True)
-    so = os.path.join(d, f"hostsim_task_{h}.so")
-    if not os.path.exists(so):
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-o", so + f".{os.getpid()}",
-                               srcs[0], os.path.join(_CSRC, "rbd_model.cpp")])
-        os.replace(so + f".{os.getpid()}", so)
-    lib = ctypes.CDLL(so)
+    """tests/hostsim/hostsim_task.cpp, compiled and loaded by hostsim.shim."""
+    lib = hostsim.shim("hostsim_task")
     lib.hostsim_task_kinematics.argtypes = [ctypes.POINTER(RbdModelDesc), ctypes.POINTER(RbdTaskDesc), ctypes.c_int, ctypes.c_int64,
                                             ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
-    _lib = lib
     return lib
 
 

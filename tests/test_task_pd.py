@@ -6,11 +6,8 @@ The fp64 numpy law below builds u_task = Σ_t J_t^T f_t from explicit matrices -
 must agree with it, and the GPU rollouts with tests/test_pd_rollout.py's host integrator running this law at every stage.
 """
 import ctypes
-import hashlib
+import functools
 import math
-import os
-import subprocess
-import tempfile
 import zlib
 
 import numpy as np
@@ -23,14 +20,12 @@ from rigidbodydynamics.jl_b200 import _cabi
 from rigidbodydynamics.jl_b200._cabi import RbdModelDesc, make_desc
 from rigidbodydynamics.jl_b200.kinematics import TaskFrame
 from rigidbodydynamics.jl_b200.pd import _RbdPdDesc, _RbdTaskPdDesc
+from tests import hostsim
 from tests.task_oracle import TaskOracle, rot, rotT, to_frame
 from tests.test_pd_rollout import Ctrl, _col, _controller, _model, _pad, _state, _tau_at, integrate_pd, law
 from tests.test_task_kinematics import task_set
 from tests.util import config_distance, rand_inputs, randmech, ref_urdf, rel_err
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_CSRC = os.path.join(_HERE, "..", "rigidbodydynamics", "jl_b200", "csrc")
-_lib = None
 TOL64 = 1e-9
 # fp32 rollout against the fp64 host integrator (Atlas, 5 steps at dt = 1e-3, fp32-representable inputs).  Measured on an NVIDIA
 # H100 80GB HBM3 at 700 W: q 1.4e-6 / v 1.8e-4 (torque mode), q 3.3e-7 / v 2.4e-6 (computed torque); each bound is about 5x the
@@ -172,27 +167,13 @@ def targets(mech, q, tasks, kinds, rng, mode="random"):
 # ------------------------------------------------------------------------------------------------------------------
 # the device law on the CPU
 # ------------------------------------------------------------------------------------------------------------------
+@functools.cache
 def _shim():
-    """tests/hostsim/hostsim_task_pd.cpp, compiled on first use into a temporary directory."""
-    global _lib
-    if _lib is not None:
-        return _lib
-    srcs = [os.path.join(_HERE, "hostsim", "hostsim_task_pd.cpp")] + sorted(
-        os.path.join(_CSRC, f) for f in os.listdir(_CSRC) if f.endswith((".cuh", ".h")) or f == "rbd_model.cpp")
-    srcs.append(os.path.join(_HERE, "..", "include", "rbd_b200.h"))
-    h = hashlib.sha1(b"".join(open(s, "rb").read() for s in srcs)).hexdigest()[:16]
-    d = os.path.join(tempfile.gettempdir(), f"rbd_hostsim_task_pd_{os.getuid()}")
-    os.makedirs(d, exist_ok=True)
-    so = os.path.join(d, f"hostsim_task_pd_{h}.so")
-    if not os.path.exists(so):
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-o", so + f".{os.getpid()}",
-                               srcs[0], os.path.join(_CSRC, "rbd_model.cpp")])
-        os.replace(so + f".{os.getpid()}", so)
-    lib = ctypes.CDLL(so)
+    """tests/hostsim/hostsim_task_pd.cpp, compiled and loaded by hostsim.shim."""
+    lib = hostsim.shim("hostsim_task_pd")
     vp = ctypes.c_void_p
     lib.hostsim_task_pd_law.argtypes = [ctypes.POINTER(RbdModelDesc), ctypes.POINTER(_RbdTaskPdDesc), ctypes.c_int, ctypes.c_int64,
                                         vp, vp, vp, vp]
-    _lib = lib
     return lib
 
 

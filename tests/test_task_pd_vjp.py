@@ -7,10 +7,7 @@ GPU tier: autodiff.simulate / simulate_contact with a TaskPD against central dif
 the direct call across checkpoints, bit-identity with the JointPD and open-loop VJPs at zero task gains, a gradient-descent use
 case and Atlas fp32 at 2^20."""
 import ctypes
-import hashlib
-import os
-import subprocess
-import tempfile
+import functools
 import zlib
 
 import numpy as np
@@ -21,38 +18,21 @@ from rigidbodydynamics.jl_b200 import _cabi
 from rigidbodydynamics.jl_b200._cabi import RbdModelDesc, make_desc
 from rigidbodydynamics.jl_b200.kinematics import TaskFrame
 from rigidbodydynamics.jl_b200.pd import _RbdTaskPdDesc
+from tests import hostsim
 from tests.task_oracle import TaskOracle
 from tests.test_pd_rollout import _controller, _model
 from tests.test_pd_vjp import _tangent
 from tests.test_task_pd import TaskCtrl, _cpu_models, _gains, _rows, _task_struct, hostsim_task_law, targets, task_mix
 from tests.util import rand_inputs
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_CSRC = os.path.join(_HERE, "..", "rigidbodydynamics", "jl_b200", "csrc")
-_lib = None
 
-
+@functools.cache
 def _shim():
-    """tests/hostsim/hostsim_task_pd_vjp.cpp, compiled on first use into a temporary directory."""
-    global _lib
-    if _lib is not None:
-        return _lib
-    srcs = [os.path.join(_HERE, "hostsim", "hostsim_task_pd_vjp.cpp")] + sorted(
-        os.path.join(_CSRC, f) for f in os.listdir(_CSRC) if f.endswith((".cuh", ".h")) or f == "rbd_model.cpp")
-    srcs.append(os.path.join(_HERE, "..", "include", "rbd_b200.h"))
-    h = hashlib.sha1(b"".join(open(s, "rb").read() for s in srcs)).hexdigest()[:16]
-    d = os.path.join(tempfile.gettempdir(), f"rbd_hostsim_task_pd_vjp_{os.getuid()}")
-    os.makedirs(d, exist_ok=True)
-    so = os.path.join(d, f"hostsim_task_pd_vjp_{h}.so")
-    if not os.path.exists(so):
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-o", so + f".{os.getpid()}",
-                               srcs[0], os.path.join(_CSRC, "rbd_model.cpp")])
-        os.replace(so + f".{os.getpid()}", so)
-    lib = ctypes.CDLL(so)
+    """tests/hostsim/hostsim_task_pd_vjp.cpp, compiled and loaded by hostsim.shim."""
+    lib = hostsim.shim("hostsim_task_pd_vjp")
     vp = ctypes.c_void_p
     lib.hostsim_task_pd_law_vjp.argtypes = [ctypes.POINTER(RbdModelDesc), ctypes.POINTER(_RbdTaskPdDesc), ctypes.c_int, ctypes.c_int64,
                                             vp, vp, vp, vp, vp, vp, vp]
-    _lib = lib
     return lib
 
 

@@ -15,10 +15,7 @@ GPU tier: the kernel against the CPU run of the same code, strides and tiles, th
 autodiff.simulate, batched gradient-descent IK, and Atlas fp32 at 2^20.
 """
 import ctypes
-import hashlib
-import os
-import subprocess
-import tempfile
+import functools
 
 import numpy as np
 import pytest
@@ -33,35 +30,18 @@ from tests.task_oracle import OUTPUTS, TaskOracle
 from tests.test_task_kinematics import VEL_OUTPUTS, _rows, hostsim_tasks, task_set
 from tests.util import rand_inputs, randmech, rel_err
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_CSRC = os.path.join(_HERE, "..", "rigidbodydynamics", "jl_b200", "csrc")
-_lib = None
 
 TOL_FD = 2e-6         # central finite differences, eps = 1e-6 (test_vjp.py)
 GRADS = ("qt", "qc", "vb", "vdb")
 K_QFLOAT, K_QSPH = 4, 6
 
 
+@functools.cache
 def _shim():
-    """tests/hostsim/hostsim_task_vjp.cpp, compiled on first use into a temporary directory."""
-    global _lib
-    if _lib is not None:
-        return _lib
-    srcs = [os.path.join(_HERE, "hostsim", "hostsim_task_vjp.cpp")] + sorted(
-        os.path.join(_CSRC, f) for f in os.listdir(_CSRC) if f.endswith((".cuh", ".h")) or f == "rbd_model.cpp")
-    srcs.append(os.path.join(_HERE, "..", "include", "rbd_b200.h"))
-    h = hashlib.sha1(b"".join(open(s, "rb").read() for s in srcs)).hexdigest()[:16]
-    d = os.path.join(tempfile.gettempdir(), f"rbd_hostsim_task_vjp_{os.getuid()}")
-    os.makedirs(d, exist_ok=True)
-    so = os.path.join(d, f"hostsim_task_vjp_{h}.so")
-    if not os.path.exists(so):
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-o", so + f".{os.getpid()}",
-                               srcs[0], os.path.join(_CSRC, "rbd_model.cpp")])
-        os.replace(so + f".{os.getpid()}", so)
-    lib = ctypes.CDLL(so)
+    """tests/hostsim/hostsim_task_vjp.cpp, compiled and loaded by hostsim.shim."""
+    lib = hostsim.shim("hostsim_task_vjp")
     lib.hostsim_task_kinematics_vjp.argtypes = [ctypes.POINTER(RbdModelDesc), ctypes.POINTER(RbdTaskDesc), ctypes.c_int, ctypes.c_int64,
                                                 ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_void_p]
-    _lib = lib
     return lib
 
 

@@ -13,7 +13,6 @@ import torch
 
 import rigidbodydynamics.jl_b200 as rbd
 from tests import hostsim
-from tests.test_fold import _run, _source, shim  # noqa: F401  (shim: the fold shim fixture)
 from tests.test_reg_stash import _models, _shared_rows_used
 from tests.util import rand_inputs
 
@@ -22,7 +21,7 @@ ATLAS_TRIG_ROWS = 52                   # the 26 limb joints (legs of 6, arms of 
 
 @pytest.mark.parametrize("fold", [True, False])
 @pytest.mark.parametrize("name", ["atlas", "valkyrie", "iiwa14", "randmech1", "randmech2", "mirrored"])
-def test_trig_cache_bit_identical_cpu(shim, monkeypatch, name, fold):  # noqa: F811
+def test_trig_cache_bit_identical_cpu(built, monkeypatch, name, fold):
     mech = dict(_models())[name]
     desc = mech.flatten()
     q, v, tau, _, _ = rand_inputs(mech, 8, 7)
@@ -30,8 +29,8 @@ def test_trig_cache_bit_identical_cpu(shim, monkeypatch, name, fold):  # noqa: F
     monkeypatch.delenv("RBD_JIT_REG_ROWS", raising=False)
     for trig in ("0", "1"):
         monkeypatch.setenv("RBD_JIT_TRIG", trig)
-        srcs[trig], _ = _source(shim, desc, np.float32, fold, has_out1=True)
-        outs[trig] = _run(shim, srcs[trig], desc, np.float32, q, v, tau, has_out1=True)
+        prog = hostsim.SpecProgram(desc, "aba", np.float32, True, True, fold=fold)
+        srcs[trig], outs[trig] = prog.src, prog.run(q, v, tau)
     used = lambda src: re.search(r"RBD_T(?:LD|ST)\([\d(]|\brbd_sc\d", src) is not None     # a cache row read or written
     assert not used(srcs["0"]) and used(srcs["1"])
     assert srcs["1"].count("RBD_SINCOS(") < srcs["0"].count("RBD_SINCOS(")

@@ -7,10 +7,7 @@ tangent directions q + eps q̇(e_k), v + eps e_k, tau + eps e_k, w + eps e_r.
 CPU tier: the per-sample device functions compiled for the host (tests/hostsim/hostsim_adjoint.cpp).  GPU tier: the kernels through
 the C ABI and the torch.autograd functions."""
 import ctypes
-import hashlib
-import os
-import subprocess
-import tempfile
+import functools
 
 import numpy as np
 import pytest
@@ -29,29 +26,12 @@ TOL_FD = 2e-6         # central finite differences, eps = 1e-6
 # The bound is the derivative tests' 5e-3.
 TOL32 = 5e-3
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_CSRC = os.path.join(_HERE, "..", "rigidbodydynamics", "jl_b200", "csrc")
-_lib = None
 
-
+@functools.cache
 def _shim():
-    """tests/hostsim/hostsim_adjoint.cpp, compiled on first use into a temporary directory."""
-    global _lib
-    if _lib is not None:
-        return _lib
-    srcs = [os.path.join(_HERE, "hostsim", "hostsim_adjoint.cpp")] + sorted(
-        os.path.join(_CSRC, f) for f in os.listdir(_CSRC) if f.endswith((".cuh", ".h")) or f == "rbd_model.cpp")
-    h = hashlib.sha1(b"".join(open(s, "rb").read() for s in srcs)).hexdigest()[:16]
-    d = os.path.join(tempfile.gettempdir(), f"rbd_hostsim_adjoint_{os.getuid()}")
-    os.makedirs(d, exist_ok=True)
-    so = os.path.join(d, f"hostsim_adjoint_{h}.so")
-    if not os.path.exists(so):
-        subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-o", so + f".{os.getpid()}",
-                               srcs[0], os.path.join(_CSRC, "rbd_model.cpp")])
-        os.replace(so + f".{os.getpid()}", so)
-    lib = ctypes.CDLL(so)
+    """tests/hostsim/hostsim_adjoint.cpp, compiled and loaded by hostsim.shim."""
+    lib = hostsim.shim("hostsim_adjoint")
     lib.hostsim_vjp.argtypes = [ctypes.POINTER(RbdModelDesc), ctypes.c_int, ctypes.c_int, ctypes.c_int64] + [ctypes.c_void_p] * 11
-    _lib = lib
     return lib
 
 
