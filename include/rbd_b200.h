@@ -776,6 +776,27 @@ int32_t rbd_task_pd_torques_vjp(const rbd_model* model, int32_t dtype, int64_t B
                                 const rbd_task_pd_desc* ctrl, int32_t step, const void* tau_out_bar, void* q_bar_tan, void* q_bar_cfg,
                                 void* v_bar, void* tau_ff_bar, const rbd_task_pd_bar* ctrl_bar, void* stream);
 
+/* Linearisation of every step of a recorded rollout (DESIGN 4.25): for the trajectory rbd_integrate_trajectory recorded with the
+ * same tau, tau_step_stride, dt and nsteps (q_traj [(nsteps+1) x nq x B], v_traj [(nsteps+1) x nv x B]), the Jacobians of the
+ * Munthe-Kaas RK4 step of rbd_integrate_schedule at x_s = (q_traj[s], v_traj[s]) for every step s and sample b:
+ *   A_s = ∂x_{s+1}/∂x_s  (2nv x 2nv),  B_s = ∂x_{s+1}/∂τ_s  (2nv x nv),  x = (q, v).
+ * Input configuration direction j: q̇ = velocity_to_configuration_derivative(e_j) (the tangent convention of
+ * rbd_dynamics_derivatives; for QuaternionFloating q exp(ε e_j)).  Output configuration rows: the change of q_{s+1} through
+ * configuration_derivative_to_velocity (exact for unit quaternions, whose norm the step preserves).  Torque columns: the [nv x B]
+ * block step s reads, held over its four stages.  Rows and columns 0..nv-1 are the configuration tangent, nv..2nv-1 the velocity.
+ * Layout (batch fastest, column-major per sample): A_out [nsteps x 4nv^2 x B], entry (i, j) of step s at row s 4nv^2 + i + j 2nv;
+ * B_out [nsteps x 2nv^2 x B], entry (i, j) at row s 2nv^2 + i + j 2nv.  Either output may be NULL, not both; every entry is
+ * written.  The (step, sample) pairs are one batch, processed in chunks within RBD_DERIV_SCRATCH_MB (the dynamics Jacobians keep
+ * their own scratch within the same budget); a chunked call equals an unchunked one bit for bit.  Argument errors, before any CUDA
+ * call: dtype other than fp32 / fp64 and the model limits of rbd_dynamics_derivatives: RBD_EUNSUPPORTED; tau_stage_stride != 0
+ * (per-stage schedules), tau_step_stride < 0, nsteps < 0, dt <= 0, both outputs NULL, NULL q_traj / v_traj: RBD_EINVAL.  B == 0 or
+ * nsteps == 0: nothing to do.  Tree rollouts only (no contact, loops or feedback).  Kernels per chunk: one gather, the recompute of
+ * rbd_integrate_vjp's backward step, four stage kernels, four dynamics Jacobians without their forward dynamics, three products and
+ * one finishing kernel. */
+int32_t rbd_integrate_derivatives(const rbd_model* model, int32_t dtype, int64_t B, const void* q_traj, const void* v_traj,
+                                  const void* tau, int64_t tau_step_stride, int64_t tau_stage_stride, double dt, int32_t nsteps,
+                                  void* A_out, void* B_out, void* stream);
+
 /* Host-pointer variants: same semantics, host buffers in, host buffers out, copies inside the call. */
 int32_t rbd_dynamics_host(rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                           const void* tau, const void* wext, void* vd_out, void* qd_out);

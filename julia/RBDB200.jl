@@ -556,6 +556,32 @@ function inverse_dynamics_derivatives!(dtau_dq, dtau_dv, state::BatchedState{T},
     dtau_dq, dtau_dv
 end
 
+"""
+    integrate_derivatives!(A, Bjac, model, q_traj, v_traj, torques = nothing; dt)
+
+The Jacobians of every step of a recorded RK4 rollout (rbd_integrate_derivatives, DESIGN 4.25): for trajectories `q_traj`
+(B x nq x (nsteps+1)) and `v_traj` (B x nv x (nsteps+1)) recorded with the same `torques` (B x nv constant, or B x nv x nsteps per
+step) and `dt`, `A` (B x 4nv² x nsteps) receives A_s = ∂x_{s+1}/∂x_s, entry (i, j) of sample b at `[b, i + (j - 1) * 2nv, s]`, and
+`Bjac` (B x 2nv² x nsteps) receives B_s = ∂x_{s+1}/∂τ_s in the same layout; x = (q, v) with the configuration in the tangent space
+(columns along `velocity_to_configuration_derivative(e_j)`, rows through `configuration_derivative_to_velocity`).  Either output may
+be `nothing`, not both.  (Not run here: no Julia installation is available to the project's tests; the Python binding exercises the
+same entry point.)
+"""
+function integrate_derivatives!(A, Bjac, model, q_traj::AbstractArray{T, 3}, v_traj::AbstractArray{T, 3}, torques = nothing;
+                                dt) where {T <: Union{Float32, Float64}}
+    B, nv, n1 = size(v_traj)
+    step = torques === nothing || ndims(torques) == 2 ? 0 : B * nv
+    GC.@preserve A Bjac q_traj v_traj torques begin
+        check(ccall((:rbd_integrate_derivatives, librbd), Int32,
+                    (Ptr{Cvoid}, Int32, Int64, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Int64, Int64, Float64, Int32, Ptr{Cvoid}, Ptr{Cvoid},
+                     Ptr{Cvoid}),
+                    model.handle, dtype_code(T), B, devptr(q_traj), devptr(v_traj), torques === nothing ? C_NULL : devptr(torques),
+                    step, 0, Float64(dt), Int32(n1 - 1), A === nothing ? C_NULL : devptr(A), Bjac === nothing ? C_NULL : devptr(Bjac),
+                    stream_ptr()))
+    end
+    A, Bjac
+end
+
 "Compile the model-specialised solve kernel of `dynamics_derivatives!` ahead of time (cubin cache; no GPU needed)."
 precompile_derivatives(model, ::Type{T}) where {T <: Union{Float32, Float64}} =
     check(ccall((:rbd_model_precompile_derivatives, librbd), Int32, (Ptr{Cvoid}, Int32), model.handle, dtype_code(T)))

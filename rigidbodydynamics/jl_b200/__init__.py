@@ -36,6 +36,6 @@ from .mechanism import maximal_coordinates  # noqa: F401
 from .mechanism import Bounds, effort_bounds  # noqa: F401
 from .pd import JointPD, TaskPD, task_pd_torques  # noqa: F401
 from . import autodiff  # noqa: F401  (rbd.autodiff.dynamics / inverse_dynamics: differentiable, kept out of this namespace)
-from .autodiff import (dynamics_vjp_, integrate_contact_vjp_, integrate_pd_vjp_, integrate_task_pd_vjp_, integrate_vjp_,  # noqa: F401
+from .autodiff import (dynamics_vjp_, integrate_contact_vjp_, integrate_derivatives, integrate_derivatives_, integrate_pd_vjp_, integrate_task_pd_vjp_, integrate_vjp_,  # noqa: F401
                        inverse_dynamics_vjp_)
 from ._cabi import RbdError, launch_info, load_library  # noqa: F401

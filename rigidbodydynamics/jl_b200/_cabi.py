@@ -142,6 +142,7 @@ SYMBOLS = {
     "rbd_integrate_schedule": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _i64, _i64, c_double, _i32, _vp]),
     "rbd_integrate_trajectory": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _i64, _i64, c_double, _i32, _vp, _vp, _vp]),
     "rbd_integrate_vjp": (c_int32, [_vp, _i32, _i64, _vp, _vp, _vp, _i64, _i64, c_double, _i32] + [_vp] * 7),
+    "rbd_integrate_derivatives": (c_int32, [_vp, _i32, _i64, _vp, _vp, _vp, _i64, _i64, c_double, _i32, _vp, _vp, _vp]),
     "rbd_integrate_contact": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _vp, c_double, _i32, _vp, _vp, _vp, _vp]),
     "rbd_integrate_loops": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, c_double, _i32, _vp, _vp, _vp, _vp]),
     "rbd_integrate_pd": (c_int32, [_vp, _i32, _i64, _i64, _vp, _vp, _vp, _vp, _i64, _i64, _vp, _vp, _vp, c_double, _i32, _vp, _vp, _vp, _vp]),

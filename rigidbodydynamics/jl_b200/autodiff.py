@@ -3,6 +3,7 @@
     dynamics_vjp_          ν̄ᵀ ∂v̇/∂(q, v, τ, w_ext)        rbd_dynamics_vjp          (include/rbd_b200.h, csrc/rbd_adjoint.cuh)
     inverse_dynamics_vjp_  τ̄ᵀ ∂τ/∂(q, v, v̇, w_ext)         rbd_inverse_dynamics_vjp
     integrate_vjp_         gradient of a recorded rollout       rbd_integrate_vjp         (csrc/rbd_integrate_adjoint.cuh)
+    integrate_derivatives_ Jacobians ∂x_{s+1}/∂(x_s, τ_s) of every recorded step  rbd_integrate_derivatives  (csrc/rbd_integrate_deriv.cuh)
     integrate_contact_vjp_ gradient of a recorded contact rollout  rbd_integrate_contact_vjp  (csrc/rbd_contact_adjoint.cuh)
     integrate_pd_vjp_      gradient of a recorded closed-loop rollout  rbd_integrate_pd_vjp  (csrc/rbd_integrate_adjoint.cuh)
     integrate_task_pd_vjp_ gradient of a recorded task-space closed-loop rollout  rbd_integrate_task_pd_vjp  (csrc/rbd_task_pd_adjoint.cuh)
@@ -49,7 +50,7 @@ from .kinematics import _NEEDS_V, _ROWS, _TASK_NEEDS_V, _TASK_ROWS, TaskFrame, T
 from .mechanism import Mechanism
 from .state import _DT, MechanismState, _model_handle
 
-__all__ = ["dynamics_vjp_", "inverse_dynamics_vjp_", "integrate_vjp_", "integrate_contact_vjp_", "integrate_pd_vjp_", "integrate_task_pd_vjp_",
+__all__ = ["dynamics_vjp_", "inverse_dynamics_vjp_", "integrate_vjp_", "integrate_derivatives_", "integrate_derivatives", "integrate_contact_vjp_", "integrate_pd_vjp_", "integrate_task_pd_vjp_",
            "task_pd_torques_vjp_", "task_pd_torques", "dynamics",
            "inverse_dynamics", "simulate", "simulate_contact", "task_kinematics_vjp_", "task_kinematics", "kinematics_vjp_", "kinematics"]
 
@@ -455,6 +456,39 @@ def integrate_vjp_(mechanism: Mechanism, q_traj: torch.Tensor, v_traj: torch.Ten
     _cabi.check(_cabi.load_library().rbd_integrate_vjp(h.ptr, _DT[q_traj.dtype], B, _ptr(q_traj), _ptr(v_traj), _ptr(torques), step,
                                                        stage, float(dt), nsteps, _ptr(q_traj_bar), _ptr(v_traj_bar), _ptr(q0_bar_tan),
                                                        _ptr(q0_bar_cfg), _ptr(v0_bar), _ptr(tau_bar), _stream(q_traj)))
+
+
+def integrate_derivatives_(mechanism: Mechanism, q_traj: torch.Tensor, v_traj: torch.Tensor, torques: Optional[torch.Tensor] = None, *,
+                           dt: float, A_out: Optional[torch.Tensor] = None, B_out: Optional[torch.Tensor] = None):
+    """Linearisation of every step of a trajectory recorded by ``simulate_trajectory_`` ([nsteps + 1, nq, B] / [nsteps + 1, nv, B])
+    with the same ``torques`` (None, [nv, B] or [nsteps, nv, B]; a per-stage schedule raises) and ``dt``: ``A_out`` [nsteps, 4 nv^2, B]
+    receives A_s = ∂x_{s+1}/∂x_s and ``B_out`` [nsteps, 2 nv^2, B] receives B_s = ∂x_{s+1}/∂τ_s, x = (q, v) with the configuration in
+    the tangent space (columns along ``velocity_to_configuration_derivative(e_j)``, rows through
+    ``configuration_derivative_to_velocity``), entry (i, j) at row i + j 2nv of a step's block.  Either may be None, not both."""
+    what = "integrate_derivatives_"
+    nsteps = q_traj.shape[0] - 1
+    h, B, step, stage = _rollout_inputs(mechanism, what, q_traj[0], v_traj[0], torques, nsteps)
+    if stage:
+        raise ValueError(f"{what}: per-stage torque schedules are not supported")
+    if A_out is None and B_out is None:
+        raise ValueError(f"{what}: A_out and B_out must not both be None")
+    nq, nv = h.info.nq, h.info.nv
+    _check_blocks(what, q_traj, [(q_traj, (nsteps + 1, nq, B), "q_traj"), (v_traj, (nsteps + 1, nv, B), "v_traj"),
+                                 (A_out, (nsteps, 4 * nv * nv, B), "A_out"), (B_out, (nsteps, 2 * nv * nv, B), "B_out")])
+    _cabi.check(_cabi.load_library().rbd_integrate_derivatives(h.ptr, _DT[q_traj.dtype], B, _ptr(q_traj), _ptr(v_traj), _ptr(torques),
+                                                               step, 0, float(dt), nsteps, _ptr(A_out), _ptr(B_out), _stream(q_traj)))
+
+
+def integrate_derivatives(mechanism: Mechanism, q_traj: torch.Tensor, v_traj: torch.Tensor, torques: Optional[torch.Tensor] = None, *,
+                          dt: float):
+    """``integrate_derivatives_`` into new tensors; returns views ``A[s, i, j, b]`` [nsteps, 2nv, 2nv, B] and ``B[s, i, j, b]``
+    [nsteps, 2nv, nv, B]."""
+    nsteps, B = q_traj.shape[0] - 1, q_traj.shape[2]
+    nv = v_traj.shape[1]
+    A = torch.empty((max(nsteps, 0), 4 * nv * nv, B), dtype=q_traj.dtype, device=q_traj.device)
+    Bm = torch.empty((max(nsteps, 0), 2 * nv * nv, B), dtype=q_traj.dtype, device=q_traj.device)
+    integrate_derivatives_(mechanism, q_traj, v_traj, torques, dt=dt, A_out=A, B_out=Bm)
+    return A.view(-1, 2 * nv, 2 * nv, B).transpose(1, 2), Bm.view(-1, nv, 2 * nv, B).transpose(1, 2)
 
 
 def _trajectory(h, q0, v0, tau, s0, m, step, stage, dt):

@@ -248,6 +248,7 @@ template <class T> struct DerivCall {
   const T* q; const T* v; const T* tau_in; const T* wext;
   T* vd;                 // forward: written; inverse: the caller's v̇ (read only)
   T* dq; T* dv; T* dtau; T* tau_out; T* M;
+  bool vd_given = false;  // forward: vd already holds v̇ at (q, v, tau) and the forward dynamics is not run again
 };
 
 template <class T>
@@ -311,7 +312,7 @@ int derivatives_t(const char* fn, const rbd_model* model, int32_t dtype, int64_t
     const int64_t c = std::min<int64_t>(C, B - b0);
     T* vd = r.vd + b0;
     // v̇ itself: the library's own forward dynamics (model-specialised kernels when available)
-    if (!r.inverse)
+    if (!r.inverse && !r.vd_given)
       if (int rc = rbd_dynamics(model, dtype, c, ld, r.q + b0, r.v + b0, at(r.tau_in, b0), at(r.wext, b0), vd, nullptr, stream)) return rc;
     DerivArgs<T> a{r.q + b0, r.v + b0, vd, r.dq + b0, r.dv + b0, scratch, ld, sld, c,
                    at(r.wext, b0), at(r.dtau, b0), at(r.tau_out, b0), at(r.M, b0)};
@@ -372,6 +373,23 @@ int32_t derivatives_entry(const char* fn, const rbd_model* model, int32_t dtype,
 }
 
 }  // namespace
+
+namespace rbd {
+int dynamics_derivatives_dense(const rbd_model* model, int32_t dtype, int64_t B, const void* q, const void* v, const void* tau,
+                               const void* vd, void* dq, void* dv, void* dtau, cudaStream_t stream) {
+  const char* fn = "rbd_integrate_derivatives";
+  if (dtype == RBD_F32) {
+    DerivCall<float> r{false, (const float*)q, (const float*)v, (const float*)tau, nullptr, (float*)const_cast<void*>(vd),
+                       (float*)dq, (float*)dv, (float*)dtau, nullptr, nullptr};
+    r.vd_given = true;
+    return derivatives_t<float>(fn, model, dtype, B, B, r, stream);
+  }
+  DerivCall<double> r{false, (const double*)q, (const double*)v, (const double*)tau, nullptr, (double*)const_cast<void*>(vd),
+                      (double*)dq, (double*)dv, (double*)dtau, nullptr, nullptr};
+  r.vd_given = true;
+  return derivatives_t<double>(fn, model, dtype, B, B, r, stream);
+}
+}  // namespace rbd
 
 extern "C" int32_t rbd_dynamics_derivatives_ext(const rbd_model* model, int32_t dtype, int64_t B, int64_t ld, const void* q, const void* v,
                                                 const void* tau, const void* wext, void* vd_out, void* dvd_dq_out, void* dvd_dv_out,

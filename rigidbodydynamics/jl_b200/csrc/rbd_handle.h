@@ -204,6 +204,11 @@ int dynamics_vjp_dense(const rbd_model* model, int32_t dtype, int64_t B, const v
 // ... and the inverse-dynamics VJP on dense arrays (no external wrenches): q̄_cfg, v̄, v̇̄ of τ = ID(q, v, v̇) from τ̄; outputs may be NULL
 int inverse_dynamics_vjp_dense(const rbd_model* model, int32_t dtype, int64_t B, const void* q, const void* v, const void* vd,
                                const void* tau_bar, void* q_bar_cfg, void* v_bar, void* vd_bar, cudaStream_t stream);
+// rbd_deriv.cu's rbd_dynamics_derivatives_ext on dense [rows x B] arrays (no external wrenches) at a v̇ the caller already has:
+// dq, dv, dtau = ∂v̇/∂(q, v, τ) [nv*nv x B] each, with the public call's path selection (specialised or generic solve, factor on the
+// scratch, chunks of RBD_DERIV_SCRATCH_MB); the forward dynamics is not rerun
+int dynamics_derivatives_dense(const rbd_model* model, int32_t dtype, int64_t B, const void* q, const void* v, const void* tau,
+                               const void* vd, void* dq, void* dv, void* dtau, cudaStream_t stream);
 // The model limits of rbd_dynamics_vjp / rbd_inverse_dynamics_vjp (those of rbd_dynamics_derivatives): RBD_OK or RBD_EUNSUPPORTED
 int check_vjp_limits(const HostModel& hm, const char* who);
 // rbd_b200.cu's controller checks of rbd_integrate_pd (pd not NULL), leading dimension ld
